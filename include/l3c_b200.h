@@ -306,6 +306,16 @@ int l3c_partition_streams(int sm_a, int n_a, void **streams_a, int n_b, void **s
 int l3c_partition_streams2(int sm_a, int n_a, void **streams_a, int n_b_high, void **streams_b_high,
                            int n_b_low, void **streams_b_low, int *sm_a_out, int *sm_b_out);
 
+/* Test knob for the persistent tensor-core convolutions (3x3, 5x5/s2, 1x1, fused DMLL head), process-wide, from
+ * the next launch on.  0 = default for either argument.
+ *   max_sms > 0:      the SM count these kernels size their grid with becomes min(max_sms, SMs of the stream's
+ *                     partition group or of the device) -- few CTAs, many tiles per CTA and per pipe.
+ *   conv_smem_kb > 0: replaces L3C_CONV_SMEM_KB as the shared-memory budget (KB, clamped to [112, 227]) from which
+ *                     the FP16 kernels choose their number of pipeline stages.
+ * Lets small inputs exercise the stage rings, both pipes and every stage count; with both at 0 every launch
+ * configuration is the default one.  Not meant for production use. */
+int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb);
+
 #ifdef __cplusplus
 }
 #endif

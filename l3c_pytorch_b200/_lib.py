@@ -72,6 +72,7 @@ _SIGNATURES = {
     'l3c_pack_streams': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'l3c_partition_streams': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_partition_streams2': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    'l3c_set_conv_launch_limits': (c_int, [c_int, c_int]),
 }
 
 EXPORTS = sorted(_SIGNATURES)

@@ -46,6 +46,7 @@ int conv1x1_tc(const l3c_conv_t &p, cudaStream_t st);
 
 int sm_count();                          // SMs of the current device
 int stream_sm_count(cudaStream_t st);    // SMs available to kernels launched into `st` (partition.cu)
+int conv_smem_kb_override();             // l3c_set_conv_launch_limits' conv_smem_kb, 0 = none (partition.cu)
 
 // cudaFuncSetAttribute is per DEVICE: "done once" flags must be kept per device, or a process that drives a second
 // GPU launches its kernels there without the opt-in for > 48 KB of dynamic shared memory

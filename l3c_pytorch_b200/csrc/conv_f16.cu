@@ -654,17 +654,18 @@ lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
 
 // dynamic shared memory a conv CTA may take (bytes).  Default: everything an SM has (227 KB).  L3C_CONV_SMEM_KB
 // lowers it so that small latency-bound CTAs (the range decoders: 16 KB per stream) can be resident BESIDE a
-// conv CTA when no SM partition separates them (codec.lanes, L3C_SM_PARTITION=0).
+// conv CTA when no SM partition separates them (codec.lanes, L3C_SM_PARTITION=0).  l3c_set_conv_launch_limits
+// overrides both at the next launch.
 static int conv_smem_cap() {
-    static int cap = 0;
-    if (cap == 0) {
+    static const int env_kb = [] {
         const char *e = getenv("L3C_CONV_SMEM_KB");
-        int kb = e ? atoi(e) : 227;
-        if (kb < 112) kb = 112;
-        if (kb > 227) kb = 227;
-        cap = kb * 1024;
-    }
-    return cap;
+        return e ? atoi(e) : 227;
+    }();
+    const int over = conv_smem_kb_override();
+    int kb = over > 0 ? over : env_kb;
+    if (kb < 112) kb = 112;
+    if (kb > 227) kb = 227;
+    return kb * 1024;
 }
 
 namespace f16 {

@@ -8,6 +8,7 @@
 // so the decoders own theirs.  Everything stays in the primary context (same memory, same events).
 #include <cuda.h>
 
+#include <atomic>
 #include <mutex>
 #include <vector>
 
@@ -66,24 +67,45 @@ __global__ void partition_probe_kernel(int *out) {
 
 }  // namespace
 
-// SMs a kernel launched into `st` can use: the group size for a partition stream handed out by
-// l3c_partition_streams, the whole device otherwise (persistent kernels size their grid with it)
-int stream_sm_count(cudaStream_t st) {
-    {
-        std::lock_guard<std::mutex> lock(g_mu);
-        for (const Partition *p : g_parts) {
-            for (CUstream s : p->streams_a)
-                if ((cudaStream_t)s == st) return p->sm_a;
-            for (CUstream s : p->streams_b)
-                if ((cudaStream_t)s == st) return p->sm_b;
-            for (CUstream s : p->streams_b_low)
-                if ((cudaStream_t)s == st) return p->sm_b;
-        }
+namespace {
+// l3c_set_conv_launch_limits: 0 = no limit
+std::atomic<int> g_max_sms{0}, g_conv_smem_kb{0};
+
+int group_sm_count(cudaStream_t st) {
+    std::lock_guard<std::mutex> lock(g_mu);
+    for (const Partition *p : g_parts) {
+        for (CUstream s : p->streams_a)
+            if ((cudaStream_t)s == st) return p->sm_a;
+        for (CUstream s : p->streams_b)
+            if ((cudaStream_t)s == st) return p->sm_b;
+        for (CUstream s : p->streams_b_low)
+            if ((cudaStream_t)s == st) return p->sm_b;
     }
     return sm_count();
 }
 
+}  // namespace
+
+// SMs a kernel launched into `st` can use: the group size for a partition stream handed out by
+// l3c_partition_streams, the whole device otherwise, capped by l3c_set_conv_launch_limits (persistent kernels
+// size their grid with it)
+int stream_sm_count(cudaStream_t st) {
+    const int n = group_sm_count(st);
+    const int cap = g_max_sms.load(std::memory_order_relaxed);
+    return (cap > 0 && cap < n) ? cap : n;
+}
+
+int conv_smem_kb_override() { return g_conv_smem_kb.load(std::memory_order_relaxed); }
+
 }  // namespace l3c
+
+extern "C" int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb) {
+    L3C_REQUIRE(max_sms >= 0 && conv_smem_kb >= 0, "l3c_set_conv_launch_limits: bad arguments (%d, %d)", max_sms,
+                conv_smem_kb);
+    l3c::g_max_sms.store(max_sms);
+    l3c::g_conv_smem_kb.store(conv_smem_kb);
+    return L3C_OK;
+}
 
 extern "C" int l3c_partition_streams2(int sm_a, int n_a, void **streams_a, int n_b_high, void **streams_b_high,
                                       int n_b_low, void **streams_b_low, int *sm_a_out, int *sm_b_out);

@@ -3,6 +3,7 @@ streams); every computation on the hot path is a kernel of libl3c_b200.so.
 
 Activation convention inside the package: NHWC fp32 contiguous tensors `[N, H, W, pitch]`.
 """
+import contextlib
 import ctypes
 import os
 
@@ -93,6 +94,18 @@ def partition_streams2(device, sm_a, n_a, n_b_high, n_b_low):
             mk = lambda arr, n: [torch.cuda.ExternalStream(int(arr[i]), device=key[0]) for i in range(n)]
             _PARTITIONS[key] = (mk(a, n_a), mk(bh, n_b_high), mk(bl, n_b_low), got_a.value, got_b.value)
     return _PARTITIONS[key]
+
+
+@contextlib.contextmanager
+def conv_launch_limits(max_sms=0, conv_smem_kb=0):
+    """Test knob (l3c_set_conv_launch_limits): inside the block the persistent tensor-core convolutions size their
+    grid for at most `max_sms` SMs and choose their pipeline stages from a `conv_smem_kb` KB budget (0 = default).
+    Process-wide; the defaults are restored on exit."""
+    check(lib.l3c_set_conv_launch_limits(int(max_sms), int(conv_smem_kb)))
+    try:
+        yield
+    finally:
+        check(lib.l3c_set_conv_launch_limits(0, 0))
 
 
 def require_cuda(t, name):

@@ -228,8 +228,8 @@ def test_f16_conv_vs_torch_on_fp16_operands(cout, rate, H, W, kw):
 @pytest.mark.parametrize('cin,cout,H,W', [(192, 120, 9, 31), (192, 150, 16, 16), (64, 64, 8, 16), (192, 120, 64, 64),
                                           (128, 256, 5, 7)])
 def test_f16_1x1_conv(cin, cout, H, W):
-    """1x1 convs with Cin % 64 == 0 (the 192 -> Kp head) as one GEMM tile of 128 pixels x all output
-    channels; pixel counts that are not multiples of 128 and Cout that is not a multiple of 64."""
+    """1x1 convs with Cin % 64 == 0 (the 192 -> Kp head) as GEMM tiles of 64 pixels x all output
+    channels; pixel counts that are not multiples of 64 and Cout that is not a multiple of 64."""
     from l3c_pytorch_b200 import engine as E, _lib
     conv = _conv_module(cin, cout, 1)
     x = torch.randn(2, cin, H, W)

@@ -58,14 +58,18 @@ def test_forward_matches_oracle(cfg, H, W, prec):
 
 
 def test_get_P_reproduces_forward_bit_exactly(prec):
-    """decoder side (three incremental get_P calls, other batch size) == encoder side."""
+    """decoder side (three incremental get_P calls, other batch size) == encoder side; also when the decoder's
+    persistent conv kernels run on 3 SMs (a decode lane's SM group) and the forward on the whole device."""
+    from l3c_pytorch_b200 import engine as E
     bp = util.blueprint('cr')
     imgs = torch.stack([util.make_image(i, 48, 80) for i in range(3)]).cuda()
     out = bp.net(imgs)
-    F_prev = None
-    for s in (2, 1, 0):
-        l, F_prev = bp.net.get_P_nhwc(s, out.bn8[s + 1][1:2].contiguous(), F_prev)
-        assert torch.equal(l, out.P_nhwc[s][1:2]), s
+    for max_sms in (0, 3):
+        F_prev = None
+        with E.conv_launch_limits(max_sms=max_sms):
+            for s in (2, 1, 0):
+                l, F_prev = bp.net.get_P_nhwc(s, out.bn8[s + 1][1:2].contiguous(), F_prev)
+                assert torch.equal(l, out.P_nhwc[s][1:2]), (s, max_sms)
     # reference-shaped entry point
     l, F = bp.net.get_P(2, out.bn[3][1:2])
     assert torch.equal(l, out.P[2][1:2])
