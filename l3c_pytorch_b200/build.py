@@ -33,12 +33,13 @@ def build(verbose=False, force=False):
     build_dir = os.path.join(HERE, 'build')
     os.makedirs(build_dir, exist_ok=True)
     procs = []
+    # every object depends on every header: which source includes which is not tracked
+    headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith('.cuh')]
     for src in SOURCES:
         obj = os.path.join(build_dir, src.replace('.cu', '.o'))
         objs.append(obj)
         srcp = os.path.join(CSRC, src)
-        deps = [srcp, os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_ptx.cuh'),
-                os.path.join(os.path.dirname(HERE), 'include', 'l3c_b200.h')]
+        deps = [srcp, os.path.join(os.path.dirname(HERE), 'include', 'l3c_b200.h')] + headers
         if not force and os.path.isfile(obj) and os.path.getmtime(obj) >= max(map(os.path.getmtime, deps)):
             continue
         cmd = [nvcc] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-c', srcp, '-o', obj]

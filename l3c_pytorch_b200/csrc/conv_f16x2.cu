@@ -15,146 +15,64 @@
 // Kernel structure: conv_f16.cu's (weights resident, one halo box per filter column and plane, two consumer
 // warpgroups on alternate tiles); one stage per pipe, one pipe for dilations > 1 (shared memory: 144 KB of weights
 // + 40-64 KB per stage).  The 1x1 layers run conv1x1_tc_kernel<2, NB> (conv_f16.cu).
-#include <cuda.h>
-#include <cuda_fp16.h>
-
-#include "common.cuh"
-#include "tc_ptx.cuh"
+#include "tc_conv.cuh"
 
 namespace l3c {
 namespace f16x2 {
 using namespace tcx;
 
-constexpr int TH = 8, TW = 16;
 constexpr int W_TAP_BYTES = 64 * 128;
 constexpr int W_PLANE_BYTES = 9 * W_TAP_BYTES;        // 73728 per plane (hi / lo)
-constexpr float LO_SCALE = 2048.0f, LO_INV = 1.0f / 2048.0f;
-
-struct Params {
-    const float *bias;
-    const float *residual;
-    float *y;
-    __half *yh;            // split image or null
-    int N, H, W;
-    int Cout, y_pitch, y_coff;
-    int yh_pitch, yh_lo_off;
-    int dilation;
-    unsigned flags;
-    int tiles_x, tiles_y;
-};
-
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    uint32_t r;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
-    return r;
-}
-// (hi, lo) pair images of two floats
-__device__ __forceinline__ void split_h2(float a, float b, uint32_t &hi, uint32_t &lo) {
-    hi = pack_h2(a, b);
-    const float2 h = __half22float2(*reinterpret_cast<const __half2 *>(&hi));
-    lo = pack_h2((a - h.x) * LO_SCALE, (b - h.y) * LO_SCALE);
-}
-__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int tq) {
-    const bool hi2 = (tq & 2) != 0;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const uint32_t send = hi2 ? v[i] : v[i + 2];
-        const uint32_t got = __shfl_xor_sync(0xFFFFFFFFu, send, 2);
-        if (hi2) v[i] = got; else v[i + 2] = got;
-    }
-    const bool hi1 = (tq & 1) != 0;
-#pragma unroll
-    for (int i = 0; i < 4; i += 2) {
-        const uint32_t send = hi1 ? v[i] : v[i + 1];
-        const uint32_t got = __shfl_xor_sync(0xFFFFFFFFu, send, 1);
-        if (hi1) v[i] = got; else v[i + 1] = got;
-    }
-}
-
-// barriers per pipe: full, empty (one stage per pipe: 144 KB of weights + 40-64 KB per stage)
-constexpr int BARS_PER_PIPE = 2;
 
 __global__ void __launch_bounds__(THREADS, 1)
 conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                      const Params p, const int n_pipes, const int a_bytes, const int ptiles) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     // [weights hi 72 KB][weights lo 72 KB][pipe 0: hi box, lo box][pipe 1: ...][barriers]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 2 * W_PLANE_BYTES + n_pipes * 2 * a_bytes);
+    const uint32_t w_base = smem_u32(smem_aligned());
+    const uint32_t bars = w_base + 2 * W_PLANE_BYTES + n_pipes * 2 * a_bytes;
+    pipeline_init(bars, &map_x, &map_w);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t w_base = smem_u32(smem);
-    const uint32_t bar_base = smem_u32(bars);
-    const uint32_t wbar = bar_base + 8u * (2 * BARS_PER_PIPE);
-
-    if (threadIdx.x == 0) {
-        for (int k = 0; k < 2; ++k) {
-            mbar_init(bar_base + 8u * (BARS_PER_PIPE * k), 1);          // full
-            mbar_init(bar_base + 8u * (BARS_PER_PIPE * k + 1), 4);      // empty: one per consumer warp
-        }
-        mbar_init(wbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    }
-    __syncthreads();
-
+    const int k = warp < CONSUMER_WARPS ? warp >> 2 : warp - CONSUMER_WARPS;   // pipe
+    if (k >= n_pipes) return;
     const int d = p.dilation;
     const int ct = blockIdx.y;
     const int lo_ch = 64;                                  // lo plane of a 64-channel operand image
+    Ring ring(w_base + 2 * W_PLANE_BYTES, 2 * a_bytes, 1, bars, k);   // one stage (hi and lo box) per pipe
 
     if (warp >= CONSUMER_WARPS) {
         // ===================== TMA producer of pipe k =====================
-        const int k = warp - CONSUMER_WARPS;
-        if (k >= n_pipes || lane != 0) return;
-        const uint32_t a_base = w_base + 2 * W_PLANE_BYTES + k * 2 * a_bytes;
-        const uint32_t full = bar_base + 8u * (BARS_PER_PIPE * k), empty = full + 8u;
+        if (lane != 0) return;
         if (k == 0) {
-            mbar_expect_tx(wbar, 2 * W_PLANE_BYTES);
+            mbar_expect_tx(weight_bar(bars), 2 * W_PLANE_BYTES);
             for (int tap = 0; tap < 9; ++tap) {
                 const int row = tap * (int)gridDim.y * 64 + ct * 64;
-                tma_load_2d(w_base + tap * W_TAP_BYTES, &map_w, wbar, 0, row);                      // hi
-                tma_load_2d(w_base + W_PLANE_BYTES + tap * W_TAP_BYTES, &map_w, wbar, 64, row);     // lo
+                tma_load_2d(w_base + tap * W_TAP_BYTES, &map_w, weight_bar(bars), 0, row);                      // hi
+                tma_load_2d(w_base + W_PLANE_BYTES + tap * W_TAP_BYTES, &map_w, weight_bar(bars), 64, row);     // lo
             }
         }
-        uint32_t phase = 0;
-        for (int t = blockIdx.x + k * gridDim.x; t < ptiles; t += n_pipes * gridDim.x) {
-            int q = t;
-            const int tx = q % p.tiles_x; q /= p.tiles_x;
-            const int ty = q % p.tiles_y; q /= p.tiles_y;
-            const int n = q;
+        for_each_tile(k, n_pipes, ptiles, [&](int t) {
+            const Tile c = tile_of(p, t);
             for (int dx = 0; dx < 3; ++dx) {
-                mbar_wait(empty, phase ^ 1u);
-                mbar_expect_tx(full, 2 * a_bytes);
-                tma_load_4d(a_base, &map_x, full, 0, tx * TW + (dx - 1) * d, ty * TH - d, n);
-                tma_load_4d(a_base + a_bytes, &map_x, full, lo_ch, tx * TW + (dx - 1) * d, ty * TH - d, n);
-                phase ^= 1u;
+                const Slot s = ring.acquire(2 * a_bytes);
+                tma_load_4d(s.dst, &map_x, s.bar, 0, c.tx * TW + (dx - 1) * d, c.ty * TH - d, c.n);
+                tma_load_4d(s.dst + a_bytes, &map_x, s.bar, lo_ch, c.tx * TW + (dx - 1) * d, c.ty * TH - d, c.n);
             }
-        }
+        });
         return;
     }
 
     // ===================== consumer warpgroup k: wgmma + epilogue =====================
-    const int k = warp >> 2, w = warp & 3;
-    if (k >= n_pipes) return;
-    const uint32_t a_base = w_base + 2 * W_PLANE_BYTES + k * 2 * a_bytes;
-    const uint32_t full = bar_base + 8u * (BARS_PER_PIPE * k), empty = full + 8u;
-    const int tq = lane & 3, tr = lane >> 2;
-    const bool relu = (p.flags & L3C_CONV_RELU) != 0;
-    const bool shuffle = (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0;
-    uint32_t phase = 0;
-    mbar_wait(wbar, 0);
-    for (int t = blockIdx.x + k * gridDim.x; t < ptiles; t += n_pipes * gridDim.x) {
-        int q = t;
-        const int tx = q % p.tiles_x; q /= p.tiles_x;
-        const int ty = q % p.tiles_y; q /= p.tiles_y;
-        const int n = q;
+    const int w = warp & 3;
+    mbar_wait(weight_bar(bars), 0);
+    for_each_tile(k, n_pipes, ptiles, [&](int t) {
+        const Tile c = tile_of(p, t);
         float acc1[2][32], acc2[2][32];                   // hi*hi | hi*lo + lo*hi; rows 0..63 / 64..127
 #pragma unroll
         for (int h = 0; h < 2; ++h) { acc_zero(acc1[h]); acc_zero(acc2[h]); }
         for (int dx = 0; dx < 3; ++dx) {
-            mbar_wait(full, phase);
+            const uint32_t a_base = ring.wait();
             wgmma_fence();
 #pragma unroll
             for (int dy = 0; dy < 3; ++dy) {
@@ -177,95 +95,15 @@ conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
             wgmma_wait0();
 #pragma unroll
             for (int h = 0; h < 2; ++h) { acc_fence(acc1[h]); acc_fence(acc2[h]); }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty);
-            phase ^= 1u;
+            ring.release();
         }
-        // epilogue: fragment (h, column half c) = tile row 4h + w, pixels tr / tr + 8, columns 32c + 8jb + 2tq
+        // x = hi*hi + (hi*lo + lo*hi) / 2^11: combined before the epilogue, so that acc2 is dead there
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int oy = ty * TH + 4 * h + w;
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const float *v1 = acc1[h] + 16 * c, *v2 = acc2[h] + 16 * c;
-                const int cb = ct * 64 + 32 * c;
-#pragma unroll
-                for (int rh = 0; rh < 2; ++rh) {
-                    const int ox = tx * TW + tr + 8 * rh;
-                    const bool inside = (oy < p.H) && (ox < p.W);
-                    const size_t pix = ((size_t)n * p.H + oy) * p.W + ox;
-                    float a[4], b[4];
-#pragma unroll
-                    for (int jb = 0; jb < 4; ++jb) {
-                        const float2 bb = __ldg(reinterpret_cast<const float2 *>(p.bias + cb + 8 * jb + 2 * tq));
-                        a[jb] = __fmaf_rn(v2[4 * jb + 2 * rh], LO_INV, v1[4 * jb + 2 * rh]) + bb.x;
-                        b[jb] = __fmaf_rn(v2[4 * jb + 2 * rh + 1], LO_INV, v1[4 * jb + 2 * rh + 1]) + bb.y;
-                        if (relu) { a[jb] = fmaxf(a[jb], 0.f); b[jb] = fmaxf(b[jb], 0.f); }
-                    }
-                    if (!shuffle) {
-                        if (p.residual != nullptr && inside) {
-#pragma unroll
-                            for (int jb = 0; jb < 4; ++jb) {
-                                const float2 r = __ldg(reinterpret_cast<const float2 *>(
-                                    p.residual + pix * p.y_pitch + p.y_coff + cb + 8 * jb + 2 * tq));
-                                a[jb] += r.x; b[jb] += r.y;
-                            }
-                        }
-                        if (p.y != nullptr && inside) {
-                            const size_t off = pix * p.y_pitch + p.y_coff + cb;
-#pragma unroll
-                            for (int jb = 0; jb < 4; ++jb)
-                                *reinterpret_cast<float2 *>(p.y + off + 8 * jb + 2 * tq) = make_float2(a[jb], b[jb]);
-                        }
-                        if (p.yh != nullptr) {
-                            uint32_t hv[4], lv[4];
-#pragma unroll
-                            for (int jb = 0; jb < 4; ++jb) split_h2(a[jb], b[jb], hv[jb], lv[jb]);
-                            quad_transpose(hv, tq);
-                            quad_transpose(lv, tq);
-                            if (inside) {
-                                const size_t offh = pix * p.yh_pitch + p.y_coff + cb + 8 * tq;
-                                *reinterpret_cast<uint4 *>(p.yh + offh) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
-                                *reinterpret_cast<uint4 *>(p.yh + offh + p.yh_lo_off) = make_uint4(lv[0], lv[1], lv[2], lv[3]);
-                            }
-                        }
-                    } else {
-                        // out[n, 2*oy+si, 2*ox+sj, cq] = conv[n, oy, ox, 4*cq + 2*si + sj]   (edsr.py:92-101)
-                        const size_t W2 = 2 * (size_t)p.W;
-                        const size_t row0 = ((size_t)n * (2 * p.H) + 2 * oy) * W2 + 2 * ox;
-                        uint32_t fa[4], fb[4];
-#pragma unroll
-                        for (int jb = 0; jb < 4; ++jb) { fa[jb] = __float_as_uint(a[jb]); fb[jb] = __float_as_uint(b[jb]); }
-                        quad_transpose(fa, tq);               // fa[s] = channel c0 + 2s, fb[s] = channel c0 + 2s + 1
-                        quad_transpose(fb, tq);
-                        if (inside) {
-                            const int cq0 = (cb + 8 * tq) >> 2;
-#pragma unroll
-                            for (int si = 0; si < 2; ++si) {
-                                const float x00 = __uint_as_float(fa[si]), x01 = __uint_as_float(fa[2 + si]);   // sj = 0: cq0, cq0+1
-                                const float x10 = __uint_as_float(fb[si]), x11 = __uint_as_float(fb[2 + si]);   // sj = 1
-                                if (p.y != nullptr) {
-                                    const size_t o2 = (row0 + si * W2) * p.y_pitch + p.y_coff + cq0;
-                                    *reinterpret_cast<float2 *>(p.y + o2) = make_float2(x00, x01);
-                                    *reinterpret_cast<float2 *>(p.y + o2 + p.y_pitch) = make_float2(x10, x11);
-                                }
-                                if (p.yh != nullptr) {
-                                    const size_t oh = (row0 + si * W2) * p.yh_pitch + p.y_coff + cq0;
-                                    uint32_t h0, l0, h1, l1;
-                                    split_h2(x00, x01, h0, l0);
-                                    split_h2(x10, x11, h1, l1);
-                                    *reinterpret_cast<uint32_t *>(p.yh + oh) = h0;
-                                    *reinterpret_cast<uint32_t *>(p.yh + oh + p.yh_lo_off) = l0;
-                                    *reinterpret_cast<uint32_t *>(p.yh + oh + p.yh_pitch) = h1;
-                                    *reinterpret_cast<uint32_t *>(p.yh + oh + p.yh_pitch + p.yh_lo_off) = l1;
-                                }
-                            }
-                        }
-                    }
-                }
-            }
-        }
-    }
+            for (int i = 0; i < 32; ++i) acc1[h][i] = __fmaf_rn(acc2[h][i], LO_INV, acc1[h][i]);
+        image_epilogue<true>(p, c, ct, w, acc1);
+    });
 }
 
 // fp32 [n_px][C] -> split image [n_px][2*C]: for the activations that CUDA-core layers (5x5/s2, Cin = 3 / 5)
@@ -307,16 +145,6 @@ int conv2d_f16x2(const l3c_conv_t &p, cudaStream_t st) {
     L3C_REQUIRE(p.x_h && p.w_h && (p.y || p.y_h), "l3c_conv2d[f16x2]: x_h / w_h and an output are required");
     L3C_REQUIRE(p.cout_pad % 64 == 0 && p.cout_pad >= p.Cout, "l3c_conv2d[f16x2]: cout_pad=%d", p.cout_pad);
     L3C_REQUIRE(!(p.flags & ~(L3C_CONV_RELU | L3C_CONV_PIXEL_SHUFFLE2)), "l3c_conv2d[f16x2]: unsupported flags %u", p.flags);
-    EncodeTiledFn encode = get_encode_fn();
-    L3C_REQUIRE(encode != nullptr, "l3c_conv2d: cuTensorMapEncodeTiled is not available from the driver");
-    const int n_sm = stream_sm_count(st);
-    static bool configured_dev[64] = {};
-    bool &configured = configured_dev[current_device_slot()];
-    if (!configured) {
-        L3C_CUDA(cudaFuncSetAttribute(conv3x3_f16x2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        configured = true;
-    }
-    alignas(64) CUtensorMap map_x, map_w;
     if (k3) {
         L3C_REQUIRE(p.Cout % 64 == 0, "l3c_conv2d[f16x2]: 3x3 layers need Cout %% 64 == 0 (got %d)", p.Cout);
         const bool ps = (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0;
@@ -328,46 +156,18 @@ int conv2d_f16x2(const l3c_conv_t &p, cudaStream_t st) {
         const int d = p.dilation;
         const int a_rows = TH + 2 * d;
         const int a_bytes = a_rows * TW * 128;
-        const int room = 227 * 1024 - 1024 - 512 - 2 * W_PLANE_BYTES;
-        const int n_pipes = (2 * 2 * a_bytes <= room) ? 2 : 1;
-        L3C_REQUIRE(2 * a_bytes <= room, "l3c_conv2d[f16x2]: halo of dilation %d does not fit in shared memory", d);
-        {
-            cuuint64_t dims[4] = {128, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
-            cuuint64_t strides[3] = {256, (cuuint64_t)p.W * 256, (cuuint64_t)p.H * p.W * 256};
-            cuuint32_t box[4] = {64, TW, (cuuint32_t)a_rows, 1};
-            cuuint32_t estr[4] = {1, 1, 1, 1};
-            CUresult r = encode(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void *>(p.x_h), dims, strides, box,
-                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            L3C_REQUIRE(r == CUDA_SUCCESS, "l3c_conv2d[f16x2]: cuTensorMapEncodeTiled(x) failed with %d", (int)r);
-        }
-        {
-            cuuint64_t dims[2] = {128, (cuuint64_t)9 * p.cout_pad};
-            cuuint64_t strides[1] = {256};
-            cuuint32_t box[2] = {64, 64};
-            cuuint32_t estr[2] = {1, 1};
-            CUresult r = encode(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(p.w_h), dims, strides, box,
-                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            L3C_REQUIRE(r == CUDA_SUCCESS, "l3c_conv2d[f16x2]: cuTensorMapEncodeTiled(w) failed with %d", (int)r);
-        }
-        Params q;
-        q.bias = p.bias; q.residual = p.residual; q.y = p.y; q.yh = reinterpret_cast<__half *>(p.y_h);
-        q.N = p.N; q.H = p.H; q.W = p.W;
-        q.Cout = p.Cout; q.y_pitch = p.y_pitch; q.y_coff = p.y_coff;
-        q.yh_pitch = p.yh_pitch; q.yh_lo_off = p.yh_lo_off;
-        q.dilation = d; q.flags = p.flags;
-        q.tiles_x = ceil_div(p.W, TW);
-        q.tiles_y = ceil_div(p.H, TH);
-        const int cout_tiles = p.cout_pad / 64;
+        const RingPlan r = plan_ring(SMEM_MAX, 2 * W_PLANE_BYTES + SMEM_RESERVE, 2 * a_bytes, 1, true);
+        L3C_REQUIRE(r.n_stages >= 1, "l3c_conv2d[f16x2]: halo of dilation %d does not fit in shared memory", d);
+        alignas(64) CUtensorMap map_x, map_w;
+        if (!encode_tmap(&map_x, "l3c_conv2d[f16x2]", "x", CU_TENSOR_MAP_DATA_TYPE_FLOAT16, p.x_h, {128, p.W, p.H, p.N},
+                         {256, 256LL * p.W, 256LL * p.H * p.W}, {64, TW, a_rows, 1}) ||
+            !encode_tmap(&map_w, "l3c_conv2d[f16x2]", "w", CU_TENSOR_MAP_DATA_TYPE_FLOAT16, p.w_h, {128, 9LL * p.cout_pad},
+                         {256}, {64, 64}))
+            return L3C_EINVAL;
+        const Params q = conv_params(p, p.H, p.W);
         const int ptiles = p.N * q.tiles_x * q.tiles_y;
-        int per_ct = n_sm / cout_tiles;
-        if (per_ct < 1) per_ct = 1;
-        if (per_ct > ptiles) per_ct = ptiles;
-        const int smem_bytes = 2 * W_PLANE_BYTES + n_pipes * 2 * a_bytes + 1024 + 512;
-        conv3x3_f16x2_kernel<<<dim3(per_ct, cout_tiles), THREADS, smem_bytes, st>>>(map_x, map_w, q, n_pipes, a_bytes, ptiles);
-        L3C_LAUNCH_CHECK("conv3x3_f16x2_kernel");
-        return L3C_OK;
+        return launch_tc<conv3x3_f16x2_kernel>("conv3x3_f16x2_kernel", grid_3x3(st, p.cout_pad / 64, ptiles),
+                                               r.smem_bytes, st, map_x, map_w, q, r.n_pipes, a_bytes, ptiles);
     }
     return conv1x1_tc(p, st);
 }

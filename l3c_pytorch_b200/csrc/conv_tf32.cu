@@ -23,115 +23,65 @@
 // host side, activations by the producing layer's epilogue, which writes a second, rounded copy (`y_tf32`) next
 // to the fp32 tensor that residual adds and the fp32 layers keep using.
 // (The faster FP16-operand variant of this path is conv_f16.cu, precision L3C_PREC_F16.)
-#include <cuda.h>
-
-#include "common.cuh"
-#include "tc_ptx.cuh"
+#include "tc_conv.cuh"
 
 namespace l3c {
 
 namespace tc {
 using namespace tcx;
 
-constexpr int TH = 8, TW = 16;                 // 128 output pixels per tile
 constexpr int B_HALF = 64 * 128;               // 64 cout rows x 128 B (32 fp32 channels)
 constexpr int W_RES_BYTES = 9 * 2 * B_HALF;    // 147456
-constexpr int MAX_STAGES = 2;
-constexpr int BARS_PER_PIPE = 2 * MAX_STAGES;  // full[2], empty[2]
-
-struct Params {
-    const float *bias;      // padded to cout_pad
-    const float *residual;
-    float *y;
-    float *y_tf32;
-    int N, H, W;
-    int Cout, y_pitch, y_coff;
-    int dilation;
-    unsigned flags;
-    int tiles_x, tiles_y;
-};
 
 __global__ void __launch_bounds__(THREADS, 1)
 conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                     const Params p, const int n_pipes, const int n_stages, const int a_bytes, const int ptiles) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     // [weights 144 KB][pipe 0 stages][pipe 1 stages][barriers]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + W_RES_BYTES + n_pipes * n_stages * a_bytes);
+    const uint32_t w_base = smem_u32(smem_aligned());
+    const uint32_t bars = w_base + W_RES_BYTES + n_pipes * n_stages * a_bytes;
+    pipeline_init(bars, &map_x, &map_w);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t w_base = smem_u32(smem);
-    const uint32_t bar_base = smem_u32(bars);
-    const uint32_t wbar = bar_base + 8u * (2 * BARS_PER_PIPE);
-
-    if (threadIdx.x == 0) {
-        for (int k = 0; k < 2; ++k)
-            for (int s = 0; s < MAX_STAGES; ++s) {
-                mbar_init(bar_base + 8u * (BARS_PER_PIPE * k + s), 1);                  // full
-                mbar_init(bar_base + 8u * (BARS_PER_PIPE * k + MAX_STAGES + s), 4);     // empty: one per consumer warp
-            }
-        mbar_init(wbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    }
-    __syncthreads();
-
+    const int k = warp < CONSUMER_WARPS ? warp >> 2 : warp - CONSUMER_WARPS;   // pipe
+    if (k >= n_pipes) return;
     const int d = p.dilation;
     const int ct = blockIdx.y;                        // this CTA's Cout tile (weights stay resident)
+    Ring ring(w_base + W_RES_BYTES, a_bytes, n_stages, bars, k);
 
     if (warp >= CONSUMER_WARPS) {
         // ===================== TMA producer of pipe k =====================
-        const int k = warp - CONSUMER_WARPS;
-        if (k >= n_pipes || lane != 0) return;
-        const uint32_t a_base = w_base + W_RES_BYTES + k * n_stages * a_bytes;
-        const uint32_t full0 = bar_base + 8u * (BARS_PER_PIPE * k), empty0 = full0 + 8u * MAX_STAGES;
+        if (lane != 0) return;
         if (k == 0) {
-            mbar_expect_tx(wbar, W_RES_BYTES);
+            mbar_expect_tx(weight_bar(bars), W_RES_BYTES);
             for (int slab = 0; slab < 18; ++slab)     // slab = tap*2 + K-half; rows [slab][cout_pad]
-                tma_load_2d(w_base + slab * B_HALF, &map_w, wbar, 0, slab * (int)gridDim.y * 64 + ct * 64);
+                tma_load_2d(w_base + slab * B_HALF, &map_w, weight_bar(bars), 0, slab * (int)gridDim.y * 64 + ct * 64);
         }
-        uint32_t stage = 0, phase = 0;
-        for (int t = blockIdx.x + k * gridDim.x; t < ptiles; t += n_pipes * gridDim.x) {
-            int q = t;
-            const int tx = q % p.tiles_x; q /= p.tiles_x;
-            const int ty = q % p.tiles_y; q /= p.tiles_y;
-            const int n = q;
+        for_each_tile(k, n_pipes, ptiles, [&](int t) {
+            const Tile c = tile_of(p, t);
             for (int unit = 0; unit < 6; ++unit) {    // unit = dx*2 + K-half
-                mbar_wait(empty0 + 8u * stage, phase ^ 1u);
-                mbar_expect_tx(full0 + 8u * stage, a_bytes);
-                tma_load_4d(a_base + stage * a_bytes, &map_x, full0 + 8u * stage, (unit & 1) * 32,
-                            tx * TW + ((unit >> 1) - 1) * d, ty * TH - d, n);
-                if (++stage == (uint32_t)n_stages) { stage = 0; phase ^= 1u; }
+                const Slot s = ring.acquire(a_bytes);
+                tma_load_4d(s.dst, &map_x, s.bar, (unit & 1) * 32, c.tx * TW + ((unit >> 1) - 1) * d, c.ty * TH - d, c.n);
             }
-        }
+        });
         return;
     }
 
     // ===================== consumer warpgroup k: wgmma + epilogue =====================
-    const int k = warp >> 2, w = warp & 3;
-    if (k >= n_pipes) return;
-    const uint32_t a_base = w_base + W_RES_BYTES + k * n_stages * a_bytes;
-    const uint32_t full0 = bar_base + 8u * (BARS_PER_PIPE * k), empty0 = full0 + 8u * MAX_STAGES;
+    const int w = warp & 3;
     const int tq = lane & 3, tr = lane >> 2;              // column pair / row inside the fragment
     const bool relu = (p.flags & L3C_CONV_RELU) != 0;
     const bool shuffle = (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0;
     const bool round_y = (p.flags & L3C_CONV_ROUND_TF32) != 0;
-    uint32_t stage = 0, phase = 0;
-    mbar_wait(wbar, 0);
-    for (int t = blockIdx.x + k * gridDim.x; t < ptiles; t += n_pipes * gridDim.x) {
-        int q = t;
-        const int tx = q % p.tiles_x; q /= p.tiles_x;
-        const int ty = q % p.tiles_y; q /= p.tiles_y;
-        const int n = q;
+    mbar_wait(weight_bar(bars), 0);
+    for_each_tile(k, n_pipes, ptiles, [&](int t) {
+        const Tile c = tile_of(p, t);
         float acc[2][32];                                 // rows 0..63 / 64..127 of the tile
         acc_zero(acc[0]);
         acc_zero(acc[1]);
         for (int unit = 0; unit < 6; ++unit) {
-            mbar_wait(full0 + 8u * stage, phase);
             const int dx = unit >> 1, kh = unit & 1;
-            const uint32_t a0 = a_base + stage * a_bytes;
+            const uint32_t a0 = ring.wait();
             wgmma_fence();
 #pragma unroll
             for (int dy = 0; dy < 3; ++dy) {
@@ -148,25 +98,24 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
             wgmma_wait0();
             acc_fence(acc[0]);
             acc_fence(acc[1]);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty0 + 8u * stage);
-            if (++stage == (uint32_t)n_stages) { stage = 0; phase ^= 1u; }
+            ring.release();
         }
-        // epilogue: fragment (h, column half c) = tile row 4h + w, pixels tr / tr + 8, columns 32c + 8jb + 2tq
+        // epilogue: element pairs, so that y and its TF32 twin need no transpose; fragment (h, column half cc) =
+        // tile row 4h + w, pixels tr / tr + 8, columns 32cc + 8jb + 2tq
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            const int oy = ty * TH + 4 * h + w;
+            const int oy = c.ty * TH + 4 * h + w;
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const float *v = acc[h] + 16 * c;
+            for (int cc = 0; cc < 2; ++cc) {
+                const float *v = acc[h] + 16 * cc;
 #pragma unroll
                 for (int rh = 0; rh < 2; ++rh) {
-                    const int ox = tx * TW + tr + 8 * rh;
+                    const int ox = c.tx * TW + tr + 8 * rh;
                     if (oy >= p.H || ox >= p.W) continue;
-                    const size_t pix = ((size_t)n * p.H + oy) * p.W + ox;
+                    const size_t pix = ((size_t)c.n * p.H + oy) * p.W + ox;
 #pragma unroll
                     for (int jb = 0; jb < 4; ++jb) {
-                        const int co = ct * 64 + 32 * c + 8 * jb + 2 * tq;
+                        const int co = ct * 64 + 32 * cc + 8 * jb + 2 * tq;
                         const float2 bb = __ldg(reinterpret_cast<const float2 *>(p.bias + co));
                         float a = v[4 * jb + 2 * rh] + bb.x;
                         float b = v[4 * jb + 2 * rh + 1] + bb.y;
@@ -184,7 +133,7 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
                             // out[n, 2*oy+i, 2*ox+jj, cq] = conv[n, oy, ox, 4*cq + 2*i + jj]; co is even:
                             // (co, co+1) -> same cq and i, jj = 0 / 1 -> two horizontally adjacent pixels
                             const int cq = co >> 2, si = (co >> 1) & 1;
-                            const size_t o2 = (((size_t)n * (2 * p.H) + 2 * oy + si) * (2 * p.W) + 2 * ox) * p.y_pitch +
+                            const size_t o2 = (((size_t)c.n * (2 * p.H) + 2 * oy + si) * (2 * p.W) + 2 * ox) * p.y_pitch +
                                               p.y_coff + cq;
                             if (p.y_tf32) { p.y_tf32[o2] = round_tf32(a); p.y_tf32[o2 + p.y_pitch] = round_tf32(b); }
                             if (round_y) { a = round_tf32(a); b = round_tf32(b); }
@@ -195,24 +144,10 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
                 }
             }
         }
-    }
+    });
 }
 
 }  // namespace tc
-
-namespace tcx {
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-}  // namespace tcx
 
 int conv2d_tf32(const l3c_conv_t &p, cudaStream_t st) {
     using namespace tc;
@@ -231,70 +166,24 @@ int conv2d_tf32(const l3c_conv_t &p, cudaStream_t st) {
     L3C_REQUIRE(eligible, "l3c_conv2d: tf32 tensor-core path needs 3x3/Cin=64 or 1x1/Cin%%64==0, stride 1 "
                           "(got k=%d s=%d Cin=%d pitch=%d Cout=%d)", p.ksize, p.stride, p.Cin, p.x_pitch, p.Cout);
     if (k1) return conv1x1_tc(p, st);
-    EncodeTiledFn encode = get_encode_fn();
-    L3C_REQUIRE(encode != nullptr, "l3c_conv2d: cuTensorMapEncodeTiled is not available from the driver");
 
     const int d = p.dilation;
     const int a_rows = TH + 2 * d;
     const int a_bytes = a_rows * TW * 128;
-    const int room = 227 * 1024 - 1024 - 512 - W_RES_BYTES;
-    int n_pipes = 2, n_stages = 2;
-    if (2 * 2 * a_bytes > room) n_stages = 1;
-    if (2 * a_bytes > room) n_pipes = 1;
-    L3C_REQUIRE(a_rows <= 256 && a_bytes <= room, "l3c_conv2d[tf32]: halo of dilation %d does not fit in shared memory", d);
+    const RingPlan r = plan_ring(SMEM_MAX, W_RES_BYTES + SMEM_RESERVE, a_bytes, 2, true);
+    L3C_REQUIRE(a_rows <= 256 && r.n_stages >= 1, "l3c_conv2d[tf32]: halo of dilation %d does not fit in shared memory", d);
 
+    // tensor-core weight image: [tap][K-half = Cin/32][cout_pad][32] fp32 (engine.PackedConv.get_tc)
     alignas(64) CUtensorMap map_x, map_w;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
-        cuuint64_t strides[3] = {(cuuint64_t)p.x_pitch * 4, (cuuint64_t)p.W * p.x_pitch * 4,
-                                 (cuuint64_t)p.H * p.W * p.x_pitch * 4};
-        cuuint32_t box[4] = {32, TW, (cuuint32_t)a_rows, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = encode(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float *>(p.x), dims, strides, box,
-                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        L3C_REQUIRE(r == CUDA_SUCCESS, "l3c_conv2d: cuTensorMapEncodeTiled(x) failed with %d", (int)r);
-    }
-    const int cout_tiles = p.cout_pad / 64;
-    {
-        // tensor-core weight image: [tap][K-half = Cin/32][cout_pad][32] fp32 (engine.PackedConv.get_tc)
-        cuuint64_t dims[2] = {32, (cuuint64_t)9 * 2 * p.cout_pad};
-        cuuint64_t strides[1] = {128};
-        cuuint32_t box[2] = {32, 64};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = encode(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(p.w), dims, strides, box,
-                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        L3C_REQUIRE(r == CUDA_SUCCESS, "l3c_conv2d: cuTensorMapEncodeTiled(w) failed with %d", (int)r);
-    }
-    Params q;
-    q.bias = p.bias;
-    q.residual = p.residual;
-    q.y = p.y;
-    q.y_tf32 = p.y_tf32;
-    q.N = p.N; q.H = p.H; q.W = p.W;
-    q.Cout = p.Cout; q.y_pitch = p.y_pitch; q.y_coff = p.y_coff;
-    q.dilation = p.dilation;
-    q.flags = p.flags;
-    q.tiles_x = ceil_div(p.W, TW);
-    q.tiles_y = ceil_div(p.H, TH);
-
-    static bool configured_dev[64] = {};
-    bool &configured = configured_dev[current_device_slot()];
-    const int n_sm = stream_sm_count(st);          // the stream may be confined to a group of SMs
-    if (!configured) {
-        L3C_CUDA(cudaFuncSetAttribute(conv3x3_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        configured = true;
-    }
+    if (!encode_tmap(&map_x, "l3c_conv2d[tf32]", "x", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.x, {p.Cin, p.W, p.H, p.N},
+                     {4LL * p.x_pitch, 4LL * p.W * p.x_pitch, 4LL * p.H * p.W * p.x_pitch}, {32, TW, a_rows, 1}) ||
+        !encode_tmap(&map_w, "l3c_conv2d[tf32]", "w", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.w, {32, 18LL * p.cout_pad},
+                     {128}, {32, 64}))
+        return L3C_EINVAL;
+    const Params q = conv_params(p, p.H, p.W);
     const int ptiles = p.N * q.tiles_x * q.tiles_y;
-    int per_ct = n_sm / cout_tiles;
-    if (per_ct < 1) per_ct = 1;
-    if (per_ct > ptiles) per_ct = ptiles;
-    const int smem_bytes = W_RES_BYTES + n_pipes * n_stages * a_bytes + 1024 + 512;
-    conv3x3_tf32_kernel<<<dim3(per_ct, cout_tiles), THREADS, smem_bytes, st>>>(map_x, map_w, q, n_pipes, n_stages,
-                                                                               a_bytes, ptiles);
-    L3C_LAUNCH_CHECK("conv3x3_tf32_kernel");
-    return L3C_OK;
+    return launch_tc<conv3x3_tf32_kernel>("conv3x3_tf32_kernel", grid_3x3(st, p.cout_pad / 64, ptiles), r.smem_bytes,
+                                          st, map_x, map_w, q, r.n_pipes, r.n_stages, a_bytes, ptiles);
 }
 
 }  // namespace l3c

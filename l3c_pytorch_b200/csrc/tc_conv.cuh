@@ -1,0 +1,331 @@
+// tc_conv.cuh -- what the persistent tensor-core convolution kernels (conv_f16.cu, conv_tf32.cu, conv_f16x2.cu)
+// share: the shared-memory stage ring of a pipe with its mbarrier protocol, the tile walk, the epilogue of the
+// FP16-image 3x3 / 5x5 kernels, and the host side of a launch (tensor maps, shared-memory opt-in, stage and pipe
+// planning, grid size).
+//
+// CTA layout: warps 0..7 are two consumer warpgroups ("pipes"), each with its own TMA producer warp (warps 8, 9),
+// its own ring of shared-memory stages and its own tiles (alternate tiles of the CTA's sequence).  A consumer
+// issues wgmma on the staged operands, keeps the fp32 accumulators in registers and runs the fused epilogue
+// itself, so the epilogue of one pipe overlaps the MMAs of the other.  Accumulator fragment of wgmma m64nNk*:
+// thread t of the warpgroup, warp w = t / 32, lane l holds
+//   d[4j + 0], d[4j + 1] = (row 16w + l/4    , columns 8j + 2*(l%4) + {0,1})
+//   d[4j + 2], d[4j + 3] = (row 16w + l/4 + 8, same columns)
+// Dynamic shared memory, from a 1024 B (swizzle atom) aligned start: [resident weights][pipe 0 stages]
+// [pipe 1 stages][buffers of the kernel's own][barriers].
+#pragma once
+#include <initializer_list>
+
+#include "common.cuh"
+#include "tc_ptx.cuh"
+
+namespace l3c {
+namespace tcx {
+
+constexpr int MAX_STAGES = 4;                  // per pipe
+constexpr int SMEM_MAX = 227 * 1024;           // dynamic shared memory one CTA can opt in to
+constexpr int SMEM_RESERVE = 1024 + 512;       // alignment slack + barriers, part of every launch's fixed bytes
+constexpr int TH = 8, TW = 16;                 // output tile of the 3x3 / 5x5 kernels: 128 pixels
+
+// ----------------------------------------------------------------------------------------------------------------
+// device side
+// ----------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint8_t *smem_aligned() {
+    extern __shared__ uint8_t smem_raw[];
+    return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+}
+
+// barriers at `bars`: full[MAX_STAGES], empty[MAX_STAGES] of pipe 0, the same of pipe 1, then the weight barrier
+__device__ __forceinline__ uint32_t weight_bar(uint32_t bars) { return bars + 8u * (4 * MAX_STAGES); }
+
+// Thread 0 initialises the barriers (full: the producer's expect_tx; empty: one arrival per consumer warp) and
+// prefetches both tensor maps; then the whole CTA syncs.
+__device__ __forceinline__ void pipeline_init(uint32_t bars, const CUtensorMap *map_x, const CUtensorMap *map_w) {
+    if (threadIdx.x == 0) {
+        for (int k = 0; k < 2; ++k)
+            for (int s = 0; s < MAX_STAGES; ++s) {
+                mbar_init(bars + 8u * (2 * MAX_STAGES * k + s), 1);
+                mbar_init(bars + 8u * (2 * MAX_STAGES * k + MAX_STAGES + s), 4);
+            }
+        mbar_init(weight_bar(bars), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(map_x) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(map_w) : "memory");
+    }
+    __syncthreads();
+}
+
+struct Slot {
+    uint32_t dst, bar;     // stage address, its full barrier
+};
+
+// The ring of pipe k: n_stages stages of `stride` bytes from `base` (pipe 0's stages, then pipe 1's).  Producer
+// and consumer each walk it with their own copy; phase flips every time the ring wraps.
+struct Ring {
+    uint32_t base, stride, bars, n_stages, stage, phase;
+
+    __device__ __forceinline__ Ring(uint32_t stages_base, uint32_t stride_, uint32_t n_stages_, uint32_t bars_, int k)
+        : base(stages_base + k * n_stages_ * stride_), stride(stride_), bars(bars_ + 8u * (2 * MAX_STAGES * k)),
+          n_stages(n_stages_), stage(0), phase(0) {}
+
+    __device__ __forceinline__ void advance() {
+        if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+    }
+    // producer: wait until the consumer has released the next stage, arm its full barrier for `bytes` of TMA
+    __device__ __forceinline__ Slot acquire(uint32_t bytes) {
+        mbar_wait(bars + 8u * (MAX_STAGES + stage), phase ^ 1u);
+        const Slot s = {base + stage * stride, bars + 8u * stage};
+        mbar_expect_tx(s.bar, bytes);
+        advance();
+        return s;
+    }
+    // consumer: wait until the next stage has landed; returns its address
+    __device__ __forceinline__ uint32_t wait() {
+        mbar_wait(bars + 8u * stage, phase);
+        return base + stage * stride;
+    }
+    // consumer, after wgmma_wait0() and the accumulator fences: hand the stage back (one arrival per warp)
+    __device__ __forceinline__ void release() {
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(bars + 8u * (MAX_STAGES + stage));
+        advance();
+    }
+};
+
+// The tiles pipe k of this CTA runs: from blockIdx.x + k * gridDim.x in steps of n_pipes * gridDim.x, so that the
+// pipes of a CTA take alternate tiles of the CTA's sequence.
+template <class F>
+__device__ __forceinline__ void for_each_tile(int k, int n_pipes, int n_tiles, F &&f) {
+    for (int t = blockIdx.x + k * gridDim.x; t < n_tiles; t += n_pipes * gridDim.x) f(t);
+}
+
+// 3x3 / 5x5 layers (conv3x3_tf32_kernel, conv_f16_kernel, conv3x3_f16x2_kernel)
+struct Params {
+    const float *bias;      // padded to cout_pad
+    const float *residual;  // fp32, layout of y, or null
+    float *y;               // fp32 output or null
+    float *y_tf32;          // tf32: TF32-rounded twin of y or null
+    __half *yh;             // f16: FP16 image of the output, f16x2: split image; or null
+    int N, H, W;            // H, W: the output pixels the tiles cover
+    int Cout, y_pitch, y_coff;
+    int yh_pitch, yh_lo_off;   // f16x2: pitch of the split image, offset of its lo plane
+    int dilation;
+    unsigned flags;
+    int tiles_x, tiles_y;
+};
+
+struct Tile {
+    int tx, ty, n;
+};
+__device__ __forceinline__ Tile tile_of(const Params &p, int t) {
+    return {t % p.tiles_x, t / p.tiles_x % p.tiles_y, t / p.tiles_x / p.tiles_y};
+}
+
+// fp32 pair -> operand image: FP16 pair, or with SPLIT its hi and lo pairs
+template <bool SPLIT>
+__device__ __forceinline__ void to_image(float a, float b, uint32_t &hi, uint32_t &lo) {
+    if (SPLIT) split_h2(a, b, hi, lo);
+    else hi = pack_h2(a, b);
+}
+
+// Epilogue of the FP16-image 3x3 / 5x5 kernels (conv_f16_kernel, conv3x3_f16x2_kernel; SPLIT: f16x2) for tile c of
+// Cout tile ct, consumer warp w; acc[h] holds the conv values of tile half h.  Adds the bias, ReLU, the fp32
+// residual, and writes the fp32 output (float2: full sectors) and the operand image (16-byte vectors after a 4x4
+// transpose inside each quad; SPLIT: hi and lo planes yh_lo_off apart), or PixelShuffle(2) of both.
+// Fragment (h, column half cc) = tile row 4h + w, pixels tr / tr + 8, columns 32cc + 8jb + 2tq.
+template <bool SPLIT>
+__device__ __forceinline__ void image_epilogue(const Params &p, const Tile &c, int ct, int w, const float (&acc)[2][32]) {
+    const int lane = threadIdx.x & 31, tq = lane & 3, tr = lane >> 2;   // column pair / row inside the fragment
+    const bool relu = (p.flags & L3C_CONV_RELU) != 0;
+    const bool shuffle = (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0;
+    const int hp = SPLIT ? p.yh_pitch : p.y_pitch;                        // pitch of the operand image
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int oy = c.ty * TH + 4 * h + w;
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+            const int cb = ct * 64 + 32 * cc;                             // first conv channel of this fragment
+#pragma unroll
+            for (int rh = 0; rh < 2; ++rh) {
+                const int ox = c.tx * TW + tr + 8 * rh;
+                const bool inside = (oy < p.H) && (ox < p.W);
+                const size_t pix = ((size_t)c.n * p.H + oy) * p.W + ox;
+                float a[4], b[4];
+#pragma unroll
+                for (int jb = 0; jb < 4; ++jb) {
+                    const float2 bb = __ldg(reinterpret_cast<const float2 *>(p.bias + cb + 8 * jb + 2 * tq));
+                    a[jb] = acc[h][16 * cc + 4 * jb + 2 * rh] + bb.x;
+                    b[jb] = acc[h][16 * cc + 4 * jb + 2 * rh + 1] + bb.y;
+                    if (relu) { a[jb] = fmaxf(a[jb], 0.f); b[jb] = fmaxf(b[jb], 0.f); }
+                }
+                if (!shuffle) {
+                    const size_t off = pix * p.y_pitch + p.y_coff + cb;
+                    if (p.residual != nullptr && inside) {
+#pragma unroll
+                        for (int jb = 0; jb < 4; ++jb) {
+                            const float2 r = __ldg(reinterpret_cast<const float2 *>(p.residual + off + 8 * jb + 2 * tq));
+                            a[jb] += r.x; b[jb] += r.y;
+                        }
+                    }
+                    if (p.y != nullptr && inside) {
+#pragma unroll
+                        for (int jb = 0; jb < 4; ++jb)
+                            *reinterpret_cast<float2 *>(p.y + off + 8 * jb + 2 * tq) = make_float2(a[jb], b[jb]);
+                    }
+                    if (p.yh != nullptr) {
+                        uint32_t hv[4], lv[4];
+#pragma unroll
+                        for (int jb = 0; jb < 4; ++jb) to_image<SPLIT>(a[jb], b[jb], hv[jb], lv[jb]);
+                        quad_transpose(hv, tq);               // -> channels cb + 8*tq + 0..7
+                        if (SPLIT) quad_transpose(lv, tq);
+                        if (inside) {
+                            const size_t oh = pix * hp + p.y_coff + cb + 8 * tq;
+                            *reinterpret_cast<uint4 *>(p.yh + oh) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
+                            if (SPLIT) *reinterpret_cast<uint4 *>(p.yh + oh + p.yh_lo_off) = make_uint4(lv[0], lv[1], lv[2], lv[3]);
+                        }
+                    }
+                } else {
+                    // out[n, 2*oy+si, 2*ox+sj, cq] = conv[n, oy, ox, 4*cq + 2*si + sj]   (edsr.py:92-101)
+                    const size_t W2 = 2 * (size_t)p.W;
+                    const size_t row0 = ((size_t)c.n * (2 * p.H) + 2 * oy) * W2 + 2 * ox;   // output pixel (si=0, sj=0)
+                    // after the transpose thread tq owns conv channels c0 + 0..7 (c0 = cb + 8*tq) = output channels
+                    // cq0, cq0 + 1 of the four sub-pixels, and a quad writes 32 contiguous bytes per output pixel
+                    uint32_t fa[4], fb[4];
+#pragma unroll
+                    for (int jb = 0; jb < 4; ++jb) { fa[jb] = __float_as_uint(a[jb]); fb[jb] = __float_as_uint(b[jb]); }
+                    quad_transpose(fa, tq);                   // fa[s] = channel c0 + 2s, fb[s] = channel c0 + 2s + 1
+                    quad_transpose(fb, tq);
+                    if (inside) {
+                        const int cq0 = (cb + 8 * tq) >> 2;
+#pragma unroll
+                        for (int si = 0; si < 2; ++si) {
+                            const float x00 = __uint_as_float(fa[si]), x01 = __uint_as_float(fa[2 + si]);   // sj = 0: cq0, cq0+1
+                            const float x10 = __uint_as_float(fb[si]), x11 = __uint_as_float(fb[2 + si]);   // sj = 1
+                            if (p.y != nullptr) {
+                                const size_t o2 = (row0 + si * W2) * p.y_pitch + p.y_coff + cq0;
+                                *reinterpret_cast<float2 *>(p.y + o2) = make_float2(x00, x01);
+                                *reinterpret_cast<float2 *>(p.y + o2 + p.y_pitch) = make_float2(x10, x11);
+                            }
+                            if (p.yh != nullptr) {
+                                const size_t oh = (row0 + si * W2) * hp + p.y_coff + cq0;
+                                uint32_t h0, l0, h1, l1;
+                                to_image<SPLIT>(x00, x01, h0, l0);
+                                to_image<SPLIT>(x10, x11, h1, l1);
+                                *reinterpret_cast<uint32_t *>(p.yh + oh) = h0;
+                                if (SPLIT) *reinterpret_cast<uint32_t *>(p.yh + oh + p.yh_lo_off) = l0;
+                                *reinterpret_cast<uint32_t *>(p.yh + oh + hp) = h1;
+                                if (SPLIT) *reinterpret_cast<uint32_t *>(p.yh + oh + hp + p.yh_lo_off) = l1;
+                            }
+                        }
+                    }
+                }
+            }
+        }
+    }
+}
+
+// ----------------------------------------------------------------------------------------------------------------
+// host side
+// ----------------------------------------------------------------------------------------------------------------
+
+// Params of a 3x3 / 5x5 launch whose tiles cover H x W output pixels
+static inline Params conv_params(const l3c_conv_t &p, int H, int W) {
+    Params q;
+    q.bias = p.bias; q.residual = p.residual; q.y = p.y; q.y_tf32 = p.y_tf32;
+    q.yh = reinterpret_cast<__half *>(p.y_h);
+    q.N = p.N; q.H = H; q.W = W;
+    q.Cout = p.Cout; q.y_pitch = p.y_pitch; q.y_coff = p.y_coff;
+    q.yh_pitch = p.yh_pitch; q.yh_lo_off = p.yh_lo_off;
+    q.dilation = p.dilation; q.flags = p.flags;
+    q.tiles_x = ceil_div(W, TW);
+    q.tiles_y = ceil_div(H, TH);
+    return q;
+}
+
+// TMA map of a dense tensor at `base` as the kernels read it: 128B swizzle, 128 B L2 promotion, zero fill out of
+// bounds (the conv padding).  dims innermost first, strides in bytes of dims 1.., box in elements, element strides
+// 1 unless given.  On failure sets the error (`who`: the entry point, `what`: the operand) and returns false.
+inline bool encode_tmap(CUtensorMap *map, const char *who, const char *what, CUtensorMapDataType dt, const void *base,
+                        std::initializer_list<long long> dims, std::initializer_list<long long> strides,
+                        std::initializer_list<int> box, std::initializer_list<int> estr = {}) {
+    typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
+                                      const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
+                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    static EncodeTiledFn encode = nullptr;
+    if (!encode) {
+        void *fn = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess &&
+            qres == cudaDriverEntryPointSuccess)
+            encode = reinterpret_cast<EncodeTiledFn>(fn);
+    }
+    if (!encode) {
+        set_error("%s: cuTensorMapEncodeTiled is not available from the driver", who);
+        return false;
+    }
+    const int rank = (int)dims.size();
+    cuuint64_t d[5], s[5];
+    cuuint32_t b[5], e[5];
+    for (int i = 0; i < rank; ++i) {
+        d[i] = (cuuint64_t)dims.begin()[i];
+        s[i] = i + 1 < rank ? (cuuint64_t)strides.begin()[i] : 0;
+        b[i] = (cuuint32_t)box.begin()[i];
+        e[i] = estr.size() ? (cuuint32_t)estr.begin()[i] : 1;
+    }
+    const CUresult r = encode(map, dt, rank, const_cast<void *>(base), d, s, b, e, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("%s: cuTensorMapEncodeTiled(%s) failed with %d", who, what, (int)r);
+        return false;
+    }
+    return true;
+}
+
+struct RingPlan {
+    int n_pipes, n_stages, smem_bytes;   // n_stages == 0: the layer does not fit
+};
+
+// Stages per pipe: as many as fit in `budget` beside `fixed` bytes (resident weights, the kernel's own buffers,
+// SMEM_RESERVE) with two pipes, at most max_stages.  If not even one fits: one stage per pipe above the budget if
+// two pipes fit in SMEM_MAX, else one pipe with one stage where the kernel can run with one pipe.
+static inline RingPlan plan_ring(int budget, int fixed, int stage_bytes, int max_stages, bool one_pipe_ok = false) {
+    int n = (budget - fixed) / (2 * stage_bytes);
+    if (n > max_stages) n = max_stages;
+    if (n < 1 && fixed + 2 * stage_bytes <= SMEM_MAX) n = 1;
+    if (n >= 1) return {2, n, fixed + 2 * n * stage_bytes};
+    if (one_pipe_ok && fixed + stage_bytes <= SMEM_MAX) return {1, 1, fixed + stage_bytes};
+    return {2, 0, 0};
+}
+
+// 3x3 / 5x5 grid: gridDim.y = Cout tiles (resident weights), gridDim.x = the stream's SMs shared among them, at
+// least 1 and at most one CTA per pixel tile
+static inline dim3 grid_3x3(cudaStream_t st, int cout_tiles, int ptiles) {
+    int per_ct = stream_sm_count(st) / cout_tiles;
+    if (per_ct < 1) per_ct = 1;
+    if (per_ct > ptiles) per_ct = ptiles;
+    return dim3(per_ct, cout_tiles);
+}
+
+// 1x1 grid: two pipes per CTA, at most one CTA per SM of the stream
+static inline int grid_1x1(cudaStream_t st, int n_tiles) {
+    const int n_sm = stream_sm_count(st);
+    return ceil_div(n_tiles, 2) < n_sm ? ceil_div(n_tiles, 2) : n_sm;
+}
+
+// Launches a persistent tensor-core kernel under `name` (the launch log).  The opt-in to SMEM_MAX bytes of
+// dynamic shared memory is per device, so it is done once per device and kernel.
+template <auto Kernel, class... Args>
+int launch_tc(const char *name, dim3 grid, int smem_bytes, cudaStream_t st, const Args &...args) {
+    static bool configured_dev[64] = {};
+    bool &configured = configured_dev[current_device_slot()];
+    if (!configured) {
+        L3C_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
+        configured = true;
+    }
+    Kernel<<<grid, THREADS, smem_bytes, st>>>(args...);
+    L3C_LAUNCH_CHECK(name);
+    return L3C_OK;
+}
+
+}  // namespace tcx
+}  // namespace l3c

@@ -1,15 +1,9 @@
 // tc_ptx.cuh -- thin PTX wrappers shared by the tensor-core convolution kernels (sm_90a): mbarriers, TMA
-// (cp.async.bulk.tensor), wgmma shared-memory descriptors and warpgroup MMA issue.
-//
-// Kernel layout shared by conv_tf32.cu, conv_f16.cu and conv_f16x2.cu: warps 0..7 are two consumer warpgroups
-// ("pipes"), each with its own TMA producer warp (warps 8, 9), its own shared-memory stages and its own tiles
-// (alternate tiles of the CTA's sequence).  A consumer issues wgmma on the staged operands, keeps the fp32
-// accumulators in registers and runs the fused epilogue itself, so the epilogue of one pipe overlaps the MMAs of
-// the other.  Accumulator fragment of wgmma m64nNk*: thread t of the warpgroup, warp w = t / 32, lane l holds
-//   d[4j + 0], d[4j + 1] = (row 16w + l/4    , columns 8j + 2*(l%4) + {0,1})
-//   d[4j + 2], d[4j + 3] = (row 16w + l/4 + 8, same columns)
+// (cp.async.bulk.tensor), wgmma shared-memory descriptors and warpgroup MMA issue, and the FP16 operand-image
+// conversions.  The kernel skeleton built on them is in tc_conv.cuh.
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace l3c {
@@ -115,10 +109,39 @@ __device__ __forceinline__ float round_tf32(float x) {      // round-to-nearest 
 // named barrier of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode_fn();    // conv_tf32.cu
+// two floats -> packed fp16 pair, round-to-nearest-even, saturating to +-65504
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+    uint32_t r;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));   // d.hi = first source
+    return r;
+}
+constexpr float LO_SCALE = 2048.0f, LO_INV = 1.0f / 2048.0f;   // precision mode f16x2: x = hi + lo / 2^11
+// (hi, lo) pair images of two floats (precision mode f16x2)
+__device__ __forceinline__ void split_h2(float a, float b, uint32_t &hi, uint32_t &lo) {
+    hi = pack_h2(a, b);
+    const float2 h = __half22float2(*reinterpret_cast<const __half2 *>(&hi));
+    lo = pack_h2((a - h.x) * LO_SCALE, (b - h.y) * LO_SCALE);
+}
+
+// 4x4 transpose inside each quad of lanes: before, thread tq holds v[j] = element (column block j, pair tq);
+// after, thread tq holds v[s] = element (column block tq, pair s) -> 8 consecutive channels = 16 bytes.
+// Must be executed by all 32 lanes.
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int tq) {
+    const bool hi2 = (tq & 2) != 0;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const uint32_t send = hi2 ? v[i] : v[i + 2];
+        const uint32_t got = __shfl_xor_sync(0xFFFFFFFFu, send, 2);
+        if (hi2) v[i] = got; else v[i + 2] = got;
+    }
+    const bool hi1 = (tq & 1) != 0;
+#pragma unroll
+    for (int i = 0; i < 4; i += 2) {
+        const uint32_t send = hi1 ? v[i] : v[i + 1];
+        const uint32_t got = __shfl_xor_sync(0xFFFFFFFFu, send, 1);
+        if (hi1) v[i] = got; else v[i + 1] = got;
+    }
+}
 
 }  // namespace tcx
 }  // namespace l3c

@@ -25,7 +25,8 @@ RTOL, ATOL = 2e-5, 2e-5            # f16x2 against float64 (test_gpu_conv.py)
 RTOL_OP, ATOL_OP = 1e-4, 1e-4      # f16 / tf32 against fp32 on the same rounded operands
 
 # ---------------------------------------------------------------------------------------------
-# launch plans: the host code of conv_f16.cu, conv_tf32.cu and conv_f16x2.cu restated (test infrastructure)
+# launch plans: the host code (plan_ring, grid_3x3, grid_1x1 in tc_conv.cuh and their callers) restated
+# (test infrastructure)
 # ---------------------------------------------------------------------------------------------
 SMEM_MAX = 227 * 1024
 RESERVE = 1024 + 512               # alignment slack + barriers, reserved by every launcher

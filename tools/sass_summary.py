@@ -31,7 +31,7 @@ def main():
             continue
         if cur is None:
             continue
-        m = re.match(r'\s*/\*[0-9a-f]{4}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_]+)', line)
+        m = re.match(r'\s*/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_]+)', line)
         if m:
             op = m.group(1)
             per[cur]['_all'] += 1
