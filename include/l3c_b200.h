@@ -252,6 +252,25 @@ int l3c_rgb_prep(const uint8_t *img_dev, const float *A1, const float *b1, const
  * (0 outside the image), elements 27..63 zero -- the 3 -> 64 conv then runs as a K = 64 GEMM on the tensor cores. */
 int l3c_rgb_im2col_f16(const uint8_t *img_dev, const float *A1, const float *b1, const float *A2, const float *b2,
                        int N, int H, int W, void *out_h_dev, void *stream);
+/* l3c_rgb_im2col_f16 for a ragged batch (DESIGN §4.6): image n occupies [0,h_n) x [0,w_n) of the padded H x W
+ * planes, extents_dev int32 [N][2] = (h_n, w_n), and taps outside that extent are 0 as at the tensor border.
+ * extents_dev = NULL is l3c_rgb_im2col_f16. */
+int l3c_rgb_im2col_f16_ragged(const uint8_t *img_dev, const float *A1, const float *b1, const float *A2,
+                              const float *b2, int N, int H, int W, const int *extents_dev, void *out_h_dev,
+                              void *stream);
+
+/* Ragged batches (DESIGN §4.6): padded NHWC / planar tensors in which image n occupies [0,h_n) x [0,w_n);
+ * extents_dev int32 [N][2] = (h_n, w_n) at the tensor's resolution.
+ * l3c_ragged_zero_halo: sets the band of `halo` pixels right of and below every image (clipped to the tensor) of an
+ * NHWC tensor with px_bytes bytes per pixel (a multiple of 4) to +0 -- run on the input of a k x k conv, it gives
+ * every output pixel inside its image the operands of the per-image launch.
+ * l3c_ragged_pack: N * planes planes of H x W elements of elem_bytes bytes (plane n * planes + q belongs to image
+ * n); to_compact != 0: padded raster -> compact planes of compact_len elements holding the h_n * w_n elements of
+ * the image row-major, then zeros; to_compact == 0: compact -> padded raster with zeros outside the image. */
+int l3c_ragged_zero_halo(void *x_dev, int px_bytes, int N, int H, int W, const int *extents_dev, int halo,
+                         void *stream);
+int l3c_ragged_pack(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
+                    const int *extents_dev, long long compact_len, int to_compact, void *stream);
 
 /* L3C_PREC_F16X2: fp32 [n_px][C] -> split operand image FP16 [n_px][2*C] (hi = fp16(x) in channels [0,C),
  * lo = fp16((x - hi) * 2^11) in [C,2C)); C % 4 == 0.  For the outputs of the CUDA-core layers of that mode (no

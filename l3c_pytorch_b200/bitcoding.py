@@ -7,7 +7,9 @@ bpsp` (int64 CHW/1CHW image; asserts `pout` does not exist; crops -> `pout.part{
 file bytes * 8 / PADDED sub-pixels, crops combined weighted by unpadded H*W, :63-71,108-110),
 `decode(pin) -> int64 1CHW`, the helper functions for the header fields and the magic separator.
 
-Added (H100-first): `encode_batch` / `decode_batch` for many equally sized images per call.
+Added (H100-first): `encode_batch` / `decode_batch` for many images per call.  Where the codec supports ragged
+batches (f16, learned bottlenecks, reference layout: BatchCodec.ragged_unsupported) images of any sizes share one
+network pass and one range-coder launch (DESIGN §4.6); elsewhere images are grouped by shape.
 """
 import os
 
@@ -20,6 +22,30 @@ from .codec import BatchCodec, MAGIC
 from .times import NoOp
 
 _MAGIC_VALUE_SEP = MAGIC
+
+# Largest N * Hmax * Wmax (padded pixels of the batch tensor) coded in one ragged pass: 16 images of up to 768 x 768
+# (tools/bench_mixed.py) -- the activations, mixture parameters and CDF rows of such a pass fit an 80 GB GPU.
+RAGGED_PASS_PIXELS = 16 * 768 * 768
+
+
+def plan_passes(shapes, budget=None):
+    """shapes: padded (H, W) per image -> lists of image indices, one per ragged pass.  Images are sorted by shape
+    (ties in input order) and consecutive ones share a pass while N * Hmax * Wmax stays within `budget` (default
+    RAGGED_PASS_PIXELS); an image larger than the budget is a pass of its own."""
+    budget = RAGGED_PASS_PIXELS if budget is None else budget
+    order = sorted(range(len(shapes)), key=lambda i: (tuple(shapes[i]), i))
+    passes, cur, hm, wm = [], [], 0, 0
+    for i in order:
+        h, w = shapes[i]
+        nh, nw = max(hm, h), max(wm, w)
+        if cur and (len(cur) + 1) * nh * nw > budget:
+            passes.append(cur)
+            cur, nh, nw = [], h, w
+        cur.append(i)
+        hm, wm = nh, nw
+    if cur:
+        passes.append(cur)
+    return passes
 
 
 class Bitcoding(object):
@@ -39,15 +65,44 @@ class Bitcoding(object):
     def _device(self):
         return self.blueprint.device
 
-    def _prepare(self, img):
+    def _prepare(self, img, quiet=False):
         """-> (uint8 [1,3,H',W'] padded, on device; padding tuple)."""
         factor = 2 ** self.blueprint.net.config_ms.num_scales
+        if img.dim() == 3:
+            img = img.unsqueeze(0)
         _, _, H, W = img.shape
         padding_tuple = (0, 0, 0, 0)
         if H % factor != 0 or W % factor != 0:
-            print(f'*** INFO: image shape ({H}X{W}) not divisible by {factor}, will pad.')
+            if not quiet:
+                print(f'*** INFO: image shape ({H}X{W}) not divisible by {factor}, will pad.')
             img, padding_tuple = pad.pad(img, fac=factor, mode=MultiscaleBlueprint.get_padding_mode())
         return img.to(torch.uint8).to(self._device()).contiguous(), padding_tuple
+
+    def _passes(self, prepared):
+        """Index groups of `prepared` [(uint8 [1,3,H,W], padding tuple)] coded in one pass each: ragged passes
+        (plan_passes) where the codec supports them, else one group per (shape, padding tuple)."""
+        if self.codec.ragged_unsupported(self.tile) is None:
+            return plan_passes([tuple(t.shape[-2:]) for (t, _) in prepared])
+        groups = {}
+        for i, (t, pt) in enumerate(prepared):
+            groups.setdefault((tuple(t.shape), pt), []).append(i)
+        return list(groups.values())
+
+    def _begin_pass(self, prepared, idxs):
+        """Enqueue the encode of prepared[idxs] as one batch on the current stream -> codec EncodeJob.  Images of
+        different shapes are placed top-left in a zero batch of the largest extent (a ragged batch)."""
+        imgs = [prepared[i][0] for i in idxs]
+        pts = [prepared[i][1] for i in idxs]
+        shapes = [tuple(t.shape[-2:]) for t in imgs]
+        if all(sh == shapes[0] for sh in shapes):
+            batch = torch.cat(imgs, 0) if len(imgs) > 1 else imgs[0]
+            pt = pts[0] if all(p == pts[0] for p in pts) else pts
+            return self.codec.encode_begin(batch, pt, tile=self.tile)
+        Hb, Wb = max(h for (h, _) in shapes), max(w for (_, w) in shapes)
+        batch = torch.zeros(len(imgs), 3, Hb, Wb, dtype=torch.uint8, device=self._device())
+        for k, t in enumerate(imgs):
+            batch[k, :, :t.shape[2], :t.shape[3]] = t[0]
+        return self.codec.encode_begin(batch, pts, tile=self.tile, extents=shapes)
 
     def encode(self, img, pout):
         """img: int64 (or uint8) CHW / 1CHW tensor with values 0..255; writes `pout`; returns bpsp."""
@@ -75,8 +130,15 @@ class Bitcoding(object):
         return self._encode_many([img], [pout])[0]
 
     def _encode_many(self, imgs, pouts):
-        """Images of equal (padded) shape are coded as one batch."""
+        """Images are coded in ragged passes (any mix of shapes, plan_passes) where the codec supports them;
+        otherwise, and with compare_with_theory, images of equal (padded) shape are coded as one batch."""
         prepared = [self._prepare(im) for im in imgs]
+        if not self.compare_with_theory and self.codec.ragged_unsupported(self.tile) is None:
+            datas, bpsps = self._encode_prepared(prepared).finish()
+            for i, dta in enumerate(datas):
+                with open(pouts[i], 'wb') as f:
+                    f.write(dta)
+            return bpsps
         groups = {}
         for i, (t, pt) in enumerate(prepared):
             groups.setdefault((tuple(t.shape), pt), []).append(i)
@@ -124,14 +186,33 @@ class Bitcoding(object):
     # ------------------------------------------------------------------------------------------
     # H100-first batch API
     def encode_batch(self, imgs_u8):
-        """imgs_u8: uint8 [N,3,H,W] (any device) -> (list of container bytes, bpsp list)."""
+        """imgs_u8: uint8 [N,3,H,W] (any device), or a list / tuple of uint8 [3,H,W] / [1,3,H,W] images of any
+        sizes -> (list of container bytes, bpsp list) in input order."""
         return self.encode_batch_begin(imgs_u8).finish()
+
+    def _encode_prepared(self, prepared):
+        """Enqueue the passes of `prepared` on the current stream -> _ListEncodeJob."""
+        jobs = [(idxs, self._begin_pass(prepared, idxs)) for idxs in self._passes(prepared)]
+        return _ListEncodeJob(jobs, [int(np.prod(t.shape[1:])) for (t, _) in prepared])
 
     def encode_batch_begin(self, imgs_u8, stream=None):
         """Asynchronous encode_batch: enqueues the upload and the whole GPU side on `stream` (default:
         the current stream) and returns a job at once; job.finish() -> (containers, bpsps).  With
         `stream=self.side_stream(N)` the encode runs beside a decode_batch of another batch: the
-        decode is bound by the serial range decoder and leaves most of the GPU idle."""
+        decode is bound by the serial range decoder and leaves most of the GPU idle.
+
+        A list / tuple of images: each is padded on its own (as encode() does) and the images are coded in ragged
+        passes (plan_passes): one network pass and one range-coder launch per pass, containers byte-identical to
+        coding each image alone.  Where the codec does not support ragged batches (ragged_unsupported) images of
+        different padded shapes raise NotImplementedError."""
+        if isinstance(imgs_u8, (list, tuple)):
+            stream = stream if stream is not None else torch.cuda.current_stream(self._device())
+            with torch.cuda.stream(stream):
+                prepared = [self._prepare(im, quiet=True) for im in imgs_u8]
+                why = self.codec.ragged_unsupported(self.tile)
+                if why is not None and len({tuple(t.shape) for (t, _) in prepared}) > 1:
+                    raise NotImplementedError(why)
+                return self._encode_prepared(prepared)
         factor = 2 ** self.blueprint.net.config_ms.num_scales
         pt = pad.padding_tuple(imgs_u8.shape[-2], imgs_u8.shape[-1], factor)
         stream = stream if stream is not None else torch.cuda.current_stream(self._device())
@@ -154,21 +235,44 @@ class Bitcoding(object):
         return self.codec.lanes(self._device(), 3 * n_images, n_lanes)[0]
 
     def decode_batch(self, datas, lane=None):
-        """list of container bytes (any mix of shapes) -> list of int64 1CHW tensors (GPU)."""
-        from .codec import parse_container
-        keys = {}
-        for i, d in enumerate(datas):
-            pt, scales = parse_container(d)
-            keys.setdefault((pt, tuple((C, H, W) for (C, H, W, _) in scales)), []).append(i)
+        """list of container bytes (any mix of shapes) -> list of int64 1CHW tensors (GPU).  Ragged passes
+        (plan_passes) where the codec supports them, else one pass per shape."""
+        from .codec import parse_container, container_tile
+        parsed = [parse_container(d) for d in datas]
+        if self.codec.ragged_unsupported(container_tile(datas[0]) if datas else None) is None and \
+                all(len(p[1]) and container_tile(d) is None for p, d in zip(parsed, datas)):
+            passes = plan_passes([p[1][-1][1:3] for p in parsed])
+        else:
+            keys = {}
+            for i, (pt, scales) in enumerate(parsed):
+                keys.setdefault((pt, tuple((C, H, W) for (C, H, W, _) in scales)), []).append(i)
+            passes = list(keys.values())
         outs = [None] * len(datas)
-        for (pt, _), idxs in keys.items():
+        for idxs in passes:
             S, _ = self.codec.decode_batch([datas[i] for i in idxs], to_host=False, lane=lane)
             for k, i in enumerate(idxs):
-                img = S[k:k + 1].long()
+                pt, scales = parsed[i]
+                H, W = scales[-1][1:3] if scales else S.shape[-2:]
+                img = S[k:k + 1, :, :H, :W].long()
                 if any(pt):
                     img = pad.undo_pad(img, *pt)
                 outs[i] = img
         return outs
+
+
+class _ListEncodeJob:
+    """encode_batch_begin of a list: the codec jobs of its passes; finish() -> (containers, bpsps) in input order."""
+
+    def __init__(self, jobs, nsubs):
+        self.jobs, self.nsubs = jobs, nsubs
+
+    def finish(self):
+        datas = [None] * len(self.nsubs)
+        for idxs, job in self.jobs:
+            d, _ = job.finish(to_host=True)
+            for k, i in enumerate(idxs):
+                datas[i] = d[k]
+        return datas, [len(d) * 8 / n for d, n in zip(datas, self.nsubs)]
 
 
 class _BatchEncodeJob:

@@ -3,7 +3,8 @@ reference-shaped `Bitcoding` class (bitcoding.py) drives.
 
 What the reference does one image, one scale, one channel at a time with a GPU->CPU round trip per
 channel (/root/reference/src/bitcoding/bitcoding.py:85-123,163-294, coders.py:38-90) is done here
-for a whole batch of equally sized images with
+for a whole batch of images -- equally sized, or of any mix of sizes (a ragged batch, DESIGN §4.6: f16, learned
+bottlenecks, the reference layout) -- with
   * ONE network pass,
   * one interval kernel per scale (no CDF table on the encode side),
   * ONE range-coder launch covering every stream of every image (N * 18 warps for L3C),
@@ -178,16 +179,20 @@ class EncodeJob:
         codec, N, per_img, caps, shapes = self.codec, self.N, self.per_img, self.caps, self.shapes
         self.coded.synchronize()                                                   # sync #1 (tiny)
         lens = self.lens_host.numpy().astype(np.int64).reshape(N, per_img)
-        if (lens > caps[None, :]).any():
+        if (lens > (caps if caps.ndim == 2 else caps[None, :])).any():
             raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
         with torch.cuda.stream(self.stream):
             # ---- container layout + gather + single D2H
-            layout = ContainerLayout(shapes, self.tile)
+            # a ragged batch has one layout and one padding tuple per image
+            layouts = [ContainerLayout(sh, self.tile) for sh in self.shapes_of] if self.ragged else \
+                [ContainerLayout(shapes, self.tile)] * N
+            pt = self.pad_tuple
+            pads = pt if (len(pt) and isinstance(pt[0], (tuple, list))) else [pt] * N
             sizes, pieces_all, dst = [], [], np.zeros((N, per_img), np.int64)
             pos = 0
             starts = []
             for n in range(N):
-                total, pieces, offs = layout.header_and_offsets(lens[n], self.pad_tuple)
+                total, pieces, offs = layouts[n].header_and_offsets(lens[n], pads[n])
                 starts.append(pos)
                 dst[n] = pos + np.asarray(offs, np.int64)
                 pieces_all.append(pieces)
@@ -197,6 +202,8 @@ class EncodeJob:
             E.pack_streams(self.desc_dev, self.lens_dev, dst.reshape(-1), N * per_img, blob)
             info = dict(sizes=sizes, starts=starts, lens=lens, shapes=shapes, out=self.out, stream_offsets=dst,
                         tile=self.tile)
+            if self.ragged:
+                info['shapes_of'] = self.shapes_of                                  # [image][(scale, C, H, W)]
             if not to_host:
                 self.packed = torch.cuda.Event()
                 self.packed.record(self.stream)
@@ -253,40 +260,70 @@ class BatchCodec(object):
         return self.net.nets[0].enc._consts(device)[1]
 
     # ------------------------------------------------------------------------------------------
-    def encode_batch(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, to_host=True, tile=None):
-        """imgs_u8: uint8 [N,3,H,W] on the GPU, H and W multiples of 2**num_scales.
+    def encode_batch(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, to_host=True, tile=None, extents=None):
+        """imgs_u8: uint8 [N,3,H,W] on the GPU, H and W multiples of 2**num_scales.  pad_tuple: the padding
+        tuple written into every container, or a list of one per image.
         Returns a list of N container byte strings (or, with to_host=False, the device blob,
         per-image sizes and offsets, leaving the bytes in HBM).  `out`: a precomputed network Out.
-        tile = (th, tw): tiled containers (ContainerLayout)."""
-        return self.encode_begin(imgs_u8, pad_tuple, out, tile).finish(to_host)
+        tile = (th, tw): tiled containers (ContainerLayout).
+        extents = [(h_n, w_n)]: a ragged batch (encode_begin)."""
+        return self.encode_begin(imgs_u8, pad_tuple, out, tile, extents).finish(to_host)
+
+    def ragged_unsupported(self, tile=None):
+        """Why this codec cannot code a ragged batch (a message naming it), or None when it can."""
+        if self.net._rgb:
+            return 'ragged batches are not supported by the RGB baselines (bicubic encoder)'
+        if not E.f16_mode():
+            return 'ragged batches run in precision f16 only, not %s' % E.get_conv_precision()
+        if tile is not None:
+            return 'ragged batches are not supported with tiled containers (tile=%s)' % (tuple(tile),)
+        return None
+
+    def _ragged_extents(self, extents, N, H, W, tile):
+        """Validated [(h_n, w_n)] of a ragged batch of N images in an H x W tensor, or None when every image fills
+        the tensor (then the call is the equal-size one, with the same kernel arguments)."""
+        if extents is None:
+            return None
+        ext = [(int(h), int(w)) for (h, w) in extents]
+        fac = 2 ** self.net.config_ms.num_scales
+        if len(ext) != N:
+            raise ValueError('%d extents for a batch of %d images' % (len(ext), N))
+        for (h, w) in ext:
+            if not (1 <= h <= H and 1 <= w <= W) or h % fac or w % fac:
+                raise ValueError('extent %dx%d must lie in the %dx%d batch and be a multiple of %d'
+                                 % (h, w, H, W, fac))
+        if all(e == (H, W) for e in ext):
+            return None
+        why = self.ragged_unsupported(tile)
+        if why is not None:
+            raise NotImplementedError(why)
+        return ext
 
     @_on_device
-    def encode_begin(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, tile=None):
+    def encode_begin(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, tile=None, extents=None):
         """First half of encode_batch: enqueues the whole GPU side of an encode (networks, intervals,
         the range-coder launch, the copy of the stream lengths to pinned memory) on the CURRENT stream
         and returns without waiting.  EncodeJob.finish() completes it.  Lets a caller overlap the
-        encode of one batch with other work, e.g. the latency-bound decode of the previous batch."""
+        encode of one batch with other work, e.g. the latency-bound decode of the previous batch.
+
+        extents = [(h_n, w_n)]: a ragged batch (DESIGN §4.6): image n is the top-left h_n x w_n of imgs_u8[n]
+        (zero elsewhere; multiples of 2**num_scales), pad_tuple is then a list of per-image tuples (or one for
+        all), and every container is byte-identical to the one of that image encoded on its own -- one network
+        pass and one range-coder launch for the batch.  f16, learned bottlenecks, reference layout only.
+        Extents that all equal the tensor are the equal-size call."""
         assert imgs_u8.dtype == torch.uint8 and imgs_u8.dim() == 4 and imgs_u8.shape[1] == 3
         dev = imgs_u8.device
         N = imgs_u8.shape[0]
+        ext = self._ragged_extents(extents, N, imgs_u8.shape[2], imgs_u8.shape[3], tile)
+        if ext is not None:
+            return self._encode_begin_ragged(imgs_u8, pad_tuple, out, ext)
         if out is None:
             out = self.net(imgs_u8, intervals_of=self.blueprint.losses)      # f16 mode: DMLL head fused into the convs
-        K = self.net.config_ms.prob.K
 
         # ---- per-symbol intervals, scale by scale (coarse -> fine = container order)
-        ivs, shapes = [], []
-        for scale, dmll, uniform in self.iter_scale_dmll():
-            S = out.S_u8[scale]
-            _, C, H, W = S.shape
-            shapes.append((scale, C, H, W))
-            if uniform:
-                ivs.append(E.lut_intervals(S, self._uniform(dmll.L, dev)[0]))
-            elif out.IV is not None and out.IV[scale] is not None:
-                ivs.append(out.IV[scale])                                    # produced by the fused head
-            else:
-                l = out.P_nhwc[scale]
-                assert non_shared_get_K(l.shape[-1], C) == K
-                ivs.append(E.dmll_intervals(l, S, dmll.targets(dev), C, K, dmll.L, dmll.rgb_scale))
+        scale_ivs = self._scale_intervals(out, dev)
+        shapes = [sh for (sh, _) in scale_ivs]
+        ivs = [iv for (_, iv) in scale_ivs]
 
         # ---- one range-coder launch for all streams; descriptor order = (image, scale, channel[, tile])
         if tile is not None:
@@ -321,21 +358,102 @@ class BatchCodec(object):
         job.keep = (imgs_u8, ivs, slots)                       # alive until finish()
         job.N, job.per_img, job.caps, job.shapes, job.out, job.tile = N, per_img, caps, shapes, out, tile
         job.pad_tuple, job.desc_dev, job.lens_dev, job.lens_host, job.dev = pad_tuple, desc_dev, lens_dev, lens_host, dev
+        job.ragged = False
+        return job
+
+    def _scale_intervals(self, out, dev):
+        """Coding intervals of every scale, coarse -> fine: [(shape (scale, C, H, W), int32 [N][C][H*W])]."""
+        K = self.net.config_ms.prob.K
+        res = []
+        for scale, dmll, uniform in self.iter_scale_dmll():
+            S = out.S_u8[scale]
+            _, C, H, W = S.shape
+            if uniform:
+                iv = E.lut_intervals(S, self._uniform(dmll.L, dev)[0])
+            elif out.IV is not None and out.IV[scale] is not None:
+                iv = out.IV[scale]                                           # produced by the fused head
+            else:
+                l = out.P_nhwc[scale]
+                assert non_shared_get_K(l.shape[-1], C) == K
+                iv = E.dmll_intervals(l, S, dmll.targets(dev), C, K, dmll.L, dmll.rgb_scale)
+            res.append(((scale, C, H, W), iv))
+        return res
+
+    def _encode_begin_ragged(self, imgs_u8, pad_tuple, out, ext):
+        """encode_begin of a ragged batch: the interval planes of every scale are gathered into per-image compact
+        planes (the order the streams read them in) and every stream gets its own length and slot."""
+        dev = imgs_u8.device
+        N, _, Hb, Wb = imgs_u8.shape
+        if pad_tuple and isinstance(pad_tuple[0], (tuple, list)):
+            pads = [tuple(int(v) for v in p) for p in pad_tuple]
+            if len(pads) != N:
+                raise ValueError('%d padding tuples for a batch of %d images' % (len(pads), N))
+        else:
+            pads = [tuple(int(v) for v in pad_tuple)] * N
+        if out is None:
+            out = self.net(imgs_u8, intervals_of=self.blueprint.losses, extents=ext)
+        shapes, ivs, ext_s, planes = [], [], [], []
+        for (scale, C, H, W), iv in self._scale_intervals(out, dev):
+            f = Hb // H
+            es = [(h // f, w // f) for (h, w) in ext]
+            plane = max(h * w for (h, w) in es)
+            shapes.append((scale, C, H, W))
+            ivs.append(E.ragged_pack(iv, C, H, W, E._to_device_async(np.asarray(es, np.int32), dev), plane, True))
+            ext_s.append(es)
+            planes.append(plane)
+        shapes_of = [[(scale, C, ext_s[si][n][0], ext_s[si][n][1]) for si, (scale, C, _, _) in enumerate(shapes)]
+                     for n in range(N)]
+        # one range-coder launch; descriptor order = (image, scale, channel) as in the equal-size call
+        streams = [(si, c) for si, (_, C, _, _) in enumerate(shapes) for c in range(C)]
+        per_img = len(streams)
+        st = np.array(streams, np.int64)
+        hw = np.array([[h * w for (h, w) in es] for es in ext_s], np.int64).T                # [N][scale]
+        n_sym = hw[:, st[:, 0]]                                                                # [N][per_img]
+        caps = ((n_sym * 17 + 7) // 8 + 64 + 3) & ~3                                          # _slot_cap
+        slot_off = np.concatenate([[0], np.cumsum(caps.reshape(-1))])
+        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
+        desc = np.zeros(N * per_img, dtype=_lib.ENC_STREAM_DTYPE)
+        d = desc.reshape(N, per_img)
+        bases = np.array([iv.data_ptr() for iv in ivs], np.int64)
+        Cs = np.array([C for (_, C, _, _) in shapes], np.int64)[st[:, 0]]
+        pl = np.array(planes, np.int64)[st[:, 0]]
+        img = np.arange(N, dtype=np.int64)[:, None]
+        d['intervals'][:] = bases[st[:, 0]][None, :] + ((img * Cs[None, :] + st[None, :, 1]) * pl[None, :]) * 4
+        d['n_sym'][:] = n_sym
+        d['out_cap'][:] = caps
+        d['out'][:] = slots.data_ptr() + slot_off[:-1].reshape(N, per_img)
+        desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
+        lens_host = torch.empty(lens_dev.shape, dtype=lens_dev.dtype, pin_memory=True)
+        lens_host.copy_(lens_dev, non_blocking=True)
+        job = EncodeJob()
+        job.codec, job.stream = self, torch.cuda.current_stream()
+        job.coded = torch.cuda.Event()
+        job.coded.record(job.stream)
+        job.keep = (imgs_u8, ivs, slots)
+        job.N, job.per_img, job.caps, job.shapes, job.out, job.tile = N, per_img, caps, shapes, out, None
+        job.pad_tuple, job.desc_dev, job.lens_dev, job.lens_host, job.dev = pads, desc_dev, lens_dev, lens_host, dev
+        job.ragged, job.shapes_of = True, shapes_of
         return job
 
     # ------------------------------------------------------------------------------------------
     @_on_device
     def decode_batch(self, datas, to_host=True, lane=None):
-        """datas: list of container byte strings of equally shaped images.
+        """datas: list of container byte strings of equally shaped images -- or, where ragged batches are supported
+        (ragged_unsupported), of any mix of shapes: image n then is the top-left H_n x W_n of the result (the
+        finest scale of its container), zero elsewhere.
         Returns (uint8 [N,3,H,W] incl. padding, pad_tuple list)."""
         dev = self.blueprint.device
         N = len(datas)
         parsed = [parse_container(d) for d in datas]
         ref_shapes = [(C, H, W) for (C, H, W, _) in parsed[0][1]]
         tile = container_tile(datas[0])
+        shapes_of = [[(C, H, W) for (C, H, W, _) in p[1]] for p in parsed]
         for p, dta in zip(parsed, datas):
-            if [(C, H, W) for (C, H, W, _) in p[1]] != ref_shapes or container_tile(dta) != tile:
+            if container_tile(dta) != tile or \
+                    ([(C, H, W) for (C, H, W, _) in p[1]] != ref_shapes and self.ragged_unsupported(tile) is not None):
                 raise ValueError('decode_batch needs containers of identical shape')
+        if any(len(sh) != len(ref_shapes) for sh in shapes_of):
+            raise ValueError('decode_batch: containers with different numbers of scales')
         # one upload of everything
         starts = np.zeros(N, np.int64)
         pos = 0
@@ -350,7 +468,7 @@ class BatchCodec(object):
         offs = np.array([[starts[n] + o for (_, _, _, st) in parsed[n][1] for (o, _) in st] for n in range(N)],
                         np.int64)
         lens = np.array([[ln for (_, _, _, st) in parsed[n][1] for (_, ln) in st] for n in range(N)], np.int64)
-        S = self.decode_device(blob, offs, lens, ref_shapes, lane=lane, tile=tile)
+        S = self.decode_device(blob, offs, lens, shapes_of, lane=lane, tile=tile)
         pads = [p[0] for p in parsed]
         if to_host:
             return S.cpu(), pads
@@ -471,9 +589,21 @@ class BatchCodec(object):
         has made `lane.main` the current stream.  Without it the range decoders of the bottleneck scales run
         on the current stream and the RGB scale on lane 0 of a one-lane partition.
         `tile` = (th, tw): the streams are the tiles of a tiled container (ContainerLayout): thousands of short
-        streams, so the three RGB channels are simply decoded one after the other, all tiles at once."""
+        streams, so the three RGB channels are simply decoded one after the other, all tiles at once.
+        shapes may also be one list per image: a ragged batch (DESIGN §4.6) when they differ; image n then is the
+        top-left H_n x W_n of the result, zero elsewhere."""
         dev = blob.device
         N = offs.shape[0]
+        if shapes and isinstance(shapes[0][0], (tuple, list)):
+            shapes = [[tuple(int(v) for v in s) for s in sh] for sh in shapes]
+            if len(shapes) != N:
+                raise ValueError('%d shape lists for %d images' % (len(shapes), N))
+            if any(sh != shapes[0] for sh in shapes):
+                why = self.ragged_unsupported(tile)
+                if why is not None:
+                    raise NotImplementedError(why)
+                return self._decode_ragged(blob, offs, lens, shapes, lane)
+            shapes = shapes[0]
         if len(shapes) != self.net.scales + 1:
             raise ValueError('container has %d scales, model expects %d' % (len(shapes), self.net.scales + 1))
         K = self.net.config_ms.prob.K
@@ -533,6 +663,67 @@ class BatchCodec(object):
                     self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
             if tile is not None:
                 S = E.reorder_tiles(S, H, W, tile, False)                   # back to raster planes
+            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else 'S%d' % scale))
+            if scale > 0:
+                bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
+        return S
+
+    def _decode_ragged(self, blob, offs, lens, shapes_of, lane):
+        """decode_device of a ragged batch: the streams of image n decode into the first H_n * W_n symbols of
+        per-image compact planes (the CDF rows are built there too, from the gathered mixture parameters); the
+        decoded planes are scattered back into the zero-padded planes the networks of the next scale read."""
+        dev = blob.device
+        N = len(shapes_of)
+        for sh in shapes_of:
+            if len(sh) != self.net.scales + 1:
+                raise ValueError('container has %d scales, model expects %d' % (len(sh), self.net.scales + 1))
+            self._check_shapes(sh)
+        K = self.net.config_ms.prob.K
+        fin = [(sh[-1][1], sh[-1][2]) for sh in shapes_of]
+        Hb, Wb = max(h for (h, _) in fin), max(w for (_, w) in fin)
+        bn8, F_prev, S = None, None, None
+        j0 = 0
+        self._mark('start')
+        for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll()):
+            C = shapes_of[0][idx][0]
+            H, W = Hb >> scale, Wb >> scale
+            es = [(sh[idx][1], sh[idx][2]) for sh in shapes_of]
+            hw = np.array([h * w for (h, w) in es], np.int64)
+            plane = int(hw.max())
+            ext_dev = E._to_device_async(np.asarray(es, np.int32), dev)
+            Sc = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # compact planes (stream order)
+            desc = np.zeros(N * C, dtype=_lib.DEC_STREAM_DTYPE)
+            d = desc.reshape(N, C)
+            d['in'][:] = blob.data_ptr() + offs[:, j0:j0 + C]
+            d['in_len'][:] = lens[:, j0:j0 + C]
+            j0 += C
+            d['n_sym'][:] = hw[:, None]
+            pl = (np.arange(N)[:, None] * C + np.arange(C)[None, :]) * plane
+            d['sym_out'][:] = Sc.data_ptr() + pl
+            if uniform:
+                d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
+                d['row_pitch'][:] = 0
+                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
+            else:
+                l, F_prev = self.net.get_P_nhwc(scale, bn8, F_prev if self.net._fuse_feat else None, extents=fin)
+                self._mark('net%d' % scale)
+                if tuple(l.shape[1:3]) != (H, W) or non_shared_get_K(l.shape[-1], C) != K:
+                    raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
+                                     % (scale, C, H, W, tuple(l.shape)))
+                # per-pixel kernels from here on: the compact planes are an N x 1 x plane "image" each
+                lc = E.ragged_pack(l, 1, H, W, ext_dev, plane, True).view(N, 1, plane, l.shape[-1])
+                Sv = Sc.view(N, C, 1, plane)
+                pitch = E.table_pitch(dmll.L)
+                table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
+                d['table'][:] = table.data_ptr() + pl * (pitch * 2)
+                d['row_pitch'][:] = pitch
+                tg = dmll.targets(dev)
+                if dmll.rgb_scale:
+                    self._decode_rgb_pipelined(lc, Sv, tg, C, K, dmll.L, table, d, dev, lane=lane)
+                else:
+                    E.dmll_build_table(lc, Sv, tg, C, K, dmll.L, False, -1, table)
+                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
+            S = E.ragged_pack(Sc, C, H, W, ext_dev, plane, False)                 # zero-padded [N][C][H][W]
             self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else 'S%d' % scale))
             if scale > 0:
                 bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))

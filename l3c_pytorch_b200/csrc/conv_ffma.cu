@@ -311,17 +311,20 @@ __global__ void rgb_prep_kernel(const uint8_t *__restrict__ img, const float *__
 // (conv1x1_f16_kernel) instead of 3.2 ms of CUDA-core work per 16 x 512^2 batch.
 __global__ void rgb_im2col_kernel(const uint8_t *__restrict__ img, const float *__restrict__ A1,
                                   const float *__restrict__ b1, const float *__restrict__ A2,
-                                  const float *__restrict__ b2, int H, int W, uint4 *__restrict__ out) {
+                                  const float *__restrict__ b2, int H, int W, const int *__restrict__ ext,
+                                  uint4 *__restrict__ out) {
     const int n = blockIdx.y;
     const int HW = H * W;
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= HW) return;
     const int y0 = p / W, x0 = p % W;
+    // ragged batch: image n is [0,Hn) x [0,Wn) of the padded tensor, and its zero padding starts there
+    const int Hn = ext ? ext[2 * n] : H, Wn = ext ? ext[2 * n + 1] : W;
     float v[28];
 #pragma unroll
     for (int tap = 0; tap < 9; ++tap) {
         const int yy = y0 + tap / 3 - 1, xx = x0 + tap % 3 - 1;
-        const bool in = yy >= 0 && yy < H && xx >= 0 && xx < W;
+        const bool in = yy >= 0 && yy < Hn && xx >= 0 && xx < Wn;
         float x[3], y[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) x[c] = in ? (float)img[((size_t)n * 3 + c) * HW + yy * W + xx] : 0.f;
@@ -436,16 +439,22 @@ extern "C" int l3c_rgb_prep(const uint8_t *img_dev, const float *A1, const float
     return L3C_OK;
 }
 
-extern "C" int l3c_rgb_im2col_f16(const uint8_t *img_dev, const float *A1, const float *b1, const float *A2,
-                                  const float *b2, int N, int H, int W, void *out_h_dev, void *stream) {
+extern "C" int l3c_rgb_im2col_f16_ragged(const uint8_t *img_dev, const float *A1, const float *b1, const float *A2,
+                                         const float *b2, int N, int H, int W, const int *extents_dev, void *out_h_dev,
+                                         void *stream) {
     using namespace l3c;
     L3C_REQUIRE(img_dev && A1 && b1 && A2 && b2 && out_h_dev && N >= 1 && H >= 1 && W >= 1 && N <= 65535,
                 "l3c_rgb_im2col_f16: bad arguments");
     dim3 grid(ceil_div(H * W, 128), N);
-    rgb_im2col_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(img_dev, A1, b1, A2, b2, H, W,
+    rgb_im2col_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(img_dev, A1, b1, A2, b2, H, W, extents_dev,
                                                               reinterpret_cast<uint4 *>(out_h_dev));
     L3C_LAUNCH_CHECK("rgb_im2col_kernel");
     return L3C_OK;
+}
+
+extern "C" int l3c_rgb_im2col_f16(const uint8_t *img_dev, const float *A1, const float *b1, const float *A2,
+                                  const float *b2, int N, int H, int W, void *out_h_dev, void *stream) {
+    return l3c_rgb_im2col_f16_ragged(img_dev, A1, b1, A2, b2, N, H, W, nullptr, out_h_dev, stream);
 }
 
 extern "C" int l3c_quantize_head(const float *f_dev, const float *w_dev, const float *bias_dev,

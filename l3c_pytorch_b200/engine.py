@@ -108,6 +108,79 @@ def conv_launch_limits(max_sms=0, conv_smem_kb=0):
         check(lib.l3c_set_conv_launch_limits(0, 0))
 
 
+# ----------------------------------------------------------------------------------------------
+# ragged batches (DESIGN §4.6)
+# ----------------------------------------------------------------------------------------------
+_RAGGED = {'v': None}       # inside ragged_extents(): (finest H, W, [(h_n, w_n)], {(H, W): device extents})
+
+
+@contextlib.contextmanager
+def ragged_extents(extents, H, W):
+    """Inside the block the tensors of the conv stack are padded batches [N][H'][W'][..] of differently sized
+    images: image n occupies [0, h_n) x [0, w_n) of the finest H x W (`extents` = [(h_n, w_n)]) and
+    (h_n * H' / H, w_n * W' / W) at a coarser H' x W'.  Before every k x k conv the band of its halo around each
+    image is set to +0 in the tensor it reads (l3c_ragged_zero_halo), so every output pixel inside an image is
+    bit-identical to the per-image conv.  extents None: a no-op (equally sized images)."""
+    if extents is None:
+        yield
+        return
+    prev = _RAGGED['v']
+    _RAGGED['v'] = (int(H), int(W), [(int(h), int(w)) for (h, w) in extents], {})
+    try:
+        yield
+    finally:
+        _RAGGED['v'] = prev
+
+
+def ragged_active():
+    return _RAGGED['v'] is not None
+
+
+def extents_at(H, W, device):
+    """Device int32 [N][2] extents of the active ragged batch at resolution H x W (cached per block)."""
+    H0, W0, ext, cache = _RAGGED['v']
+    key = (int(H), int(W), str(device))
+    if key not in cache:
+        fh, fw = H0 // H, W0 // W
+        if fh * H != H0 or fw * W != W0:
+            raise ValueError('ragged batch: a %dx%d tensor is not a scale of the %dx%d batch' % (H, W, H0, W0))
+        arr = np.array([(h // fh, w // fw) for (h, w) in ext], np.int32)
+        cache[key] = _to_device_async(arr, device)
+    return cache[key]
+
+
+def zero_halo(x, halo):
+    """Ragged batch: +0 into the `halo`-pixel band around every image of the NHWC tensor x (in place)."""
+    N, H, W = x.shape[:3]
+    ext = extents_at(H, W, x.device)
+    assert x.is_contiguous()
+    check(lib.l3c_ragged_zero_halo(_ptr(x), x.shape[-1] * x.element_size(), N, H, W, _ptr(ext), int(halo),
+                                   _stream_ptr()))
+    LAUNCHES['n'] += 1
+
+
+def ragged_pack(src, planes, H, W, extents_dev, compact_len, to_compact, out=None):
+    """l3c_ragged_pack: padded planes [N][planes][H][W] of elements (trailing dims) <-> compact planes
+    [N][planes][compact_len] of the same elements.  -> the new tensor."""
+    assert src.is_contiguous()
+    N = extents_dev.shape[0]
+    elem = src.numel() // (N * planes * (compact_len if not to_compact else H * W))
+    elem_bytes = elem * src.element_size()
+    if out is None:
+        shape = (N, planes, compact_len) if to_compact else (N, planes, H, W)
+        out = torch.empty(shape + ((elem,) if elem > 1 else ()), dtype=src.dtype, device=src.device)
+    check(lib.l3c_ragged_pack(_ptr(src), _ptr(out), elem_bytes, planes, N, H, W, _ptr(extents_dev),
+                              int(compact_len), 1 if to_compact else 0, _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return out
+
+
+def _ragged_guard(kh, dil, x):
+    """Before a k x k conv of a ragged batch: zero the halo band of the tensor it reads."""
+    if _RAGGED['v'] is not None and kh > 1:
+        zero_halo(x, dil * (kh // 2))
+
+
 def require_cuda(t, name):
     if not t.is_cuda:
         raise ValueError('%s must be a CUDA tensor (l3c_pytorch_b200 has no CPU path)' % name)
@@ -312,6 +385,9 @@ def conv2d(conv, x, cin=None, relu=False, residual=None, pixel_shuffle=False, ou
     mode = _PRECISION['mode'] if precision is None else precision
     if mode == _lib.PREC_F16:
         return _conv2d_f16(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want)
+    if _RAGGED['v'] is not None:
+        raise NotImplementedError('ragged batches run in precision f16 only, not %s'
+                                  % {v: k for k, v in _lib.PRECISIONS.items()}[mode])
     if mode == _lib.PREC_F16X2:
         return _conv2d_f16x2(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want)
     x = xa.f
@@ -405,6 +481,7 @@ def _conv2d_f16(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, wan
         if xa.r is None or xa.r.dtype != torch.float16:
             xa = as_operand(xa.f)                     # callers from outside the network (tests, bench)
         w_h, b = pc.get_f16()
+        _ragged_guard(kh, dil, xa.r)
         d = ConvDesc(x_h=xa.r.data_ptr(), w_h=w_h.data_ptr(), bias=b.data_ptr(),
                      residual=residual.data_ptr() if residual is not None else None,
                      y=_dp(y), y_h=_dp(y_h), N=N, H=H, W=W, Cin=cin, x_pitch=xp, Cout=cout, cout_pad=b.shape[0],
@@ -415,6 +492,7 @@ def _conv2d_f16(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, wan
         if y is None:                                 # the FFMA kernel always writes fp32
             y = torch.empty(shape, dtype=torch.float32, device=src.device)
         w, b = pc.get()
+        _ragged_guard(kh, dil, xa.f)
         d = ConvDesc(x=xa.f.data_ptr(), w=w.data_ptr(), bias=b.data_ptr(),
                      residual=residual.data_ptr() if residual is not None else None,
                      y=_dp(y), y_h=_dp(y_h), N=N, H=H, W=W, Cin=cin, x_pitch=xp, Cout=cout, cout_pad=b.shape[0],
@@ -530,6 +608,8 @@ def rgb_prep(img_u8, conv1, conv2):
     MeanShift convs are applied as per-pixel 3x3 affines (parameters read from the modules)."""
     require_cuda(img_u8, 'img')
     assert img_u8.dtype == torch.uint8 and img_u8.is_contiguous()
+    if _RAGGED['v'] is not None:
+        raise NotImplementedError('ragged batches need the f16 RGB head (precision f16)')
     N, _, H, W = img_u8.shape
     A1 = conv1.weight.detach().float().reshape(9).contiguous()
     b1 = conv1.bias.detach().float().contiguous()
@@ -560,8 +640,12 @@ def rgb_head_f16(img_u8, conv1, conv2, head_conv):
     A2 = conv2.weight.detach().float().reshape(9).contiguous()
     b2 = conv2.bias.detach().float().contiguous()
     cols = torch.empty(N, H, W, 64, dtype=torch.float16, device=img_u8.device)
-    check(lib.l3c_rgb_im2col_f16(_ptr(img_u8), _ptr(A1), _ptr(b1), _ptr(A2), _ptr(b2), N, H, W, _ptr(cols),
-                                 _stream_ptr()))
+    if _RAGGED['v'] is not None:
+        check(lib.l3c_rgb_im2col_f16_ragged(_ptr(img_u8), _ptr(A1), _ptr(b1), _ptr(A2), _ptr(b2), N, H, W,
+                                            _ptr(extents_at(H, W, img_u8.device)), _ptr(cols), _stream_ptr()))
+    else:
+        check(lib.l3c_rgb_im2col_f16(_ptr(img_u8), _ptr(A1), _ptr(b1), _ptr(A2), _ptr(b2), N, H, W, _ptr(cols),
+                                     _stream_ptr()))
     LAUNCHES['n'] += 1
     pc = _packed_obj(head_conv)
     _, b = pc.get()
@@ -608,6 +692,8 @@ def symbols_to_values(sym, values, shift=None):
 
 
 def bicubic_half(img_u8):
+    if _RAGGED['v'] is not None:
+        raise NotImplementedError('ragged batches are not supported by the RGB baselines (bicubic encoder)')
     N, C, H, W = img_u8.shape
     assert C == 3 and img_u8.dtype == torch.uint8 and img_u8.is_contiguous()
     out = torch.empty(N, 3, int(H * 0.5), int(W * 0.5), dtype=torch.uint8, device=img_u8.device)

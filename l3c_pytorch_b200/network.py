@@ -396,9 +396,23 @@ class MultiscaleNetwork(nn.Module):
             return E.rgb_head_f16(img, self.sub_rgb_mean, self.heads[0].head[0], self.heads[0].head[1].head)
         return E.rgb_prep(img, self.sub_rgb_mean, self.heads[0].head[0])[1]
 
-    def forward(self, x, auto_recurse=0, intervals_of=None):
+    def _check_ragged(self, extents, auto_recurse=0):
+        if extents is None:
+            return
+        if self._rgb:
+            raise NotImplementedError('ragged batches are not supported by the RGB baselines (bicubic encoder)')
+        if auto_recurse:
+            raise NotImplementedError('ragged batches are not supported with auto_recurse')
+        if not E.f16_mode():
+            raise NotImplementedError('ragged batches run in precision f16 only, not %s' % E.get_conv_precision())
+
+    def forward(self, x, auto_recurse=0, intervals_of=None, extents=None):
         """intervals_of: a Losses object -> encode-side pass in f16 mode: the probability heads emit the coding
         intervals of the symbols directly (Out.IV) and no parameter tensor is materialised (Out.P entries None).
+
+        extents: [(h_n, w_n)] -> `x` is a ragged batch (DESIGN §4.6, f16 only): image n occupies [0, h_n) x [0, w_n)
+        of the padded batch (multiples of 2**num_scales, zero outside) and every output inside an image's extent at
+        every scale is bit-identical to the forward of that image alone; outside it the outputs are unspecified.
 
         x: image batch NCHW in [0,255] (uint8 / long / float).  Eval-mode forward
         (multiscale_network.py:226-306) -> Out.  auto_recurse: how many times the last trained scale is
@@ -406,6 +420,11 @@ class MultiscaleNetwork(nn.Module):
         multiscale_network.py:235-238,291-294); the extra scales use scale index -1, never fuse decoder
         features, and `Out.auto_recursive_from` marks where they start."""
         img = self._as_u8_planes(x)
+        self._check_ragged(extents, auto_recurse)
+        with E.ragged_extents(extents, img.shape[2], img.shape[3]):
+            return self._forward(img, auto_recurse, intervals_of)
+
+    def _forward(self, img, auto_recurse, intervals_of):
         forward_scales = list(range(self.scales)) + [-1] * int(auto_recurse)
         out = Out(targets_style='S' if self._rgb else 'bn',
                   auto_recursive_from=self.scales if auto_recurse > 0 else None)
@@ -498,12 +517,16 @@ class MultiscaleNetwork(nn.Module):
                 prev_x = loss_dmm.sample(nchw_view(P), C=C)
         return prev_x
 
-    def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False):
+    def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False, extents=None):
         """-> (parameters NHWC, decoder features as engine.Act for the next finer scale).  At scale 0 the
-        features feed nothing else (need_F=True keeps their fp32 tensor for the reference-shaped get_P)."""
+        features feed nothing else (need_F=True keeps their fp32 tensor for the reference-shaped get_P).
+        extents: [(h_n, w_n)] at the FINEST scale -> bn8 is a ragged batch (forward())."""
         assert 0 <= scale < self.config_ms.num_scales, 'Out of range: {}'.format(scale)
-        F = self.nets[scale].dec(bn8, dec_F_prev, operand_only=(scale == 0 and not need_F)).F
-        return self.prob_clfs[scale](F), F
+        self._check_ragged(extents)
+        f = 2 ** (scale + 1)
+        with E.ragged_extents(extents, bn8.shape[1] * f, bn8.shape[2] * f):
+            F = self.nets[scale].dec(bn8, dec_F_prev, operand_only=(scale == 0 and not need_F)).F
+            return self.prob_clfs[scale](F), F
 
     def get_P(self, scale, bn_q, dec_F_prev=None):
         """multiscale_network.py:308-322 with NCHW-shaped tensors in and out."""
