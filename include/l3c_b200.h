@@ -335,6 +335,12 @@ int l3c_partition_streams2(int sm_a, int n_a, void **streams_a, int n_b_high, vo
  * configuration is the default one.  Not meant for production use. */
 int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb);
 
+/* Test knob for the L = 256 range decoder, process-wide, from the next launch on: streams per CTA (1, 2 or 4) of
+ * v3::ac_decode256_kernel<SPC>; 0 = the L3C_DEC_SPC environment variable or, without it, the default (1).  Any
+ * other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant for
+ * production use. */
+int l3c_set_decoder_streams_per_cta(int spc);
+
 #ifdef __cplusplus
 }
 #endif

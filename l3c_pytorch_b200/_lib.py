@@ -76,6 +76,7 @@ _SIGNATURES = {
     'l3c_partition_streams': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_partition_streams2': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_set_conv_launch_limits': (c_int, [c_int, c_int]),
+    'l3c_set_decoder_streams_per_cta': (c_int, [c_int]),
 }
 
 EXPORTS = sorted(_SIGNATURES)

@@ -22,6 +22,8 @@
 //     rows are still being built (RGB channel pipelining).
 #include <stdlib.h>
 
+#include <atomic>
+
 #include "common.cuh"
 
 namespace l3c {
@@ -1011,6 +1013,17 @@ extern "C" int l3c_ac_encode_streams(const l3c_enc_stream_t *streams_dev, int n_
     return L3C_OK;
 }
 
+namespace l3c {
+std::atomic<int> g_dec_spc{0};   // l3c_set_decoder_streams_per_cta: 0 = L3C_DEC_SPC / the default
+}
+
+extern "C" int l3c_set_decoder_streams_per_cta(int spc) {
+    L3C_REQUIRE(spc == 0 || spc == 1 || spc == 2 || spc == 4,
+                "l3c_set_decoder_streams_per_cta: spc=%d not in {0, 1, 2, 4}", spc);
+    l3c::g_dec_spc.store(spc);
+    return L3C_OK;
+}
+
 extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_streams, int L,
                                      uint32_t first, uint32_t count, void *stream) {
     using namespace l3c;
@@ -1024,13 +1037,14 @@ extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_
     if (L <= 32) {
         ac_decode32_kernel<<<grid, blk, 0, st>>>(streams_dev, n_streams, L, first, count);
     } else if (L == 256) {
-        static int spc = 0;
-        static bool configured_dev[64] = {};
-        if (spc == 0) {
+        static const int env_spc = [] {
             const char *e = getenv("L3C_DEC_SPC");
-            spc = e ? atoi(e) : 1;
-            if (spc != 1 && spc != 2 && spc != 4) spc = 1;
-        }
+            const int v = e ? atoi(e) : 1;
+            return (v == 1 || v == 2 || v == 4) ? v : 1;
+        }();
+        static bool configured_dev[64] = {};
+        const int forced = g_dec_spc.load(std::memory_order_relaxed);
+        const int spc = forced ? forced : env_spc;
         bool &configured = configured_dev[current_device_slot()];
         if (!configured) {
             L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode256_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,

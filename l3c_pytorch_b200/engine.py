@@ -108,6 +108,17 @@ def conv_launch_limits(max_sms=0, conv_smem_kb=0):
         check(lib.l3c_set_conv_launch_limits(0, 0))
 
 
+@contextlib.contextmanager
+def decoder_streams_per_cta(spc):
+    """Test knob (l3c_set_decoder_streams_per_cta): inside the block the L = 256 range decoder packs `spc` streams
+    (1, 2 or 4) into one CTA; 0 = the L3C_DEC_SPC / default choice.  Process-wide; the default is restored on exit."""
+    check(lib.l3c_set_decoder_streams_per_cta(int(spc)))
+    try:
+        yield
+    finally:
+        check(lib.l3c_set_decoder_streams_per_cta(0))
+
+
 # ----------------------------------------------------------------------------------------------
 # ragged batches (DESIGN §4.6)
 # ----------------------------------------------------------------------------------------------

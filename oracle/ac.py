@@ -29,6 +29,10 @@ def lib():
         _lib.oracle_ac_decode.argtypes = [
             ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
             ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+        _lib.oracle_ac_decode_trace.restype = None
+        _lib.oracle_ac_decode_trace.argtypes = [
+            ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
+            ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p]
         _lib.oracle_mixture_cdf.restype = None
         _lib.oracle_mixture_cdf.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_void_p]
     return _lib
@@ -75,6 +79,21 @@ def decode(cdf, data, n_sym=None):
     lib().oracle_ac_decode(cdf.ctypes.data, stride, n_sym, Lp,
                            buf.ctypes.data if buf.size else None, buf.size, out.ctypes.data)
     return out
+
+
+def decode_trace(cdf, data):
+    """decode() that also returns the coder state when each symbol is reached: uint32 [n_sym, 4] rows of
+    (low, high, value, code bits read so far) -- what a decoder resumed at that symbol starts from."""
+    cdf = _as_cdf(cdf)
+    Lp = cdf.shape[-1]
+    cdf = cdf.reshape(-1, Lp)
+    n_sym = cdf.shape[0]
+    buf = np.frombuffer(bytes(data), np.uint8)
+    out = np.empty(n_sym, np.int16)
+    trace = np.empty((n_sym, 4), np.uint32)
+    lib().oracle_ac_decode_trace(cdf.ctypes.data, Lp, n_sym, Lp, buf.ctypes.data if buf.size else None, buf.size,
+                                 out.ctypes.data, trace.ctypes.data)
+    return out, trace
 
 
 def mixture_cdf(targets, means, log_scales, probs):

@@ -141,16 +141,25 @@ static uint16_t row_search(const uint16_t *row, uint16_t target, uint16_t top_sy
     return left;
 }
 
-/* ---- decoder (torchac.cpp:299-381) -------------------------------------------------------- */
-void oracle_ac_decode(const uint16_t *cdf, int64_t row_stride, int n_sym, int Lp,
-                      const uint8_t *in, size_t in_len, int16_t *out) {
+/* ---- decoder (torchac.cpp:299-381) --------------------------------------------------------
+ * trace (may be NULL): 4 words per symbol, trace[4*i ..] = (low, high, value, code bits read)
+ * when symbol i is reached -- the coder state a decoder resumed at symbol i starts from. */
+void oracle_ac_decode_trace(const uint16_t *cdf, int64_t row_stride, int n_sym, int Lp,
+                            const uint8_t *in, size_t in_len, int16_t *out, uint32_t *trace) {
     bitsrc_t src = {in, in_len, 0, 0, 0};
     uint32_t low = 0, high = 0xFFFFFFFFu, value = 0;
+    uint32_t nbits = 32;
     const int top_symbol = Lp - 2;
 
     for (int i = 0; i < 32; ++i) src_shift_in(&src, &value);
 
     for (int i = 0; i < n_sym; ++i) {
+        if (trace) {
+            trace[4 * (size_t)i + 0] = low;
+            trace[4 * (size_t)i + 1] = high;
+            trace[4 * (size_t)i + 2] = value;
+            trace[4 * (size_t)i + 3] = nbits;
+        }
         const uint16_t *row = cdf + (int64_t)i * row_stride;
         const uint64_t span = (uint64_t)high - (uint64_t)low + 1u;
         const uint16_t count =
@@ -176,8 +185,14 @@ void oracle_ac_decode(const uint16_t *cdf, int64_t row_stride, int n_sym, int Lp
                 break;
             }
             src_shift_in(&src, &value);
+            nbits++;
         }
     }
+}
+
+void oracle_ac_decode(const uint16_t *cdf, int64_t row_stride, int n_sym, int Lp,
+                      const uint8_t *in, size_t in_len, int16_t *out) {
+    oracle_ac_decode_trace(cdf, row_stride, n_sym, Lp, in, in_len, out, NULL);
 }
 
 /* ---- logistic-mixture CDF table (torchac_kernel.cu:16-76) --------------------------------

@@ -62,14 +62,16 @@ def test_encode_decode_cdf_bit_exact(L, n_sym):
 
 
 def _underflow_case(rng, n_sym, L=3):
-    """Symbols whose interval straddles the midpoint: `u` underflow shifts and no decided bit per
-    symbol, so the owed ("pending") bits pile up over many symbols -- well past 31, across the
-    encoder's 32-symbol batches -- until an off-centre symbol releases them (torchac.cpp:196-206)."""
+    """Symbols whose interval [32768 - w, 32768 + w), w a power of two, is centred on the midpoint: from the full
+    interval each one owes log2(2^15 / w) underflow shifts, decides no bit and leaves the coder at the full interval
+    again, so the owed ("pending") bits pile up over many symbols -- well past 31, across the encoder's 32-symbol
+    batches -- until an off-centre symbol releases them (torchac.cpp:196-206).  (With unequal halves the midpoint
+    leaves the coder's interval after a symbol or two and no run grows past ~15 bits.)"""
     half = 32768
     rows = np.zeros((n_sym, L + 1), np.int64)
     for i in range(n_sym):
-        w = int(rng.integers(1, 200))
-        rows[i, :L] = [0, half - w, half + int(rng.integers(1, 200))]
+        w = 1 << int(rng.integers(5, 9))
+        rows[i, :L] = [0, half - w, half + w]
     sym = np.ones(n_sym, np.int16)                       # the straddling symbol ...
     for i in rng.integers(0, n_sym, size=max(1, n_sym // 37)):
         sym[i] = int(rng.integers(0, 3))                 # ... with a few releases sprinkled in
