@@ -104,7 +104,9 @@ typedef struct {
     uint8_t *sym_out;           /* dev: n_sym decoded symbols                                    */
     uint32_t *state;            /* dev: 4 words of coder state (low, high, value, bitpos);        */
                                 /*      lets one stream be decoded in several launches (chunks)   */
-    int64_t row_pitch;          /* entries between consecutive rows; 0 = one shared row           */
+    int64_t row_pitch;          /* entries between consecutive rows; 0 = one shared row.  Every   */
+                                /*      row is read whole: 32 entries for L <= 32, 256 for L > 32, */
+                                /*      16-byte aligned.  Entries past L may hold anything.       */
     uint32_t n_sym;             /* total symbols of the stream                                    */
     uint32_t in_len;
 } l3c_dec_stream_t;
@@ -335,10 +337,10 @@ int l3c_partition_streams2(int sm_a, int n_a, void **streams_a, int n_b_high, vo
  * configuration is the default one.  Not meant for production use. */
 int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb);
 
-/* Test knob for the L = 256 range decoder, process-wide, from the next launch on: streams per CTA (1, 2 or 4) of
- * v3::ac_decode256_kernel<SPC>; 0 = the L3C_DEC_SPC environment variable or, without it, the default (1).  Any
- * other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant for
- * production use. */
+/* Test knob for the range decoder of alphabets L > 32, process-wide, from the next launch on: streams per CTA (1, 2
+ * or 4) of v3::ac_decode_kernel<FULLROW, SPC>; 0 = the L3C_DEC_SPC environment variable or, without it, the default
+ * (1).  Any other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant
+ * for production use. */
 int l3c_set_decoder_streams_per_cta(int spc);
 
 #ifdef __cplusplus

@@ -30,7 +30,6 @@ namespace l3c {
 
 constexpr unsigned FULL = 0xFFFFFFFFu;
 constexpr int ENC_WARPS_PER_CTA = 1;
-constexpr int DEC_WARPS_PER_CTA = 1;
 
 // ---------------------------------------------------------------------------------------------
 // encoder
@@ -416,69 +415,53 @@ struct CoderState {
     }
 };
 
-// CDF row held by a warp.  EPL = 8: lane l holds entries 8l..8l+7 (two per register) plus the first
-// entry of lane l+1; EPL = 1: lane l holds entry l.  Padding entries (index >= L) are stored as 0.
-template <int EPL>
-struct RowRegs;
-template <>
-struct RowRegs<8> {
-    uint4 v;
-    __device__ __forceinline__ void load(const uint16_t *row, int lane) {
-        v = __ldg(reinterpret_cast<const uint4 *>(row) + lane);
+// The symbols [first, last) of a stream of n that a launch for [first, first + count) decodes; false when there
+// are none.  Symbols below upd_end update the coder state, the stream's final symbol does not (torchac.cpp:335-337).
+__device__ __forceinline__ bool chunk_of(uint32_t n, uint32_t first, uint32_t count, uint32_t &last, uint32_t &upd_end) {
+    if (first >= n) return false;
+    last = (count > n - first) ? n : first + count;
+    upd_end = (last == n) ? n - 1u : last;
+    return true;
+}
+
+// Opens the stream at symbol `first`: at its head when first == 0, else where the previous launch saved its state.
+// Returns the bit position of the stream's first code bit (save_stream() needs it).
+__device__ __forceinline__ uint32_t open_stream(const l3c_dec_stream_t &st, uint32_t first, BitSource &src,
+                                                CoderState &cs) {
+    const uint32_t bit0 = src.open(st.in, st.in_len);
+    if (first == 0) {
+        src.seek(bit0);
+        cs.reset(src.take(32));
+    } else {
+        cs.restore(st.state);
+        src.seek(st.state[3] + bit0);
     }
-};
-template <>
-struct RowRegs<1> {
-    uint32_t v;
-    __device__ __forceinline__ void load(const uint16_t *row, int lane) { v = (uint32_t)__ldg(row + lane); }
-};
+    return bit0;
+}
+
+// one lane per stream
+__device__ __forceinline__ void save_stream(const l3c_dec_stream_t &st, const CoderState &cs, const BitSource &src,
+                                            uint32_t bit0) {
+    if (st.state != nullptr) {
+        cs.save(st.state);
+        st.state[3] = src.pos - bit0;
+    }
+}
 
 __device__ __forceinline__ bool below(uint32_t e, uint32_t r, uint64_t target) {   // e * (r+1) < target
     return ((uint64_t)r * e + e) < target;
 }
 
-// Search the row for the symbol whose interval contains the code value.  Returns the symbol and
-// its bounds: c_lo = cdf[sym], c_hi = cdf[sym+1] (2^16 for the last symbol).
+// One exact, branchy decoding step: the replay of a group the speculative loop gave up on, and the symbols
+// outside whole groups.  pk holds this lane's P packed proposals (cdf[m] << 16) | (cdf[m+1] - 1) of the entries
+// m = P*lane .. P*lane + P-1; past the alphabet they are 0 or repeat entry L-1's (see v3::ac_decode_kernel), so
+// they never change the largest passing proposal.  Returns that winning proposal and updates the state with its
+// interval unless `update` is false (the stream's final symbol).
 //   reference: count = ((value-low+1)*2^16-1)/span; sym = largest m with cdf[m] <= count, floor 0
 //   here:      cdf[m] <= count  <=>  cdf[m]*span < (value-low+1)<<16      (no division)
-template <bool FULLROW>
-__device__ __forceinline__ int search_row(const RowRegs<8> &row, uint32_t r, uint64_t target, int lane, int L,
-                                          uint32_t &c_lo, uint32_t &c_hi) {
-    // every lane tests its 8 entries; rows are non-decreasing, so cdf[sym] is the largest "true" entry
-    // and cdf[sym+1] the smallest "false" one: two warp reductions (REDUX) + one for the index
-    const uint32_t w[4] = {row.v.x, row.v.y, row.v.z, row.v.w};
-    uint32_t lane_lo = 0u, lane_hi = 0x10000u;
-    int n_true = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const uint32_t e = (j & 1) ? (w[j >> 1] >> 16) : (w[j >> 1] & 0xFFFFu);
-        const bool valid = FULLROW || (lane * 8 + j) < L;         // padding entries are never true
-        const bool f = ((lane | j) == 0) || (valid && below(e, r, target));
-        lane_lo = f ? max(lane_lo, e) : lane_lo;
-        lane_hi = (f || !valid) ? lane_hi : min(lane_hi, e);
-        n_true += f ? 1 : 0;
-    }
-    c_lo = __reduce_max_sync(FULL, lane_lo);
-    c_hi = __reduce_min_sync(FULL, lane_hi);
-    return __reduce_add_sync(FULL, n_true) - 1;
-}
-
-template <bool FULLROW>
-__device__ __forceinline__ int search_row(const RowRegs<1> &row, uint32_t r, uint64_t target, int lane, int L,
-                                          uint32_t &c_lo, uint32_t &c_hi) {
-    const bool f = (lane == 0) || ((lane < L) && below(row.v, r, target));
-    const int n = __popc(__ballot_sync(FULL, f));
-    const int sym = n - 1;
-    c_lo = __shfl_sync(FULL, row.v, sym);
-    const uint32_t nxt = __shfl_sync(FULL, row.v, n & 31);
-    c_hi = (n >= L) ? 0x10000u : nxt;
-    return sym;
-}
-
-// one symbol: search, update [low, high], renormalise, shift code bits into `value`
-template <int EPL, bool FULLROW>
-__device__ __forceinline__ int decode_step(const RowRegs<EPL> &cur, CoderState &cs, BitSource &src, int lane, int L,
-                                           bool update) {
+template <int P>
+__device__ __forceinline__ uint32_t exact_step(const uint32_t (&pk)[P], CoderState &cs, BitSource &src, int lane,
+                                               bool update) {
     const uint32_t r = cs.r;                                    // span - 1
     const uint32_t dv = cs.dv;
     uint64_t target = ((uint64_t)dv + 1ull) << 16;
@@ -489,122 +472,58 @@ __device__ __forceinline__ int decode_step(const RowRegs<EPL> &cur, CoderState &
         target = (uint64_t)foreign_count16(cs.low + dv, cs.low, r) + 1ull;
         r_cmp = 0u;
     }
-    uint32_t c_lo, c_hi;
-    const int sym = search_row<FULLROW>(cur, r_cmp, target, lane, L, c_lo, c_hi);
-    if (update) cs.update(c_lo, c_hi, src);
-    return sym;
+    uint32_t best = 0u;
+#pragma unroll
+    for (int j = 0; j < P; ++j) {
+        const bool fj = ((lane | j) == 0) || below(pk[j] >> 16, r_cmp, target);
+        best = fj ? max(best, pk[j]) : best;
+    }
+    const uint32_t top = __reduce_max_sync(FULL, best);
+    if (update) cs.update(top >> 16, (top & 0xFFFFu) + 1u, src);
+    return top;
 }
 
-template <int EPL, bool FULLROW>
-__global__ void __launch_bounds__(32 * DEC_WARPS_PER_CTA)
-ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, int L,
-                 uint32_t first, uint32_t count) {
-    constexpr int D = 8;   // row prefetch distance (symbols)
-    const int sid = blockIdx.x * DEC_WARPS_PER_CTA + (threadIdx.x >> 5);
-    if (sid >= n_streams) return;
-    const int lane = threadIdx.x & 31;
-    const l3c_dec_stream_t st = streams[sid];
-    const uint32_t n = st.n_sym;
-    if (first >= n) return;
-    const uint32_t last = (count > n - first) ? n : first + count;   // exclusive
-
-    BitSource src;
-    const uint32_t bit0 = src.open(st.in, st.in_len);
-
-    CoderState cs;
-    if (first == 0) {
-        src.seek(bit0);
-        cs.reset(src.take(32));
+// Writes a group of cnt <= 8 decoded symbols, packed four to a word, to out[0, cnt): as two words when the group
+// is whole and out is 4-byte aligned, else byte by byte.  (The byte loop stays rolled: unrolled, the register
+// allocation and schedule it brings made both decoders slower, by about 2 % at L = 256 and 10 % at L = 25 on an
+// H100 80GB HBM3 at 700 W.)
+__device__ __forceinline__ void store_group(uint8_t *out, const uint32_t (&packed)[2], uint32_t cnt) {
+    if (cnt == 8u && (reinterpret_cast<uintptr_t>(out) & 3u) == 0u) {
+        reinterpret_cast<uint32_t *>(out)[0] = packed[0];
+        reinterpret_cast<uint32_t *>(out)[1] = packed[1];
     } else {
-        cs.restore(st.state);
-        src.seek(st.state[3] + bit0);
-    }
-
-    const uint16_t *__restrict__ table = st.table;
-    const int64_t pitch = st.row_pitch;
-    uint8_t *__restrict__ sym_out = st.sym_out;
-    const bool vec_out = ((reinterpret_cast<uintptr_t>(sym_out) | first) & 3u) == 0u;
-
-    // symbols handled by the unrolled main loop: whole groups of D, never the stream's final symbol
-    const uint32_t upd_end = (last == n) ? n - 1 : last;          // symbols < upd_end update the state
-    const uint32_t main_end = first + ((upd_end - first) / D) * D;
-
-    RowRegs<EPL> ring[D];
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-        const uint32_t i = first + d;
-        if (i < last) ring[d].load(table + (int64_t)i * pitch, lane);
-    }
-    uint32_t base = first;
-    for (; base < main_end; base += D) {
-        uint32_t packed[D / 4];
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-            const uint32_t i = base + d;
-            const RowRegs<EPL> cur = ring[d];
-            if (i + D < last) ring[d].load(table + (int64_t)(i + D) * pitch, lane);
-            const int sym = decode_step<EPL, FULLROW>(cur, cs, src, lane, L, true);
-            if ((d & 3) == 0) packed[d >> 2] = 0u;
-            packed[d >> 2] |= (uint32_t)sym << (8 * (d & 3));
-            if (!vec_out && lane == 0) sym_out[i] = (uint8_t)sym;
-        }
-        if (vec_out && lane == 0) {
-#pragma unroll
-            for (int q = 0; q < D / 4; ++q) *reinterpret_cast<uint32_t *>(sym_out + base + 4 * q) = packed[q];
-        }
-    }
-    // tail (< D symbols, may contain the final symbol, which leaves the state untouched:
-    // torchac.cpp:335-337)
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-        const uint32_t i = base + d;
-        if (i < last) {
-            const int sym = decode_step<EPL, FULLROW>(ring[d], cs, src, lane, L, i < upd_end);
-            if (lane == 0) sym_out[i] = (uint8_t)sym;
-        }
-    }
-
-    if (lane == 0 && st.state != nullptr) {
-        cs.save(st.state);
-        st.state[3] = src.pos - bit0;
+        const uint64_t p = ((uint64_t)packed[1] << 32) | packed[0];   // a register, not a local-memory array
+#pragma unroll 1
+        for (uint32_t d = 0; d < cnt; ++d) out[d] = (uint8_t)(p >> (8 * d));
     }
 }
 
 // ---------------------------------------------------------------------------------------------
 // decoder, alphabets of at most 32 symbols (bottleneck and uniform-prior streams): one CDF entry per
-// lane, ballot + popc + two shuffles.  Groups of 8 symbols run as straight-line speculative code
-// (see v3::ac_decode256_kernel); a group that trips the sticky flag is replayed with decode_step().
+// lane, one compare and one max-reduction.  Groups of 8 symbols run as straight-line speculative code
+// (see v3::ac_decode_kernel); a group that trips the sticky flag is replayed with exact_step().
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(32 * DEC_WARPS_PER_CTA)
+__global__ void __launch_bounds__(32)
 ac_decode32_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, int L,
                    uint32_t first, uint32_t count) {
     constexpr int D = 8;   // symbols per group = row prefetch distance
-    const int sid = blockIdx.x * DEC_WARPS_PER_CTA + (threadIdx.x >> 5);
+    const int sid = blockIdx.x;
     if (sid >= n_streams) return;
     const int lane = threadIdx.x & 31;
     const l3c_dec_stream_t st = streams[sid];
-    const uint32_t n = st.n_sym;
-    if (first >= n) return;
-    const uint32_t last = (count > n - first) ? n : first + count;   // exclusive
+    uint32_t last, upd_end;
+    if (!chunk_of(st.n_sym, first, count, last, upd_end)) return;
 
     BitSource src;
-    const uint32_t bit0 = src.open(st.in, st.in_len);
     CoderState cs;
-    if (first == 0) {
-        src.seek(bit0);
-        cs.reset(src.take(32));
-    } else {
-        cs.restore(st.state);
-        src.seek(st.state[3] + bit0);
-    }
+    const uint32_t bit0 = open_stream(st, first, src, cs);
 
     const uint16_t *__restrict__ table = st.table;
     const int64_t pitch = st.row_pitch;
     uint8_t *__restrict__ sym_out = st.sym_out;
-    const bool vec_out = ((reinterpret_cast<uintptr_t>(sym_out) | first) & 3u) == 0u;
     const bool in_row = lane < L;
 
-    const uint32_t upd_end = (last == n) ? n - 1 : last;          // symbols < upd_end update the state
+    // the speculative groups: whole groups of D, never the stream's final symbol
     const uint32_t main_end = first + ((upd_end - first) / D) * D;
 
     // lane l keeps entry l as the packed proposal (cdf[l] << 16) | (cdf[l+1] - 1) (2^16 after the last
@@ -617,6 +536,13 @@ ac_decode32_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, 
         uint32_t nx = __shfl_down_sync(FULL, v, 1);
         if (lane + 1 >= L) nx = 0x10000u;
         return in_row ? ((v << 16) | ((nx - 1u) & 0xFFFFu)) : 0u;
+    };
+    // symbol i on the exact path; the symbol is the number of the row's proposals up to the winner, minus 1
+    auto exact = [&](uint32_t i) {
+        const uint32_t pk[1] = {pack_row((uint32_t)__ldg(table + (int64_t)i * pitch + lane))};
+        const uint32_t top = exact_step(pk, cs, src, lane, i < upd_end);
+        const int sym = __popc(__ballot_sync(FULL, in_row && pk[0] <= top)) - 1;
+        if (lane == 0) sym_out[i] = (uint8_t)sym;
     };
     // rows are fetched two groups ahead: a group's rows are packed at its start, so they must have been
     // requested at least a whole group (~1.5 us) earlier for HBM latency to stay hidden
@@ -656,48 +582,25 @@ ac_decode32_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, 
                 packed[d >> 2] |= (uint32_t)(nt - 1) << (8 * (d & 3));
             }
             if (__builtin_expect(!bad, 1)) {
-                if (lane == 0) {
-                    if (vec_out) {
-#pragma unroll
-                        for (int q = 0; q < D / 4; ++q)
-                            *reinterpret_cast<uint32_t *>(sym_out + base + 4 * q) = packed[q];
-                    } else {
-#pragma unroll
-                        for (int d = 0; d < D; ++d) sym_out[base + d] = (uint8_t)(packed[d >> 2] >> (8 * (d & 3)));
-                    }
-                }
+                if (lane == 0) store_group(sym_out + base, packed, D);
                 continue;
             }
             cs = cs0;                 // replay this group exactly (the ring already holds the next group's rows)
             src = src0;
         }
 #pragma unroll 1
-        for (int d = 0; d < D; ++d) {
-            const uint32_t i = base + d;
-            RowRegs<1> cur;
-            cur.load(table + (int64_t)i * pitch, lane);
-            const int sym = decode_step<1, false>(cur, cs, src, lane, L, true);
-            if (lane == 0) sym_out[i] = (uint8_t)sym;
-        }
+        for (int d = 0; d < D; ++d) exact(base + d);
     }
-    // tail (< D symbols, may contain the stream's final symbol, which leaves the state untouched:
-    // torchac.cpp:335-337)
+    // tail (< D symbols, may contain the stream's final symbol)
 #pragma unroll 1
-    for (uint32_t i = base; i < last; ++i) {
-        RowRegs<1> cur;
-        cur.load(table + (int64_t)i * pitch, lane);
-        const int sym = decode_step<1, false>(cur, cs, src, lane, L, i < upd_end);
-        if (lane == 0) sym_out[i] = (uint8_t)sym;
-    }
+    for (uint32_t i = base; i < last; ++i) exact(i);
 
-    if (lane == 0 && st.state != nullptr) {
-        cs.save(st.state);
-        st.state[3] = src.pos - bit0;
-    }
+    if (lane == 0) save_stream(st, cs, src, bit0);
 }
 
 // ---------------------------------------------------------------------------------------------
-// decoder, 256-symbol alphabets (the RGB streams): CTA = decoder warp + helper warp per stream
+// decoder, alphabets of 33 to 256 symbols (the RGB streams have 256): CTA = decoder warp + helper warp
+// per stream; rows are read as 256 entries whatever L is
 //
 // A single warp issues one dependent instruction every ~4-5 cycles, so the serial rate of the coder
 // is set by the number of instructions the decoding warp executes per symbol.  Everything that does
@@ -781,9 +684,16 @@ __device__ __forceinline__ bool spec_group(CoderState &cs, BitSource &src, const
     return bad;
 }
 
-template <int SPC>
+// FULLROW: L = 256.  Otherwise (33 <= L <= 255) only the helper warp differs, and nothing it does depends on what
+// the row holds past entry L-1:
+//   * entry L-1's upper bound is 2^16;
+//   * entries m >= L propose 0, which passes every compare but never exceeds entry 0's proposal (that always
+//     passes) -- except entry L when it shares a pair of spec_group's select tree with entry L-1 (odd L): a 0 there
+//     would pass and hide entry L-1, so it repeats entry L-1's proposal, which passes exactly when that one does;
+//   * only entries m < L count towards the symbol index.
+template <bool FULLROW, int SPC>
 __global__ void __launch_bounds__(64 * SPC)
-ac_decode256_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, uint32_t first, uint32_t count) {
+ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, int L, uint32_t first, uint32_t count) {
     extern __shared__ __align__(16) uint8_t dec_smem[];
     const int warp_id = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -807,9 +717,8 @@ ac_decode256_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams,
     const int sid = blockIdx.x * SPC + sslot;
     if (sid >= n_streams) return;
     const l3c_dec_stream_t st = streams[sid];
-    const uint32_t n = st.n_sym;
-    if (first >= n) return;
-    const uint32_t last = (count > n - first) ? n : first + count;   // exclusive
+    uint32_t last, upd_end;
+    if (!chunk_of(st.n_sym, first, count, last, upd_end)) return;
     const uint32_t n_groups = (last - first + G - 1) / G;
 
     if (warp == 1) {
@@ -840,32 +749,23 @@ ac_decode256_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams,
                 // winning proposals into symbols, then the slots may be overwritten
                 mbar_wait(bar0 + 16 + 8 * g, ((gi >> 1) - 1) & 1u);
                 const uint32_t ibase = first + (gi - 2) * G;
-                uint32_t pack0 = 0u, pack1 = 0u;
+                uint32_t packed[2] = {0u, 0u};
 #pragma unroll
                 for (int d = 0; d < G; ++d) {
                     if (ibase + d < last) {
                         const uint32_t top = tops[g * G + d];
                         const uint4 a = ring[g * G + d][0][lane];
                         const uint4 b = ring[g * G + d][1][lane];
-                        int c = (a.x <= top) + (a.y <= top) + (a.z <= top) + (a.w <= top) + (b.x <= top) + (b.y <= top) +
-                                (b.z <= top) + (b.w <= top);
+                        const uint32_t pk[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                        int c = 0;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) c += (pk[j] <= top && (FULLROW || 8 * lane + j < L)) ? 1 : 0;
                         int tot = __reduce_add_sync(FULL, c);
                         tot = tot > 0 ? tot - 1 : 0;
-                        if (d < 4) pack0 |= (uint32_t)tot << (8 * d);
-                        else pack1 |= (uint32_t)tot << (8 * (d - 4));
+                        packed[d >> 2] |= (uint32_t)tot << (8 * (d & 3));
                     }
                 }
-                if (lane == 0) {
-                    const bool vec = ((reinterpret_cast<uintptr_t>(sym_out) | ibase) & 3u) == 0u && ibase + G <= last;
-                    if (vec) {
-                        *reinterpret_cast<uint32_t *>(sym_out + ibase) = pack0;
-                        *reinterpret_cast<uint32_t *>(sym_out + ibase + 4) = pack1;
-                    } else {
-                        for (int d = 0; d < G; ++d)
-                            if (ibase + d < last)
-                                sym_out[ibase + d] = (uint8_t)(((d < 4 ? pack0 : pack1) >> (8 * (d & 3))) & 0xFFu);
-                    }
-                }
+                if (lane == 0) store_group(sym_out + ibase, packed, min(last - ibase, (uint32_t)G));
                 __syncwarp();
             }
             if (gi < n_groups) {
@@ -874,18 +774,25 @@ ac_decode256_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams,
                     const uint4 v = cur[d];
                     uint32_t nx = __shfl_down_sync(FULL, v.x, 1);
                     if (lane == 31) nx = 0u;                                  // row end -> upper bound 2^16
-                    uint4 lo, hi;
-                    // proposal of entry m: (cdf[m] << 16) | ((cdf[m+1] - 1) & 0xFFFF)
-                    lo.x = (v.x << 16) | (((v.x >> 16) - 1u) & 0xFFFFu);
-                    lo.y = (v.x & 0xFFFF0000u) | (((v.y & 0xFFFFu) - 1u) & 0xFFFFu);
-                    lo.z = (v.y << 16) | (((v.y >> 16) - 1u) & 0xFFFFu);
-                    lo.w = (v.y & 0xFFFF0000u) | (((v.z & 0xFFFFu) - 1u) & 0xFFFFu);
-                    hi.x = (v.z << 16) | (((v.z >> 16) - 1u) & 0xFFFFu);
-                    hi.y = (v.z & 0xFFFF0000u) | (((v.w & 0xFFFFu) - 1u) & 0xFFFFu);
-                    hi.z = (v.w << 16) | (((v.w >> 16) - 1u) & 0xFFFFu);
-                    hi.w = (v.w & 0xFFFF0000u) | (((nx & 0xFFFFu) - 1u) & 0xFFFFu);
-                    ring[g * G + d][0][lane] = lo;
-                    ring[g * G + d][1][lane] = hi;
+                    // proposal of entry m = 8 * lane + j: (cdf[m] << 16) | ((cdf[m+1] - 1) & 0xFFFF)
+                    uint32_t p[8] = {(v.x << 16) | (((v.x >> 16) - 1u) & 0xFFFFu),
+                                     (v.x & 0xFFFF0000u) | (((v.y & 0xFFFFu) - 1u) & 0xFFFFu),
+                                     (v.y << 16) | (((v.y >> 16) - 1u) & 0xFFFFu),
+                                     (v.y & 0xFFFF0000u) | (((v.z & 0xFFFFu) - 1u) & 0xFFFFu),
+                                     (v.z << 16) | (((v.z >> 16) - 1u) & 0xFFFFu),
+                                     (v.z & 0xFFFF0000u) | (((v.w & 0xFFFFu) - 1u) & 0xFFFFu),
+                                     (v.w << 16) | (((v.w >> 16) - 1u) & 0xFFFFu),
+                                     (v.w & 0xFFFF0000u) | (((nx & 0xFFFFu) - 1u) & 0xFFFFu)};
+                    if (!FULLROW) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const int m = 8 * lane + j;
+                            if (m == L - 1) p[j] |= 0xFFFFu;
+                            else if (m >= L) p[j] = (m == L && (j & 1)) ? p[j - 1] : 0u;
+                        }
+                    }
+                    ring[g * G + d][0][lane] = make_uint4(p[0], p[1], p[2], p[3]);
+                    ring[g * G + d][1][lane] = make_uint4(p[4], p[5], p[6], p[7]);
                 }
                 mbar_arrive(bar0 + 8 * g);                                    // full[g]
             }
@@ -895,16 +802,8 @@ ac_decode256_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams,
 
     // ============================ decoder warp ============================
     BitSource src;
-    const uint32_t bit0 = src.open(st.in, st.in_len);
     CoderState cs;
-    if (first == 0) {
-        src.seek(bit0);
-        cs.reset(src.take(32));
-    } else {
-        cs.restore(st.state);
-        src.seek(st.state[3] + bit0);
-    }
-    const uint32_t upd_end = (last == n) ? n - 1u : last;                     // symbols < upd_end update the state
+    const uint32_t bit0 = open_stream(st, first, src, cs);
     for (uint32_t gi = 0; gi < n_groups; ++gi) {
         const uint32_t g = gi & 1u;
         mbar_wait(bar0 + 8 * g, (gi >> 1) & 1u);                              // full[g]
@@ -937,34 +836,15 @@ ac_decode256_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams,
                 if (i >= last) break;
                 const uint4 a = ring[g * G + d][0][lane];
                 const uint4 b = ring[g * G + d][1][lane];
-                const uint32_t r = cs.r;
-                const uint32_t dv = cs.dv;
-                uint64_t target = ((uint64_t)dv + 1ull) << 16;
-                uint32_t r_cmp = r;
-                if (dv > r) {                                                 // corrupt / foreign input only
-                    target = (uint64_t)foreign_count16(cs.low + dv, cs.low, r) + 1ull;
-                    r_cmp = 0u;
-                }
                 const uint32_t pk[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                uint32_t best = 0u;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const bool fj = ((lane | j) == 0) || below(pk[j] >> 16, r_cmp, target);
-                    best = fj ? max(best, pk[j]) : best;
-                }
-                const uint32_t top = __reduce_max_sync(FULL, best);
+                const uint32_t top = exact_step(pk, cs, src, lane, i < upd_end);
                 if (lane == 0) tops[g * G + d] = top;
-                if (i != n - 1)                                               // torchac.cpp:335-337
-                    cs.update(top >> 16, (top & 0xFFFFu) + 1u, src);
             }
         }
         __syncwarp();
         mbar_arrive(bar0 + 16 + 8 * g);                                       // empty[g]
     }
-    if (lane == 0 && st.state != nullptr) {
-        cs.save(st.state);
-        st.state[3] = src.pos - bit0;
-    }
+    if (lane == 0) save_stream(st, cs, src, bit0);
 }
 
 }  // namespace v3
@@ -1015,7 +895,20 @@ extern "C" int l3c_ac_encode_streams(const l3c_enc_stream_t *streams_dev, int n_
 
 namespace l3c {
 std::atomic<int> g_dec_spc{0};   // l3c_set_decoder_streams_per_cta: 0 = L3C_DEC_SPC / the default
+
+template <bool FULLROW>
+void launch_decode(const l3c_dec_stream_t *streams, int n, int L, uint32_t first, uint32_t count, int spc,
+                   cudaStream_t st) {
+    using v3::ac_decode_kernel;
+    using v3::STREAM_SMEM;
+    if (spc == 4)
+        ac_decode_kernel<FULLROW, 4><<<ceil_div(n, 4), 256, 4 * STREAM_SMEM, st>>>(streams, n, L, first, count);
+    else if (spc == 2)
+        ac_decode_kernel<FULLROW, 2><<<ceil_div(n, 2), 128, 2 * STREAM_SMEM, st>>>(streams, n, L, first, count);
+    else
+        ac_decode_kernel<FULLROW, 1><<<n, 64, STREAM_SMEM, st>>>(streams, n, L, first, count);
 }
+}  // namespace l3c
 
 extern "C" int l3c_set_decoder_streams_per_cta(int spc) {
     L3C_REQUIRE(spc == 0 || spc == 1 || spc == 2 || spc == 4,
@@ -1031,12 +924,10 @@ extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_
     L3C_REQUIRE(L >= 1 && L <= 256, "l3c_ac_decode_streams: L=%d not in [1,256]", L);
     if (n_streams == 0 || count == 0) return L3C_OK;
     L3C_REQUIRE(streams_dev, "l3c_ac_decode_streams: null pointer");
-    const int grid = ceil_div(n_streams, DEC_WARPS_PER_CTA);
-    const dim3 blk(32 * DEC_WARPS_PER_CTA);
     cudaStream_t st = (cudaStream_t)stream;
     if (L <= 32) {
-        ac_decode32_kernel<<<grid, blk, 0, st>>>(streams_dev, n_streams, L, first, count);
-    } else if (L == 256) {
+        ac_decode32_kernel<<<n_streams, 32, 0, st>>>(streams_dev, n_streams, L, first, count);
+    } else {
         static const int env_spc = [] {
             const char *e = getenv("L3C_DEC_SPC");
             const int v = e ? atoi(e) : 1;
@@ -1046,19 +937,17 @@ extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_
         const int forced = g_dec_spc.load(std::memory_order_relaxed);
         const int spc = forced ? forced : env_spc;
         bool &configured = configured_dev[current_device_slot()];
-        if (!configured) {
-            L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode256_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        if (!configured) {   // the SPC = 4 variants are the ones above 48 KB of shared memory
+            L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          4 * v3::STREAM_SMEM));
+            L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           4 * v3::STREAM_SMEM));
             configured = true;
         }
-        if (spc == 4)
-            v3::ac_decode256_kernel<4><<<ceil_div(n_streams, 4), 256, 4 * v3::STREAM_SMEM, st>>>(streams_dev, n_streams, first, count);
-        else if (spc == 2)
-            v3::ac_decode256_kernel<2><<<ceil_div(n_streams, 2), 128, 2 * v3::STREAM_SMEM, st>>>(streams_dev, n_streams, first, count);
+        if (L == 256)
+            launch_decode<true>(streams_dev, n_streams, L, first, count, spc, st);
         else
-            v3::ac_decode256_kernel<1><<<n_streams, 64, v3::STREAM_SMEM, st>>>(streams_dev, n_streams, first, count);
-    } else {
-        ac_decode_kernel<8, false><<<grid, blk, 0, st>>>(streams_dev, n_streams, L, first, count);
+            launch_decode<false>(streams_dev, n_streams, L, first, count, spc, st);
     }
     L3C_LAUNCH_CHECK("ac_decode_kernel");
     return L3C_OK;

@@ -1,7 +1,7 @@
 """Every launch path of the range coder against the CPU oracle (oracle.ac, bit-exact by construction).
 
 The decoder kernel is chosen by the alphabet (range_coder.cu, l3c_ac_decode_streams): L <= 32 runs
-ac_decode32_kernel, 33..255 ac_decode_kernel<8,false>, 256 v3::ac_decode256_kernel<SPC> with SPC streams per CTA
+ac_decode32_kernel, larger alphabets v3::ac_decode_kernel<FULLROW, SPC> (FULLROW: L = 256) with SPC streams per CTA
 (engine.decoder_streams_per_cta).  Here every one of them decodes many ragged streams per launch, in place from odd
 byte offsets of one blob, resumed from saved state under several chunk schedules, with corrupt and truncated
 streams beside valid ones in the same launches.  After every launch the saved coder state of every stream is
@@ -26,17 +26,15 @@ KINDS = ('flat', 'peaked', 'tail', 'straddle', 'uniform', 'mix')
 EXTRA = (('uniform', 1501), ('straddle-run', 5003), ('straddle-run', 65))
 HALF = 32768
 
-# (L, streams per CTA of the L = 256 decoder): every decoder kernel of the library
-DECODE_CASES = [(L, 0) for L in ALPHABETS if L != 256] + [(256, 1), (256, 2), (256, 4)]
+# (L, streams per CTA of the L > 32 decoder): every decoder kernel of the library, each SPC with L < 256 (odd and even)
+DECODE_CASES = [(L, 0) for L in ALPHABETS if L <= 32] + [(L, spc) for L in ALPHABETS if L > 32 for spc in (1, 2, 4)]
 
 
 def decoder_kernel(L, spc):
     """the kernel l3c_ac_decode_streams launches for alphabet L under decoder_streams_per_cta(spc)"""
     if L <= 32:
         return 'ac_decode32_kernel'
-    if L < 256:
-        return 'ac_decode_kernel<8,false>'
-    return 'v3::ac_decode256_kernel<%d>' % (spc or 1)
+    return 'v3::ac_decode_kernel<%s,%d>' % ('true' if L == 256 else 'false', spc or 1)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -233,12 +231,11 @@ def test_stream_factory_round_trips_on_the_oracle():
         # corrupt positions lie in every launch (the smallest launch has len(ss) - 3 streams) on long streams
         assert max(JUNK + tuple(TRUNCATE)) < len(ss) - 3
     # bookkeeping, not evidence: decoder_kernel() restates the library's dispatch rule, so this only says that
-    # DECODE_CASES names an alphabet / SPC for each of the five decoder kernels.  The launch log does not name the
-    # variant; that the knob really switches the L = 256 kernel is shown by breaking one variant (e.g. its grid)
-    # and watching test_chunked_ragged_decode_matches_oracle fail for that SPC only.
-    assert {decoder_kernel(L, spc) for (L, spc) in DECODE_CASES} == {
-        'ac_decode32_kernel', 'ac_decode_kernel<8,false>', 'v3::ac_decode256_kernel<1>',
-        'v3::ac_decode256_kernel<2>', 'v3::ac_decode256_kernel<4>'}
+    # DECODE_CASES names an alphabet / SPC for each instantiation of the two decoder kernels.  The launch log does
+    # not name the variant; that the knob really switches the L > 32 kernel is shown by breaking one variant (e.g.
+    # its grid) and watching test_chunked_ragged_decode_matches_oracle fail for that SPC only.
+    assert {decoder_kernel(L, spc) for (L, spc) in DECODE_CASES} == {'ac_decode32_kernel'} | {
+        'v3::ac_decode_kernel<%s,%d>' % (full, spc) for full in ('true', 'false') for spc in (1, 2, 4)}
 
 
 def test_decoder_streams_per_cta_knob_rejects_other_values():
