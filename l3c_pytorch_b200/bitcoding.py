@@ -48,6 +48,15 @@ def plan_passes(shapes, budget=None):
     return passes
 
 
+def _groups(keys):
+    """Indices of equal keys -- one group per (shape, padding tuple) where ragged passes are unsupported -- in
+    order of first appearance."""
+    groups = {}
+    for i, k in enumerate(keys):
+        groups.setdefault(k, []).append(i)
+    return list(groups.values())
+
+
 class Bitcoding(object):
     def __init__(self, blueprint, times=NoOp, compare_with_theory=False, tile=None):
         """tile = (th, tw): write TILED containers (codec.ContainerLayout): every channel plane of every scale is
@@ -83,10 +92,7 @@ class Bitcoding(object):
         (plan_passes) where the codec supports them, else one group per (shape, padding tuple)."""
         if self.codec.ragged_unsupported(self.tile) is None:
             return plan_passes([tuple(t.shape[-2:]) for (t, _) in prepared])
-        groups = {}
-        for i, (t, pt) in enumerate(prepared):
-            groups.setdefault((tuple(t.shape), pt), []).append(i)
-        return list(groups.values())
+        return _groups((tuple(t.shape), pt) for (t, pt) in prepared)
 
     def _begin_pass(self, prepared, idxs):
         """Enqueue the encode of prepared[idxs] as one batch on the current stream -> codec EncodeJob.  Images of
@@ -139,12 +145,10 @@ class Bitcoding(object):
                 with open(pouts[i], 'wb') as f:
                     f.write(dta)
             return bpsps
-        groups = {}
-        for i, (t, pt) in enumerate(prepared):
-            groups.setdefault((tuple(t.shape), pt), []).append(i)
         bpsps = [None] * len(imgs)
-        for (shape, pt), idxs in groups.items():
+        for idxs in _groups((tuple(t.shape), pt) for (t, pt) in prepared):
             batch = torch.cat([prepared[i][0] for i in idxs], 0)
+            pt = prepared[idxs[0]][1]
             with self.times.run('[-] encode forwardpass'):
                 # without --compare_theory nobody reads the parameter tensors: the probability heads emit the
                 # coding intervals directly (f16 mode; MultiscaleNetwork.forward(intervals_of=...))
@@ -155,7 +159,7 @@ class Bitcoding(object):
                     loss_out = self.blueprint.get_loss(out)
             with self.times.run('[-] entropy coding'):
                 datas, info = self.codec.encode_batch(batch, pt, out=out, tile=self.tile)
-            num_subpixels = int(np.prod(shape))
+            num_subpixels = int(np.prod(batch.shape[1:]))
             for k, i in enumerate(idxs):
                 with open(pouts[i], 'wb') as f:
                     f.write(datas[k])
@@ -222,7 +226,8 @@ class Bitcoding(object):
                 x = torch.nn.functional.pad(x, pt, 'constant')
             x = x.contiguous()
             job = self.codec.encode_begin(x, pt, tile=self.tile)
-        return _BatchEncodeJob(job, int(np.prod(x.shape[1:])))
+        N = x.shape[0]
+        return _ListEncodeJob([(list(range(N)), job)], [int(np.prod(x.shape[1:]))] * N)
 
     def side_stream(self, n_images, n_lanes=1):
         """Stream for encode_batch_begin() calls that should overlap decode_batch calls of `n_images` each."""
@@ -243,10 +248,7 @@ class Bitcoding(object):
                 all(len(p[1]) and container_tile(d) is None for p, d in zip(parsed, datas)):
             passes = plan_passes([p[1][-1][1:3] for p in parsed])
         else:
-            keys = {}
-            for i, (pt, scales) in enumerate(parsed):
-                keys.setdefault((pt, tuple((C, H, W) for (C, H, W, _) in scales)), []).append(i)
-            passes = list(keys.values())
+            passes = _groups((tuple((C, H, W) for (C, H, W, _) in scales), pt) for (pt, scales) in parsed)
         outs = [None] * len(datas)
         for idxs in passes:
             S, _ = self.codec.decode_batch([datas[i] for i in idxs], to_host=False, lane=lane)
@@ -261,7 +263,8 @@ class Bitcoding(object):
 
 
 class _ListEncodeJob:
-    """encode_batch_begin of a list: the codec jobs of its passes; finish() -> (containers, bpsps) in input order."""
+    """encode_batch_begin: the codec jobs of its passes (one for a batch tensor); finish() -> (containers, bpsps) in
+    input order."""
 
     def __init__(self, jobs, nsubs):
         self.jobs, self.nsubs = jobs, nsubs
@@ -273,15 +276,6 @@ class _ListEncodeJob:
             for k, i in enumerate(idxs):
                 datas[i] = d[k]
         return datas, [len(d) * 8 / n for d, n in zip(datas, self.nsubs)]
-
-
-class _BatchEncodeJob:
-    def __init__(self, job, nsub):
-        self.job, self.nsub = job, nsub
-
-    def finish(self):
-        datas, _ = self.job.finish(to_host=True)
-        return datas, [len(d) * 8 / self.nsub for d in datas]
 
 
 # --- header field helpers (bitcoding.py:326-375), little-endian -------------------------------

@@ -2,7 +2,7 @@
 reference-shaped `Bitcoding` class (bitcoding.py) drives.
 
 What the reference does one image, one scale, one channel at a time with a GPU->CPU round trip per
-channel (/root/reference/src/bitcoding/bitcoding.py:85-123,163-294, coders.py:38-90) is done here
+channel (src/bitcoding/bitcoding.py:85-123,163-294, coders.py:38-90) is done here
 for a whole batch of images -- equally sized, or of any mix of sizes (a ragged batch, DESIGN §4.6: f16, learned
 bottlenecks, the reference layout) -- with
   * ONE network pass,
@@ -12,6 +12,11 @@ bottlenecks, the reference layout) -- with
     (bitcoding.py:326-363: 4 x u16 padding | per scale: u8 C, u16 H, u16 W | per channel: u32 len +
     stream | 4-byte magic).
 Decoding uploads the concatenated containers once and decodes every stream in place.
+
+Equal-size, tiled and ragged batches share one encode and one decode path: `stream_layout` says where every
+stream's intervals (encode) or symbols and CDF rows (decode) sit in the `[N][C][plane]` tensor of its scale, and
+only the step between those stream planes and the raster planes of the networks differs (a view, l3c_reorder_tiles
+or l3c_ragged_pack).
 """
 import os
 import struct
@@ -83,6 +88,37 @@ def tile_grid(H, W, tile):
             out.append((off, h * w))
             off += h * w
     return out
+
+
+def stream_layout(shapes_of, tile=None):
+    """Where every stream of a batch lives (DESIGN §4.6 "Stream order").  shapes_of: [image][(C, h, w)] coarse ->
+    fine.  Scale si has the plane length plane[si] = max_n h_n * w_n (H * W when the images are equal), and stream
+    (n, si, c, t) covers the elements [(n*C + c) * plane[si] + off_t, ... + n_t) of that scale's [N][C][plane]
+    tensor, (off_t, n_t) = tile_grid(h_n, w_n, tile)[t].
+    -> (scale, elem, n_sym, plane): the scale index, first element and symbol count of every stream, int64
+    [N][streams per image] in container order (image, scale, channel[, tile]), and plane int64 [scales]."""
+    N = len(shapes_of)
+    dims = np.array(shapes_of, np.int64).reshape(N, -1, 3)                 # [N][scale][C, h, w]
+    if (dims[:, :, 0] != dims[:1, :, 0]).any():
+        raise ValueError('images with different channel counts in one batch')
+    plane = (dims[:, :, 1] * dims[:, :, 2]).max(0)
+    img = np.arange(N)[:, None, None]
+    grids, si, elem, n_sym = {}, [], [], []
+    for k in range(dims.shape[1]):
+        C = int(dims[0, k, 0])
+        ext = list(map(tuple, dims[:, k, 1:].tolist()))
+        distinct = set(ext)
+        for e in distinct - grids.keys():
+            grids[e] = np.array(tile_grid(e[0], e[1], tile), np.int64).T      # [offset, n_sym][tile]
+        if len({grids[e].shape for e in distinct}) > 1:
+            raise ValueError('images with different numbers of tiles in one batch')
+        g = grids[ext[0]][:, None] if len(distinct) == 1 else np.stack([grids[e] for e in ext], 1)
+        off, cnt = g[:, :, None, :]                                          # [N or 1][1][tiles] each
+        shape = (N, C, off.shape[-1])
+        si.append(np.full(shape, k))
+        elem.append((img * C + np.arange(C)[None, :, None]) * plane[k] + off)
+        n_sym.append(np.broadcast_to(cnt, shape))
+    return tuple(np.concatenate([x.reshape(N, -1) for x in xs], 1) for xs in (si, elem, n_sym)) + (plane,)
 
 
 class ContainerLayout(object):
@@ -170,40 +206,46 @@ class DecodeLane(object):
 
 
 class EncodeJob:
-    """An encode in flight (BatchCodec.encode_begin).  finish() waits for the stream lengths, lays the
-    containers out, gathers the streams into one blob on the job's stream and (to_host) brings the
-    bytes back: same results as encode_batch."""
+    """An encode in flight (BatchCodec.encode_begin): the range coder is queued on the current stream and the
+    stream lengths are on their way to pinned memory.  finish() waits for them, lays the containers out, gathers
+    the streams into one blob on the job's stream and (to_host) brings the bytes back: same results as
+    encode_batch.  shapes: [(scale, C, H, W)] of the batch tensors; shapes_of / pads: the container shapes
+    [(scale, C, h_n, w_n)] and the padding tuple of every image; caps: slot bytes [N][streams per image]."""
+
+    def __init__(self, codec, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, keep):
+        self.codec, self.shapes, self.shapes_of, self.pads, self.tile, self.out = codec, shapes, shapes_of, pads, tile, out
+        self.caps, self.desc_dev, self.lens_dev = caps, desc_dev, lens_dev
+        self.keep = keep                                       # alive until finish()
+        self.lens_host = torch.empty(lens_dev.shape, dtype=lens_dev.dtype, pin_memory=True)
+        self.lens_host.copy_(lens_dev, non_blocking=True)
+        self.stream = torch.cuda.current_stream()
+        self.coded = torch.cuda.Event()
+        self.coded.record(self.stream)
 
     @_on_device
     def finish(self, to_host=True):
-        codec, N, per_img, caps, shapes = self.codec, self.N, self.per_img, self.caps, self.shapes
+        N, per_img = self.caps.shape
         self.coded.synchronize()                                                   # sync #1 (tiny)
         lens = self.lens_host.numpy().astype(np.int64).reshape(N, per_img)
-        if (lens > (caps if caps.ndim == 2 else caps[None, :])).any():
+        if (lens > self.caps).any():
             raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
         with torch.cuda.stream(self.stream):
             # ---- container layout + gather + single D2H
-            # a ragged batch has one layout and one padding tuple per image
-            layouts = [ContainerLayout(sh, self.tile) for sh in self.shapes_of] if self.ragged else \
-                [ContainerLayout(shapes, self.tile)] * N
-            pt = self.pad_tuple
-            pads = pt if (len(pt) and isinstance(pt[0], (tuple, list))) else [pt] * N
             sizes, pieces_all, dst = [], [], np.zeros((N, per_img), np.int64)
             pos = 0
             starts = []
             for n in range(N):
-                total, pieces, offs = layouts[n].header_and_offsets(lens[n], pads[n])
+                layout = ContainerLayout(self.shapes_of[n], self.tile)
+                total, pieces, offs = layout.header_and_offsets(lens[n], self.pads[n])
                 starts.append(pos)
                 dst[n] = pos + np.asarray(offs, np.int64)
                 pieces_all.append(pieces)
                 sizes.append(total)
                 pos += (total + 15) & ~15
-            blob = torch.empty(pos + 16, dtype=torch.uint8, device=self.dev)
+            blob = torch.empty(pos + 16, dtype=torch.uint8, device=self.lens_dev.device)
             E.pack_streams(self.desc_dev, self.lens_dev, dst.reshape(-1), N * per_img, blob)
-            info = dict(sizes=sizes, starts=starts, lens=lens, shapes=shapes, out=self.out, stream_offsets=dst,
-                        tile=self.tile)
-            if self.ragged:
-                info['shapes_of'] = self.shapes_of                                  # [image][(scale, C, H, W)]
+            info = dict(sizes=sizes, starts=starts, lens=lens, shapes=self.shapes, shapes_of=self.shapes_of,
+                        out=self.out, stream_offsets=dst, tile=self.tile)
             if not to_host:
                 self.packed = torch.cuda.Event()
                 self.packed.record(self.stream)
@@ -271,13 +313,10 @@ class BatchCodec(object):
 
     def ragged_unsupported(self, tile=None):
         """Why this codec cannot code a ragged batch (a message naming it), or None when it can."""
-        if self.net._rgb:
-            return 'ragged batches are not supported by the RGB baselines (bicubic encoder)'
-        if not E.f16_mode():
-            return 'ragged batches run in precision f16 only, not %s' % E.get_conv_precision()
-        if tile is not None:
-            return 'ragged batches are not supported with tiled containers (tile=%s)' % (tuple(tile),)
-        return None
+        why = self.net.ragged_unsupported()
+        if why is None and tile is not None:
+            why = 'ragged batches are not supported with tiled containers (tile=%s)' % (tuple(tile),)
+        return why
 
     def _ragged_extents(self, extents, N, H, W, tile):
         """Validated [(h_n, w_n)] of a ragged batch of N images in an H x W tensor, or None when every image fills
@@ -306,60 +345,56 @@ class BatchCodec(object):
         and returns without waiting.  EncodeJob.finish() completes it.  Lets a caller overlap the
         encode of one batch with other work, e.g. the latency-bound decode of the previous batch.
 
+        pad_tuple: one padding tuple for every container, or a list of one per image.
         extents = [(h_n, w_n)]: a ragged batch (DESIGN §4.6): image n is the top-left h_n x w_n of imgs_u8[n]
-        (zero elsewhere; multiples of 2**num_scales), pad_tuple is then a list of per-image tuples (or one for
-        all), and every container is byte-identical to the one of that image encoded on its own -- one network
-        pass and one range-coder launch for the batch.  f16, learned bottlenecks, reference layout only.
-        Extents that all equal the tensor are the equal-size call."""
+        (zero elsewhere; multiples of 2**num_scales), and every container is byte-identical to the one of that
+        image encoded on its own -- one network pass and one range-coder launch for the batch.  f16, learned
+        bottlenecks, reference layout only.  Extents that all equal the tensor are the equal-size call."""
         assert imgs_u8.dtype == torch.uint8 and imgs_u8.dim() == 4 and imgs_u8.shape[1] == 3
         dev = imgs_u8.device
-        N = imgs_u8.shape[0]
-        ext = self._ragged_extents(extents, N, imgs_u8.shape[2], imgs_u8.shape[3], tile)
-        if ext is not None:
-            return self._encode_begin_ragged(imgs_u8, pad_tuple, out, ext)
-        if out is None:
-            out = self.net(imgs_u8, intervals_of=self.blueprint.losses)      # f16 mode: DMLL head fused into the convs
-
-        # ---- per-symbol intervals, scale by scale (coarse -> fine = container order)
-        scale_ivs = self._scale_intervals(out, dev)
-        shapes = [sh for (sh, _) in scale_ivs]
-        ivs = [iv for (_, iv) in scale_ivs]
-
-        # ---- one range-coder launch for all streams; descriptor order = (image, scale, channel[, tile])
+        N, _, Hb, Wb = imgs_u8.shape
+        ext = self._ragged_extents(extents, N, Hb, Wb, tile)
+        if len(pad_tuple) and isinstance(pad_tuple[0], (tuple, list)):
+            pads = [tuple(int(v) for v in p) for p in pad_tuple]
+            if len(pads) != N:
+                raise ValueError('%d padding tuples for a batch of %d images' % (len(pads), N))
+        else:
+            pads = [tuple(int(v) for v in pad_tuple)] * N
         if tile is not None:
             tile = (int(tile[0]), int(tile[1]))
-            # intervals are produced in raster order; the streams of a tiled container read them tile by tile
-            ivs = [E.reorder_tiles(iv, H, W, tile, True) for iv, (_, C, H, W) in zip(ivs, shapes)]
-        streams = [(si, c, off, n) for si, (_, C, H, W) in enumerate(shapes) for c in range(C)
-                   for (off, n) in tile_grid(H, W, tile)]
-        per_img = len(streams)
-        caps = np.array([_slot_cap(n) for (_, _, _, n) in streams], np.int64)
+        if out is None:
+            # f16 mode: DMLL head fused into the convs
+            out = self.net(imgs_u8, intervals_of=self.blueprint.losses, extents=ext)
+
+        # ---- per-symbol intervals, scale by scale (coarse -> fine = container order), as stream planes
+        shapes, shapes_of, ivs = [], [[] for _ in range(N)], []
+        for (scale, C, H, W), iv in self._scale_intervals(out, dev):
+            f = Hb // H
+            es = [(H, W)] * N if ext is None else [(h // f, w // f) for (h, w) in ext]
+            if ext is not None:
+                iv = E.ragged_pack(iv, C, H, W, E._to_device_async(np.asarray(es, np.int32), dev),
+                                   max(h * w for (h, w) in es), True)
+            elif tile is not None:
+                # intervals are produced in raster order; the streams of a tiled container read them tile by tile
+                iv = E.reorder_tiles(iv, H, W, tile, True)
+            shapes.append((scale, C, H, W))
+            ivs.append(iv)
+            for sh, (h, w) in zip(shapes_of, es):
+                sh.append((scale, C, h, w))
+
+        # ---- one range-coder launch for all streams, each with its own slot
+        si, elem, n_sym, _ = stream_layout([[s[1:] for s in sh] for sh in shapes_of], tile)
+        caps = _slot_cap(n_sym)
         slot_off = np.concatenate([[0], np.cumsum(caps)])
-        img_slot_bytes = int(slot_off[-1])
-        slots = torch.empty(N * img_slot_bytes, dtype=torch.uint8, device=dev)
-        desc = np.zeros(N * per_img, dtype=_lib.ENC_STREAM_DTYPE)
-        d = desc.reshape(N, per_img)
+        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
+        desc = np.zeros(caps.size, dtype=_lib.ENC_STREAM_DTYPE)
         bases = np.array([iv.data_ptr() for iv in ivs], np.int64)
-        st = np.array(streams, np.int64)                                    # [per_img][4]
-        CHW = np.array([(C, H * W) for (_, C, H, W) in shapes], np.int64)[st[:, 0]]      # per stream: C, HW of its scale
-        img = np.arange(N, dtype=np.int64)[:, None]
-        d['intervals'][:] = bases[st[:, 0]][None, :] + ((img * CHW[None, :, 0] + st[None, :, 1]) * CHW[None, :, 1]
-                                                        + st[None, :, 2]) * 4
-        d['n_sym'][:] = st[None, :, 3]
-        d['out_cap'][:] = caps[None, :]
-        d['out'][:] = slots.data_ptr() + img * img_slot_bytes + slot_off[None, :-1]
+        desc['intervals'] = (bases[si] + elem * 4).reshape(-1)
+        desc['n_sym'] = n_sym.reshape(-1)
+        desc['out_cap'] = caps.reshape(-1)
+        desc['out'] = slots.data_ptr() + slot_off[:-1]
         desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
-        lens_host = torch.empty(lens_dev.shape, dtype=lens_dev.dtype, pin_memory=True)
-        lens_host.copy_(lens_dev, non_blocking=True)
-        job = EncodeJob()
-        job.codec, job.stream = self, torch.cuda.current_stream()
-        job.coded = torch.cuda.Event()
-        job.coded.record(job.stream)
-        job.keep = (imgs_u8, ivs, slots)                       # alive until finish()
-        job.N, job.per_img, job.caps, job.shapes, job.out, job.tile = N, per_img, caps, shapes, out, tile
-        job.pad_tuple, job.desc_dev, job.lens_dev, job.lens_host, job.dev = pad_tuple, desc_dev, lens_dev, lens_host, dev
-        job.ragged = False
-        return job
+        return EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, (imgs_u8, ivs, slots))
 
     def _scale_intervals(self, out, dev):
         """Coding intervals of every scale, coarse -> fine: [(shape (scale, C, H, W), int32 [N][C][H*W])]."""
@@ -379,62 +414,6 @@ class BatchCodec(object):
             res.append(((scale, C, H, W), iv))
         return res
 
-    def _encode_begin_ragged(self, imgs_u8, pad_tuple, out, ext):
-        """encode_begin of a ragged batch: the interval planes of every scale are gathered into per-image compact
-        planes (the order the streams read them in) and every stream gets its own length and slot."""
-        dev = imgs_u8.device
-        N, _, Hb, Wb = imgs_u8.shape
-        if pad_tuple and isinstance(pad_tuple[0], (tuple, list)):
-            pads = [tuple(int(v) for v in p) for p in pad_tuple]
-            if len(pads) != N:
-                raise ValueError('%d padding tuples for a batch of %d images' % (len(pads), N))
-        else:
-            pads = [tuple(int(v) for v in pad_tuple)] * N
-        if out is None:
-            out = self.net(imgs_u8, intervals_of=self.blueprint.losses, extents=ext)
-        shapes, ivs, ext_s, planes = [], [], [], []
-        for (scale, C, H, W), iv in self._scale_intervals(out, dev):
-            f = Hb // H
-            es = [(h // f, w // f) for (h, w) in ext]
-            plane = max(h * w for (h, w) in es)
-            shapes.append((scale, C, H, W))
-            ivs.append(E.ragged_pack(iv, C, H, W, E._to_device_async(np.asarray(es, np.int32), dev), plane, True))
-            ext_s.append(es)
-            planes.append(plane)
-        shapes_of = [[(scale, C, ext_s[si][n][0], ext_s[si][n][1]) for si, (scale, C, _, _) in enumerate(shapes)]
-                     for n in range(N)]
-        # one range-coder launch; descriptor order = (image, scale, channel) as in the equal-size call
-        streams = [(si, c) for si, (_, C, _, _) in enumerate(shapes) for c in range(C)]
-        per_img = len(streams)
-        st = np.array(streams, np.int64)
-        hw = np.array([[h * w for (h, w) in es] for es in ext_s], np.int64).T                # [N][scale]
-        n_sym = hw[:, st[:, 0]]                                                                # [N][per_img]
-        caps = ((n_sym * 17 + 7) // 8 + 64 + 3) & ~3                                          # _slot_cap
-        slot_off = np.concatenate([[0], np.cumsum(caps.reshape(-1))])
-        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
-        desc = np.zeros(N * per_img, dtype=_lib.ENC_STREAM_DTYPE)
-        d = desc.reshape(N, per_img)
-        bases = np.array([iv.data_ptr() for iv in ivs], np.int64)
-        Cs = np.array([C for (_, C, _, _) in shapes], np.int64)[st[:, 0]]
-        pl = np.array(planes, np.int64)[st[:, 0]]
-        img = np.arange(N, dtype=np.int64)[:, None]
-        d['intervals'][:] = bases[st[:, 0]][None, :] + ((img * Cs[None, :] + st[None, :, 1]) * pl[None, :]) * 4
-        d['n_sym'][:] = n_sym
-        d['out_cap'][:] = caps
-        d['out'][:] = slots.data_ptr() + slot_off[:-1].reshape(N, per_img)
-        desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
-        lens_host = torch.empty(lens_dev.shape, dtype=lens_dev.dtype, pin_memory=True)
-        lens_host.copy_(lens_dev, non_blocking=True)
-        job = EncodeJob()
-        job.codec, job.stream = self, torch.cuda.current_stream()
-        job.coded = torch.cuda.Event()
-        job.coded.record(job.stream)
-        job.keep = (imgs_u8, ivs, slots)
-        job.N, job.per_img, job.caps, job.shapes, job.out, job.tile = N, per_img, caps, shapes, out, None
-        job.pad_tuple, job.desc_dev, job.lens_dev, job.lens_host, job.dev = pads, desc_dev, lens_dev, lens_host, dev
-        job.ragged, job.shapes_of = True, shapes_of
-        return job
-
     # ------------------------------------------------------------------------------------------
     @_on_device
     def decode_batch(self, datas, to_host=True, lane=None):
@@ -445,14 +424,12 @@ class BatchCodec(object):
         dev = self.blueprint.device
         N = len(datas)
         parsed = [parse_container(d) for d in datas]
-        ref_shapes = [(C, H, W) for (C, H, W, _) in parsed[0][1]]
         tile = container_tile(datas[0])
         shapes_of = [[(C, H, W) for (C, H, W, _) in p[1]] for p in parsed]
-        for p, dta in zip(parsed, datas):
-            if container_tile(dta) != tile or \
-                    ([(C, H, W) for (C, H, W, _) in p[1]] != ref_shapes and self.ragged_unsupported(tile) is not None):
-                raise ValueError('decode_batch needs containers of identical shape')
-        if any(len(sh) != len(ref_shapes) for sh in shapes_of):
+        if any(container_tile(dta) != tile for dta in datas) or \
+                (any(sh != shapes_of[0] for sh in shapes_of) and self.ragged_unsupported(tile) is not None):
+            raise ValueError('decode_batch needs containers of identical shape')
+        if any(len(sh) != len(shapes_of[0]) for sh in shapes_of):
             raise ValueError('decode_batch: containers with different numbers of scales')
         # one upload of everything
         starts = np.zeros(N, np.int64)
@@ -591,115 +568,48 @@ class BatchCodec(object):
         `tile` = (th, tw): the streams are the tiles of a tiled container (ContainerLayout): thousands of short
         streams, so the three RGB channels are simply decoded one after the other, all tiles at once.
         shapes may also be one list per image: a ragged batch (DESIGN §4.6) when they differ; image n then is the
-        top-left H_n x W_n of the result, zero elsewhere."""
+        top-left H_n x W_n of the result, zero elsewhere.
+        Every scale decodes into [N][C][plane] stream planes (stream_layout), where the CDF rows are built too, and
+        then goes back to the raster planes the networks of the next scale read."""
         dev = blob.device
         N = offs.shape[0]
         if shapes and isinstance(shapes[0][0], (tuple, list)):
-            shapes = [[tuple(int(v) for v in s) for s in sh] for sh in shapes]
-            if len(shapes) != N:
-                raise ValueError('%d shape lists for %d images' % (len(shapes), N))
-            if any(sh != shapes[0] for sh in shapes):
-                why = self.ragged_unsupported(tile)
-                if why is not None:
-                    raise NotImplementedError(why)
-                return self._decode_ragged(blob, offs, lens, shapes, lane)
-            shapes = shapes[0]
-        if len(shapes) != self.net.scales + 1:
-            raise ValueError('container has %d scales, model expects %d' % (len(shapes), self.net.scales + 1))
-        K = self.net.config_ms.prob.K
-        self._check_shapes(shapes)
-        bn8, F_prev, S = None, None, None
-        j0 = 0
-        self._mark('start')
-        if tile is not None:
-            tile = (int(tile[0]), int(tile[1]))
-        for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll()):
-            C, H, W = shapes[idx]
-            HW = H * W
-            S = torch.empty(N, C, H, W, dtype=torch.uint8, device=dev)      # symbols in STREAM order (tile order if tiled)
-            grid = tile_grid(H, W, tile)
-            T = len(grid)
-            g_off = np.array([o for (o, _) in grid], np.int64)[None, None, :]
-            g_n = np.array([n for (_, n) in grid], np.int64)[None, None, :]
-            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
-            d = desc.reshape(N, C, T)
-            d['in'][:] = (blob.data_ptr() + offs[:, j0:j0 + C * T]).reshape(N, C, T)
-            d['in_len'][:] = lens[:, j0:j0 + C * T].reshape(N, C, T)
-            j0 += C * T
-            d['n_sym'][:] = g_n
-            plane = (np.arange(N)[:, None, None] * C + np.arange(C)[None, :, None]) * HW + g_off     # first symbol of the stream
-            d['sym_out'][:] = S.data_ptr() + plane
-            pitch = E.table_pitch(dmll.L)
-            if uniform:
-                row_dev = self._uniform(dmll.L, dev)[1]
-                d['table'][:] = row_dev.data_ptr()
-                d['row_pitch'][:] = 0
-                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            else:
-                l, F_prev = self.net.get_P_nhwc(scale, bn8, F_prev if self.net._fuse_feat else None)
-                self._mark('net%d' % scale)
-                if tuple(l.shape[1:3]) != (H, W) or non_shared_get_K(l.shape[-1], C) != K:
-                    raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
-                                     % (scale, C, H, W, tuple(l.shape)))
-                table = torch.empty(N * C * HW * pitch, dtype=torch.int16, device=dev)
-                d['table'][:] = table.data_ptr() + plane * (pitch * 2)
-                d['row_pitch'][:] = pitch
-                tg = dmll.targets(dev)
-                if tile is not None:
-                    if dmll.rgb_scale:
-                        # channel c's means depend on the decoded channels < c of the same pixel: R, G, B one
-                        # after the other, every tile of every image at once (N*T streams per launch)
-                        for c in range(C):
-                            E.dmll_build_table_tiled(l, S, tg, C, K, dmll.L, True, c, table, tile)
-                            dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
-                            self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
-                    else:
-                        E.dmll_build_table_tiled(l, S, tg, C, K, dmll.L, False, -1, table, tile)
-                        self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-                elif dmll.rgb_scale:
-                    self._decode_rgb_pipelined(l, S, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane)
-                else:
-                    E.dmll_build_table(l, S, tg, C, K, dmll.L, False, -1, table)
-                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            if tile is not None:
-                S = E.reorder_tiles(S, H, W, tile, False)                   # back to raster planes
-            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else 'S%d' % scale))
-            if scale > 0:
-                bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
-        return S
-
-    def _decode_ragged(self, blob, offs, lens, shapes_of, lane):
-        """decode_device of a ragged batch: the streams of image n decode into the first H_n * W_n symbols of
-        per-image compact planes (the CDF rows are built there too, from the gathered mixture parameters); the
-        decoded planes are scattered back into the zero-padded planes the networks of the next scale read."""
-        dev = blob.device
-        N = len(shapes_of)
-        for sh in shapes_of:
+            shapes_of = [[tuple(int(v) for v in s) for s in sh] for sh in shapes]
+            if len(shapes_of) != N:
+                raise ValueError('%d shape lists for %d images' % (len(shapes_of), N))
+        else:
+            shapes_of = [[tuple(int(v) for v in s) for s in shapes]] * N
+        ragged = any(sh != shapes_of[0] for sh in shapes_of)
+        if ragged:
+            why = self.ragged_unsupported(tile)
+            if why is not None:
+                raise NotImplementedError(why)
+        for sh in {tuple(sh): sh for sh in shapes_of}.values():               # every distinct shape list once
             if len(sh) != self.net.scales + 1:
                 raise ValueError('container has %d scales, model expects %d' % (len(sh), self.net.scales + 1))
             self._check_shapes(sh)
+        if tile is not None:
+            tile = (int(tile[0]), int(tile[1]))
+        si, elem, n_sym, planes = stream_layout(shapes_of, tile)
+        bounds = np.searchsorted(si[0], np.arange(len(planes) + 1))     # scale idx: columns bounds[idx]:bounds[idx+1]
+        fin = [sh[-1][1:] for sh in shapes_of] if ragged else None      # extents at the finest scale
         K = self.net.config_ms.prob.K
-        fin = [(sh[-1][1], sh[-1][2]) for sh in shapes_of]
-        Hb, Wb = max(h for (h, _) in fin), max(w for (_, w) in fin)
         bn8, F_prev, S = None, None, None
-        j0 = 0
         self._mark('start')
         for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll()):
             C = shapes_of[0][idx][0]
-            H, W = Hb >> scale, Wb >> scale
-            es = [(sh[idx][1], sh[idx][2]) for sh in shapes_of]
-            hw = np.array([h * w for (h, w) in es], np.int64)
-            plane = int(hw.max())
-            ext_dev = E._to_device_async(np.asarray(es, np.int32), dev)
-            Sc = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # compact planes (stream order)
-            desc = np.zeros(N * C, dtype=_lib.DEC_STREAM_DTYPE)
-            d = desc.reshape(N, C)
-            d['in'][:] = blob.data_ptr() + offs[:, j0:j0 + C]
-            d['in_len'][:] = lens[:, j0:j0 + C]
-            j0 += C
-            d['n_sym'][:] = hw[:, None]
-            pl = (np.arange(N)[:, None] * C + np.arange(C)[None, :]) * plane
-            d['sym_out'][:] = Sc.data_ptr() + pl
+            H, W = max(sh[idx][1] for sh in shapes_of), max(sh[idx][2] for sh in shapes_of)
+            plane = int(planes[idx])
+            ext_dev = E._to_device_async(np.array([sh[idx][1:] for sh in shapes_of], np.int32), dev) if ragged else None
+            cols = slice(bounds[idx], bounds[idx + 1])
+            T = (cols.stop - cols.start) // C
+            Sp = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # symbols in stream order
+            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
+            d = desc.reshape(N, C, T)
+            d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
+            d['in_len'][:] = lens[:, cols].reshape(N, C, T)
+            d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
+            d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
             if uniform:
                 d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
                 d['row_pitch'][:] = 0
@@ -710,20 +620,40 @@ class BatchCodec(object):
                 if tuple(l.shape[1:3]) != (H, W) or non_shared_get_K(l.shape[-1], C) != K:
                     raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
                                      % (scale, C, H, W, tuple(l.shape)))
-                # per-pixel kernels from here on: the compact planes are an N x 1 x plane "image" each
-                lc = E.ragged_pack(l, 1, H, W, ext_dev, plane, True).view(N, 1, plane, l.shape[-1])
-                Sv = Sc.view(N, C, 1, plane)
                 pitch = E.table_pitch(dmll.L)
                 table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
-                d['table'][:] = table.data_ptr() + pl * (pitch * 2)
+                d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
                 d['row_pitch'][:] = pitch
                 tg = dmll.targets(dev)
-                if dmll.rgb_scale:
-                    self._decode_rgb_pipelined(lc, Sv, tg, C, K, dmll.L, table, d, dev, lane=lane)
+                if tile is not None:
+                    if dmll.rgb_scale:
+                        # channel c's means depend on the decoded channels < c of the same pixel: R, G, B one
+                        # after the other, every tile of every image at once (N*T streams per launch)
+                        for c in range(C):
+                            E.dmll_build_table_tiled(l, Sp, tg, C, K, dmll.L, True, c, table, tile)
+                            dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
+                            self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
+                    else:
+                        E.dmll_build_table_tiled(l, Sp, tg, C, K, dmll.L, False, -1, table, tile)
+                        self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
                 else:
-                    E.dmll_build_table(lc, Sv, tg, C, K, dmll.L, False, -1, table)
-                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            S = E.ragged_pack(Sc, C, H, W, ext_dev, plane, False)                 # zero-padded [N][C][H][W]
+                    # per-pixel kernels from here on: the stream planes are an N x 1 x plane "image" each
+                    if ragged:
+                        l = E.ragged_pack(l, 1, H, W, ext_dev, plane, True)
+                    l = l.view(N, 1, plane, l.shape[-1])
+                    Sv = Sp.view(N, C, 1, plane)
+                    if dmll.rgb_scale:
+                        self._decode_rgb_pipelined(l, Sv, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane)
+                    else:
+                        E.dmll_build_table(l, Sv, tg, C, K, dmll.L, False, -1, table)
+                        self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
+            # back to raster planes
+            if ragged:
+                S = E.ragged_pack(Sp, C, H, W, ext_dev, plane, False)          # zero-padded [N][C][H][W]
+            elif tile is not None:
+                S = E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
+            else:
+                S = Sp.view(N, C, H, W)
             self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else 'S%d' % scale))
             if scale > 0:
                 bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))

@@ -396,15 +396,20 @@ class MultiscaleNetwork(nn.Module):
             return E.rgb_head_f16(img, self.sub_rgb_mean, self.heads[0].head[0], self.heads[0].head[1].head)
         return E.rgb_prep(img, self.sub_rgb_mean, self.heads[0].head[0])[1]
 
-    def _check_ragged(self, extents, auto_recurse=0):
-        if extents is None:
-            return
+    def ragged_unsupported(self, auto_recurse=0):
+        """Why this network cannot run a ragged batch (a message naming it), or None when it can."""
         if self._rgb:
-            raise NotImplementedError('ragged batches are not supported by the RGB baselines (bicubic encoder)')
+            return 'ragged batches are not supported by the RGB baselines (bicubic encoder)'
         if auto_recurse:
-            raise NotImplementedError('ragged batches are not supported with auto_recurse')
+            return 'ragged batches are not supported with auto_recurse'
         if not E.f16_mode():
-            raise NotImplementedError('ragged batches run in precision f16 only, not %s' % E.get_conv_precision())
+            return 'ragged batches run in precision f16 only, not %s' % E.get_conv_precision()
+        return None
+
+    def _check_ragged(self, extents, auto_recurse=0):
+        why = None if extents is None else self.ragged_unsupported(auto_recurse)
+        if why is not None:
+            raise NotImplementedError(why)
 
     def forward(self, x, auto_recurse=0, intervals_of=None, extents=None):
         """intervals_of: a Losses object -> encode-side pass in f16 mode: the probability heads emit the coding

@@ -1,5 +1,6 @@
-"""Ragged batches (DESIGN §4.6), host side: the pass policy and Python models of the index maps of the two ragged
-kernels (ragged.cu) -- which pixels l3c_ragged_zero_halo writes and how l3c_ragged_pack moves elements."""
+"""Ragged batches (DESIGN §4.6), host side: the pass policy, the stream layout shared by all batches, and Python
+models of the index maps of the two ragged kernels (ragged.cu) -- which pixels l3c_ragged_zero_halo writes and how
+l3c_ragged_pack moves elements."""
 import numpy as np
 import pytest
 
@@ -80,6 +81,58 @@ def test_pack_round_trips_and_zero_fills():
         m[:h, :w] = True
         assert np.array_equal(back[pl].reshape(H, W)[m], src[pl].reshape(H, W)[m])
         assert not back[pl].reshape(H, W)[~m].any()
+
+
+# ---------------------------------------------------------------------------------------------
+# stream layout (codec.stream_layout): the one rule the encode and decode descriptors are built from
+# ---------------------------------------------------------------------------------------------
+@pytest.mark.parametrize('case', ['equal', 'tiled', 'ragged'])
+def test_stream_layout_follows_the_container_order(case):
+    from l3c_pytorch_b200 import codec as C
+    fin, tile = {'equal': ([(32, 48)] * 3, None),
+                 'tiled': ([(40, 56)] * 3, (16, 24)),                   # edge tiles of every scale are partial
+                 'ragged': ([(40, 24), (16, 48), (40, 48), (8, 8)], None)}[case]
+    # cr-like: three 5-channel bottlenecks over the 3-channel image, coarse -> fine
+    shapes_of = [[(s, 3 if s == 0 else 5, h >> s, w >> s) for s in (3, 2, 1, 0)] for (h, w) in fin]
+    si, elem, n_sym, plane = C.stream_layout([[sh[1:] for sh in shs] for shs in shapes_of], tile)
+    N = len(fin)
+    assert si.shape == elem.shape == n_sym.shape and si.shape[0] == N
+    assert plane.tolist() == [max(h * w for (_, _, h, w) in (shs[k] for shs in shapes_of)) for k in range(4)]
+    for n, shs in enumerate(shapes_of):
+        # the order ContainerLayout writes and parse_container reads: scale, channel, tile (row-major), each tile
+        # holding min(th, rows left) x min(tw, columns left) symbols
+        want = []
+        for k, (_, Cc, h, w) in enumerate(shs):
+            th, tw = tile or (h, w)
+            offs = np.cumsum([0] + [min(th, h - y) * min(tw, w - x) for y in range(0, h, th) for x in range(0, w, tw)])
+            want += [(k, c, o, m) for c in range(Cc) for (o, m) in zip(offs[:-1], np.diff(offs))]
+        lens = np.arange(len(want)) % 5
+        total, pieces, _ = C.ContainerLayout(shs, tile).header_and_offsets(lens, (0, 0, 0, 0))
+        buf = bytearray(total)
+        for (o, b) in pieces:
+            buf[o:o + len(b)] = b
+        _, scales = C.parse_container(bytes(buf))
+        assert [k for k, (_, _, _, st) in enumerate(scales) for _ in st] == [k for (k, _, _, _) in want]
+        assert si[n].tolist() == [k for (k, _, _, _) in want]
+        assert n_sym[n].tolist() == [m for (_, _, _, m) in want]
+        # equal-size and tiled batches: the element index the descriptors used before stream_layout existed
+        if case != 'ragged':
+            assert elem[n].tolist() == [(n * Cc + c) * shs[k][2] * shs[k][3] + o for (k, c, o, _) in want
+                                        for Cc in [shs[k][1]]]
+    # the streams of every scale cover disjoint ranges of [N][C][plane], image n channel c from (n*C + c) * plane on
+    for k in range(4):
+        Cc = shapes_of[0][k][1]
+        m = si == k
+        lo, hi = elem[m], elem[m] + n_sym[m]
+        order = np.argsort(lo)
+        assert (hi[order][:-1] <= lo[order][1:]).all() and lo.min() >= 0 and hi.max() <= N * Cc * plane[k]
+        for n, shs in enumerate(shapes_of):
+            covered = sorted(zip(elem[n][si[n] == k], n_sym[n][si[n] == k]))
+            for c in range(Cc):
+                start = (n * Cc + c) * plane[k]
+                mine = [(a, b) for (a, b) in covered if start <= a < start + plane[k]]
+                assert mine[0][0] == start and sum(b for (_, b) in mine) == shs[k][2] * shs[k][3]
+                assert all(a + b == a2 for (a, b), (a2, _) in zip(mine, mine[1:]))        # one contiguous run
 
 
 # ---------------------------------------------------------------------------------------------

@@ -15,8 +15,8 @@ marks = []
 def mark(name):
     e = torch.cuda.Event(enable_timing=True); e.record(); marks.append((name, e))
 orig_getP = bp.net.get_P_nhwc
-def getP(scale, bn8, F):
-    mark('getP%d_begin' % scale); r = orig_getP(scale, bn8, F); mark('getP%d_end' % scale); return r
+def getP(scale, bn8, F, **kw):
+    mark('getP%d_begin' % scale); r = orig_getP(scale, bn8, F, **kw); mark('getP%d_end' % scale); return r
 bp.net.get_P_nhwc = getP
 orig_tab = E.dmll_build_table
 orig_dec = E.ac_decode_streams
