@@ -273,6 +273,14 @@ int l3c_ragged_zero_halo(void *x_dev, int px_bytes, int N, int H, int W, const i
                          void *stream);
 int l3c_ragged_pack(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
                     const int *extents_dev, long long compact_len, int to_compact, void *stream);
+/* l3c_dmll_nll of a ragged batch: l_dev NHWC [N][H][W][Kp] and sym_dev [N][C][H][W] are padded, nll_dev f64 [N]
+ * gets the nats of the h_n * w_n pixels of every image, bit-identical to l3c_dmll_nll on that image alone (the same
+ * 128-pixel blocks in raster order of the extent, the same summation order).  Nothing outside an extent is read.
+ * Every extent must satisfy 1 <= h_n <= H and 1 <= w_n <= W; an image whose extent does not reads nothing and
+ * gets NaN. */
+int l3c_dmll_nll_ragged(const float *l_dev, const uint8_t *sym_dev, const float *values_dev, int N, int H, int W,
+                        int C, int K, int L, int rgb, float x_min, float x_max, const int *extents_dev,
+                        double *nll_dev, void *stream);
 
 /* L3C_PREC_F16X2: fp32 [n_px][C] -> split operand image FP16 [n_px][2*C] (hi = fp16(x) in channels [0,C),
  * lo = fp16((x - hi) * 2^11) in [C,2C)); C % 4 == 0.  For the outputs of the CUDA-core layers of that mode (no

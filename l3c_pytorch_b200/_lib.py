@@ -67,6 +67,7 @@ _SIGNATURES = {
     'l3c_rgb_im2col_f16_ragged': (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 3),
     'l3c_ragged_zero_halo': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_int, c_void_p]),
     'l3c_ragged_pack': (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, ctypes.c_longlong, c_int, c_void_p]),
+    'l3c_dmll_nll_ragged': (c_int, [c_void_p] * 3 + [c_int] * 7 + [c_float, c_float] + [c_void_p] * 3),
     'l3c_quantize_head': (c_int, [c_void_p] * 4 + [c_int] * 5 + [c_void_p, c_void_p, c_void_p]),
     'l3c_symbols_to_values': (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_void_p, c_void_p]),
     'l3c_bicubic_half_u8': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),

@@ -28,17 +28,18 @@ _MAGIC_VALUE_SEP = MAGIC
 RAGGED_PASS_PIXELS = 16 * 768 * 768
 
 
-def plan_passes(shapes, budget=None):
+def plan_passes(shapes, budget=None, max_images=None):
     """shapes: padded (H, W) per image -> lists of image indices, one per ragged pass.  Images are sorted by shape
     (ties in input order) and consecutive ones share a pass while N * Hmax * Wmax stays within `budget` (default
-    RAGGED_PASS_PIXELS); an image larger than the budget is a pass of its own."""
+    RAGGED_PASS_PIXELS) and N within `max_images` (default: no limit); an image larger than the budget is a pass of
+    its own."""
     budget = RAGGED_PASS_PIXELS if budget is None else budget
     order = sorted(range(len(shapes)), key=lambda i: (tuple(shapes[i]), i))
     passes, cur, hm, wm = [], [], 0, 0
     for i in order:
         h, w = shapes[i]
         nh, nw = max(hm, h), max(wm, w)
-        if cur and (len(cur) + 1) * nh * nw > budget:
+        if cur and ((len(cur) + 1) * nh * nw > budget or (max_images is not None and len(cur) >= max_images)):
             passes.append(cur)
             cur, nh, nw = [], h, w
         cur.append(i)

@@ -30,12 +30,13 @@ class MultiscaleBlueprint(nn.Module):
         self.losses.loss_dmol_n.eval()
         return self
 
-    def forward(self, in_batch, auto_recurse=0) -> Out:
-        """in_batch: NCHW 0..255 (float / long / uint8) on the GPU."""
+    def forward(self, in_batch, auto_recurse=0, extents=None) -> Out:
+        """in_batch: NCHW 0..255 (float / long / uint8) on the GPU.  extents: [(h_n, w_n)] -> a ragged batch
+        (MultiscaleNetwork.forward): the losses of the returned Out cover every image's own extent only."""
         if self.device.type != 'cuda':
-            return self.net(in_batch, auto_recurse)   # raises: there is no CPU path
+            return self.net(in_batch, auto_recurse, extents=extents)   # raises: there is no CPU path
         with torch.cuda.device(self.device):          # kernels launch on the CURRENT device
-            return self.net(in_batch, auto_recurse)
+            return self.net(in_batch, auto_recurse, extents=extents)
 
     def forward_for_coding(self, in_batch) -> Out:
         """forward() for the bit-coder: in f16 mode the DMLL head is fused into the 1x1 convs of the probability
@@ -69,10 +70,14 @@ class MultiscaleBlueprint(nn.Module):
     def get_loss_per_image(self, out: Out, num_subpixels_before_pad=None):
         """Total theoretical bpsp (all scales + the uniform-prior final scale) of every image of the
         batch, as a list of floats: what get_loss() gives for a batch of one, without running the
-        images one at a time.  `num_subpixels_before_pad` counts ONE image."""
+        images one at a time.  `num_subpixels_before_pad` counts ONE image (an int), or is one count per image (a
+        sequence), e.g. the unpadded sub-pixels of every image of a ragged batch (Out.extents)."""
         costs, final_cost_uniform, num_subpixels = self.losses.get_per_image(out)
-        if num_subpixels_before_pad:
-            assert num_subpixels_before_pad <= num_subpixels, num_subpixels_before_pad
+        if num_subpixels_before_pad is not None and np.ndim(num_subpixels_before_pad) > 0:
+            num_subpixels_before_pad = np.asarray(num_subpixels_before_pad, np.int64)
+            assert num_subpixels_before_pad.shape == (out.S_u8[0].shape[0],), num_subpixels_before_pad.shape
+        if np.ndim(num_subpixels_before_pad) > 0 or num_subpixels_before_pad:
+            assert np.all(num_subpixels_before_pad <= num_subpixels), num_subpixels_before_pad
             num_subpixels = num_subpixels_before_pad
         if out.auto_recursive_from is not None:                  # sum(recursive_bpsps): the last scale is the uniform one
             final_cost_uniform = out.get_nat_count(-1) / out.S_u8[0].shape[0]

@@ -213,18 +213,40 @@ __device__ __forceinline__ float softplus_f(float x) {   // torch.nn.functional.
 
 constexpr int NLL_THREADS = 128;
 
-template <int K>
+// Pixels of image n the NLL visits: all H*W of the plane, or (RAGGED) the h_n x w_n of its extent, which must lie
+// inside the plane -- an extent that does not covers no pixel here and makes nll_finish_kernel report NaN.
+__device__ __forceinline__ int nll_pixels(const int *__restrict__ extents, int n, int H, int W, int &wn) {
+    if (!extents) {
+        wn = W;
+        return H * W;
+    }
+    const int hn = extents[2 * n];
+    wn = extents[2 * n + 1];
+    return (hn >= 1 && hn <= H && wn >= 1 && wn <= W) ? hn * wn : 0;
+}
+
+// One CTA sums NLL_THREADS consecutive pixels of one image.  Pixel q of image n is taken in raster order of the
+// pixels it visits (nll_pixels): with RAGGED the plane is a padded H x W and q lies at row q / w_n, column q % w_n
+// of it, so image n is cut into the same CTAs, partials and per-pixel math as a launch on that image alone.
+template <int K, bool RAGGED>
 __global__ void __launch_bounds__(NLL_THREADS)
 dmll_nll_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
-                const float *__restrict__ values, int HW, int C, int L, int rgb, float x_min,
-                float x_max, double *__restrict__ partial /* [N][gridDim.x] */,
+                const float *__restrict__ values, int H, int W, int C, int L, int rgb, float x_min,
+                float x_max, const int *__restrict__ extents /* [N][2], RAGGED only */,
+                double *__restrict__ partial /* [N][gridDim.x] */,
                 float *__restrict__ nll_map /* [N][C][HW] or null */) {
+    // first: the fp64 division is a call, and the ragged pixel mapping held across it spilled to local memory
+    const float half_bin = (float)(((double)x_max - (double)x_min) / (double)(L - 1) / 2.0);
+    const int HW = H * W;
     const int Kp = (rgb ? 4 : 3) * C * K;
     const int n = blockIdx.y;
-    const int p = blockIdx.x * NLL_THREADS + threadIdx.x;
-    const float half_bin = (float)(((double)x_max - (double)x_min) / (double)(L - 1) / 2.0);
+    const int q = blockIdx.x * NLL_THREADS + threadIdx.x;
+    int wn;
+    const int npix = nll_pixels(RAGGED ? extents : nullptr, n, H, W, wn);
+    if (RAGGED && (int)blockIdx.x * NLL_THREADS >= npix) return;       // the whole CTA: beyond this image
+    const int p = RAGGED ? q + (q / wn) * (W - wn) : q;                // row q / w_n, column q % w_n
     double mine = 0.0;
-    if (p < HW) {
+    if (q < npix) {
         const float *lp = l + ((size_t)n * HW + p) * Kp;
         float xr = 0.f, xg = 0.f;
         for (int c = 0; c < C; ++c) {
@@ -282,12 +304,21 @@ dmll_nll_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
     }
 }
 
-__global__ void nll_finish_kernel(const double *__restrict__ partial, int per_image,
-                                  double *__restrict__ out) {
-    // one warp per image, fixed summation order
+__global__ void nll_finish_kernel(const double *__restrict__ partial, int per_image, int H, int W,
+                                  const int *__restrict__ extents, double *__restrict__ out) {
+    // one warp per image, fixed summation order; a ragged image sums only the partials of its own CTAs
     const int n = blockIdx.x;
+    int count = per_image, wn;
+    if (extents) {
+        const int npix = nll_pixels(extents, n, H, W, wn);
+        if (npix == 0) {
+            if (threadIdx.x == 0) out[n] = __longlong_as_double(0x7FF8000000000000LL);
+            return;
+        }
+        count = (npix + NLL_THREADS - 1) / NLL_THREADS;
+    }
     double t = 0.0;
-    for (int i = threadIdx.x; i < per_image; i += 32) t += partial[(size_t)n * per_image + i];
+    for (int i = threadIdx.x; i < count; i += 32) t += partial[(size_t)n * per_image + i];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) t += __shfl_down_sync(0xFFFFFFFFu, t, o);
     if (threadIdx.x == 0) out[n] = t;
@@ -468,11 +499,32 @@ extern "C" int l3c_dmll_nll(const float *l_dev, const uint8_t *sym_dev, const fl
     const int per_image = ceil_div(HW, NLL_THREADS);
     double *partial = nullptr;
     L3C_CUDA(cudaMallocAsync(&partial, sizeof(double) * (size_t)N * per_image, (cudaStream_t)stream));
-    dim3 grid(per_image, N);
-    dmll_nll_kernel<10><<<grid, NLL_THREADS, 0, (cudaStream_t)stream>>>(
-        l_dev, sym_dev, values_dev, HW, C, L, rgb, x_min, x_max, partial, nll_map_dev);
+    dim3 grid(per_image, N);                                 // the plane as one row of HW pixels
+    dmll_nll_kernel<10, false><<<grid, NLL_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, values_dev, 1, HW, C, L, rgb, x_min, x_max, nullptr, partial, nll_map_dev);
     L3C_LAUNCH_CHECK("dmll_nll_kernel");
-    nll_finish_kernel<<<N, 32, 0, (cudaStream_t)stream>>>(partial, per_image, nll_dev);
+    nll_finish_kernel<<<N, 32, 0, (cudaStream_t)stream>>>(partial, per_image, 1, HW, nullptr, nll_dev);
+    L3C_LAUNCH_CHECK("nll_finish_kernel");
+    L3C_CUDA(cudaFreeAsync(partial, (cudaStream_t)stream));
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_nll_ragged(const float *l_dev, const uint8_t *sym_dev, const float *values_dev, int N, int H,
+                                   int W, int C, int K, int L, int rgb, float x_min, float x_max,
+                                   const int *extents_dev, double *nll_dev, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(H >= 1 && W >= 1 && (int64_t)H * W <= INT32_MAX, "l3c_dmll_nll_ragged: H=%d W=%d", H, W);
+    if (int e = check_common("l3c_dmll_nll_ragged", N, H * W, C, K, L, rgb)) return e;
+    L3C_REQUIRE(l_dev && sym_dev && values_dev && extents_dev && nll_dev, "l3c_dmll_nll_ragged: null pointer");
+    // CTAs for the largest image the plane can hold; those beyond an image's own pixels exit at once
+    const int per_image = ceil_div(H * W, NLL_THREADS);
+    double *partial = nullptr;
+    L3C_CUDA(cudaMallocAsync(&partial, sizeof(double) * (size_t)N * per_image, (cudaStream_t)stream));
+    dim3 grid(per_image, N);
+    dmll_nll_kernel<10, true><<<grid, NLL_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, values_dev, H, W, C, L, rgb, x_min, x_max, extents_dev, partial, nullptr);
+    L3C_LAUNCH_CHECK("dmll_nll_kernel");
+    nll_finish_kernel<<<N, 32, 0, (cudaStream_t)stream>>>(partial, per_image, H, W, extents_dev, nll_dev);
     L3C_LAUNCH_CHECK("nll_finish_kernel");
     L3C_CUDA(cudaFreeAsync(partial, (cudaStream_t)stream));
     return L3C_OK;

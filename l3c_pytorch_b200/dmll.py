@@ -105,10 +105,17 @@ class DiscretizedMixLogisticLoss(nn.Module):
             u_x = torch.empty(N, C, H, W, dtype=torch.float32, device=lh.device).uniform_(1e-5, 1. - 1e-5)
         return E.dmll_sample(lh.contiguous(), u_sel, u_x, C, K, self.use_coeffs)
 
-    def nll_sum(self, sym_u8, l_nhwc, want_map=False):
-        """per-image NLL in nats (float64 [N]) of uint8 symbol planes under NHWC parameters."""
+    def nll_sum(self, sym_u8, l_nhwc, want_map=False, extents=None):
+        """per-image NLL in nats (float64 [N]) of uint8 symbol planes under NHWC parameters.
+        extents: [(h_n, w_n)] at this resolution -> a ragged batch: image n is summed over [0, h_n) x [0, w_n) only,
+        bit-identical to its own call (no per-sub-pixel map)."""
         C = sym_u8.shape[1]
         K = non_shared_get_K(l_nhwc.shape[-1], C)
+        if extents is not None:
+            if want_map:
+                raise NotImplementedError('per-sub-pixel NLL maps are not built for ragged batches')
+            return E.dmll_nll_ragged(l_nhwc, sym_u8, self.values(l_nhwc.device), C, K, self.L, self.rgb_scale,
+                                     self.x_min, self.x_max, extents)
         s, m = E.dmll_nll(l_nhwc, sym_u8, self.values(l_nhwc.device), C, K, self.L, self.rgb_scale,
                           self.x_min, self.x_max, want_map)
         return (s, m) if want_map else s

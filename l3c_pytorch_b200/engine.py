@@ -783,6 +783,27 @@ def dmll_nll(l, sym, values, C, K, L, rgb, x_min, x_max, want_map=False):
     return out, nmap
 
 
+def dmll_nll_ragged(l, sym, values, C, K, L, rgb, x_min, x_max, extents):
+    """dmll_nll of a ragged batch: l NHWC [N,H,W,Kp] and sym [N,C,H,W] padded, image n occupies [0, h_n) x [0, w_n)
+    (`extents` = [(h_n, w_n)] at this resolution).  -> per-image nats float64 [N], bit-identical to dmll_nll on each
+    image alone; nothing outside an extent is read."""
+    N, H, W, _ = l.shape
+    ext = [(int(h), int(w)) for (h, w) in extents]
+    if len(ext) != N:
+        raise ValueError('%d extents for a batch of %d images' % (len(ext), N))
+    for n, (h, w) in enumerate(ext):
+        if not (1 <= h <= H and 1 <= w <= W):
+            raise ValueError('extent %dx%d of image %d does not fit the %dx%d batch' % (h, w, n, H, W))
+    assert tuple(sym.shape) == (N, C, H, W) and sym.dtype == torch.uint8, (tuple(sym.shape), sym.dtype)
+    l, sym = l.contiguous(), sym.contiguous()
+    ext_dev = _to_device_async(np.array(ext, np.int32).reshape(N, 2), l.device)
+    out = torch.empty(N, dtype=torch.float64, device=l.device)
+    check(lib.l3c_dmll_nll_ragged(_ptr(l), _ptr(sym), _ptr(values), N, H, W, C, K, L, int(rgb), float(x_min),
+                                  float(x_max), _ptr(ext_dev), _ptr(out), _stream_ptr()))
+    LAUNCHES['n'] += 2
+    return out
+
+
 def dmll_channel_params(l, x_dec, C, K, rgb, c):
     """l NHWC; x_dec f32 [N,C,H,W] contiguous (values of already coded channels) or None.
     -> (softmax pi, mu, log sigma), each [N,K,H,W] f32."""

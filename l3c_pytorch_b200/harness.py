@@ -19,8 +19,12 @@ What it mirrors (flag names and meaning as in /root/reference/src/test.py:44-141
     real bpsp reported, per-stage times collected (test/multiscale_tester.py:347-373).
 --sample writes the ground truth and three sampled images per test image (row f3).
 
-H100-first difference: in the default mode images of equal size are pushed through the network as
-one batch (`--batch`, default 16) instead of one at a time.
+H100-first difference: in the default mode up to `--batch` images (default 16) share one network pass instead
+of going one at a time.  Where the network runs ragged batches (precision f16, learned bottlenecks, no
+--recursive; DESIGN §4.6) every crop is padded on its own and crops of ANY sizes are planned into passes
+(bitcoding.plan_passes), each placed top-left in a zero batch: the bpsp of every image is bit-identical to
+evaluating it alone.  Elsewhere (fp32 / tf32 / f16x2, the RGB baselines, --recursive) only crops of equal shape
+share a pass.
 """
 import argparse
 import fnmatch
@@ -190,6 +194,29 @@ def save_png(img_1chw, path):
     Image.fromarray(np.ascontiguousarray(a)).save(path)
 
 
+def ragged_theory_bpsps(blueprint, crops, fac, batch_max):
+    """Theoretical bpsp of every crop (uint8 CHW, any sizes) in ragged passes (DESIGN §4.6): each crop is padded on
+    its own to a multiple of `fac`, the padded shapes are planned into passes of at most `batch_max` images
+    (bitcoding.plan_passes), each pass is placed top-left in a zero batch and run with forward(extents=).  The bpsp
+    counts the crop's unpadded sub-pixels and is bit-identical to evaluating the crop alone.  -> [float] per crop."""
+    from .bitcoding import plan_passes
+    padded_shapes = [(c.shape[1] + (-c.shape[1]) % fac, c.shape[2] + (-c.shape[2]) % fac) for c in crops]
+    bpsps = [None] * len(crops)
+    for idxs in plan_passes(padded_shapes, max_images=batch_max):
+        padded = [blueprint.unpack_batch_pad(crops[i].unsqueeze(0), fac=fac)[0] for i in idxs]
+        shapes = [tuple(t.shape[-2:]) for t in padded]
+        assert shapes == [padded_shapes[i] for i in idxs], shapes
+        Hb, Wb = max(h for h, _ in shapes), max(w for _, w in shapes)
+        batch = torch.zeros(len(idxs), 3, Hb, Wb, dtype=padded[0].dtype, device=padded[0].device)
+        for k, t in enumerate(padded):
+            batch[k, :, :t.shape[2], :t.shape[3]] = t[0]
+        out = blueprint.forward(batch, 0, extents=shapes)
+        n_sub = [crops[i].numel() for i in idxs]
+        for i, bpsp in zip(idxs, blueprint.get_loss_per_image(out, num_subpixels_before_pad=n_sub)):
+            bpsps[i] = float(bpsp)
+    return bpsps
+
+
 class TestResult(object):
     def __init__(self, metric_name='bpsp'):
         self.metric_name = metric_name
@@ -304,13 +331,48 @@ class Tester(object):
         self._cache_put(key, result)
         return result
 
-    # ---- default mode: theoretical bpsp, equal-sized images batched
+    # ---- default mode: theoretical bpsp, images of any sizes (ragged passes) or of equal size batched
+    def _ragged(self):
+        """True when the blueprint evaluates ragged batches (MultiscaleNetwork.ragged_unsupported is None)."""
+        why = getattr(self.blueprint.net, 'ragged_unsupported', None)
+        return why is not None and why(self.recursive) is None
+
     def _theory(self, testset):
-        from . import auto_crop
         result = TestResult('bpsp recursive' if self.recursive else 'bpsp')
         # multiscale_tester.py:222-225: every recursion halves the image once more
         fac = 2 ** (self.recursive + 1) if self.recursive else 2 ** self.config_ms.num_scales
         batch_max = max(1, int(getattr(self.flags, 'batch', 16) or 1))
+        if self._ragged():
+            combos = self._theory_ragged(testset, fac, batch_max)
+        else:
+            combos = self._theory_by_shape(testset, fac, batch_max)
+        for name, comb in combos.items():
+            result[name] = comb.get_bpsp()
+        print('{}: {} images: mean {}={}'.format(self.log_date, len(combos), result.metric_name, result.mean()))
+        return result
+
+    def _theory_ragged(self, testset, fac, batch_max):
+        """Every crop of the test set through ragged passes (ragged_theory_bpsps); crops combined in test-set
+        order."""
+        from . import auto_crop
+        combos = OrderedDict()                  # image name -> CropLossCombinator
+        crops = []                              # [(name, crop uint8 CHW)] in test-set order
+        for p in testset.ps:
+            name = os.path.splitext(os.path.basename(p))[0]
+            img = read_image_chw(p, self.flags.crop)
+            combos[name] = auto_crop.CropLossCombinator()
+            crops += [(name, crop[0]) for crop in auto_crop.iter_crops(img.unsqueeze(0))]
+        bpsps = ragged_theory_bpsps(self.blueprint, [c for _, c in crops], fac, batch_max)
+        for (name, crop), bpsp in zip(crops, bpsps):
+            combos[name].add(bpsp, crop.numel())
+        if getattr(self.flags, 'sample', None):            # multiscale_tester.py:327-328 (one image at a time)
+            for (name, crop) in crops:
+                self._sample(name, crop, fac)
+        return combos
+
+    def _theory_by_shape(self, testset, fac, batch_max):
+        """Crops of equal shape share a pass of at most `batch_max` images."""
+        from . import auto_crop
         combos = OrderedDict()                  # image name -> CropLossCombinator
         pending = OrderedDict()                 # (C,H,W) -> [(name, crop uint8 CHW)]
 
@@ -340,10 +402,7 @@ class Tester(object):
                     flush(shape)
         for shape in list(pending):
             flush(shape)
-        for name, comb in combos.items():
-            result[name] = comb.get_bpsp()
-        print('{}: {} images: mean {}={}'.format(self.log_date, len(combos), result.metric_name, result.mean()))
-        return result
+        return combos
 
     # ---- --sample: images sampled from the model (multiscale_tester.py:436-448)
     def _sample(self, name, raw_u8, fac):
@@ -420,7 +479,10 @@ def build_parser():
     p.add_argument('--time_report', type=str, metavar='TIME_REPORT_PATH')
     p.add_argument('--sort_output', '-s', choices=['testset', 'exp', 'itr', 'res'], default='testset')
     p.add_argument('--configs_dir', default=None, help='Root of the ms/ and dl/ config trees (default: the package\'s).')
-    p.add_argument('--batch', type=int, default=16, help='Images of equal size per network pass (default mode).')
+    p.add_argument('--batch', type=int, default=16,
+                   help='Most images per network pass (default mode): images of any sizes share a pass where the '
+                        'network runs ragged batches (precision f16, learned bottlenecks, no --recursive), '
+                        'else only images of equal size.')
     return p
 
 

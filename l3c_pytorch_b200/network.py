@@ -280,6 +280,7 @@ class Out(object):
         assert targets_style in ('S', 'bn')
         self.S_u8, self.bn8, self.P_nhwc, self.L = [], [], [], []
         self.IV = None          # per scale: coding intervals from the fused head (forward(intervals_of=...)), P is None then
+        self.extents = None     # ragged batch (forward(extents=...)): [(h_n, w_n)] of every image at the finest scale
         self.auto_recursive_from = auto_recursive_from
         self.targets_style = targets_style
 
@@ -311,9 +312,23 @@ class Out(object):
         self.bn8.append(enc_out.bn_q)
         assert len(self.S_u8) == len(self.L) == len(self.bn8) == len(self.P_nhwc) + 1
 
+    def extents_at(self, i):
+        """Ragged batch: [(h_n, w_n)] of every image at the resolution of S_u8[i] (scale index, -1 the coarsest)."""
+        s = i % len(self.S_u8)
+        return [(h >> s, w >> s) for (h, w) in self.extents]
+
     def get_nat_count(self, i):
+        if self.extents is not None:
+            return float(self.get_nat_counts_per_image(i).sum())
         N, C, H, W = self.S_u8[i].shape
         return N * C * H * W * np.log(self.L[i])
+
+    def get_nat_counts_per_image(self, i):
+        """Uniform-prior nats of S_u8[i] for every image, float64 [N]: priced over each image's own extent in a
+        ragged batch, exactly as get_nat_count() of that image alone."""
+        N, C, H, W = self.S_u8[i].shape
+        ext = self.extents_at(i) if self.extents is not None else [(H, W)] * N
+        return np.array([C * h * w * np.log(self.L[i]) for (h, w) in ext], np.float64)
 
 
 class Losses(nn.Module):
@@ -329,7 +344,11 @@ class Losses(nn.Module):
 
     def get(self, out):
         """(per-scale costs in nats [python floats, summed over the batch], uniform-scale nats,
-        number of sub-pixels) -- multiscale_network.py:145-165."""
+        number of sub-pixels) -- multiscale_network.py:145-165.  A ragged Out (Out.extents) counts every image over
+        its own extent only, never the padding."""
+        if out.extents is not None:
+            costs, uniform, num_subpixels = self.get_per_image(out)
+            return [float(c.sum()) for c in costs], float(uniform.sum()), int(num_subpixels.sum())
         costs = [float(self.loss_dmol_rgb.nll_sum(out.S_u8[0], out.P_nhwc[0]).sum())]
         for s in range(1, len(out.P_nhwc)):
             costs.append(float(self.loss_dmol_n.nll_sum(out.S_u8[s], out.P_nhwc[s]).sum()))
@@ -338,7 +357,16 @@ class Losses(nn.Module):
 
     def get_per_image(self, out):
         """Same quantities as get(), kept apart per image of the batch: (per-scale nats as float64
-        arrays [N], uniform-scale nats of ONE image, sub-pixels of ONE image)."""
+        arrays [N], uniform-scale nats of ONE image, sub-pixels of ONE image).
+        A ragged Out (Out.extents): every image over its own extent, (h_n >> s, w_n >> s) at scale s, bit-identical to
+        the Out of that image alone; the uniform-scale nats and the sub-pixels are then arrays [N] as well."""
+        if out.extents is not None:
+            dms = [self.loss_dmol_rgb] + [self.loss_dmol_n] * (len(out.P_nhwc) - 1)
+            costs = [dm.nll_sum(out.S_u8[s], out.P_nhwc[s], extents=out.extents_at(s)).double().cpu().numpy()
+                     for s, dm in enumerate(dms)]
+            final_idx = -1 if out.auto_recursive_from is None else out.auto_recursive_from
+            subpixels = np.array([out.S_u8[0].shape[1] * h * w for (h, w) in out.extents], np.int64)
+            return costs, out.get_nat_counts_per_image(final_idx), subpixels
         costs = [self.loss_dmol_rgb.nll_sum(out.S_u8[0], out.P_nhwc[0]).double().cpu().numpy()]
         for s in range(1, len(out.P_nhwc)):
             costs.append(self.loss_dmol_n.nll_sum(out.S_u8[s], out.P_nhwc[s]).double().cpu().numpy())
@@ -427,7 +455,10 @@ class MultiscaleNetwork(nn.Module):
         img = self._as_u8_planes(x)
         self._check_ragged(extents, auto_recurse)
         with E.ragged_extents(extents, img.shape[2], img.shape[3]):
-            return self._forward(img, auto_recurse, intervals_of)
+            out = self._forward(img, auto_recurse, intervals_of)
+        if extents is not None:
+            out.extents = [(int(h), int(w)) for (h, w) in extents]
+        return out
 
     def _forward(self, img, auto_recurse, intervals_of):
         forward_scales = list(range(self.scales)) + [-1] * int(auto_recurse)
