@@ -51,7 +51,11 @@ long long l3c_launch_log(char *buf, size_t cap, int reset);
  * A. Drop-in native exports (reference: torchac.cpp:433-443; python shim torchac.py:87-166)
  * ---------------------------------------------------------------------------------------- */
 
-/* replaces `cuda_supported()` (torchac.cpp:439,441): 1 iff an sm_90 device is usable. */
+/* The four coding functions accept every Lp in [2, 32769] (L = Lp - 1 symbols, int16 symbols as in the reference);
+ * any other Lp is L3C_EINVAL.  Rows must be strictly increasing over entries 0..L-1, as the reference's binary
+ * search assumes; the last entry is never read.
+ *
+ * replaces `cuda_supported()` (torchac.cpp:439,441): 1 iff an sm_90 device is usable. */
 int l3c_cuda_supported(void);
 
 /* replaces `encode_cdf(cdf, sym) -> bytes` (torchac.cpp:262-269 -> encode() :152-227).
@@ -101,19 +105,25 @@ typedef struct {
     const uint16_t *table;      /* dev: CDF rows for symbols [0, n_sym) of this stream           */
     const uint8_t *in;          /* dev: code bytes at ANY byte address (decoded in place from the  */
                                 /*      container); the buffer must be readable 4 bytes past the end */
-    uint8_t *sym_out;           /* dev: n_sym decoded symbols                                    */
+    uint8_t *sym_out;           /* dev: n_sym decoded symbols, uint8; for L > 256 n_sym           */
+                                /*      little-endian uint16, 2-byte aligned.  Nothing past n_sym  */
+                                /*      symbols is written.                                       */
     uint32_t *state;            /* dev: 4 words of coder state (low, high, value, bitpos);        */
                                 /*      lets one stream be decoded in several launches (chunks)   */
     int64_t row_pitch;          /* entries between consecutive rows; 0 = one shared row.  Every   */
-                                /*      row is read whole: 32 entries for L <= 32, 256 for L > 32, */
-                                /*      16-byte aligned.  Entries past L may hold anything.       */
+                                /*      row is read whole: 32 entries for L <= 32, 256 for L <= 256,*/
+                                /*      round_up(L, 8) for L > 256, 16-byte aligned.  Entries past */
+                                /*      L may hold anything.  For L > 256 the pitch must be 0 or a */
+                                /*      multiple of 8 that is >= L.                               */
     uint32_t n_sym;             /* total symbols of the stream                                    */
     uint32_t in_len;
 } l3c_dec_stream_t;
 
 /* Decodes symbols [first, first+count) of every stream (count clipped to n_sym).  first == 0
  * initialises the coder state from the stream head, otherwise it is resumed from `state`.
- * L = number of symbols of the alphabet (<= 256). */
+ * L = number of symbols of the alphabet, 1 to 32768.  For L > 256 the descriptors are first copied to the host and
+ * checked (row_pitch, 16-byte aligned table, 2-byte aligned sym_out; L3C_EINVAL otherwise), so the call waits for
+ * `stream`. */
 int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_streams, int L,
                           uint32_t first, uint32_t count, void *stream);
 

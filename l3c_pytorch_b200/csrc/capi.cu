@@ -166,12 +166,16 @@ static int run_encode(const uint32_t *iv_dev, int64_t n_sym, uint8_t *out_host, 
     return L3C_OK;
 }
 
+// row pitch of the decoder's tables: 32 entries for L <= 32, 256 up to L = 256, else L rounded up to a multiple of 8
+static int decode_pitch(int L) { return (L <= 32) ? 32 : (L <= 256) ? 256 : (L + 7) & ~7; }
+
 static int run_decode(const uint16_t *table_dev, int pitch, int64_t n_sym, int L,
                       const uint8_t *in_host, size_t in_len, int16_t *sym_out_host) {
     const size_t padded = ((in_len + 3) & ~(size_t)3) + 8;
+    const size_t sym_bytes = (L > 256) ? 2 : 1;        // the decoder writes uint16 symbols for L > 256
     DevBuf in, sym, desc;
     if (int e = in.alloc(padded)) return e;
-    if (int e = sym.alloc((size_t)n_sym)) return e;
+    if (int e = sym.alloc((size_t)n_sym * sym_bytes)) return e;
     if (int e = desc.alloc(sizeof(l3c_dec_stream_t))) return e;
     L3C_CUDA(cudaMemset(in.p, 0, padded));
     if (in_len) L3C_CUDA(cudaMemcpy(in.p, in_host, in_len, cudaMemcpyHostToDevice));
@@ -185,15 +189,20 @@ static int run_decode(const uint16_t *table_dev, int pitch, int64_t n_sym, int L
     d.in_len = (uint32_t)in_len;
     L3C_CUDA(cudaMemcpy(desc.p, &d, sizeof(d), cudaMemcpyHostToDevice));
     if (int e = l3c_ac_decode_streams(desc.as<l3c_dec_stream_t>(), 1, L, 0, (uint32_t)n_sym, nullptr)) return e;
+    if (sym_bytes == 2) {
+        L3C_CUDA(cudaMemcpy(sym_out_host, sym.p, (size_t)n_sym * 2, cudaMemcpyDeviceToHost));
+        return L3C_OK;
+    }
     std::vector<uint8_t> tmp((size_t)n_sym);
     L3C_CUDA(cudaMemcpy(tmp.data(), sym.p, (size_t)n_sym, cudaMemcpyDeviceToHost));
     for (int64_t i = 0; i < n_sym; ++i) sym_out_host[i] = (int16_t)tmp[(size_t)i];
     return L3C_OK;
 }
 
+// Lp <= 32769: the reference passes symbols as int16, so L = 32768 is the largest alphabet it can code
 static int check_stream_args(const char *fn, int64_t n_sym, int Lp) {
     L3C_REQUIRE(n_sym >= 1 && n_sym < (1ll << 31), "%s: n_sym=%lld", fn, (long long)n_sym);
-    L3C_REQUIRE(Lp >= 2 && Lp <= 257, "%s: Lp=%d not in [2,257]", fn, Lp);
+    L3C_REQUIRE(Lp >= 2 && Lp <= 32769, "%s: Lp=%d not in [2,32769]", fn, Lp);
     return L3C_OK;
 }
 
@@ -266,7 +275,7 @@ extern "C" int l3c_decode_cdf(const uint16_t *cdf_host, int64_t n_sym, int Lp, c
     if (int e = check_stream_args("l3c_decode_cdf", n_sym, Lp)) return e;
     L3C_REQUIRE(cdf_host && sym_out_host && (in_host || in_len == 0), "l3c_decode_cdf: null pointer");
     const int L = Lp - 1;
-    const int pitch = (L <= 32) ? 32 : 256;
+    const int pitch = decode_pitch(L);
     DevBuf cdf, table;
     if (int e = cdf.alloc((size_t)n_sym * Lp * 2)) return e;
     if (int e = table.alloc((size_t)n_sym * pitch * 2)) return e;
@@ -305,7 +314,7 @@ extern "C" int l3c_decode_logistic_mixture(const float *targets_dev, const float
                     (in_host || in_len == 0),
                 "l3c_decode_logistic_mixture: bad arguments");
     const int L = Lp - 1;
-    const int pitch = (L <= 32) ? 32 : 256;
+    const int pitch = decode_pitch(L);
     DevBuf table;
     if (int e = table.alloc((size_t)n_sym * pitch * 2)) return e;
     plane_table_kernel<<<(unsigned)ceil_div64(n_sym * pitch, 256), 256>>>(

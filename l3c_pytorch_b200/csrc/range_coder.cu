@@ -22,7 +22,9 @@
 //     rows are still being built (RGB channel pipelining).
 #include <stdlib.h>
 
+#include <algorithm>
 #include <atomic>
+#include <vector>
 
 #include "common.cuh"
 
@@ -850,6 +852,147 @@ ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, in
 }  // namespace v3
 
 // ---------------------------------------------------------------------------------------------
+// decoder, alphabets of 257 to 32768 symbols (reached through the drop-in torchac API): CTA = decoder warp +
+// helper warp, one stream per CTA.  A row no longer fits the warp's registers, so it is staged whole in shared
+// memory and searched in two levels, each one exact_step() (floor rule, foreign count) over at most 8 proposals
+// per lane:
+//   helper warp : copies every row into a ring of shared-memory slots with one cp.async.bulk (its mbarrier
+//                 completes on the transaction bytes), up to ring_n - 1 rows ahead of the decoder; once a row has
+//                 landed it writes the row's 256 bucket heads (cdf[j*s] << 16) | j, s = ceil(L/256), 8 per lane
+//                 in v3's ring layout (heads of buckets past the row propose 0, which never wins).
+//   decoder warp: level 1: the largest passing head gives the bucket j (rows are sorted, so the head of bucket j+1
+//                 fails whenever it exists); level 2: entries m0 + lane + 32t of bucket j (m0 = j*s, s <= 128)
+//                 propose (cdf[m] << 16) | (cdf[m+1] - 1), 2^16 above entry L-1; entry m0 always passes (floor
+//                 0 for j = 0, its head passed otherwise), the largest passing proposal carries the interval, and
+//                 the number of proposals up to it gives the symbol.  No speculation: every symbol runs the exact
+//                 step, so corrupt input needs no replay.
+// Symbols are written as uint16.
+// ---------------------------------------------------------------------------------------------
+namespace wide {
+
+constexpr int MAX_RING = 8;                   // row slots at most
+constexpr int BAR_BYTES = 3 * MAX_RING * 8;   // tx / full / empty mbarrier per slot
+constexpr int HEAD_BYTES = 256 * 4;           // 256 packed bucket heads per slot
+
+__host__ __device__ inline uint32_t row_bytes(int L) { return (uint32_t)((L + 7) & ~7) * 2u; }
+inline size_t smem_bytes(int ring_n, int L) { return BAR_BYTES + (size_t)ring_n * (HEAD_BYTES + row_bytes(L)); }
+
+// one row, global -> shared, completing `bar`'s current phase on its bytes (16-byte aligned, multiple of 16)
+__device__ __forceinline__ void stage_row(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
+                 : "memory");
+}
+
+__global__ void __launch_bounds__(64)
+ac_decode_wide_kernel(const l3c_dec_stream_t *__restrict__ streams, int L, int ring_n, uint32_t first,
+                      uint32_t count) {
+    using v3::mbar_arrive;
+    using v3::mbar_init;
+    using v3::mbar_wait;
+    using v3::smem_u32;
+    extern __shared__ __align__(16) uint8_t dec_smem[];
+    const int warp = threadIdx.x >> 5;                 // 0 = decoder, 1 = helper
+    const int lane = threadIdx.x & 31;
+    const uint32_t bars = smem_u32(dec_smem);
+    const uint32_t rb = row_bytes(L);
+    uint4 (*heads)[2][32] = reinterpret_cast<uint4 (*)[2][32]>(dec_smem + BAR_BYTES);          // [slot][half][lane]
+    const uint16_t *rows = reinterpret_cast<const uint16_t *>(dec_smem + BAR_BYTES + ring_n * HEAD_BYTES);
+    const uint32_t rent = rb / 2u;                                                            // entries per slot
+    auto tx_bar = [&](int k) { return bars + 8u * k; };                         // row bytes landed
+    auto full_bar = [&](int k) { return bars + 8u * (MAX_RING + k); };          // heads written (helper -> decoder)
+    auto empty_bar = [&](int k) { return bars + 8u * (2 * MAX_RING + k); };     // slot consumed (decoder -> helper)
+    if (threadIdx.x == 0) {
+        for (int k = 0; k < ring_n; ++k) {
+            mbar_init(tx_bar(k), 1);
+            mbar_init(full_bar(k), 32);
+            mbar_init(empty_bar(k), 32);
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    const l3c_dec_stream_t st = streams[blockIdx.x];
+    uint32_t last, upd_end;
+    if (!chunk_of(st.n_sym, first, count, last, upd_end)) return;
+    const uint32_t n = last - first;
+    const uint32_t s = ((uint32_t)L + 255u) / 256u;                             // entries per bucket, <= 128
+
+    if (warp == 1) {
+        // ============================ helper warp ============================
+        const uint8_t *table = reinterpret_cast<const uint8_t *>(st.table);
+        const int64_t pitch_bytes = 2 * st.row_pitch;
+        int k_in = 0, k_out = 0;                  // slot of the next row to request / to index
+        uint32_t ph_in = 0, ph_out = 0;           // and the parity of that slot's current use
+        for (uint32_t q = 0; q < n + (uint32_t)ring_n - 1u; ++q) {
+            if (q < n) {
+                if (q >= (uint32_t)ring_n) mbar_wait(empty_bar(k_in), ph_in ^ 1u);   // the decoder is done with it
+                if (lane == 0)
+                    stage_row(smem_u32(rows + (size_t)k_in * rent), table + (int64_t)(first + q) * pitch_bytes, rb,
+                              tx_bar(k_in));
+                if (++k_in == ring_n) { k_in = 0; ph_in ^= 1u; }
+            }
+            if (q + 1u >= (uint32_t)ring_n) {     // row q - (ring_n - 1): build its heads
+                mbar_wait(tx_bar(k_out), ph_out);
+                const uint16_t *row = rows + (size_t)k_out * rent;
+                uint32_t h[8];
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                    const uint32_t j = 8u * lane + jj, m = j * s;
+                    h[jj] = (m < (uint32_t)L) ? (((uint32_t)row[m] << 16) | j) : 0u;
+                }
+                heads[k_out][0][lane] = make_uint4(h[0], h[1], h[2], h[3]);
+                heads[k_out][1][lane] = make_uint4(h[4], h[5], h[6], h[7]);
+                mbar_arrive(full_bar(k_out));
+                if (++k_out == ring_n) { k_out = 0; ph_out ^= 1u; }
+            }
+        }
+        return;
+    }
+
+    // ============================ decoder warp ============================
+    BitSource src;
+    CoderState cs;
+    const uint32_t bit0 = open_stream(st, first, src, cs);
+    uint16_t *__restrict__ sym_out = reinterpret_cast<uint16_t *>(st.sym_out);
+    int k = 0;
+    uint32_t ph = 0;
+    for (uint32_t i = first; i < last; ++i) {
+        mbar_wait(full_bar(k), ph);
+        mbar_wait(tx_bar(k), ph);                 // complete already; makes the staged bytes visible to this warp
+        // level 1: the bucket
+        const uint4 a = heads[k][0][lane], b = heads[k][1][lane];
+        const uint32_t hk[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+        const uint32_t m0 = (exact_step(hk, cs, src, lane, false) & 0xFFFFu) * s;
+        // level 2: the entry inside it
+        const uint16_t *row = rows + (size_t)k * rent;
+        const uint32_t m_end = min(m0 + s, (uint32_t)L);
+        uint32_t pk[4];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const uint32_t m = m0 + lane + 32u * t;
+            pk[t] = 0u;
+            if (m < m_end) {
+                const uint32_t hi = (m + 1u == (uint32_t)L) ? 0x10000u : (uint32_t)row[m + 1u];
+                pk[t] = ((uint32_t)row[m] << 16) | ((hi - 1u) & 0xFFFFu);
+            }
+        }
+        const uint32_t top = exact_step(pk, cs, src, lane, i < upd_end);
+        int c = 0;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) c += (m0 + lane + 32u * t < m_end && pk[t] <= top) ? 1 : 0;
+        const int tot = __reduce_add_sync(FULL, c);   // >= 1: entry m0 passes
+        mbar_arrive(empty_bar(k));
+        if (lane == 0) sym_out[i] = (uint16_t)(m0 + (uint32_t)tot - 1u);
+        if (++k == ring_n) { k = 0; ph ^= 1u; }
+    }
+    if (lane == 0) save_stream(st, cs, src, bit0);
+}
+
+}  // namespace wide
+
+// ---------------------------------------------------------------------------------------------
 // gather the variable-length code streams into one contiguous blob (container layout, byte offsets)
 // ---------------------------------------------------------------------------------------------
 constexpr int PACK_CHUNK = 16384;
@@ -917,14 +1060,53 @@ extern "C" int l3c_set_decoder_streams_per_cta(int spc) {
     return L3C_OK;
 }
 
+namespace l3c {
+// L > 256: the descriptors are checked on the host first (row pitch, alignment of the rows and of the uint16
+// output), so a bad one is L3C_EINVAL instead of a misaligned bulk copy; this waits for `st`.
+static int decode_wide(const l3c_dec_stream_t *streams_dev, int n, int L, uint32_t first, uint32_t count,
+                       cudaStream_t st) {
+    using wide::ac_decode_wide_kernel;
+    std::vector<l3c_dec_stream_t> d((size_t)n);
+    L3C_CUDA(cudaMemcpyAsync(d.data(), streams_dev, sizeof(l3c_dec_stream_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    L3C_CUDA(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i) {
+        const int64_t p = d[(size_t)i].row_pitch;
+        L3C_REQUIRE(p == 0 || (p % 8 == 0 && p >= L),
+                    "l3c_ac_decode_streams: stream %d: row_pitch=%lld for L=%d (L > 256 needs 0 or a multiple of 8 "
+                    ">= L)", i, (long long)p, L);
+        L3C_REQUIRE((reinterpret_cast<uintptr_t>(d[(size_t)i].table) & 15u) == 0 &&
+                        (reinterpret_cast<uintptr_t>(d[(size_t)i].sym_out) & 1u) == 0,
+                    "l3c_ac_decode_streams: stream %d: table must be 16-byte and sym_out 2-byte aligned for L > 256", i);
+    }
+    static int optin_dev[64] = {};
+    int &optin = optin_dev[current_device_slot()];
+    if (!optin) {   // opt in once per device to all the shared memory a block may have
+        int dev = 0, v = 0;
+        L3C_CUDA(cudaGetDevice(&dev));
+        L3C_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        L3C_CUDA(cudaFuncSetAttribute(ac_decode_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+        optin = v;
+    }
+    // as many row slots as fit, 2 to MAX_RING (3 at L = 32768 with 227 KB)
+    const int ring_n = (int)std::min<size_t>(wide::MAX_RING, ((size_t)optin - wide::BAR_BYTES) /
+                                                                 (wide::HEAD_BYTES + wide::row_bytes(L)));
+    L3C_REQUIRE(ring_n >= 2, "l3c_ac_decode_streams: L=%d needs %zu bytes of shared memory, the device offers %d", L,
+                wide::smem_bytes(2, L), optin);
+    ac_decode_wide_kernel<<<n, 64, wide::smem_bytes(ring_n, L), st>>>(streams_dev, L, ring_n, first, count);
+    L3C_LAUNCH_CHECK("ac_decode_wide_kernel");
+    return L3C_OK;
+}
+}  // namespace l3c
+
 extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_streams, int L,
                                      uint32_t first, uint32_t count, void *stream) {
     using namespace l3c;
     L3C_REQUIRE(n_streams >= 0, "l3c_ac_decode_streams: n_streams=%d", n_streams);
-    L3C_REQUIRE(L >= 1 && L <= 256, "l3c_ac_decode_streams: L=%d not in [1,256]", L);
+    L3C_REQUIRE(L >= 1 && L <= 32768, "l3c_ac_decode_streams: L=%d not in [1,32768]", L);
     if (n_streams == 0 || count == 0) return L3C_OK;
     L3C_REQUIRE(streams_dev, "l3c_ac_decode_streams: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
+    if (L > 256) return decode_wide(streams_dev, n_streams, L, first, count, st);
     if (L <= 32) {
         ac_decode32_kernel<<<n_streams, 32, 0, st>>>(streams_dev, n_streams, L, first, count);
     } else {

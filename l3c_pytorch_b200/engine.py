@@ -742,7 +742,8 @@ def lut_intervals(sym, lut):
 
 
 def table_pitch(L):
-    return 32 if L <= 32 else 256
+    """row pitch (entries) of the decoder's CDF tables for alphabet L"""
+    return 32 if L <= 32 else 256 if L <= 256 else (L + 7) // 8 * 8
 
 
 def dmll_build_table(l, sym, targets, C, K, L, rgb, c, table, pix0=0, npix=None):

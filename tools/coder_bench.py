@@ -5,7 +5,7 @@ import numpy as np
 import torch
 from l3c_pytorch_b200 import engine as E, _lib
 
-def run(L, n_streams, n_sym, peaked, rare=False, own_tables=False, uniform=False):
+def run(L, n_streams, n_sym, peaked, rare=False, own_tables=False, uniform=False, ref_cpu=False):
     dev = torch.device('cuda')
     rng = np.random.default_rng(0)
     pitch = E.table_pitch(L)
@@ -45,7 +45,8 @@ def run(L, n_streams, n_sym, peaked, rare=False, own_tables=False, uniform=False
     lens = torch.empty(n_streams, dtype=torch.int32, device=dev)
     t_enc = timed(lambda: E.check(E.lib.l3c_ac_encode_streams(E._ptr(ddev), n_streams, E._ptr(lens), E._stream_ptr())))
     nbytes = int(lens[0])
-    out = torch.zeros(n_streams * n_sym, dtype=torch.uint8, device=dev)
+    esz = 2 if L > 256 else 1         # the decoder writes uint16 symbols above 256
+    out = torch.zeros(n_streams * n_sym * esz, dtype=torch.uint8, device=dev)
     dd = np.zeros(n_streams, dtype=_lib.DEC_STREAM_DTYPE)
     if own_tables:      # every stream streams its own rows from HBM (as in the real pipeline)
         big = tab_dev.repeat(n_streams, 1)
@@ -53,16 +54,40 @@ def run(L, n_streams, n_sym, peaked, rare=False, own_tables=False, uniform=False
     else:
         dd['table'] = tab_dev.data_ptr()
     dd['in'] = slots.data_ptr() + cap * np.arange(n_streams)
-    dd['sym_out'] = out.data_ptr() + n_sym * np.arange(n_streams); dd['row_pitch'] = 0 if (uniform and not own_tables) else pitch
+    dd['sym_out'] = out.data_ptr() + esz * n_sym * np.arange(n_streams); dd['row_pitch'] = 0 if (uniform and not own_tables) else pitch
     dd['n_sym'] = n_sym; dd['in_len'] = nbytes
     dddev = E._desc_to_device(dd, dev)
     t_dec = timed(lambda: E.check(E.lib.l3c_ac_decode_streams(E._ptr(dddev), n_streams, L, 0, n_sym, E._stream_ptr())))
-    ok = bool((out.reshape(n_streams, n_sym).cpu().numpy() == sym[None, :]).all())
+    got = out.cpu().numpy().view(np.uint16 if esz == 2 else np.uint8).reshape(n_streams, n_sym)
+    ok = bool((got == sym[None, :]).all())
+    extra = {}
+    if ref_cpu:       # the compiled reference's decode_cdf of stream 0, one CPU thread
+        import time
+        from oracle import build_ref
+        ref = build_ref.load()
+        if ref is not None:
+            torch.set_num_threads(1)
+            t_cdf = torch.from_numpy(np.concatenate([tab[:, :L], np.zeros((n_sym, 1), np.uint16)], 1).view(np.int16))
+            data = slots[:nbytes].cpu().numpy().tobytes()
+            t0 = time.perf_counter()
+            back = ref.decode_cdf(t_cdf.reshape(1, 1, n_sym, L + 1), data)
+            extra = dict(ref_cpu_ns_per_sym=(time.perf_counter() - t0) * 1e9 / n_sym,
+                         ref_ok=bool((back.numpy().astype(np.int64) == sym).all()))
     print(json.dumps(dict(L=L, streams=n_streams, n_sym=n_sym, peaked=peaked, rare=rare, own_tables=own_tables, uniform=uniform, bits_per_sym=nbytes * 8 / n_sym,
-                          enc_ns_per_sym=t_enc * 1e6 / n_sym, dec_ns_per_sym=t_dec * 1e6 / n_sym, ok=ok)))
+                          enc_ns_per_sym=t_enc * 1e6 / n_sym, dec_ns_per_sym=t_dec * 1e6 / n_sym, ok=ok, **extra)))
 
 if __name__ == '__main__':
     only = int(sys.argv[sys.argv.index('--only') + 1]) if '--only' in sys.argv else None
+    if '--wide' in sys.argv:          # alphabets above 256 (drop-in torchac range), against the reference on the CPU
+        import subprocess
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', '0'],
+                           capture_output=True, text=True).stdout.strip()
+        print(json.dumps(dict(gpu=torch.cuda.get_device_name(0), nvidia_smi=q)))
+        for L in (257, 1024, 4096, 32768):
+            n = min(16384, (128 << 20) // (2 * E.table_pitch(L)))      # <= 128 MB of rows per stream
+            for ns in (1, 48):
+                run(L, ns, n, True, own_tables=ns > 1, ref_cpu=ns == 1)
+        sys.exit(0)
     if '--custom' in sys.argv:        # --custom L,streams,n_sym,peaked,rare,own_tables,uniform  (0/1 flags)
         v = [int(x) for x in sys.argv[sys.argv.index('--custom') + 1].split(',')]
         run(v[0], v[1], v[2], bool(v[3]), bool(v[4]), bool(v[5]), bool(v[6]))
