@@ -49,6 +49,25 @@ constexpr int W_RES_BYTES = 9 * W_TAP_BYTES;   // 73728
 constexpr int K5_A_BYTES = 10 * TW * 128;                  // 20480: strided halo box
 constexpr int K5_STAGE_BYTES = K5_A_BYTES + 3 * W_TAP_BYTES;   // 45056: box + up to three weight slabs
 
+// The wgmmas of one unit of an 8x16 tile: NTAPS taps j, tap j reading the staged box at a0 from row j * row_step
+// (rows of 16 pixels) and the weight slab at w0 + j * w_step, each for both 64-pixel halves and four k-steps.
+// `first`: the unit starts the tile's accumulation (its first k-step overwrites the accumulators).
+template <int NTAPS>
+__device__ __forceinline__ void unit_mma(float (&acc)[2][32], uint32_t a0, int row_step, uint32_t w0, uint32_t w_step,
+                                         bool first) {
+#pragma unroll
+    for (int j = 0; j < NTAPS; ++j) {
+        const uint64_t db = make_desc(w0 + j * w_step);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint64_t da = make_desc(a0 + (j * row_step * TW + 64 * h) * 128);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)                                          // +32 B = 16 fp16 along K
+                wgmma_f16(acc[h], da + 2u * kk, db + 2u * kk, (first && j == 0 && kk == 0) ? 0u : 1u);
+        }
+    }
+}
+
 template <int KIND>
 __global__ void __launch_bounds__(THREADS, 1)
 conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
@@ -100,42 +119,33 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     if (KIND == 0) mbar_wait(weight_bar(bars), 0);
     for_each_tile(k, 2, ptiles, [&](int t) {
         const Tile c = tile_of(p, t);
+        prefetch_residual(p, c, ct, w);
         float acc[2][32];                                 // rows 0..63 / 64..127 of the tile
         acc_zero(acc[0]);
         acc_zero(acc[1]);
-        for (int u = 0; u < UNITS; ++u) {
+        // one unit: wait for its stage, issue(stage address) its wgmmas as one group, wait for them, hand it back
+        auto unit = [&](auto &&issue) {
             const uint32_t a0 = ring.wait();
             wgmma_fence();
-            if (KIND == 0) {
-#pragma unroll
-                for (int dy = 0; dy < 3; ++dy) {
-                    const uint64_t db = make_desc(w_base + (dy * 3 + u) * W_TAP_BYTES);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const uint64_t da = make_desc(a0 + (dy * d * TW + 64 * h) * 128);   // dy*d rows of 16 px
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk)                                       // +32 B = 16 fp16 along K
-                            wgmma_f16(acc[h], da + 2u * kk, db + 2u * kk, (u | dy | kk) != 0 ? 1u : 0u);
-                    }
-                }
-            } else {
-                const int ntaps = 3 - (u & 1);
-                for (int j = 0; j < ntaps; ++j) {
-                    const uint64_t db = make_desc(a0 + K5_A_BYTES + j * W_TAP_BYTES);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const uint64_t da = make_desc(a0 + (j * TW + 64 * h) * 128);        // box row j = tap ky0 + 2j
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk)
-                            wgmma_f16(acc[h], da + 2u * kk, db + 2u * kk, (u | j | kk) != 0 ? 1u : 0u);
-                    }
-                }
-            }
+            issue(a0);
             wgmma_commit();
             wgmma_wait0();
             acc_fence(acc[0]);
             acc_fence(acc[1]);
             ring.release();
+        };
+        if (KIND == 0) {
+#pragma unroll
+            for (int u = 0; u < UNITS; ++u)          // filter column dx = u: taps dy = 0..2, dy*d rows of 16 px apart
+                unit([&](uint32_t a0) { unit_mma<3>(acc, a0, d, w_base + u * W_TAP_BYTES, 3 * W_TAP_BYTES, u == 0); });
+        } else {
+            // unit (kx, row parity): taps ky = par + 2j, box row j, weight slab j after the box.  The two parities
+            // are separate bodies so that both tap loops have compile-time trip counts: with a runtime count ptxas
+            // serialises every wgmma of the kernel.
+            for (int kx = 0; kx < 5; ++kx) {
+                unit([&](uint32_t a0) { unit_mma<3>(acc, a0, 1, a0 + K5_A_BYTES, W_TAP_BYTES, kx == 0); });
+                unit([&](uint32_t a0) { unit_mma<2>(acc, a0, 1, a0 + K5_A_BYTES, W_TAP_BYTES, false); });
+            }
         }
         image_epilogue<false>(p, c, ct, w, acc);
     });

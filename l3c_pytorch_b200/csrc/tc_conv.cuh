@@ -127,6 +127,28 @@ __device__ __forceinline__ void to_image(float a, float b, uint32_t &hi, uint32_
     else hi = pack_h2(a, b);
 }
 
+// L2 prefetch of the fp32 residual lines image_epilogue() reads for tile c of Cout tile ct, consumer warp w
+// (one 128 B line per pixel and column half, issued by the first lane of each quad).  Issued before the tile's
+// MMAs, so that the epilogue's residual loads find their lines in L2 instead of waiting on HBM.  Without
+// residual or with PixelShuffle(2) (no residual there) nothing is fetched.
+__device__ __forceinline__ void prefetch_residual(const Params &p, const Tile &c, int ct, int w) {
+    if (p.residual == nullptr || (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0 || (threadIdx.x & 3) != 0) return;
+    const int tr = (threadIdx.x & 31) >> 2;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int oy = c.ty * TH + 4 * h + w;
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) {
+            const int ox = c.tx * TW + tr + 8 * rh;
+            if (oy >= p.H || ox >= p.W) continue;
+            const size_t pix = ((size_t)c.n * p.H + oy) * p.W + ox;
+#pragma unroll
+            for (int cc = 0; cc < 2; ++cc)
+                asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + pix * p.y_pitch + p.y_coff + ct * 64 + 32 * cc));
+        }
+    }
+}
+
 // Epilogue of the FP16-image 3x3 / 5x5 kernels (conv_f16_kernel, conv3x3_f16x2_kernel; SPLIT: f16x2) for tile c of
 // Cout tile ct, consumer warp w; acc[h] holds the conv values of tile half h.  Adds the bias, ReLU, the fp32
 // residual, and writes the fp32 output (float2: full sectors) and the operand image (16-byte vectors after a 4x4

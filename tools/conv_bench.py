@@ -1,7 +1,7 @@
 """Micro-benchmark of the conv kernels by layer type and precision mode (CUDA events, L2-cold inputs by
 size: every tensor is far larger than the 50 MB L2 at the default shape).
 
-    python tools/conv_bench.py [--n 16] [--hw 256] [--modes f16,tf32] [--reps 20]
+    python tools/conv_bench.py [--n 16] [--hw 256] [--modes f16,tf32] [--reps 20] [--cases pair,down]
 
 Layer types (the shapes an L3C round trip is made of):
   res1   first conv of a ResBlock: 3x3 64->64 + ReLU, output feeds only the next tensor-core conv ('round')
@@ -12,7 +12,9 @@ Layer types (the shapes an L3C round trip is made of):
   atr4   3x3 dilation 4 into a slice of the 192-channel concat buffer ('round')
   lin    1x1 192->120 on the concat buffer (the DMLL parameters); lin_fused: the same conv with the DMLL head in
          its epilogue (coding intervals out, encode side; tf32: the two-step path for comparison)
-  down   5x5 stride 2 (CUDA cores in every mode)
+  down   5x5 stride 2 on the operand image: f16 runs the tensor-core kernel (conv5x5s2_f16_kernel), tf32 and
+         f16x2 the CUDA-core kernel on the fp32 input; its FLOPs and bytes are per INPUT pixel (four per output
+         pixel)
 Prints ms per launch, TFLOP/s, and algorithmic HBM bytes per launch / GB/s (what the layer must move, per
 DESIGN.md 4.1).
 """
@@ -32,6 +34,7 @@ def main():
     ap.add_argument('--hw', type=int, default=256)
     ap.add_argument('--modes', default='f16,tf32')
     ap.add_argument('--reps', type=int, default=20)
+    ap.add_argument('--cases', default=None, help='comma-separated subset of the layer types (default: all)')
     ap.add_argument('--json', default=None)
     args = ap.parse_args()
     import l3c_pytorch_b200 as l3c
@@ -85,9 +88,13 @@ def main():
             'lin_fused': ((lambda: E.lin_dmll_intervals(clin, cat, sym, tgt, 3, 10, 256, True)) if mode == 'f16'
                           else (lambda: E.dmll_intervals(E.conv2d(clin, cat_act), sym, tgt, 3, 10, 256, True)),
                           2 * 192 * 120, 192 * op_b + 3 + 12),
-            'down': (lambda: E.conv2d(cdown, x, want='act'), 2 * 25 * 64 * 64 / 4.0, 256 + (256 + 64 * op_b) / 4.0),
+            # f16 reads the FP16 operand image, the CUDA-core kernel of the other modes the fp32 input
+            'down': (lambda: E.conv2d(cdown, xa, want='act'), 2 * 25 * 64 * 64 / 4.0,
+                     (64 * op_b if mode == 'f16' else 256) + (256 + 64 * op_b) / 4.0),
         }
         for name, (fn, flop_px, bytes_px) in cases.items():
+            if args.cases and name not in args.cases.split(','):
+                continue
             try:
                 for _ in range(3):
                     fn()
