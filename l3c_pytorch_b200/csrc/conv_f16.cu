@@ -12,7 +12,7 @@
 // below), but
 //   * one wgmma covers K = 16 instead of 8 at twice the TF32 rate;
 //   * an activation's operand image is 128 B per pixel (64 channels) = exactly ONE 128B-swizzle row, so a halo
-//     box needs one TMA load per filter column (no K-halves) and half the L2->smem bytes;
+//     box is one TMA load (no K-halves) and half the L2->smem bytes;
 //   * operand twins cost 128 instead of 256 B per pixel in HBM, and a layer whose output only feeds tensor-core
 //     convs (first conv of a ResBlock, atrous convs, the finest decoder features) writes ONLY the 2-byte image.
 // Per pixel a 64->64 conv moves 256 B (operand in / operand out) to 768 B (operand + fp32 residual in, fp32 +
@@ -21,11 +21,15 @@
 // Structure of the 3x3 kernel (persistent, tc_conv.cuh layout: two consumer warpgroups with a TMA producer warp
 // each):
 //   * the 9 weight slabs of the CTA's Cout tile (9 x 64 rows x 128 B = 72 KB) stay in shared memory;
-//   * per filter column dx ONE box of (8 + 2d) rows x 16 pixels x 64 channels is staged by TMA; the three dy taps
-//     read it at row offsets dy*d*2048 B (multiples of the 1024 B swizzle atom);
-//   * the consumer warpgroup accumulates the two 64-pixel halves of the 8x16 tile (2 x 32 registers per
-//     thread), then fuses bias / ReLU / residual / PixelShuffle(2), writes fp32 float2 (full sectors) and the FP16
-//     image as 16-byte vectors after a 4x4 transpose inside each quad.
+//   * per tile ONE halo box of (8 + 2d) rows x halo_w(d) pixels (24 for d <= 4) x 64 channels is staged by TMA,
+//     so every input pixel crosses L2 -> smem once per tile (240 / 288 / 384 B per output pixel at d = 1 / 2 / 4
+//     instead of three boxes of 16 px, one per filter column, at twice that);
+//   * the two 64-pixel halves of the 8x16 tile are its left and right 8-pixel columns (Halves::COLS): the 8-row
+//     core-matrix groups of a half are 8 box rows one box row (a multiple of 1024 B) apart, so every tap (dy, dx)
+//     of a half is one descriptor, started at pixel dx*d, i.e. anywhere inside the swizzle atom (halo_mma);
+//   * the consumer warpgroup accumulates both halves (2 x 32 registers per thread), then fuses bias / ReLU /
+//     residual / PixelShuffle(2), writes fp32 float2 (full sectors) and the FP16 image as 16-byte vectors after a
+//     4x4 transpose inside each quad.
 // Accumulation order per output element: (dx, dy, k-step) -- fixed, independent of batch / image size / tile
 // position / pipe: encoder-side and decoder-side evaluations are bit-identical.
 #include <stdlib.h>
@@ -48,6 +52,31 @@ constexpr int W_RES_BYTES = 9 * W_TAP_BYTES;   // 73728
 //   brings its 3 (2) weight slabs along with its box.  10 units, 100 k-steps per tile.
 constexpr int K5_A_BYTES = 10 * TW * 128;                  // 20480: strided halo box
 constexpr int K5_STAGE_BYTES = K5_A_BYTES + 3 * W_TAP_BYTES;   // 45056: box + up to three weight slabs
+
+// KIND 0: width (pixels) of the halo box, TW + 2d rounded up to whole 8-pixel groups so that one box row (the
+// descriptors' SBO) is a multiple of the 1024 B swizzle atom.  24 for d = 1..4.
+__host__ __device__ constexpr int halo_w(int d) { return (TW + 2 * d + 7) & ~7; }
+
+// The 72 wgmmas of a 3x3 tile on its halo box (bw pixels wide, its row 0 / pixel 0 the input row / pixel d before
+// the tile's first): tap (dy, dx) of half h reads box rows dy*d + g (g = 0..7, the tile rows), pixels
+// 8h + dx*d + 0..7.  Every output element accumulates in the order (dx, dy, k-step); the two halves alternate
+// per k-step, which measured ~1 % faster than four k-steps of one half after the other.
+__device__ __forceinline__ void halo_mma(float (&acc)[2][32], uint32_t box, int d, int bw, uint32_t w_base) {
+#pragma unroll
+    for (int dx = 0; dx < 3; ++dx) {
+#pragma unroll
+        for (int dy = 0; dy < 3; ++dy) {
+            const uint64_t db = make_desc(w_base + (dy * 3 + dx) * W_TAP_BYTES);
+            const uint32_t a0 = box + (dy * d * bw + dx * d) * 128;
+            const uint64_t da[2] = {make_desc(a0, bw * 128), make_desc(a0 + 8 * 128, bw * 128)};
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)                                          // +32 B = 16 fp16 along K
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    wgmma_f16(acc[h], da[h] + 2u * kk, db + 2u * kk, (dx | dy | kk) != 0 ? 1u : 0u);
+        }
+    }
+}
 
 // The wgmmas of one unit of an 8x16 tile: NTAPS taps j, tap j reading the staged box at a0 from row j * row_step
 // (rows of 16 pixels) and the weight slab at w0 + j * w_step, each for both 64-pixel halves and four k-steps.
@@ -73,7 +102,8 @@ __global__ void __launch_bounds__(THREADS, 1)
 conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                 const Params p, const int n_stages, const int a_bytes, const int ptiles) {
     constexpr int W_RES = (KIND == 0) ? W_RES_BYTES : 0;    // resident weights
-    constexpr int UNITS = (KIND == 0) ? 3 : 10;
+    constexpr int UNITS = (KIND == 0) ? 1 : 10;
+    constexpr Halves HV = (KIND == 0) ? Halves::COLS : Halves::ROWS;
     // [weights 72 KB][pipe 0 stages][pipe 1 stages][barriers]
     const uint32_t w_base = smem_u32(smem_aligned());
     const uint32_t bars = w_base + W_RES + 2 * n_stages * a_bytes;
@@ -98,8 +128,8 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
             const Tile c = tile_of(p, t);
             for (int u = 0; u < UNITS; ++u) {
                 if (KIND == 0) {
-                    const Slot s = ring.acquire(a_bytes);
-                    tma_load_4d(s.dst, &map_x, s.bar, 0, c.tx * TW + (u - 1) * d, c.ty * TH - d, c.n);
+                    const Slot s = ring.acquire(a_bytes);       // the tile's halo box
+                    tma_load_4d(s.dst, &map_x, s.bar, 0, c.tx * TW - d, c.ty * TH - d, c.n);
                 } else {
                     const int kx = u >> 1, par = u & 1, ntaps = 3 - par;
                     const Slot s = ring.acquire(K5_A_BYTES + ntaps * W_TAP_BYTES);
@@ -119,8 +149,8 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     if (KIND == 0) mbar_wait(weight_bar(bars), 0);
     for_each_tile(k, 2, ptiles, [&](int t) {
         const Tile c = tile_of(p, t);
-        prefetch_residual(p, c, ct, w);
-        float acc[2][32];                                 // rows 0..63 / 64..127 of the tile
+        prefetch_residual<HV>(p, c, ct, w);
+        float acc[2][32];                                 // the two halves of the tile (HV)
         acc_zero(acc[0]);
         acc_zero(acc[1]);
         // one unit: wait for its stage, issue(stage address) its wgmmas as one group, wait for them, hand it back
@@ -135,9 +165,8 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
             ring.release();
         };
         if (KIND == 0) {
-#pragma unroll
-            for (int u = 0; u < UNITS; ++u)          // filter column dx = u: taps dy = 0..2, dy*d rows of 16 px apart
-                unit([&](uint32_t a0) { unit_mma<3>(acc, a0, d, w_base + u * W_TAP_BYTES, 3 * W_TAP_BYTES, u == 0); });
+            const int bw = halo_w(d);
+            unit([&](uint32_t a0) { halo_mma(acc, a0, d, bw, w_base); });   // all 9 taps on the one halo box
         } else {
             // unit (kx, row parity): taps ky = par + 2j, box row j, weight slab j after the box.  The two parities
             // are separate bodies so that both tap loops have compile-time trip counts: with a runtime count ptxas
@@ -147,7 +176,7 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 unit([&](uint32_t a0) { unit_mma<2>(acc, a0, 1, a0 + K5_A_BYTES, W_TAP_BYTES, false); });
             }
         }
-        image_epilogue<false>(p, c, ct, w, acc);
+        image_epilogue<false, HV>(p, c, ct, w, acc);
     });
 }
 
@@ -529,13 +558,15 @@ int conv2d_f16(const l3c_conv_t &p, cudaStream_t st) {
                     "l3c_conv2d[f16]: output pitch/offset alignment (pitch=%d coff=%d)", p.y_pitch, p.y_coff);
         L3C_REQUIRE(!(ps && p.residual), "l3c_conv2d[f16]: residual with pixel shuffle is not built");
         const int d = p.dilation;
-        const int a_rows = TH + 2 * d;
+        const int a_rows = TH + 2 * d, a_w = halo_w(d);
         L3C_REQUIRE(a_rows <= 256, "l3c_conv2d[f16]: dilation %d too large", d);
-        const int a_bytes = a_rows * TW * 128;
-        const RingPlan r = plan_ring(conv_smem_cap(), W_RES_BYTES + SMEM_RESERVE, a_bytes, 3);
+        const int a_bytes = a_rows * a_w * 128;          // one halo box = one stage = one tile
+        // One stage per pipe: a second one (a tile of lookahead) measured no faster, and the 60 KB it takes at
+        // d = 1 leave room on the SM for the CTAs of the other kernels that run beside this one in a codec step.
+        const RingPlan r = plan_ring(conv_smem_cap(), W_RES_BYTES + SMEM_RESERVE, a_bytes, 1);
         L3C_REQUIRE(r.n_stages >= 1, "l3c_conv2d[f16]: halo of dilation %d does not fit in shared memory", d);
         if (!encode_tmap(&map_x, "l3c_conv2d[f16]", "x", dt, p.x_h, {64, p.W, p.H, p.N}, {img[0], img[1], img[2]},
-                         {64, TW, a_rows, 1}) ||
+                         {64, a_w, a_rows, 1}) ||
             !encode_tmap(&map_w, "l3c_conv2d[f16]", "w", dt, p.w_h, {64, 9LL * p.cout_pad}, {128}, {64, 64}))
             return L3C_EINVAL;
         const Params q = conv_params(p, p.H, p.W);

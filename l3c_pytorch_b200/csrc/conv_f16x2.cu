@@ -102,7 +102,7 @@ conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
         for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int i = 0; i < 32; ++i) acc1[h][i] = __fmaf_rn(acc2[h][i], LO_INV, acc1[h][i]);
-        image_epilogue<true>(p, c, ct, w, acc1);
+        image_epilogue<true, Halves::ROWS>(p, c, ct, w, acc1);
     });
 }
 

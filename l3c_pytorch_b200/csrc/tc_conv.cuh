@@ -120,6 +120,18 @@ __device__ __forceinline__ Tile tile_of(const Params &p, int t) {
     return {t % p.tiles_x, t / p.tiles_x % p.tiles_y, t / p.tiles_x / p.tiles_y};
 }
 
+// Which pixels of an 8x16 tile the two 64-row halves (acc[0], acc[1]) of the MMA are.
+//   ROWS: half h = tile rows 4h..4h+3 (8-row group g = row 4h + g/2, pixels 8(g%2)..+7): conv3x3_f16x2_kernel and
+//         the 5x5/s2 kernel, whose boxes are 16 px wide
+//   COLS: half h = pixels 8h..8h+7 of all 8 rows (group g = row g): the 3x3 f16 kernel, whose groups are evenly
+//         spaced rows of one wide halo box
+// Accumulator row 16w + tr + 8rh of half h (consumer warp w, tr = lane / 4) is tile row half_row(), pixel half_px().
+enum class Halves { ROWS, COLS };
+template <Halves HV>
+__device__ __forceinline__ int half_row(int h, int w, int rh) { return HV == Halves::ROWS ? 4 * h + w : 2 * w + rh; }
+template <Halves HV>
+__device__ __forceinline__ int half_px(int h, int tr, int rh) { return HV == Halves::ROWS ? tr + 8 * rh : 8 * h + tr; }
+
 // fp32 pair -> operand image: FP16 pair, or with SPLIT its hi and lo pairs
 template <bool SPLIT>
 __device__ __forceinline__ void to_image(float a, float b, uint32_t &hi, uint32_t &lo) {
@@ -131,15 +143,16 @@ __device__ __forceinline__ void to_image(float a, float b, uint32_t &hi, uint32_
 // (one 128 B line per pixel and column half, issued by the first lane of each quad).  Issued before the tile's
 // MMAs, so that the epilogue's residual loads find their lines in L2 instead of waiting on HBM.  Without
 // residual or with PixelShuffle(2) (no residual there) nothing is fetched.
+template <Halves HV>
 __device__ __forceinline__ void prefetch_residual(const Params &p, const Tile &c, int ct, int w) {
     if (p.residual == nullptr || (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0 || (threadIdx.x & 3) != 0) return;
     const int tr = (threadIdx.x & 31) >> 2;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const int oy = c.ty * TH + 4 * h + w;
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
-            const int ox = c.tx * TW + tr + 8 * rh;
+            const int oy = c.ty * TH + half_row<HV>(h, w, rh);
+            const int ox = c.tx * TW + half_px<HV>(h, tr, rh);
             if (oy >= p.H || ox >= p.W) continue;
             const size_t pix = ((size_t)c.n * p.H + oy) * p.W + ox;
 #pragma unroll
@@ -150,25 +163,47 @@ __device__ __forceinline__ void prefetch_residual(const Params &p, const Tile &c
 }
 
 // Epilogue of the FP16-image 3x3 / 5x5 kernels (conv_f16_kernel, conv3x3_f16x2_kernel; SPLIT: f16x2) for tile c of
-// Cout tile ct, consumer warp w; acc[h] holds the conv values of tile half h.  Adds the bias, ReLU, the fp32
-// residual, and writes the fp32 output (float2: full sectors) and the operand image (16-byte vectors after a 4x4
-// transpose inside each quad; SPLIT: hi and lo planes yh_lo_off apart), or PixelShuffle(2) of both.
-// Fragment (h, column half cc) = tile row 4h + w, pixels tr / tr + 8, columns 32cc + 8jb + 2tq.
-template <bool SPLIT>
+// Cout tile ct, consumer warp w; acc[h] holds the conv values of tile half h (HV: which pixels that is).  Adds the
+// bias, ReLU, the fp32 residual, and writes the fp32 output (float2: full sectors) and the operand image (16-byte
+// vectors after a 4x4 transpose inside each quad; SPLIT: hi and lo planes yh_lo_off apart), or PixelShuffle(2) of
+// both.  Fragment (h, column half cc, rh) = tile row half_row(h, w, rh), pixel half_px(h, tr, rh), columns
+// 32cc + 8jb + 2tq; either way the eight lanes tr of a fragment hold eight consecutive pixels of one row.
+template <bool SPLIT, Halves HV>
 __device__ __forceinline__ void image_epilogue(const Params &p, const Tile &c, int ct, int w, const float (&acc)[2][32]) {
     const int lane = threadIdx.x & 31, tq = lane & 3, tr = lane >> 2;   // column pair / row inside the fragment
     const bool relu = (p.flags & L3C_CONV_RELU) != 0;
     const bool shuffle = (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0;
     const int hp = SPLIT ? p.yh_pitch : p.y_pitch;                        // pitch of the operand image
+    // Without SPLIT the residual of a tile half is loaded before the half's first store: the compiler cannot tell
+    // that y / yh do not alias it, so a load left inside the loop waits behind every store before it (one L2 round
+    // trip per fragment instead of one per half).  The whole tile's residual at once would exceed the 168
+    // registers a thread has; in the split kernel, whose registers are already short, even a half's spills.
+    const bool add_res = p.residual != nullptr && !shuffle;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const int oy = c.ty * TH + 4 * h + w;
+        float2 res[2][2][4];                                              // [cc][rh][jb]
+        if (!SPLIT && add_res) {
+#pragma unroll
+            for (int cc = 0; cc < 2; ++cc)
+#pragma unroll
+                for (int rh = 0; rh < 2; ++rh) {
+                    const int oy = c.ty * TH + half_row<HV>(h, w, rh);
+                    const int ox = c.tx * TW + half_px<HV>(h, tr, rh);
+                    const size_t off = (((size_t)c.n * p.H + oy) * p.W + ox) * p.y_pitch + p.y_coff + ct * 64 + 32 * cc;
+#pragma unroll
+                    for (int jb = 0; jb < 4; ++jb)
+                        res[cc][rh][jb] = (oy < p.H && ox < p.W)
+                                              ? __ldg(reinterpret_cast<const float2 *>(p.residual + off + 8 * jb + 2 * tq))
+                                              : make_float2(0.f, 0.f);
+                }
+        }
 #pragma unroll
         for (int cc = 0; cc < 2; ++cc) {
             const int cb = ct * 64 + 32 * cc;                             // first conv channel of this fragment
 #pragma unroll
             for (int rh = 0; rh < 2; ++rh) {
-                const int ox = c.tx * TW + tr + 8 * rh;
+                const int oy = c.ty * TH + half_row<HV>(h, w, rh);
+                const int ox = c.tx * TW + half_px<HV>(h, tr, rh);
                 const bool inside = (oy < p.H) && (ox < p.W);
                 const size_t pix = ((size_t)c.n * p.H + oy) * p.W + ox;
                 float a[4], b[4];
@@ -181,10 +216,11 @@ __device__ __forceinline__ void image_epilogue(const Params &p, const Tile &c, i
                 }
                 if (!shuffle) {
                     const size_t off = pix * p.y_pitch + p.y_coff + cb;
-                    if (p.residual != nullptr && inside) {
+                    if (add_res && inside) {
 #pragma unroll
                         for (int jb = 0; jb < 4; ++jb) {
-                            const float2 r = __ldg(reinterpret_cast<const float2 *>(p.residual + off + 8 * jb + 2 * tq));
+                            const float2 r = SPLIT ? __ldg(reinterpret_cast<const float2 *>(p.residual + off + 8 * jb + 2 * tq))
+                                                   : res[cc][rh][jb];
                             a[jb] += r.x; b[jb] += r.y;
                         }
                     }

@@ -50,12 +50,15 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
 }
 
 // K-major, 128B-swizzled operand tile as TMA writes it with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128 B, 8-row
-// groups 1024 B apart.  Start addresses keep the 1024 B atom phase (whole 8-row groups); +32 B steps along K
-// inside the swizzled row are +2 on the descriptor.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+// groups `sbo` bytes apart (a multiple of 1024 B, so that every group has the start's phase in the 1024 B swizzle
+// atom).  +32 B steps along K inside the swizzled row are +2 on the descriptor.  A start may also lie on any row
+// inside the atom: the H100 applies the swizzle to the absolute shared-memory address bits, so the matrix base
+// offset (bits 49-51) stays 0.  Setting it to the start's phase, (start >> 7) & 7, reads the rows in the wrong
+// order (measured: every output of the 3x3 f16 kernel wrong).
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t sbo = 1024) {
     return (uint64_t)((smem_addr >> 4) & 0x3FFFu)      // start address
            | (1ull << 16)                              // leading byte offset (unused for SW128 K-major)
-           | (64ull << 32)                             // stride byte offset: 1024 B between 8-row groups
+           | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32)  // stride byte offset between 8-row groups
            | (1ull << 62);                             // SWIZZLE_128B
 }
 
