@@ -323,7 +323,21 @@ int l3c_bicubic_half_u8(const uint8_t *in_dev, int N, int H, int W, uint8_t *out
 int l3c_decode_rgb_pipelined(const float *l_dev, uint8_t *sym_dev, const float *targets_dev, int N, int HW, int K,
                              int L, uint16_t *table_dev, int pitch,
                              const l3c_dec_stream_t *const *desc_dev_per_channel, int chunk_px, void *cur_stream,
-                             void *const *bld_streams, void *const *dec_streams);
+                             void *const *bld_streams, void *const *dec_streams, int coarse);
+/* coarse != 0: table_dev holds coarse records instead of rows (pitch = 96, see l3c_dmll_build_coarse), built by
+ * l3c_dmll_build_coarse and decoded by l3c_ac_decode_streams_coarse; same symbols, same saved states. */
+
+/* Coarse CDF rows of RGB channel c (L = 256, K = 10) for pixels [pix0, pix0+npix) of every image: per sub-pixel one
+ * record of 96 uint16 at rec_dev[((n*3 + c)*HW + p) * 96]: the channel's mixture parameters as 32 floats (pi[10],
+ * mu[10], -log2(e)/sigma[10], 2 zeros), then the 32 entries cdf[8 i], i = 0..31, of the full row that
+ * l3c_dmll_build_table builds (cdf[256] = 2^16 is implied).  sym_dev: the decoded R (and G) symbols for c > 0. */
+int l3c_dmll_build_coarse(const float *l_dev, const uint8_t *sym_dev, const float *targets_dev, int N, int HW, int K,
+                          int L, int c, int pix0, int npix, uint16_t *rec_dev, void *stream);
+/* l3c_ac_decode_streams for L = 256 with every stream's `table` pointing at coarse records (row_pitch >= 96, 4-byte
+ * aligned); targets_dev: the 256 bin targets the records were built with.  The entries between two coarse entries
+ * are evaluated on demand, with the builder's arithmetic: symbols and saved states equal a full-row decode. */
+int l3c_ac_decode_streams_coarse(const l3c_dec_stream_t *streams_dev, int n_streams, const float *targets_dev,
+                                 uint32_t first, uint32_t count, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * E. Execution resources

@@ -451,14 +451,15 @@ class BatchCodec(object):
             return S.cpu(), pads
         return S, pads
 
-    def _decode_rgb_pipelined(self, l, S, tg, C, K, L, table, d, dev, n_chunks=None, lane=None):
+    def _decode_rgb_pipelined(self, l, S, tg, C, K, L, table, d, dev, n_chunks=None, lane=None, coarse=False):
         """RGB scale: channel c's means depend on the decoded channels < c at the same pixel
         (logistic_mixture.py:262-272), so the reference codes R, G, B strictly one after the other.
         Here the three serial decoders run concurrently, staggered by one chunk of pixels: as soon as
         chunk j of channel c-1 is decoded, the CDF rows of chunk j of channel c are built (on the SM
         group the decoders do not own, _rgb_streams) and channel c's warps continue -- coder state is
         carried across launches.  Serial depth drops from 3*HW to (1 + 2/n_chunks)*HW symbols (whole
-        decode at 16x512^2 with 32 / 64 / 128 chunks: 120.5 / 118.7 / 117.7 ms when measured)."""
+        decode at 16x512^2 with 32 / 64 / 128 chunks: 120.5 / 118.7 / 117.7 ms when measured).
+        coarse: `table` and the descriptors hold coarse records (E.COARSE_PITCH) instead of full rows."""
         N, HW = S.shape[0], S.shape[2] * S.shape[3]
         if n_chunks is None:
             n_chunks = int(os.environ.get('L3C_RGB_CHUNKS', 64))
@@ -471,7 +472,7 @@ class BatchCodec(object):
         if lane is None:
             lane = self.lanes(dev, N * C, 1)[0][0]
         # the chunk loop itself (2 x 3 x n_chunks launches + as many event records / waits) runs inside the library
-        E.decode_rgb_pipelined(l, S, tg, K, L, table, descs, csz, cur, lane.bld, lane.dec)
+        E.decode_rgb_pipelined(l, S, tg, K, L, table, descs, csz, cur, lane.bld, lane.dec, coarse=coarse)
 
     def encode_stream(self, dev, n_decoders, n_lanes=1):
         """A stream for encodes that run beside decodes (EncodeJob pipelining): confined to the SM group of
@@ -620,7 +621,12 @@ class BatchCodec(object):
                 if tuple(l.shape[1:3]) != (H, W) or non_shared_get_K(l.shape[-1], C) != K:
                     raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
                                      % (scale, C, H, W, tuple(l.shape)))
-                pitch = E.table_pitch(dmll.L)
+                # the RGB scale of an equal-size batch in f16 mode decodes from coarse records (parameters + every 8th
+                # CDF entry, 192 instead of 512 B per sub-pixel; the decoder evaluates the bracketed entries itself);
+                # tiled and ragged batches, the bottleneck scales, L < 256 and the other precision modes build full rows
+                coarse = (dmll.rgb_scale and tile is None and not ragged and dmll.L == 256 and K == 10 and
+                          E.f16_mode())
+                pitch = E.COARSE_PITCH if coarse else E.table_pitch(dmll.L)
                 table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
                 d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
                 d['row_pitch'][:] = pitch
@@ -643,7 +649,8 @@ class BatchCodec(object):
                     l = l.view(N, 1, plane, l.shape[-1])
                     Sv = Sp.view(N, C, 1, plane)
                     if dmll.rgb_scale:
-                        self._decode_rgb_pipelined(l, Sv, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane)
+                        self._decode_rgb_pipelined(l, Sv, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane,
+                                                   coarse=coarse)
                     else:
                         E.dmll_build_table(l, Sv, tg, C, K, dmll.L, False, -1, table)
                         self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))

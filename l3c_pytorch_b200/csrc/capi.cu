@@ -369,11 +369,14 @@ struct EventRing {
 extern "C" int l3c_decode_rgb_pipelined(const float *l_dev, uint8_t *sym_dev, const float *targets_dev, int N, int HW,
                                         int K, int L, uint16_t *table_dev, int pitch,
                                         const l3c_dec_stream_t *const *desc_dev_per_channel, int chunk_px,
-                                        void *cur_stream, void *const *bld_streams, void *const *dec_streams) {
+                                        void *cur_stream, void *const *bld_streams, void *const *dec_streams,
+                                        int coarse) {
     L3C_REQUIRE(l_dev && sym_dev && targets_dev && table_dev && desc_dev_per_channel && bld_streams && dec_streams,
                 "l3c_decode_rgb_pipelined: null pointer");
     L3C_REQUIRE(N >= 1 && HW >= 1 && chunk_px >= 1 && L == 256, "l3c_decode_rgb_pipelined: N=%d HW=%d chunk=%d L=%d", N, HW,
                 chunk_px, L);
+    L3C_REQUIRE(!coarse || pitch == l3c::COARSE_REC_U16, "l3c_decode_rgb_pipelined: coarse records need pitch %d, got %d",
+                l3c::COARSE_REC_U16, pitch);
     thread_local EventRing rings[64];     // per host thread and device, for the lifetime of the process
     int dev_id = 0;
     L3C_CUDA(cudaGetDevice(&dev_id));
@@ -393,13 +396,18 @@ extern "C" int l3c_decode_rgb_pipelined(const float *l_dev, uint8_t *sym_dev, co
         for (int c = 0; c < C; ++c) {
             cudaStream_t sb = (cudaStream_t)bld_streams[c], sd = (cudaStream_t)dec_streams[c];
             if (c > 0) L3C_CUDA(cudaStreamWaitEvent(sb, dec_done[c - 1], 0));      // this chunk of channel c-1 is decoded
-            if (int e = l3c_dmll_build_table(l_dev, sym_dev, targets_dev, N, HW, C, K, L, 1, c, p0, npx, table_dev, pitch, sb))
+            if (int e = coarse ? l3c_dmll_build_coarse(l_dev, sym_dev, targets_dev, N, HW, K, L, c, p0, npx, table_dev, sb)
+                               : l3c_dmll_build_table(l_dev, sym_dev, targets_dev, N, HW, C, K, L, 1, c, p0, npx, table_dev,
+                                                      pitch, sb))
                 return e;
             cudaEvent_t built = ring.get();
             L3C_REQUIRE(built != nullptr, "l3c_decode_rgb_pipelined: cudaEventCreate failed");
             L3C_CUDA(cudaEventRecord(built, sb));
             L3C_CUDA(cudaStreamWaitEvent(sd, built, 0));
-            if (int e = l3c_ac_decode_streams(desc_dev_per_channel[c], N, L, (uint32_t)p0, (uint32_t)npx, sd)) return e;
+            if (int e = coarse ? l3c_ac_decode_streams_coarse(desc_dev_per_channel[c], N, targets_dev, (uint32_t)p0,
+                                                              (uint32_t)npx, sd)
+                               : l3c_ac_decode_streams(desc_dev_per_channel[c], N, L, (uint32_t)p0, (uint32_t)npx, sd))
+                return e;
             dec_done[c] = ring.get();
             L3C_REQUIRE(dec_done[c] != nullptr, "l3c_decode_rgb_pipelined: cudaEventCreate failed");
             L3C_CUDA(cudaEventRecord(dec_done[c], sd));

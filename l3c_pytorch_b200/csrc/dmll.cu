@@ -177,6 +177,53 @@ dmll_table_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
     }
 }
 
+// Coarse rows of RGB channel c (L = 256, raster stream order): per sub-pixel the record of dmll_math.cuh
+// (COARSE_REC_U16) -- channel_params() exactly as dmll_table_kernel computes them, and the entries cdf[8 i].  One
+// warp per record: lane l writes parameter word l and evaluates coarse entry l, 32 instead of 256 entries.
+__global__ void __launch_bounds__(TB_THREADS)
+dmll_coarse_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym, const float *__restrict__ targets,
+                   int HW, int c, int pix0, int npix, uint16_t *__restrict__ rec) {
+    constexpr int K = 10, C = 3, Kp = 4 * C * K;
+    __shared__ float s_par[TB_PIX][COARSE_PARAM_WORDS + 1];          // odd pitch: conflict-free column writes
+    const int n = blockIdx.y;
+    const int q0 = blockIdx.x * TB_PIX;
+    const int np = min(TB_PIX, npix - q0);
+    if ((int)threadIdx.x < np) {
+        const int p = pix0 + q0 + threadIdx.x;
+        const float *lp = l + ((size_t)n * HW + p) * Kp;
+        float xr = 0.f, xg = 0.f;
+        if (c >= 1) xr = (float)sym[((size_t)n * C + 0) * HW + p];
+        if (c >= 2) xg = (float)sym[((size_t)n * C + 1) * HW + p];
+        ChanParams<K> cp;
+        channel_params<K>(lp, 1, C, c, true, xr, xg, cp);
+        float *o = s_par[threadIdx.x];
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            o[k] = cp.pi[k];
+            o[K + k] = cp.mu[k];
+            o[2 * K + k] = cp.inv_s[k];
+        }
+        o[3 * K] = o[3 * K + 1] = 0.f;
+    }
+    __syncthreads();
+    const float scale = (float)(65536 - 256);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float tg = __ldg(targets + COARSE_STEP * lane);
+    for (int r = warp; r < np; r += TB_THREADS / 32) {
+        float pi[K], mu[K], is[K];
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            pi[k] = s_par[r][k];
+            mu[k] = s_par[r][K + k];
+            is[k] = s_par[r][2 * K + k];
+        }
+        const uint32_t v = mixture_cdf_u16_warp<K>(pi, mu, is, tg, scale, COARSE_STEP * lane, true);
+        uint16_t *out = rec + (((size_t)n * C + c) * HW + pix0 + q0 + r) * COARSE_REC_U16;
+        reinterpret_cast<float *>(out)[lane] = s_par[r][lane];
+        out[2 * COARSE_PARAM_WORDS + lane] = (uint16_t)v;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // reference-shaped per-channel parameters (CDFOut of logistic_mixture.py:61-65,134-141):
 // softmax(pi), mu (with RGB coupling), clamped log sigma as [N][K][HW] planes
@@ -436,6 +483,22 @@ extern "C" int l3c_dmll_build_table(const float *l_dev, const uint8_t *sym_dev,
     dmll_table_kernel<10><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, pix0, npix, table_dev, pitch, 0, 0, 0, 0);
     L3C_LAUNCH_CHECK("dmll_table_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_build_coarse(const float *l_dev, const uint8_t *sym_dev, const float *targets_dev, int N,
+                                     int HW, int K, int L, int c, int pix0, int npix, uint16_t *rec_dev, void *stream) {
+    using namespace l3c;
+    if (int e = check_common("l3c_dmll_build_coarse", N, HW, 3, K, L, 1)) return e;
+    L3C_REQUIRE(L == 256, "l3c_dmll_build_coarse: coarse rows exist for L=256 only, got L=%d", L);
+    L3C_REQUIRE(l_dev && targets_dev && rec_dev, "l3c_dmll_build_coarse: null pointer");
+    L3C_REQUIRE(c >= 0 && c < 3 && (c == 0 || sym_dev), "l3c_dmll_build_coarse: c=%d (decoded symbols needed for c>0)", c);
+    L3C_REQUIRE(pix0 >= 0 && npix >= 0 && pix0 + npix <= HW, "l3c_dmll_build_coarse: pixel range");
+    if (npix == 0) return L3C_OK;
+    dim3 grid(ceil_div(npix, TB_PIX), N);
+    dmll_coarse_kernel<<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(l_dev, sym_dev, targets_dev, HW, c, pix0, npix,
+                                                                      rec_dev);
+    L3C_LAUNCH_CHECK("dmll_coarse_kernel");
     return L3C_OK;
 }
 

@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "dmll_math.cuh"
 
 namespace l3c {
 
@@ -852,6 +853,234 @@ ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, in
 }  // namespace v3
 
 // ---------------------------------------------------------------------------------------------
+// decoder, RGB streams from coarse rows (L = 256; dmll_math.cuh: per symbol the 30 mixture parameters and the
+// coarse entries cdf[8 i]): v3's CTA layout (decoder warp + helper warp per stream, SPC streams per CTA), its
+// mbarrier ring and its speculative groups of 8, with a two-level search:
+//   helper warp : prefetches each symbol's record one group ahead and writes it into the ring: the parameters
+//                 (32 words, read by every lane) and the coarse proposals (cdf[8 l] << 16) | (cdf[8 l + 8] - 1),
+//                 one per lane (2^16 above cdf[248]).
+//   decoder warp: level 1 -- lane l compares coarse entry 8 l, one REDUX.MAX gives the bracket's bounds cdf[8 j]
+//                 and cdf[8 j + 8], a ballot gives j; level 2 -- lanes 1..7 evaluate cdf[8 j + lane] on demand
+//                 (mixture_cdf_u16_warp: the builder's code, so the full row's integers; the transcendentals are
+//                 skipped when every term of the bracket is saturated), compare them, and two reductions give the
+//                 largest passing entry and the smallest failing one (or cdf[8 j + 8]): the symbol's interval.
+// The rows are sorted, so the largest passing coarse entry brackets the largest passing entry of the full row:
+// every symbol and every interval is the full-row decoder's.  The exact path (replayed groups, ragged tails, the
+// final symbol, corrupt input) runs both levels as exact_step().  The decoder writes the symbols itself.
+// ---------------------------------------------------------------------------------------------
+namespace coarse {
+
+using v3::G;
+using v3::R;
+using v3::mbar_arrive;
+using v3::mbar_init;
+using v3::mbar_wait;
+using v3::smem_u32;
+
+constexpr int SLOT_WORDS = COARSE_PARAM_WORDS + COARSE_N;     // parameters, then the coarse proposals
+constexpr int RING_BYTES = R * SLOT_WORDS * 4;                 // 4 KB per stream
+constexpr int STREAM_SMEM = RING_BYTES + 32;                   // + 4 mbarriers
+constexpr int TG_BYTES = 256 * 4;                              // the targets, shared by the CTA's streams
+constexpr float SCALE = (float)(65536 - 256);
+
+inline size_t smem_bytes(int spc) { return (size_t)TG_BYTES + (size_t)spc * STREAM_SMEM; }
+
+struct Params {
+    float w[COARSE_PARAM_WORDS];   // pi[0..9], mu[0..9], inv_s[0..9]
+    __device__ __forceinline__ void load(const uint32_t *slot) {
+        const float4 *p = reinterpret_cast<const float4 *>(slot);
+#pragma unroll
+        for (int q = 0; q < COARSE_PARAM_WORDS / 4; ++q) {
+            const float4 x = p[q];
+            w[4 * q] = x.x;
+            w[4 * q + 1] = x.y;
+            w[4 * q + 2] = x.z;
+            w[4 * q + 3] = x.w;
+        }
+    }
+};
+
+// cdf[8 j + lane] on lanes 1..7, cdf[8 j] (`head`, from the coarse entry) on lane 0; other lanes: unused
+__device__ __forceinline__ uint32_t bracket_entry(const Params &p, const float *s_tg, uint32_t j, uint32_t head,
+                                                  int lane) {
+    const bool active = lane >= 1 && lane < COARSE_STEP;
+    const int m = COARSE_STEP * (int)j + (active ? lane : 0);
+    const uint32_t v = mixture_cdf_u16_warp<10>(p.w, p.w + 10, p.w + 20, s_tg[m], SCALE, m, active);
+    return lane == 0 ? head : v;
+}
+
+// one exact step of both levels; returns the symbol
+__device__ __forceinline__ uint32_t exact_symbol(const uint32_t *slot, const float *s_tg, CoderState &cs,
+                                                 BitSource &src, int lane, bool update) {
+    Params p;
+    p.load(slot);
+    const uint32_t pk1[1] = {slot[COARSE_PARAM_WORDS + lane]};
+    const uint32_t top1 = exact_step(pk1, cs, src, lane, false);
+    const uint32_t j = (uint32_t)__popc(__ballot_sync(FULL, pk1[0] <= top1)) - 1u;
+    const uint32_t v = bracket_entry(p, s_tg, j, top1 >> 16, lane);
+    uint32_t nx = __shfl_down_sync(FULL, v, 1);
+    if (lane == COARSE_STEP - 1) nx = (top1 & 0xFFFFu) + 1u;                 // cdf[8 j + 8]
+    const uint32_t pk2[1] = {lane < COARSE_STEP ? ((v << 16) | ((nx - 1u) & 0xFFFFu)) : 0u};
+    const uint32_t top2 = exact_step(pk2, cs, src, lane, update);
+    return COARSE_STEP * j + (uint32_t)__popc(__ballot_sync(FULL, lane < COARSE_STEP && pk2[0] <= top2)) - 1u;
+}
+
+// one speculative group of G symbols (see v3::spec_group; FULL2: the group starts with a span of exactly 2^32)
+template <bool FULL2>
+__device__ __forceinline__ bool spec_group(CoderState &cs, BitSource &src, const uint32_t *ring, const float *s_tg,
+                                           int lane, uint32_t (&packed)[2]) {
+    bool bad = false;
+    uint32_t cp = ring[COARSE_PARAM_WORDS + lane];
+#pragma unroll 1
+    for (int d = 0; d < G; ++d) {
+        const uint32_t *slot = ring + d * SLOT_WORDS;
+        const uint32_t ncp = ring[((d + 1) & (G - 1)) * SLOT_WORDS + COARSE_PARAM_WORDS + lane];
+        Params p;
+        p.load(slot);                                                         // off the chain until j is known
+        const uint32_t r = cs.r, dv = cs.dv;
+        const uint32_t span = r + 1u;
+        bad |= (dv > r) || ((span == 0u) != FULL2);
+        auto passes = [&](uint32_t x) {   // cdf <= count  <=>  mulhi(cdf << 16, span) <= dv
+            return (FULL2 ? (x & 0xFFFF0000u) : __umulhi(x & 0xFFFF0000u, span)) <= dv;
+        };
+        // level 1: the bracket
+        const bool f1 = (lane == 0) || passes(cp);
+        const uint32_t top1 = __reduce_max_sync(FULL, f1 ? cp : 0u);
+        const uint32_t j = 31u - (uint32_t)__clz((int)__ballot_sync(FULL, f1));
+        // level 2: the entry inside it
+        const uint32_t v = bracket_entry(p, s_tg, j, top1 >> 16, lane);
+        const bool in = lane < COARSE_STEP;
+        const bool f2 = (lane == 0) || (in && passes(v << 16));
+        const uint32_t lo = __reduce_max_sync(FULL, f2 ? v : 0u);
+        const uint32_t hi = __reduce_min_sync(FULL, (in && !f2) ? v : (top1 & 0xFFFFu) + 1u);
+        const uint32_t sym = COARSE_STEP * j + (uint32_t)__popc(__ballot_sync(FULL, f2)) - 1u;   // off the chain
+        bad |= cs.update_flat(lo, hi, src);
+        const uint32_t sh = sym << (8 * (d & 3));
+        packed[0] |= (d < 4) ? sh : 0u;
+        packed[1] |= (d < 4) ? 0u : sh;
+        cp = ncp;
+    }
+    return bad;
+}
+
+// streams: row_pitch >= COARSE_REC_U16 (uint16), table 4-byte aligned; targets_dev: the 256 RGB bin targets
+template <int SPC>
+__global__ void __launch_bounds__(64 * SPC, 1)
+ac_decode_coarse_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, const float *__restrict__ targets,
+                        uint32_t first, uint32_t count) {
+    extern __shared__ __align__(16) uint8_t dec_smem[];
+    const int warp_id = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int sslot = warp_id % SPC;
+    const int warp = warp_id / SPC;                     // 0 = decoder, 1 = helper
+    float *s_tg = reinterpret_cast<float *>(dec_smem);
+    uint8_t *mine = dec_smem + TG_BYTES + sslot * STREAM_SMEM;
+    uint32_t *ring = reinterpret_cast<uint32_t *>(mine);                     // [slot][SLOT_WORDS]
+    const uint32_t bar0 = smem_u32(mine + RING_BYTES);                      // full[0..1], empty[0..1]
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) s_tg[i] = __ldg(targets + i);
+    if (warp == 0 && lane == 0) {
+        mbar_init(bar0 + 0, 32);
+        mbar_init(bar0 + 8, 32);
+        mbar_init(bar0 + 16, 32);
+        mbar_init(bar0 + 24, 32);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    const int sid = blockIdx.x * SPC + sslot;
+    if (sid >= n_streams) return;
+    const l3c_dec_stream_t st = streams[sid];
+    uint32_t last, upd_end;
+    if (!chunk_of(st.n_sym, first, count, last, upd_end)) return;
+    const uint32_t n_groups = (last - first + G - 1) / G;
+
+    if (warp == 1) {
+        // ============================ helper warp ============================
+        const uint16_t *__restrict__ table = st.table;
+        const int64_t pitch = st.row_pitch;
+        uint32_t nw[G], nc[G];
+        auto fetch = [&](uint32_t gi) {
+#pragma unroll
+            for (int d = 0; d < G; ++d) {
+                const uint32_t i = first + gi * G + d;
+                if (i < last) {
+                    const uint16_t *rec = table + (int64_t)i * pitch;
+                    nw[d] = __ldg(reinterpret_cast<const uint32_t *>(rec) + lane);
+                    nc[d] = __ldg(rec + 2 * COARSE_PARAM_WORDS + lane);
+                } else {
+                    nw[d] = nc[d] = 0u;
+                }
+            }
+        };
+        fetch(0);
+        for (uint32_t gi = 0; gi < n_groups; ++gi) {
+            const uint32_t g = gi & 1u;
+            uint32_t cw[G], cc[G];
+#pragma unroll
+            for (int d = 0; d < G; ++d) {
+                cw[d] = nw[d];
+                cc[d] = nc[d];
+            }
+            if (gi + 1 < n_groups) fetch(gi + 1);
+            if (gi >= 2) mbar_wait(bar0 + 16 + 8 * g, ((gi >> 1) - 1) & 1u);   // the decoder is done with this half
+#pragma unroll
+            for (int d = 0; d < G; ++d) {
+                uint32_t *slot = ring + (g * G + d) * SLOT_WORDS;
+                uint32_t nx = __shfl_down_sync(FULL, cc[d], 1);
+                if (lane == 31) nx = 0x10000u;                                   // cdf[256]
+                slot[lane] = cw[d];
+                slot[COARSE_PARAM_WORDS + lane] = (cc[d] << 16) | ((nx - 1u) & 0xFFFFu);
+            }
+            mbar_arrive(bar0 + 8 * g);                                           // full[g]
+        }
+        return;
+    }
+
+    // ============================ decoder warp ============================
+    BitSource src;
+    CoderState cs;
+    const uint32_t bit0 = open_stream(st, first, src, cs);
+    uint8_t *__restrict__ sym_out = st.sym_out;
+    for (uint32_t gi = 0; gi < n_groups; ++gi) {
+        const uint32_t g = gi & 1u;
+        mbar_wait(bar0 + 8 * g, (gi >> 1) & 1u);                                 // full[g]
+        const uint32_t ibase = first + gi * G;
+        const uint32_t *slots = ring + g * G * SLOT_WORDS;
+        bool replay = ibase + G > upd_end;                                       // ragged / final group
+        uint32_t packed[2] = {0u, 0u};
+        if (!replay) {
+            const CoderState cs0 = cs;
+            const BitSource src0 = src;
+            const bool bad = (cs.r == 0xFFFFFFFFu) ? spec_group<true>(cs, src, slots, s_tg, lane, packed)
+                                                    : spec_group<false>(cs, src, slots, s_tg, lane, packed);
+            if (__builtin_expect(bad, 0)) {
+                cs = cs0;
+                src = src0;
+                packed[0] = packed[1] = 0u;
+                replay = true;
+            }
+        }
+        if (replay) {
+#pragma unroll 1
+            for (int d = 0; d < G; ++d) {
+                const uint32_t i = ibase + d;
+                if (i >= last) break;
+                const uint32_t sym = exact_symbol(slots + d * SLOT_WORDS, s_tg, cs, src, lane, i < upd_end);
+                const uint32_t sh = sym << (8 * (d & 3));
+                packed[0] |= (d < 4) ? sh : 0u;
+                packed[1] |= (d < 4) ? 0u : sh;
+            }
+        }
+        __syncwarp();
+        mbar_arrive(bar0 + 16 + 8 * g);                                          // empty[g]
+        if (lane == 0) store_group(sym_out + ibase, packed, min(last - ibase, (uint32_t)G));
+    }
+    if (lane == 0) save_stream(st, cs, src, bit0);
+}
+
+}  // namespace coarse
+
+// ---------------------------------------------------------------------------------------------
 // decoder, alphabets of 257 to 32768 symbols (reached through the drop-in torchac API): CTA = decoder warp +
 // helper warp, one stream per CTA.  A row no longer fits the warp's registers, so it is staged whole in shared
 // memory and searched in two levels, each one exact_step() (floor rule, foreign count) over at most 8 proposals
@@ -1039,6 +1268,17 @@ extern "C" int l3c_ac_encode_streams(const l3c_enc_stream_t *streams_dev, int n_
 namespace l3c {
 std::atomic<int> g_dec_spc{0};   // l3c_set_decoder_streams_per_cta: 0 = L3C_DEC_SPC / the default
 
+// streams per CTA of the helper-warp decoders: the knob, else L3C_DEC_SPC (read once), else 1
+static int decoder_spc() {
+    static const int env_spc = [] {
+        const char *e = getenv("L3C_DEC_SPC");
+        const int v = e ? atoi(e) : 1;
+        return (v == 1 || v == 2 || v == 4) ? v : 1;
+    }();
+    const int forced = g_dec_spc.load(std::memory_order_relaxed);
+    return forced ? forced : env_spc;
+}
+
 template <bool FULLROW>
 void launch_decode(const l3c_dec_stream_t *streams, int n, int L, uint32_t first, uint32_t count, int spc,
                    cudaStream_t st) {
@@ -1110,14 +1350,8 @@ extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_
     if (L <= 32) {
         ac_decode32_kernel<<<n_streams, 32, 0, st>>>(streams_dev, n_streams, L, first, count);
     } else {
-        static const int env_spc = [] {
-            const char *e = getenv("L3C_DEC_SPC");
-            const int v = e ? atoi(e) : 1;
-            return (v == 1 || v == 2 || v == 4) ? v : 1;
-        }();
+        const int spc = decoder_spc();
         static bool configured_dev[64] = {};
-        const int forced = g_dec_spc.load(std::memory_order_relaxed);
-        const int spc = forced ? forced : env_spc;
         bool &configured = configured_dev[current_device_slot()];
         if (!configured) {   // the SPC = 4 variants are the ones above 48 KB of shared memory
             L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1131,6 +1365,30 @@ extern "C" int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_
         else
             launch_decode<false>(streams_dev, n_streams, L, first, count, spc, st);
     }
+    L3C_LAUNCH_CHECK("ac_decode_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_ac_decode_streams_coarse(const l3c_dec_stream_t *streams_dev, int n_streams,
+                                            const float *targets_dev, uint32_t first, uint32_t count, void *stream) {
+    using namespace l3c;
+    using coarse::ac_decode_coarse_kernel;
+    L3C_REQUIRE(n_streams >= 0, "l3c_ac_decode_streams_coarse: n_streams=%d", n_streams);
+    if (n_streams == 0 || count == 0) return L3C_OK;
+    L3C_REQUIRE(streams_dev && targets_dev, "l3c_ac_decode_streams_coarse: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int spc = decoder_spc();
+    if (spc == 4)
+        ac_decode_coarse_kernel<4><<<ceil_div(n_streams, 4), 256, coarse::smem_bytes(4), st>>>(streams_dev, n_streams,
+                                                                                           targets_dev, first, count);
+    else if (spc == 2)
+        ac_decode_coarse_kernel<2><<<ceil_div(n_streams, 2), 128, coarse::smem_bytes(2), st>>>(streams_dev, n_streams,
+                                                                                           targets_dev, first, count);
+    else
+        ac_decode_coarse_kernel<1><<<n_streams, 64, coarse::smem_bytes(1), st>>>(streams_dev, n_streams, targets_dev,
+                                                                                 first, count);
+    // logged under the decoder family's name, like every v3 variant: a decode makes the same launches whether its
+    // RGB scale reads coarse records or full rows
     L3C_LAUNCH_CHECK("ac_decode_kernel");
     return L3C_OK;
 }

@@ -871,16 +871,43 @@ def pack_streams(desc_dev, lens_dev, dst_off_np, n, blob):
     LAUNCHES['n'] += 1
 
 
-def decode_rgb_pipelined(l, S, targets, K, L, table, descs_dev, chunk_px, cur, bld, dec):
+COARSE_PITCH = 96     # uint16 per coarse record (l3c_dmll_build_coarse)
+
+
+def dmll_build_coarse(l, sym, targets, K, L, c, rec, pix0=0, npix=None):
+    """coarse records (parameters + cdf[8 i]) of RGB channel c, L = 256: rec int16 [N * 3 * H * W * COARSE_PITCH]"""
+    N, H, W, _ = l.shape
+    npix = H * W - pix0 if npix is None else npix
+    check(lib.l3c_dmll_build_coarse(_ptr(l), _ptr(sym), _ptr(targets), N, H * W, K, L, c, pix0, npix, _ptr(rec),
+                                    _stream_ptr()))
+    LAUNCHES['n'] += 1
+
+
+def ac_decode_streams_coarse(desc_np, device, targets, first=0, count=None, desc_dev=None, n=None):
+    """ac_decode_streams (L = 256) for streams whose `table` points at coarse records (row_pitch COARSE_PITCH)."""
+    if desc_dev is None:
+        desc_dev = _desc_to_device(desc_np, device)
+    if n is None:
+        n = desc_np.shape[0]
+    if count is None:
+        count = int(desc_np['n_sym'].max()) if n else 0
+    check(lib.l3c_ac_decode_streams_coarse(_ptr(desc_dev), n, _ptr(targets), first, count, _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return desc_dev
+
+
+def decode_rgb_pipelined(l, S, targets, K, L, table, descs_dev, chunk_px, cur, bld, dec, coarse=False):
     """l3c_decode_rgb_pipelined: the chunk-pipelined RGB scale of a decode in one native call.
-    descs_dev: three device tensors (descriptor arrays of the R, G, B streams); cur / bld / dec: torch streams."""
+    descs_dev: three device tensors (descriptor arrays of the R, G, B streams); cur / bld / dec: torch streams.
+    coarse: `table` holds coarse records (pitch COARSE_PITCH) instead of 256-entry rows."""
     N, H, W, _ = l.shape
     HW = H * W
     pp = (ctypes.c_void_p * 3)(*[d.data_ptr() for d in descs_dev])
     sb = (ctypes.c_void_p * 3)(*[s.cuda_stream for s in bld])
     sd = (ctypes.c_void_p * 3)(*[s.cuda_stream for s in dec])
-    check(lib.l3c_decode_rgb_pipelined(_ptr(l), _ptr(S), _ptr(targets), N, HW, K, L, _ptr(table), table_pitch(L), pp,
-                                       int(chunk_px), ctypes.c_void_p(cur.cuda_stream), sb, sd))
+    check(lib.l3c_decode_rgb_pipelined(_ptr(l), _ptr(S), _ptr(targets), N, HW, K, L, _ptr(table),
+                                       COARSE_PITCH if coarse else table_pitch(L), pp, int(chunk_px),
+                                       ctypes.c_void_p(cur.cuda_stream), sb, sd, 1 if coarse else 0))
     LAUNCHES['n'] += 2 * 3 * (-(-HW // int(chunk_px)))
 
 
