@@ -857,13 +857,15 @@ ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, in
 // coarse entries cdf[8 i]): v3's CTA layout (decoder warp + helper warp per stream, SPC streams per CTA), its
 // mbarrier ring and its speculative groups of 8, with a two-level search:
 //   helper warp : prefetches each symbol's record one group ahead and writes it into the ring: the parameters
-//                 (32 words, read by every lane) and the coarse proposals (cdf[8 l] << 16) | (cdf[8 l + 8] - 1),
-//                 one per lane (2^16 above cdf[248]).
+//                 (32 words), the coarse proposals (cdf[8 l] << 16) | (cdf[8 l + 8] - 1), one per lane (2^16 above
+//                 cdf[248]), and in the padding word LIN_WORD the linear-bracket mask: bit l set when every term
+//                 is saturated on the same side at both ends of bracket l (dmll_math.cuh: mixture_linear), i.e.
+//                 cdf[8 l + e] = cdf[8 l] + e.  Narrow components make most brackets of a record linear.
 //   decoder warp: level 1 -- lane l compares coarse entry 8 l, one REDUX.MAX gives the bracket's bounds cdf[8 j]
-//                 and cdf[8 j + 8], a ballot gives j; level 2 -- lanes 1..7 evaluate cdf[8 j + lane] on demand
-//                 (mixture_cdf_u16_warp: the builder's code, so the full row's integers; the transcendentals are
-//                 skipped when every term of the bracket is saturated), compare them, and two reductions give the
-//                 largest passing entry and the smallest failing one (or cdf[8 j + 8]): the symbol's interval.
+//                 and cdf[8 j + 8], a ballot gives j; level 2 -- lane e < 8 proposes cdf[8 j + e]: cdf[8 j] + e in a
+//                 linear bracket, else evaluated term-parallel on 28 lanes (bracket_entry_terms: mixture_cdf_u16's
+//                 operations in its order, so the full row's integers); one compare each, and two reductions give
+//                 the largest passing entry and the smallest failing one (or cdf[8 j + 8]): the symbol's interval.
 // The rows are sorted, so the largest passing coarse entry brackets the largest passing entry of the full row:
 // every symbol and every interval is the full-row decoder's.  The exact path (replayed groups, ragged tails, the
 // final symbol, corrupt input) runs both levels as exact_step().  The decoder writes the symbols itself.
@@ -885,39 +887,57 @@ constexpr float SCALE = (float)(65536 - 256);
 
 inline size_t smem_bytes(int spc) { return (size_t)TG_BYTES + (size_t)spc * STREAM_SMEM; }
 
-struct Params {
-    float w[COARSE_PARAM_WORDS];   // pi[0..9], mu[0..9], inv_s[0..9]
-    __device__ __forceinline__ void load(const uint32_t *slot) {
-        const float4 *p = reinterpret_cast<const float4 *>(slot);
-#pragma unroll
-        for (int q = 0; q < COARSE_PARAM_WORDS / 4; ++q) {
-            const float4 x = p[q];
-            w[4 * q] = x.x;
-            w[4 * q + 1] = x.y;
-            w[4 * q + 2] = x.z;
-            w[4 * q + 3] = x.w;
-        }
-    }
-};
+constexpr int K = 10;
+constexpr int LIN_WORD = 3 * K;          // ring slot word 30 (record padding): the linear-bracket mask
 
-// cdf[8 j + lane] on lanes 1..7, cdf[8 j] (`head`, from the coarse entry) on lane 0; other lanes: unused
-__device__ __forceinline__ uint32_t bracket_entry(const Params &p, const float *s_tg, uint32_t j, uint32_t head,
-                                                  int lane) {
-    const bool active = lane >= 1 && lane < COARSE_STEP;
-    const int m = COARSE_STEP * (int)j + (active ? lane : 0);
-    const uint32_t v = mixture_cdf_u16_warp<10>(p.w, p.w + 10, p.w + 20, s_tg[m], SCALE, m, active);
-    return lane == 0 ? head : v;
+// Entry cdf[8 j + (lane & 7)] of a bracket that is not linear, term-parallel: lane e + 8 q (e = lane & 7) evaluates
+// terms q, q + 4, q + 8 (< K) of entry 8 j + e with mixture_term()'s operations, and lane e gathers the K factors by
+// shuffles and accumulates them in term order, exactly as mixture_cdf_u16() does.  A term with u >= SAT_HI adds
+// nothing; it travels as the factor -1, which no evaluated factor can be (1, a reciprocal of a number >= 1, or
+// NaN, for which `< 0` is false) -- a zero factor would not do: fma(NaN, 0, acc) is not acc.  3 MUFU pairs per
+// lane instead of 10.  Valid on lanes 1..7 (lane 0 computes cdf[8 j] itself); warp-collective.
+__device__ __forceinline__ uint32_t bracket_entry_terms(const float *slot, const float *s_tg, uint32_t j, int lane) {
+    const int e = lane & (COARSE_STEP - 1), q = lane >> 3;
+    const int m = COARSE_STEP * (int)j + e;
+    const float t = s_tg[m];
+    float f[3];
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+        const int k = (q + 4 * s < K) ? q + 4 * s : q;             // lanes 16..31 own 2 terms; the third is unused
+        const float u = __fmul_rn(__fsub_rn(t, slot[K + k]), slot[2 * K + k]);
+        const float sig = (u <= SAT_LO) ? 1.0f : sigmoid_from_log2(u);
+        f[s] = (u >= SAT_HI) ? -1.0f : sig;
+    }
+    float acc = 0.f;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const float x = __shfl_sync(FULL, f[k >> 2], e + COARSE_STEP * (k & 3));
+        acc = (x < 0.0f) ? acc : __fmaf_rn(slot[k], x, acc);
+    }
+    return (uint32_t)(__float2int_rn(__fmul_rn(acc, SCALE)) + m) & 0xFFFFu;
+}
+
+// cdf[8 j + lane] on lanes 0..7 (lane 0: cdf[8 j], the bracket's coarse entry top1 >> 16); other lanes: unused.
+// lin: the slot's linear-bracket mask.  A linear bracket needs no evaluation: its entries are cdf[8 j] + lane.
+__device__ __forceinline__ uint32_t bracket_entry(const uint32_t *slot, uint32_t lin, const float *s_tg, uint32_t j,
+                                                  uint32_t top1, int lane) {
+    const uint32_t head = top1 >> 16;
+    uint32_t v = (head + (uint32_t)lane) & 0xFFFFu;
+    if (!((lin >> j) & 1u)) {          // warp-uniform; a select would pay for the evaluation on every symbol
+        v = bracket_entry_terms(reinterpret_cast<const float *>(slot), s_tg, j, lane);
+        v = (lane == 0) ? head : v;
+    }
+    return v;
 }
 
 // one exact step of both levels; returns the symbol
 __device__ __forceinline__ uint32_t exact_symbol(const uint32_t *slot, const float *s_tg, CoderState &cs,
                                                  BitSource &src, int lane, bool update) {
-    Params p;
-    p.load(slot);
+    const uint32_t lin = slot[LIN_WORD];
     const uint32_t pk1[1] = {slot[COARSE_PARAM_WORDS + lane]};
     const uint32_t top1 = exact_step(pk1, cs, src, lane, false);
     const uint32_t j = (uint32_t)__popc(__ballot_sync(FULL, pk1[0] <= top1)) - 1u;
-    const uint32_t v = bracket_entry(p, s_tg, j, top1 >> 16, lane);
+    const uint32_t v = bracket_entry(slot, lin, s_tg, j, top1, lane);
     uint32_t nx = __shfl_down_sync(FULL, v, 1);
     if (lane == COARSE_STEP - 1) nx = (top1 & 0xFFFFu) + 1u;                 // cdf[8 j + 8]
     const uint32_t pk2[1] = {lane < COARSE_STEP ? ((v << 16) | ((nx - 1u) & 0xFFFFu)) : 0u};
@@ -935,8 +955,7 @@ __device__ __forceinline__ bool spec_group(CoderState &cs, BitSource &src, const
     for (int d = 0; d < G; ++d) {
         const uint32_t *slot = ring + d * SLOT_WORDS;
         const uint32_t ncp = ring[((d + 1) & (G - 1)) * SLOT_WORDS + COARSE_PARAM_WORDS + lane];
-        Params p;
-        p.load(slot);                                                         // off the chain until j is known
+        const uint32_t lin = slot[LIN_WORD];                                  // off the chain until j is known
         const uint32_t r = cs.r, dv = cs.dv;
         const uint32_t span = r + 1u;
         bad |= (dv > r) || ((span == 0u) != FULL2);
@@ -948,7 +967,7 @@ __device__ __forceinline__ bool spec_group(CoderState &cs, BitSource &src, const
         const uint32_t top1 = __reduce_max_sync(FULL, f1 ? cp : 0u);
         const uint32_t j = 31u - (uint32_t)__clz((int)__ballot_sync(FULL, f1));
         // level 2: the entry inside it
-        const uint32_t v = bracket_entry(p, s_tg, j, top1 >> 16, lane);
+        const uint32_t v = bracket_entry(slot, lin, s_tg, j, top1, lane);
         const bool in = lane < COARSE_STEP;
         const bool f2 = (lane == 0) || (in && passes(v << 16));
         const uint32_t lo = __reduce_max_sync(FULL, f2 ? v : 0u);
@@ -998,6 +1017,7 @@ ac_decode_coarse_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_stre
         // ============================ helper warp ============================
         const uint16_t *__restrict__ table = st.table;
         const int64_t pitch = st.row_pitch;
+        const float t_first = s_tg[COARSE_STEP * lane], t_last = s_tg[COARSE_STEP * lane + COARSE_STEP - 1];
         uint32_t nw[G], nc[G];
         auto fetch = [&](uint32_t gi) {
 #pragma unroll
@@ -1030,6 +1050,15 @@ ac_decode_coarse_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_stre
                 if (lane == 31) nx = 0x10000u;                                   // cdf[256]
                 slot[lane] = cw[d];
                 slot[COARSE_PARAM_WORDS + lane] = (cc[d] << 16) | ((nx - 1u) & 0xFFFFu);
+            }
+            __syncwarp();
+            // bit l of word LIN_WORD: bracket l is linear (mixture_linear() at its first and last entry)
+#pragma unroll 1
+            for (int d = 0; d < G; ++d) {
+                uint32_t *slot = ring + (g * G + d) * SLOT_WORDS;
+                const float *w = reinterpret_cast<const float *>(slot);
+                const uint32_t lin = __ballot_sync(FULL, mixture_linear<K>(w + K, w + 2 * K, t_first, t_last));
+                if (lane == 0) slot[LIN_WORD] = lin;
             }
             mbar_arrive(bar0 + 8 * g);                                           // full[g]
         }

@@ -76,8 +76,86 @@ def run(L, n_streams, n_sym, peaked, rare=False, own_tables=False, uniform=False
     print(json.dumps(dict(L=L, streams=n_streams, n_sym=n_sym, peaked=peaked, rare=rare, own_tables=own_tables, uniform=uniform, bits_per_sym=nbytes * 8 / n_sym,
                           enc_ns_per_sym=t_enc * 1e6 / n_sym, dec_ns_per_sym=t_dec * 1e6 / n_sym, ok=ok, **extra)))
 
+def run_coarse(n_streams, kind, H=128, W=128):
+    """The coarse RGB decoder alone (l3c_ac_decode_streams_coarse): n_streams planes of H x W sub-pixels, records
+    from l3c_dmll_build_coarse, streams encoded on dmll_table_kernel's full rows.  kind 'bench': sigma ~ 1 bin and
+    uniform symbols, as on the noise images of bench.py (most symbols land in linear brackets); 'peaked': one
+    dominant component per sub-pixel, symbols at its mode (trained-like: the brackets are evaluated)."""
+    from l3c_pytorch_b200.dmll import DiscretizedMixLogisticLoss
+    dev = torch.device('cuda')
+    C, K, L, HW = 3, 10, 256, H * W
+    N = -(-n_streams // C)
+    rng = np.random.default_rng(0)
+    shp = (N, HW, C, K)
+    logit, mean = rng.normal(0, 1, shp), rng.uniform(0, 255, shp)
+    if kind == 'bench':
+        logs, coef = rng.normal(0, 0.5, shp), rng.normal(0, 1, shp)
+        sym = rng.integers(0, 256, (N, C, HW))
+    else:
+        dom = rng.integers(0, K, (N, HW, C))
+        np.put_along_axis(logit, dom[..., None], 8.0, axis=3)
+        logs, coef = rng.uniform(-1, 1, shp), np.full(shp, -30.0)            # no channel coupling
+        mu = np.take_along_axis(mean, dom[..., None], axis=3)[..., 0]         # [N, HW, C]
+        sym = np.clip(np.rint(mu + rng.normal(0, 1, mu.shape)), 0, 255).transpose(0, 2, 1)
+    sym = sym.astype(np.uint8)
+    l = torch.from_numpy(np.stack([logit, mean, logs, coef], 2).reshape(N, H, W, 4 * C * K).astype(np.float32)).to(dev)
+    sym_dev = torch.from_numpy(sym.reshape(N, C, H, W)).to(dev)
+    tg = DiscretizedMixLogisticLoss(True, 0, 255, L).targets(dev)
+    S = N * C
+    rows = torch.zeros(S * HW * L, dtype=torch.int16, device=dev)
+    rec = torch.zeros(S * HW * E.COARSE_PITCH, dtype=torch.int16, device=dev)
+    for c in range(C):
+        E.dmll_build_table(l, sym_dev, tg, C, K, L, True, c, rows)
+        E.dmll_build_coarse(l, sym_dev, tg, K, L, c, rec)
+    r = rows.view(S, HW, L).to(torch.int64) & 0xFFFF
+    s = torch.from_numpy(sym.reshape(S, HW).astype(np.int64)).to(dev)
+    lo = r.gather(2, s[..., None])[..., 0]
+    hi = torch.where(s < L - 1, r.gather(2, (s + 1).clamp(max=L - 1)[..., None])[..., 0], torch.full_like(s, 65536))
+    iv = lo | ((hi - 1) << 16)
+    iv = torch.where(iv >= 2 ** 31, iv - 2 ** 32, iv).to(torch.int32).contiguous()
+    del rows, r
+    # the fraction of symbols whose bracket is linear (mixture_linear() on the records' parameters)
+    par = rec.view(S, HW, E.COARSE_PITCH)[..., :64].contiguous().view(torch.float32)       # [S, HW, 32]
+    t = tg[:256]
+    u0 = (t[0::8][None, None, :, None] - par[..., None, 10:20]) * par[..., None, 20:30]
+    u1 = (t[7::8][None, None, :, None] - par[..., None, 10:20]) * par[..., None, 20:30]
+    lin = ((u0 <= -25.0) | (u1 >= 40.0)).all(-1)                                            # [S, HW, 32]
+    frac_lin = float(lin[:n_streams].gather(2, (s[:n_streams] >> 3)[..., None]).float().mean())
+    cap = ((HW * 17 + 7) // 8 + 64 + 3) & ~3
+    slots = torch.zeros(S * cap, dtype=torch.uint8, device=dev)
+    desc = np.zeros(S, dtype=_lib.ENC_STREAM_DTYPE)
+    desc['intervals'] = iv.data_ptr() + 4 * HW * np.arange(S); desc['n_sym'] = HW; desc['out_cap'] = cap
+    desc['out'] = slots.data_ptr() + cap * np.arange(S)
+    _, lens = E.ac_encode_streams(desc, dev)
+    out = torch.zeros(S * HW, dtype=torch.uint8, device=dev)
+    dd = np.zeros(S, dtype=_lib.DEC_STREAM_DTYPE)
+    dd['table'] = rec.data_ptr() + 2 * E.COARSE_PITCH * HW * np.arange(S); dd['row_pitch'] = E.COARSE_PITCH
+    dd['in'] = slots.data_ptr() + cap * np.arange(S); dd['in_len'] = lens.cpu().numpy()
+    dd['sym_out'] = out.data_ptr() + HW * np.arange(S); dd['n_sym'] = HW
+    ddev = E._desc_to_device(dd, dev)
+    times = []
+    for _ in range(4):
+        a = torch.cuda.Event(enable_timing=True); b = torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize(); a.record()
+        E.ac_decode_streams_coarse(dd, dev, tg, 0, HW, desc_dev=ddev, n=n_streams)
+        b.record(); torch.cuda.synchronize(); times.append(a.elapsed_time(b))
+    got = out.view(S, HW)[:n_streams].cpu().numpy()
+    ok = bool((got == sym.reshape(S, HW)[:n_streams]).all())
+    print(json.dumps(dict(coarse=kind, streams=n_streams, n_sym=HW, bits_per_sym=float(lens[:n_streams].float().mean()) * 8 / HW,
+                          linear_fraction=frac_lin, dec_ns_per_sym=min(times[1:]) * 1e6 / HW, ok=ok)))
+
+
 if __name__ == '__main__':
     only = int(sys.argv[sys.argv.index('--only') + 1]) if '--only' in sys.argv else None
+    if '--coarse' in sys.argv:        # the coarse RGB decoder (f16 mode, L = 256), 1 and 48 streams
+        import subprocess
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', '0'],
+                           capture_output=True, text=True).stdout.strip()
+        print(json.dumps(dict(gpu=torch.cuda.get_device_name(0), nvidia_smi=q)))
+        for kind in ('bench', 'peaked'):
+            for ns in (1, 48):
+                run_coarse(ns, kind)
+        sys.exit(0)
     if '--wide' in sys.argv:          # alphabets above 256 (drop-in torchac range), against the reference on the CPU
         import subprocess
         q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', '0'],
