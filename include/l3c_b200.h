@@ -73,7 +73,12 @@ int l3c_decode_cdf(const uint16_t *cdf_host, int64_t n_sym, int Lp, const uint8_
  * (torchac.cpp:231-258; CDF formula torchac_kernel.cu:20-76).  targets_dev f32[Lp];
  * means/log_scales/probs_dev f32 [K][n_sym] (1KHW contiguous, CUDA); sym_host int16 (CPU, as in
  * the reference).  No CDF table is materialised: only the two bounds of each coded symbol are
- * evaluated.  Synchronous. */
+ * evaluated.  Synchronous.
+ * log_scales are used as given, unclamped, as the reference's torchac does.  Below about -88 the
+ * scale factor exp(-log_scale) overflows to inf.  An entry whose target then equals a component's
+ * mean evaluates to NaN and becomes cdf[l] = l, which can make the row decrease there and leave a
+ * symbol without an interval.  The reference's callers clamp log-scales at -7
+ * (logistic_mixture.py:57), which is far from this limit. */
 int l3c_encode_logistic_mixture(const float *targets_dev, const float *means_dev,
                                 const float *log_scales_dev, const float *probs_dev, int K,
                                 int64_t n_sym, int Lp, const int16_t *sym_host,
@@ -374,6 +379,12 @@ int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb);
  * (1).  Any other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant
  * for production use. */
 int l3c_set_decoder_streams_per_cta(int spc);
+
+/* Test probe of the CDF rows' sigmoid: for the n fp32 values u_dev[i] (device), raw_dev[i] = sigmoid_from_log2(u)
+ * (~ 1 / (1 + 2^u), the MUFU.EX2 + MUFU.RCP evaluation every CDF entry uses) and term_dev[i] = mixture_term(0, 1, u)
+ * (the same with the saturation shortcuts: exactly 1 for u <= -25, 0 for u >= 40).  Both call the kernels' own
+ * __device__ functions, so a test can measure what the built library computes.  Not meant for production use. */
+int l3c_dmll_probe_sigmoid(const float *u_dev, float *raw_dev, float *term_dev, int64_t n, void *stream);
 
 #ifdef __cplusplus
 }

@@ -618,3 +618,27 @@ extern "C" int l3c_dmll_sample(const float *l_dev, const float *u_sel_dev, const
     L3C_LAUNCH_CHECK("dmll_sample_kernel");
     return L3C_OK;
 }
+
+namespace l3c {
+// the sigmoid of the CDF rows and one saturating mixture term (pi = 1, acc = 0), through the same __device__
+// functions every CDF kernel calls
+__global__ void probe_sigmoid_kernel(const float *__restrict__ u, float *__restrict__ raw, float *__restrict__ term,
+                                     int64_t n) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float v = u[i];
+        raw[i] = sigmoid_from_log2(v);
+        term[i] = mixture_term(0.f, 1.f, v);
+    }
+}
+}  // namespace l3c
+
+extern "C" int l3c_dmll_probe_sigmoid(const float *u_dev, float *raw_dev, float *term_dev, int64_t n, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(u_dev && raw_dev && term_dev && n >= 0, "l3c_dmll_probe_sigmoid: bad arguments");
+    if (n == 0) return L3C_OK;
+    const int64_t want = ceil_div64(n, 256);
+    const int blocks = (int)(want < 65536 ? want : 65536);
+    probe_sigmoid_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(u_dev, raw_dev, term_dev, n);
+    L3C_LAUNCH_CHECK("probe_sigmoid_kernel");
+    return L3C_OK;
+}
