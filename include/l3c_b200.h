@@ -11,7 +11,8 @@
  * Section A are the drop-in replacements for the FIVE exports of the reference's native module
  * (pybind module torchac_backend_{cpu,gpu}: /root/reference/src/torchac/torchac_backend/
  * torchac.cpp:433-443).  Sections B..E are the batched, device-resident building blocks the host
- * mirror (l3c_pytorch_b200.*) composes into the reference's Bitcoding / MultiscaleBlueprint API.
+ * mirror (l3c_pytorch_b200.*) composes into the reference's Bitcoding / MultiscaleBlueprint API;
+ * section F adds the ones the batched torchac calls compose with section B.
  *
  * Layout conventions
  *   activations ........ NHWC fp32, channel pitch given explicitly where slices are written
@@ -343,6 +344,48 @@ int l3c_dmll_build_coarse(const float *l_dev, const uint8_t *sym_dev, const floa
  * are evaluated on demand, with the builder's arithmetic: symbols and saved states equal a full-row decode. */
 int l3c_ac_decode_streams_coarse(const l3c_dec_stream_t *streams_dev, int n_streams, const float *targets_dev,
                                  uint32_t first, uint32_t count, void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * F. torchac, batched: the drop-in's streams, many per launch (l3c_pytorch_b200.torchac.*_batch)
+ *    Section A codes one stream per synchronous call.  These two kernels turn the sources of any number of streams
+ *    into the inputs of section B's coder: coding intervals for l3c_ac_encode_streams, decoder rows for
+ *    l3c_ac_decode_streams.  The integers are those of section A for the same stream.  The host composes them:
+ *    one interval launch, one encode launch and one pack for a whole call; the rows chunk by chunk, the decoder
+ *    resuming from its saved state.  Asynchronous on `stream`; nothing is allocated.
+ * ---------------------------------------------------------------------------------------- */
+
+/* The source of one stream.  A table stream has `table` set; a mixture stream has table = NULL and the four
+ * plane pointers set.  Lp = L + 1 as in section A (2 to 32769, checked by the caller).  The kernels assume valid
+ * descriptors and do not check them. */
+typedef struct {
+    const uint16_t *table;      /* dev [n_sym][Lp]: the 1HWLp CDF tensor, flattened; or NULL                      */
+    const float *targets;       /* mixture: dev f32 [Lp]                                                            */
+    const float *means;         /* mixture: dev f32 [K][n_sym]                                                      */
+    const float *log_scales;    /* mixture: dev f32 [K][n_sym] (unclamped, as in l3c_encode_logistic_mixture)      */
+    const float *probs;         /* mixture: dev f32 [K][n_sym]                                                      */
+    const int16_t *sym;         /* dev int16 [n_sym]: the symbols to code (read by l3c_batch_intervals only)       */
+    int64_t n_sym;              /* 1 to 2^31 - 1                                                                    */
+    int32_t Lp;
+    int32_t K;                  /* mixture components (>= 1); ignored for a table stream                            */
+} l3c_code_src_t;
+
+/* Coding intervals of every symbol of every stream, one launch.  sym_off_dev int64 [n_streams + 1]: prefix sums of
+ * n_sym (sym_off[0] = 0, sym_off[n_streams] = n_total); stream j's intervals go to intervals_dev + sym_off[j], packed
+ * c_low | (c_high - 1) << 16 as table_intervals_kernel / plane_intervals_kernel (section A) produce them.
+ * bad_dev int32 [n_streams]: stream j's first position whose symbol lies outside [0, Lp - 2], or -1 if there is
+ * none; such a symbol's interval is written as 0 and nothing else is read for it. */
+int l3c_batch_intervals(const l3c_code_src_t *src_dev, const int64_t *sym_off_dev, int n_streams, int64_t n_total,
+                        uint32_t *intervals_dev, int32_t *bad_dev, void *stream);
+
+/* Decoder rows of symbols [first, first + r_j) of every stream j, r_j = min(count, n_sym - first) (0 if
+ * first >= n_sym), one launch.  row_off_dev int64 [n_streams + 1], in uint16 entries: stream j's rows start at
+ * rows_dev + row_off[j], and row_off[j + 1] - row_off[j] = r_j * pitch_j with pitch_j the decoder's pitch for
+ * L = Lp - 1 (32 for L <= 32, 256 for L <= 256, else round_up(L, 8)); n_entries = row_off[n_streams].  rows_dev
+ * must be 16-byte aligned.  Entries 0..L-1 of a row are the CDF (a table row, or the mixture row that
+ * l3c_decode_logistic_mixture builds), the rest are 0.  A descriptor of l3c_ac_decode_streams then points its
+ * `table` at rows_dev + row_off[j] - first * pitch_j, so that symbol first + i reads row i. */
+int l3c_batch_rows(const l3c_code_src_t *src_dev, const int64_t *row_off_dev, int n_streams, int64_t n_entries,
+                   uint32_t first, uint16_t *rows_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * E. Execution resources

@@ -36,6 +36,9 @@ PRECISIONS = {'fp32': PREC_FP32, 'tf32': PREC_TF32, 'f16': PREC_F16, 'f16x2': PR
 ENC_STREAM_DTYPE = [('intervals', '<u8'), ('out', '<u8'), ('n_sym', '<u4'), ('out_cap', '<u4')]
 DEC_STREAM_DTYPE = [('table', '<u8'), ('in', '<u8'), ('sym_out', '<u8'), ('state', '<u8'),
                     ('row_pitch', '<i8'), ('n_sym', '<u4'), ('in_len', '<u4')]
+# l3c_code_src_t (section F)
+CODE_SRC_DTYPE = [('table', '<u8'), ('targets', '<u8'), ('means', '<u8'), ('log_scales', '<u8'), ('probs', '<u8'),
+                  ('sym', '<u8'), ('n_sym', '<i8'), ('Lp', '<i4'), ('K', '<i4')]
 
 _SIGNATURES = {
     'l3c_last_error': (ctypes.c_char_p, []),
@@ -81,6 +84,8 @@ _SIGNATURES = {
     'l3c_set_conv_launch_limits': (c_int, [c_int, c_int]),
     'l3c_set_decoder_streams_per_cta': (c_int, [c_int]),
     'l3c_dmll_probe_sigmoid': (c_int, [c_void_p] * 3 + [c_int64, c_void_p]),
+    'l3c_batch_intervals': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
+    'l3c_batch_rows': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_uint32, c_void_p, c_void_p]),
 }
 
 EXPORTS = sorted(_SIGNATURES)

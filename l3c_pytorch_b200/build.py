@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 SO = os.path.join(HERE, 'libl3c_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-SOURCES = ['capi.cu', 'range_coder.cu', 'dmll.cu', 'conv_ffma.cu', 'conv_tf32.cu', 'conv_f16.cu', 'conv_f16x2.cu', 'bicubic.cu', 'partition.cu', 'ragged.cu']
+SOURCES = ['capi.cu', 'range_coder.cu', 'dmll.cu', 'conv_ffma.cu', 'conv_tf32.cu', 'conv_f16.cu', 'conv_f16x2.cu', 'bicubic.cu', 'partition.cu', 'ragged.cu', 'torchac_batch.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--fmad=true',
               '-DL3C_BUILDING_DSO']

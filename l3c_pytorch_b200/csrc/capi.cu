@@ -83,22 +83,7 @@ __global__ void repitch_kernel(const uint16_t *__restrict__ cdf, int64_t n_sym, 
     out[i] = (e < Lp - 1) ? cdf[r * Lp + e] : (uint16_t)0;
 }
 
-// cdf[n][l] of torchac_kernel.cu:58-75 with parameters given as [K][N] planes.  The arithmetic is the
-// library's single CDF function (dmll_math.cuh: mixture_cdf_u16 on -log2(e)/sigma), so a stream written through
-// this per-channel entry point equals the one the batched codec writes for the same parameters.
-__device__ __forceinline__ uint32_t plane_cdf_u16(const float *__restrict__ means,
-                                                  const float *__restrict__ log_scales,
-                                                  const float *__restrict__ probs, int K, int64_t N,
-                                                  int64_t n, float target, float scale, int l) {
-    float acc = 0.f;
-    for (int k = 0; k < K; ++k) {
-        const float is = __fmul_rn(expf(-log_scales[k * N + n]), NEG_LOG2E);
-        const float u = __fmul_rn(__fsub_rn(target, means[k * N + n]), is);
-        acc = mixture_term(acc, probs[k * N + n], u);
-    }
-    return (uint32_t)(__float2int_rn(__fmul_rn(acc, scale)) + l) & 0xFFFFu;
-}
-
+// cdf[n][l] of torchac_kernel.cu:58-75 from [K][N] planes: dmll_math.cuh, plane_cdf_u16
 __global__ void plane_intervals_kernel(const float *__restrict__ targets, const float *__restrict__ means,
                                        const float *__restrict__ log_scales,
                                        const float *__restrict__ probs, int K, int64_t N, int Lp,
@@ -165,9 +150,6 @@ static int run_encode(const uint32_t *iv_dev, int64_t n_sym, uint8_t *out_host, 
     L3C_CUDA(cudaMemcpy(out_host, out.p, n, cudaMemcpyDeviceToHost));
     return L3C_OK;
 }
-
-// row pitch of the decoder's tables: 32 entries for L <= 32, 256 up to L = 256, else L rounded up to a multiple of 8
-static int decode_pitch(int L) { return (L <= 32) ? 32 : (L <= 256) ? 256 : (L + 7) & ~7; }
 
 static int run_decode(const uint16_t *table_dev, int pitch, int64_t n_sym, int L,
                       const uint8_t *in_host, size_t in_len, int16_t *sym_out_host) {

@@ -56,6 +56,9 @@ static inline int current_device_slot() {
     return dev & 63;
 }
 
+// row pitch of the decoder's tables: 32 entries for L <= 32, 256 up to L = 256, else L rounded up to a multiple of 8
+__host__ __device__ static inline int decode_pitch(int L) { return (L <= 32) ? 32 : (L <= 256) ? 256 : (L + 7) & ~7; }
+
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
