@@ -417,6 +417,39 @@ int l3c_partition_streams2(int sm_a, int n_a, void **streams_a, int n_b_high, vo
  * configuration is the default one.  Not meant for production use. */
 int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb);
 
+/* Test and diagnosis knob for the persistent tensor-core convolutions, process-wide, from the next launch on: how
+ * a launch hands its tiles to its CTAs.
+ *   0: dynamic (default): each pipe claims its next tile from a per-launch counter, so CTAs that start late run
+ *      fewer tiles;
+ *   1: static stripe: CTA b runs tiles b, b + G, ... (G = gridDim.x), its two pipes alternating;
+ *   2: dynamic with a start skew: odd CTAs wait 500 us before their first claim, so a few CTAs take most tiles
+ *      and some take none.
+ * Every mode gives the same bits.  Any other value is L3C_EINVAL.  Not meant for production use. */
+int l3c_set_conv_tile_schedule(int mode);
+
+/* *count = CTAs of the current device that ran no tile under schedule mode 2 since the last reset (waits for the
+ * device); reset != 0 then zeroes the count.  Not meant for production use. */
+int l3c_conv_idle_ctas(long long *count, int reset);
+
+/* One CTA of a persistent tensor-core convolution, as a library built with L3C_CTA_TRACE records it
+ * (`python -m l3c_pytorch_b200.build --cta-trace`, tools/cta_timeline.py). */
+typedef struct {
+    uint64_t t_start;   /* %globaltimer (ns) at the CTA's first instruction */
+    uint64_t t_end;     /* %globaltimer when the CTA's last warp left */
+    uint32_t smid;      /* the SM it ran on */
+    uint32_t tiles;     /* the tiles its consumers ran */
+    uint32_t launch;    /* launch index since l3c_cta_trace_register */
+    uint32_t cta;       /* blockIdx.y * gridDim.x + blockIdx.x */
+} l3c_cta_record_t;
+
+/* L3C_CTA_TRACE builds: from the next launch on, the CTAs of every persistent tensor-core launch write their
+ * records into records_dev (device memory, `capacity` records; launches that do not fit any more are not recorded)
+ * and the launch index starts from 0.  records_dev = NULL stops the recording.  Other builds: L3C_EUNSUPPORTED. */
+int l3c_cta_trace_register(l3c_cta_record_t *records_dev, int64_t capacity);
+/* L3C_CTA_TRACE builds: one line "launch name grid_x grid_y first_record stream" per launch since the last
+ * l3c_cta_trace_register (truncated to `cap`); *n_records = records written.  Other builds: L3C_EUNSUPPORTED. */
+int l3c_cta_trace_launches(char *buf, size_t cap, int64_t *n_records);
+
 /* Test knob for the range decoder of alphabets L > 32, process-wide, from the next launch on: streams per CTA (1, 2
  * or 4) of v3::ac_decode_kernel<FULLROW, SPC>; 0 = the L3C_DEC_SPC environment variable or, without it, the default
  * (1).  Any other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant

@@ -9,7 +9,8 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-SO_PATH = os.path.join(_HERE, 'libl3c_b200.so')
+# L3C_CTA_TRACE=1: the diagnosis build (build.py --cta-trace), whose conv CTAs record their timeline
+SO_PATH = os.path.join(_HERE, 'libl3c_b200_trace.so' if os.environ.get('L3C_CTA_TRACE') == '1' else 'libl3c_b200.so')
 
 c_void_p, c_int, c_int64, c_size_t, c_uint32, c_float = (
     ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_uint32, ctypes.c_float)
@@ -82,6 +83,10 @@ _SIGNATURES = {
     'l3c_partition_streams': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_partition_streams2': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_set_conv_launch_limits': (c_int, [c_int, c_int]),
+    'l3c_set_conv_tile_schedule': (c_int, [c_int]),
+    'l3c_conv_idle_ctas': (c_int, [ctypes.POINTER(ctypes.c_longlong), c_int]),
+    'l3c_cta_trace_register': (c_int, [c_void_p, c_int64]),
+    'l3c_cta_trace_launches': (c_int, [ctypes.c_char_p, c_size_t, ctypes.POINTER(c_int64)]),
     'l3c_set_decoder_streams_per_cta': (c_int, [c_int]),
     'l3c_dmll_probe_sigmoid': (c_int, [c_void_p] * 3 + [c_int64, c_void_p]),
     'l3c_batch_intervals': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),

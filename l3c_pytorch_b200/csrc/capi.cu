@@ -324,6 +324,74 @@ extern "C" long long l3c_launch_log(char *buf, size_t cap, int reset) {
     return total;
 }
 
+// ---- CTA trace of the persistent tensor-core kernels (L3C_CTA_TRACE builds) ----------------
+#ifdef L3C_CTA_TRACE
+namespace l3c {
+namespace {
+struct TraceLaunch {
+    const char *name;
+    unsigned gx, gy;
+    long long first;
+    cudaStream_t st;
+};
+std::mutex g_trace_mu;
+l3c_cta_record_t *g_trace_rec = nullptr;
+long long g_trace_cap = 0, g_trace_used = 0;
+std::vector<TraceLaunch> g_trace_launches;
+}  // namespace
+
+CtaTraceArg cta_trace_launch(const char *name, dim3 grid, cudaStream_t st) {
+    std::lock_guard<std::mutex> lk(g_trace_mu);
+    const long long n = (long long)grid.x * grid.y;
+    if (!g_trace_rec || g_trace_used + n > g_trace_cap) return CtaTraceArg{nullptr, -1};
+    const CtaTraceArg a{g_trace_rec + g_trace_used, (int)g_trace_launches.size()};
+    g_trace_launches.push_back(TraceLaunch{name, grid.x, grid.y, g_trace_used, st});
+    g_trace_used += n;
+    return a;
+}
+}  // namespace l3c
+#endif
+
+extern "C" int l3c_cta_trace_register(l3c_cta_record_t *records_dev, int64_t capacity) {
+    using namespace l3c;
+#ifdef L3C_CTA_TRACE
+    L3C_REQUIRE(capacity >= 0, "l3c_cta_trace_register: capacity %lld", (long long)capacity);
+    std::lock_guard<std::mutex> lk(g_trace_mu);
+    g_trace_rec = records_dev;
+    g_trace_cap = records_dev ? capacity : 0;
+    g_trace_used = 0;
+    g_trace_launches.clear();
+    return L3C_OK;
+#else
+    (void)records_dev; (void)capacity;
+    set_error("l3c_cta_trace_register: this library is built without L3C_CTA_TRACE");
+    return L3C_EUNSUPPORTED;
+#endif
+}
+
+extern "C" int l3c_cta_trace_launches(char *buf, size_t cap, int64_t *n_records) {
+    using namespace l3c;
+#ifdef L3C_CTA_TRACE
+    std::lock_guard<std::mutex> lk(g_trace_mu);
+    size_t pos = 0;
+    if (buf && cap) buf[0] = 0;
+    for (size_t i = 0; i < g_trace_launches.size(); ++i) {
+        const TraceLaunch &l = g_trace_launches[i];
+        if (buf && pos + 1 < cap) {
+            const int w = snprintf(buf + pos, cap - pos, "%zu %s %u %u %lld %p\n", i, l.name, l.gx, l.gy, l.first,
+                                   (void *)l.st);
+            if (w > 0) pos += (size_t)w < cap - pos ? (size_t)w : cap - pos - 1;
+        }
+    }
+    if (n_records) *n_records = g_trace_used;
+    return L3C_OK;
+#else
+    (void)buf; (void)cap; (void)n_records;
+    set_error("l3c_cta_trace_launches: this library is built without L3C_CTA_TRACE");
+    return L3C_EUNSUPPORTED;
+#endif
+}
+
 // ---------------------------------------------------------------------------------------------
 // RGB scale of a decode, channel-pipelined (host-side runtime piece: one call instead of ~400 Python-level
 // launches / event operations per decode).  Channel c's means depend on the decoded channels < c of the same

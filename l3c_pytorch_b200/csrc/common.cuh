@@ -47,6 +47,20 @@ int conv1x1_tc(const l3c_conv_t &p, cudaStream_t st);
 int sm_count();                          // SMs of the current device
 int stream_sm_count(cudaStream_t st);    // SMs available to kernels launched into `st` (partition.cu)
 int conv_smem_kb_override();             // l3c_set_conv_launch_limits' conv_smem_kb, 0 = none (partition.cu)
+int conv_tile_schedule();                // l3c_set_conv_tile_schedule's mode (partition.cu)
+// The tile counters of a persistent tensor-core launch into `st` (n <= TILE_COUNTERS of them, zero; no stream but
+// `st` uses them) and the device's idle-CTA count of schedule mode 2 (partition.cu)
+constexpr int TILE_COUNTERS = 32;
+int tile_counters(cudaStream_t st, int n, unsigned **counters, unsigned long long **idle_ctas);
+
+#ifdef L3C_CTA_TRACE
+// diagnosis builds: where the CTAs of the next launch record themselves (rec null: not recorded) (capi.cu)
+struct CtaTraceArg {
+    l3c_cta_record_t *rec;
+    int launch;
+};
+CtaTraceArg cta_trace_launch(const char *name, dim3 grid, cudaStream_t st);
+#endif
 
 // cudaFuncSetAttribute is per DEVICE: "done once" flags must be kept per device, or a process that drives a second
 // GPU launches its kernels there without the opt-in for > 48 KB of dynamic shared memory

@@ -100,7 +100,9 @@ __device__ __forceinline__ void unit_mma(float (&acc)[2][32], uint32_t a0, int r
 template <int KIND>
 __global__ void __launch_bounds__(THREADS, 1)
 conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
-                const Params p, const int n_stages, const int a_bytes, const int ptiles) {
+                const Params p, const int n_stages, const int a_bytes, const int ptiles,
+                const TileSchedule ts) {
+    L3C_TRACE_BEGIN;
     constexpr int W_RES = (KIND == 0) ? W_RES_BYTES : 0;    // resident weights
     constexpr int UNITS = (KIND == 0) ? 1 : 10;
     constexpr Halves HV = (KIND == 0) ? Halves::COLS : Halves::ROWS;
@@ -115,6 +117,7 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     const int d = p.dilation;
     const int ct = blockIdx.y;                        // this CTA's Cout tile (weights stay resident)
     Ring ring(w_base + W_RES, a_bytes, n_stages, bars, k);
+    TileQueue tiles(bars, k, 2, ptiles, ts);
 
     if (warp >= CONSUMER_WARPS) {
         // ===================== TMA producer of pipe k =====================
@@ -124,7 +127,7 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
             for (int tap = 0; tap < 9; ++tap)         // rows [tap][cout_pad] of the weight image
                 tma_load_2d(w_base + tap * W_TAP_BYTES, &map_w, weight_bar(bars), 0, tap * (int)gridDim.y * 64 + ct * 64);
         }
-        for_each_tile(k, 2, ptiles, [&](int t) {
+        produce_tiles(tiles, [&](int t) {
             const Tile c = tile_of(p, t);
             for (int u = 0; u < UNITS; ++u) {
                 if (KIND == 0) {
@@ -147,7 +150,7 @@ conv_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     // ===================== consumer warpgroup k: wgmma + epilogue =====================
     const int w = warp & 3;
     if (KIND == 0) mbar_wait(weight_bar(bars), 0);
-    for_each_tile(k, 2, ptiles, [&](int t) {
+    consume_tiles(tiles, [&](int t) {
         const Tile c = tile_of(p, t);
         prefetch_residual<HV>(p, c, ct, w);
         float acc[2][32];                                 // the two halves of the tile (HV)
@@ -209,8 +212,8 @@ struct Params1 {
 // each tile t (pixel tile t / nch) stages its kunits K chunks of 64 pixels, in KIND 2 with their lo plane.
 template <int KIND>
 __device__ __forceinline__ void produce_1x1(Ring &ring, const CUtensorMap *map_x, const CUtensorMap *map_w,
-                                            uint32_t w_base, uint32_t wbar, int k, int kunits, int npad, int nch,
-                                            int lo_ch, int n_tiles) {
+                                            TileQueue &tiles, uint32_t w_base, uint32_t wbar, int k, int kunits,
+                                            int npad, int nch, int lo_ch) {
     constexpr int PLANES = (KIND == 2) ? 2 : 1;
     constexpr int CH = (KIND == 0) ? 32 : 64;           // channels per K chunk
     if (k == 0) {
@@ -218,7 +221,7 @@ __device__ __forceinline__ void produce_1x1(Ring &ring, const CUtensorMap *map_x
         for (int kc = 0; kc < PLANES * kunits; ++kc)
             tma_load_2d(w_base + kc * npad * 128, map_w, wbar, 0, kc * npad);
     }
-    for_each_tile(k, 2, n_tiles, [&](int t) {
+    produce_tiles(tiles, [&](int t) {
         const int pt = t / nch;
         for (int u = 0; u < kunits; ++u) {
             const Slot s = ring.acquire(PLANES * K1_A_BYTES);
@@ -278,7 +281,8 @@ __device__ __forceinline__ void mma_1x1(Ring &ring, float (&acc)[NB][32], float 
 template <int KIND, int NB>
 __global__ void __launch_bounds__(THREADS, 1)
 conv1x1_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
-                  const Params1 p, const int n_stages, const int n_tiles) {
+                  const Params1 p, const int n_stages, const int n_tiles, const TileSchedule ts) {
+    L3C_TRACE_BEGIN;
     constexpr int PLANES = (KIND == 2) ? 2 : 1;
     const int w_plane = p.kunits * p.npad * 128;
     // [weights (hi plane, lo plane)][pipe 0 stages][pipe 1 stages][barriers]
@@ -290,10 +294,11 @@ conv1x1_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
     const int lane = threadIdx.x & 31;
     const int k = warp < CONSUMER_WARPS ? warp >> 2 : warp - CONSUMER_WARPS;   // pipe
     Ring ring(w_base + PLANES * w_plane, PLANES * K1_A_BYTES, n_stages, bars, k);
+    TileQueue tiles(bars, k, 2, n_tiles, ts);
 
     if (warp >= CONSUMER_WARPS) {
         if (lane == 0)
-            produce_1x1<KIND>(ring, &map_x, &map_w, w_base, weight_bar(bars), k, p.kunits, p.npad, p.nch, p.lo_ch, n_tiles);
+            produce_1x1<KIND>(ring, &map_x, &map_w, tiles, w_base, weight_bar(bars), k, p.kunits, p.npad, p.nch, p.lo_ch);
         return;
     }
 
@@ -303,7 +308,7 @@ conv1x1_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
     const bool relu = (p.flags & L3C_CONV_RELU) != 0;
     const bool round_y = (p.flags & L3C_CONV_ROUND_TF32) != 0;
     mbar_wait(weight_bar(bars), 0);
-    for_each_tile(k, 2, n_tiles, [&](int t) {
+    consume_tiles(tiles, [&](int t) {
         const int pt = t / p.nch, nc = t % p.nch;
         float acc[NB][32], acc2[NB][32];          // acc2: KIND 2 only
         mma_1x1<KIND, NB>(ring, acc, acc2, w_base, w_plane, p.kunits, p.npad, nc);
@@ -376,7 +381,8 @@ struct ParamsLD {
 template <int C, bool RGB, int NB>
 __global__ void __launch_bounds__(THREADS, 1)
 lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
-                    const ParamsLD p, const int n_stages, const int n_tiles) {
+                    const ParamsLD p, const int n_stages, const int n_tiles, const TileSchedule ts) {
+    L3C_TRACE_BEGIN;
     constexpr int K = 10;
     constexpr int KP = (RGB ? 4 : 3) * C * K;            // parameters per pixel (the bias has KP entries)
     constexpr int NPAD = NB * 64, S = NPAD + 1;         // staging row pitch (floats): conflict-free column reads
@@ -392,9 +398,10 @@ lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     const int lane = threadIdx.x & 31;
     const int k = warp < CONSUMER_WARPS ? warp >> 2 : warp - CONSUMER_WARPS;   // pipe
     Ring ring(w_base + w_bytes, K1_A_BYTES, n_stages, bars, k);
+    TileQueue tiles(bars, k, 2, n_tiles, ts);
 
     if (warp >= CONSUMER_WARPS) {
-        if (lane == 0) produce_1x1<1>(ring, &map_x, &map_w, w_base, weight_bar(bars), k, p.kchunks, NPAD, 1, 0, n_tiles);
+        if (lane == 0) produce_1x1<1>(ring, &map_x, &map_w, tiles, w_base, weight_bar(bars), k, p.kchunks, NPAD, 1, 0);
         return;
     }
 
@@ -404,7 +411,7 @@ lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     const int tq = lane & 3, tr = lane >> 2;
     const float scale = (float)(65536 - p.L);            // 2^16 - (Lp - 1)
     mbar_wait(weight_bar(bars), 0);
-    for_each_tile(k, 2, n_tiles, [&](int t) {
+    consume_tiles(tiles, [&](int t) {
         float acc[NB][32];
         mma_1x1<1, NB>(ring, acc, acc, w_base, 0, p.kchunks, NPAD, 0);     // acc2 is not used by KIND 1
         // accumulators (+ bias, the same add as the plain kernel's epilogue) -> staging [pixel][channel]

@@ -26,7 +26,9 @@ constexpr int W_PLANE_BYTES = 9 * W_TAP_BYTES;        // 73728 per plane (hi / l
 
 __global__ void __launch_bounds__(THREADS, 1)
 conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
-                     const Params p, const int n_pipes, const int a_bytes, const int ptiles) {
+                     const Params p, const int n_pipes, const int a_bytes, const int ptiles,
+                     const TileSchedule ts) {
+    L3C_TRACE_BEGIN;
     // [weights hi 72 KB][weights lo 72 KB][pipe 0: hi box, lo box][pipe 1: ...][barriers]
     const uint32_t w_base = smem_u32(smem_aligned());
     const uint32_t bars = w_base + 2 * W_PLANE_BYTES + n_pipes * 2 * a_bytes;
@@ -40,6 +42,7 @@ conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
     const int ct = blockIdx.y;
     const int lo_ch = 64;                                  // lo plane of a 64-channel operand image
     Ring ring(w_base + 2 * W_PLANE_BYTES, 2 * a_bytes, 1, bars, k);   // one stage (hi and lo box) per pipe
+    TileQueue tiles(bars, k, n_pipes, ptiles, ts);
 
     if (warp >= CONSUMER_WARPS) {
         // ===================== TMA producer of pipe k =====================
@@ -52,7 +55,7 @@ conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
                 tma_load_2d(w_base + W_PLANE_BYTES + tap * W_TAP_BYTES, &map_w, weight_bar(bars), 64, row);     // lo
             }
         }
-        for_each_tile(k, n_pipes, ptiles, [&](int t) {
+        produce_tiles(tiles, [&](int t) {
             const Tile c = tile_of(p, t);
             for (int dx = 0; dx < 3; ++dx) {
                 const Slot s = ring.acquire(2 * a_bytes);
@@ -66,7 +69,7 @@ conv3x3_f16x2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
     // ===================== consumer warpgroup k: wgmma + epilogue =====================
     const int w = warp & 3;
     mbar_wait(weight_bar(bars), 0);
-    for_each_tile(k, n_pipes, ptiles, [&](int t) {
+    consume_tiles(tiles, [&](int t) {
         const Tile c = tile_of(p, t);
         float acc1[2][32], acc2[2][32];                   // hi*hi | hi*lo + lo*hi; rows 0..63 / 64..127
 #pragma unroll

@@ -35,7 +35,9 @@ constexpr int W_RES_BYTES = 9 * 2 * B_HALF;    // 147456
 
 __global__ void __launch_bounds__(THREADS, 1)
 conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
-                    const Params p, const int n_pipes, const int n_stages, const int a_bytes, const int ptiles) {
+                    const Params p, const int n_pipes, const int n_stages, const int a_bytes, const int ptiles,
+                    const TileSchedule ts) {
+    L3C_TRACE_BEGIN;
     // [weights 144 KB][pipe 0 stages][pipe 1 stages][barriers]
     const uint32_t w_base = smem_u32(smem_aligned());
     const uint32_t bars = w_base + W_RES_BYTES + n_pipes * n_stages * a_bytes;
@@ -48,6 +50,7 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     const int d = p.dilation;
     const int ct = blockIdx.y;                        // this CTA's Cout tile (weights stay resident)
     Ring ring(w_base + W_RES_BYTES, a_bytes, n_stages, bars, k);
+    TileQueue tiles(bars, k, n_pipes, ptiles, ts);
 
     if (warp >= CONSUMER_WARPS) {
         // ===================== TMA producer of pipe k =====================
@@ -57,7 +60,7 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
             for (int slab = 0; slab < 18; ++slab)     // slab = tap*2 + K-half; rows [slab][cout_pad]
                 tma_load_2d(w_base + slab * B_HALF, &map_w, weight_bar(bars), 0, slab * (int)gridDim.y * 64 + ct * 64);
         }
-        for_each_tile(k, n_pipes, ptiles, [&](int t) {
+        produce_tiles(tiles, [&](int t) {
             const Tile c = tile_of(p, t);
             for (int unit = 0; unit < 6; ++unit) {    // unit = dx*2 + K-half
                 const Slot s = ring.acquire(a_bytes);
@@ -74,7 +77,7 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     const bool shuffle = (p.flags & L3C_CONV_PIXEL_SHUFFLE2) != 0;
     const bool round_y = (p.flags & L3C_CONV_ROUND_TF32) != 0;
     mbar_wait(weight_bar(bars), 0);
-    for_each_tile(k, n_pipes, ptiles, [&](int t) {
+    consume_tiles(tiles, [&](int t) {
         const Tile c = tile_of(p, t);
         float acc[2][32];                                 // rows 0..63 / 64..127 of the tile
         acc_zero(acc[0]);

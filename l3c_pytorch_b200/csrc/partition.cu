@@ -9,7 +9,10 @@
 #include <cuda.h>
 
 #include <atomic>
+#include <map>
 #include <mutex>
+#include <thread>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -97,7 +100,74 @@ int stream_sm_count(cudaStream_t st) {
 
 int conv_smem_kb_override() { return g_conv_smem_kb.load(std::memory_order_relaxed); }
 
+namespace {
+std::atomic<int> g_tile_schedule{0};
+
+// Tile counters of the persistent tensor-core kernels: a slot of TILE_COUNTERS per (device, stream), so that two
+// launches that can run at the same time never share one.  Launches on one stream run one after the other, and
+// each launch's last claim leaves its counters at zero for the next.  Slots come from chunks of device memory
+// zeroed once when the chunk is made; word 0 of a device's first chunk is its idle-CTA count.
+constexpr int SLOTS_PER_CHUNK = 256;
+struct CounterPool {
+    std::vector<unsigned *> chunks;
+    int used = 1;                                   // slot 0 of chunk 0: the idle-CTA count
+    std::map<std::pair<cudaStream_t, std::thread::id>, unsigned *> slot_of;
+};
+CounterPool g_pools[64];
+std::mutex g_pool_mu;
+}  // namespace
+
+int conv_tile_schedule() { return g_tile_schedule.load(std::memory_order_relaxed); }
+
+int tile_counters(cudaStream_t st, int n, unsigned **counters, unsigned long long **idle_ctas) {
+    L3C_REQUIRE(n >= 1 && n <= TILE_COUNTERS, "persistent tensor-core conv: %d Cout tiles (at most %d are built)", n,
+                TILE_COUNTERS);
+    const int dev = current_device_slot();
+    std::lock_guard<std::mutex> lock(g_pool_mu);
+    CounterPool &pool = g_pools[dev];
+    // the per-thread default stream is one stream per host thread under one handle
+    const auto key = std::make_pair(st, st == cudaStreamPerThread ? std::this_thread::get_id() : std::thread::id());
+    auto it = pool.slot_of.find(key);
+    if (it == pool.slot_of.end()) {
+        if (pool.chunks.empty() || pool.used == SLOTS_PER_CHUNK) {
+            const size_t bytes = (size_t)SLOTS_PER_CHUNK * TILE_COUNTERS * sizeof(unsigned);
+            unsigned *chunk = nullptr;
+            L3C_CUDA(cudaMalloc(&chunk, bytes));
+            // zeroed before any kernel can use it: a one-time synchronous set
+            L3C_CUDA(cudaMemset(chunk, 0, bytes));
+            L3C_CUDA(cudaStreamSynchronize(0));
+            pool.used = pool.chunks.empty() ? 1 : 0;
+            pool.chunks.push_back(chunk);
+        }
+        it = pool.slot_of.emplace(key, pool.chunks.back() + (size_t)pool.used++ * TILE_COUNTERS).first;
+    }
+    *counters = it->second;
+    *idle_ctas = reinterpret_cast<unsigned long long *>(pool.chunks[0]);
+    return L3C_OK;
+}
+
 }  // namespace l3c
+
+extern "C" int l3c_set_conv_tile_schedule(int mode) {
+    L3C_REQUIRE(mode >= 0 && mode <= 2, "l3c_set_conv_tile_schedule: mode %d (0: dynamic, 1: static, 2: skewed)", mode);
+    l3c::g_tile_schedule.store(mode);
+    return L3C_OK;
+}
+
+extern "C" int l3c_conv_idle_ctas(long long *count, int reset) {
+    using namespace l3c;
+    L3C_REQUIRE(count, "l3c_conv_idle_ctas: null pointer");
+    unsigned *counters = nullptr;
+    unsigned long long *idle = nullptr;
+    if (int e = tile_counters(0, 1, &counters, &idle)) return e;
+    L3C_CUDA(cudaDeviceSynchronize());
+    unsigned long long v = 0;
+    L3C_CUDA(cudaMemcpy(&v, idle, sizeof(v), cudaMemcpyDeviceToHost));
+    if (reset) L3C_CUDA(cudaMemset(idle, 0, sizeof(v)));
+    if (reset) L3C_CUDA(cudaDeviceSynchronize());
+    *count = (long long)v;
+    return L3C_OK;
+}
 
 extern "C" int l3c_set_conv_launch_limits(int max_sms, int conv_smem_kb) {
     L3C_REQUIRE(max_sms >= 0 && conv_smem_kb >= 0, "l3c_set_conv_launch_limits: bad arguments (%d, %d)", max_sms,

@@ -4,7 +4,7 @@
 // planning, grid size).
 //
 // CTA layout: warps 0..7 are two consumer warpgroups ("pipes"), each with its own TMA producer warp (warps 8, 9),
-// its own ring of shared-memory stages and its own tiles (alternate tiles of the CTA's sequence).  A consumer
+// its own ring of shared-memory stages and its own tiles (claimed from the launch's tile queue).  A consumer
 // issues wgmma on the staged operands, keeps the fp32 accumulators in registers and runs the fused epilogue
 // itself, so the epilogue of one pipe overlaps the MMAs of the other.  Accumulator fragment of wgmma m64nNk*:
 // thread t of the warpgroup, warp w = t / 32, lane l holds
@@ -12,6 +12,11 @@
 //   d[4j + 2], d[4j + 3] = (row 16w + l/4 + 8, same columns)
 // Dynamic shared memory, from a 1024 B (swizzle atom) aligned start: [resident weights][pipe 0 stages]
 // [pipe 1 stages][buffers of the kernel's own][barriers].
+//
+// Tile walk: the producer of each pipe claims tiles from a per-launch counter (one per Cout tile, blockIdx.y) with
+// atomicAdd, one claim ahead, and hands each index to its consumer through a two-slot tile ring in shared memory
+// before it issues the tile's TMA; so a CTA that starts late, on an SM another kernel still holds, simply runs fewer
+// tiles.  Which CTA runs a tile does not change any output bit: each output's accumulation order is fixed per tile.
 #pragma once
 #include <initializer_list>
 
@@ -34,19 +39,37 @@ __device__ __forceinline__ uint8_t *smem_aligned() {
     return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
 }
 
-// barriers at `bars`: full[MAX_STAGES], empty[MAX_STAGES] of pipe 0, the same of pipe 1, then the weight barrier
+// barriers at `bars` (SMEM_RESERVE keeps 512 B for them): full[MAX_STAGES], empty[MAX_STAGES] of pipe 0, the same
+// of pipe 1, then the weight barrier; from +256 the tile ring of pipe k (tile_ring()): full[TQ_SLOTS],
+// empty[TQ_SLOTS] at +256 + 32k, its index slots at +320 + 8k; at +336 the count of idle pipes (schedule mode 2).
+constexpr int TQ_SLOTS = 2;
 __device__ __forceinline__ uint32_t weight_bar(uint32_t bars) { return bars + 8u * (4 * MAX_STAGES); }
+__device__ __forceinline__ uint32_t tile_ring(uint32_t bars, int k) { return bars + 256u + 32u * k; }
+__device__ __forceinline__ uint32_t tile_slots(uint32_t bars, int k) { return bars + 320u + 8u * k; }
+__device__ __forceinline__ uint32_t idle_pipes(uint32_t bars) { return bars + 336u; }
 
-// Thread 0 initialises the barriers (full: the producer's expect_tx; empty: one arrival per consumer warp) and
-// prefetches both tensor maps; then the whole CTA syncs.
+__device__ __forceinline__ uint64_t globaltimer() {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// Thread 0 initialises the barriers (full: the producer's expect_tx or tile index; empty: one arrival per consumer
+// warp) and prefetches both tensor maps; then the whole CTA syncs.
 __device__ __forceinline__ void pipeline_init(uint32_t bars, const CUtensorMap *map_x, const CUtensorMap *map_w) {
     if (threadIdx.x == 0) {
-        for (int k = 0; k < 2; ++k)
+        for (int k = 0; k < 2; ++k) {
             for (int s = 0; s < MAX_STAGES; ++s) {
                 mbar_init(bars + 8u * (2 * MAX_STAGES * k + s), 1);
                 mbar_init(bars + 8u * (2 * MAX_STAGES * k + MAX_STAGES + s), 4);
             }
+            for (int s = 0; s < TQ_SLOTS; ++s) {
+                mbar_init(tile_ring(bars, k) + 8u * s, 1);
+                mbar_init(tile_ring(bars, k) + 8u * (TQ_SLOTS + s), 4);
+            }
+        }
         mbar_init(weight_bar(bars), 1);
+        asm volatile("st.shared.u32 [%0], 0;" ::"r"(idle_pipes(bars)) : "memory");
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(map_x) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(map_w) : "memory");
@@ -91,11 +114,129 @@ struct Ring {
     }
 };
 
-// The tiles pipe k of this CTA runs: from blockIdx.x + k * gridDim.x in steps of n_pipes * gridDim.x, so that the
-// pipes of a CTA take alternate tiles of the CTA's sequence.
+// How the tiles of a launch are handed out (l3c_set_conv_tile_schedule)
+struct TileSchedule {
+    unsigned *counters;             // one per Cout tile (blockIdx.y), zero when the launch starts (modes 0, 2)
+    unsigned long long *idle_ctas;  // mode 2: CTAs that ran no tile are counted here
+    int mode;                       // 0: dynamic, 1: static stripe, 2: dynamic, odd CTAs start SKEW_NS late
+#ifdef L3C_CTA_TRACE
+    CtaTraceArg trace;              // where this launch's CTAs record themselves
+#endif
+};
+constexpr uint64_t SKEW_NS = 500000;
+
+#ifdef L3C_CTA_TRACE
+// Diagnosis builds only (build.py --cta-trace): every CTA writes one l3c_cta_record_t (tools/cta_timeline.py).
+// Thread 0 writes the start at the first instruction, pipeline_init's sync orders it before the consumers add
+// their tile counts, and the latest warp to leave sets t_end.
+__device__ __forceinline__ l3c_cta_record_t *trace_record(const TileSchedule &s) {
+    return s.trace.rec ? s.trace.rec + blockIdx.y * gridDim.x + blockIdx.x : nullptr;
+}
+struct CtaTrace {
+    l3c_cta_record_t *r;
+    __device__ explicit CtaTrace(const TileSchedule &s) : r(trace_record(s)) {
+        if (threadIdx.x != 0 || !r) return;
+        uint32_t smid;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        r->t_start = globaltimer();
+        r->t_end = 0;
+        r->smid = smid;
+        r->tiles = 0;
+        r->launch = (uint32_t)s.trace.launch;
+        r->cta = blockIdx.y * gridDim.x + blockIdx.x;
+    }
+    __device__ ~CtaTrace() {
+        if (r && (threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned long long *>(&r->t_end), globaltimer());
+    }
+};
+#define L3C_TRACE_BEGIN const ::l3c::tcx::CtaTrace cta_trace_(ts)
+#else
+#define L3C_TRACE_BEGIN
+#endif
+
+// The tile walk of pipe k (n_pipes pipes per CTA, n_tiles tiles per Cout tile).  Producer and consumer each keep
+// their own copy, as with Ring.
+//   producer: first(), then claim() right after a tile's TMA is issued, so the atomic's latency overlaps the
+//             stage wait; publish() hands each claimed index, and at the end -1, to the consumer before the tile's
+//             TMA, so the consumer can prefetch the tile's residual while its stage is in flight.
+//   consumer: take() returns the next index or -1.
+// The claims of a launch on one counter number n_tiles + (its pipes): every pipe ends with exactly one failed
+// claim, and the last claim of all resets the counter for the next launch on the stream.
+struct TileQueue {
+    uint32_t ring, slots, idle, pos, phase;
+    int n_tiles, n_claimers, n_pipes, next, taken;
+    TileSchedule s;
+
+    __device__ __forceinline__ TileQueue(uint32_t bars, int k, int n_pipes_, int n_tiles_, const TileSchedule &s_)
+        : ring(tile_ring(bars, k)), slots(tile_slots(bars, k)), idle(idle_pipes(bars)), pos(0), phase(0),
+          n_tiles(n_tiles_), n_claimers(n_pipes_ * (int)gridDim.x), n_pipes(n_pipes_),
+          next(blockIdx.x + k * gridDim.x), taken(0), s(s_) {}
+
+    __device__ __forceinline__ void advance() {
+        if (++pos == TQ_SLOTS) { pos = 0; phase ^= 1u; }
+    }
+    __device__ __forceinline__ int claim() {
+        if (s.mode == 1) {                       // static stripe: pipes of a CTA take alternate tiles of its sequence
+            const int t = next;
+            next += n_claimers;
+            return t < n_tiles ? t : -1;
+        }
+        unsigned *c = s.counters + blockIdx.y;
+        const unsigned v = atomicAdd(c, 1u);
+        if (v == (unsigned)(n_tiles + n_claimers - 1)) atomicExch(c, 0u);
+        return v < (unsigned)n_tiles ? (int)v : -1;
+    }
+    __device__ __forceinline__ int first() {
+        if (s.mode == 2 && (blockIdx.x & 1)) {
+            const uint64_t t0 = globaltimer();
+            while (globaltimer() - t0 < SKEW_NS) __nanosleep(1000);
+        }
+        return claim();
+    }
+    __device__ __forceinline__ void publish(int t) {
+        mbar_wait(ring + 8u * (TQ_SLOTS + pos), phase ^ 1u);
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(slots + 4u * pos), "r"(t) : "memory");
+        mbar_arrive(ring + 8u * pos);
+        advance();
+    }
+    __device__ __forceinline__ int take() {
+        mbar_wait(ring + 8u * pos, phase);
+        int t;
+        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(t) : "r"(slots + 4u * pos) : "memory");
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(ring + 8u * (TQ_SLOTS + pos));
+        advance();
+        const bool leader = (threadIdx.x & 127) == 0;
+        if (t >= 0) {
+            ++taken;
+            return t;
+        }
+#ifdef L3C_CTA_TRACE
+        if (leader && trace_record(s)) atomicAdd(&trace_record(s)->tiles, (unsigned)taken);
+#endif
+        if (s.mode == 2 && taken == 0 && leader) {
+            // idle pipes count themselves; the CTA is idle when all n_pipes of them did
+            uint32_t before;
+            asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(before) : "r"(idle) : "memory");
+            if ((int)before == n_pipes - 1) atomicAdd(s.idle_ctas, 1ull);
+        }
+        return t;
+    }
+};
+
+// producer: claim tiles, publish each and then the end, call f(t) to issue tile t's TMA
 template <class F>
-__device__ __forceinline__ void for_each_tile(int k, int n_pipes, int n_tiles, F &&f) {
-    for (int t = blockIdx.x + k * gridDim.x; t < n_tiles; t += n_pipes * gridDim.x) f(t);
+__device__ __forceinline__ void produce_tiles(TileQueue &q, F &&f) {
+    for (int t = q.first();; t = q.claim()) {
+        q.publish(t);
+        if (t < 0) return;
+        f(t);
+    }
+}
+// consumer: f(t) for every tile the producer publishes
+template <class F>
+__device__ __forceinline__ void consume_tiles(TileQueue &q, F &&f) {
+    for (int t = q.take(); t >= 0; t = q.take()) f(t);
 }
 
 // 3x3 / 5x5 layers (conv3x3_tf32_kernel, conv_f16_kernel, conv3x3_f16x2_kernel)
@@ -370,8 +511,9 @@ static inline int grid_1x1(cudaStream_t st, int n_tiles) {
     return ceil_div(n_tiles, 2) < n_sm ? ceil_div(n_tiles, 2) : n_sm;
 }
 
-// Launches a persistent tensor-core kernel under `name` (the launch log).  The opt-in to SMEM_MAX bytes of
-// dynamic shared memory is per device, so it is done once per device and kernel.
+// Launches a persistent tensor-core kernel under `name` (the launch log), its tile schedule (the stream's tile
+// counters) as the last argument.  The opt-in to SMEM_MAX bytes of dynamic shared memory is per device, so it is
+// done once per device and kernel.
 template <auto Kernel, class... Args>
 int launch_tc(const char *name, dim3 grid, int smem_bytes, cudaStream_t st, const Args &...args) {
     static bool configured_dev[64] = {};
@@ -380,7 +522,13 @@ int launch_tc(const char *name, dim3 grid, int smem_bytes, cudaStream_t st, cons
         L3C_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
         configured = true;
     }
-    Kernel<<<grid, THREADS, smem_bytes, st>>>(args...);
+    TileSchedule ts;
+    ts.mode = conv_tile_schedule();
+    if (int e = tile_counters(st, (int)grid.y, &ts.counters, &ts.idle_ctas)) return e;
+#ifdef L3C_CTA_TRACE
+    ts.trace = cta_trace_launch(name, grid, st);
+#endif
+    Kernel<<<grid, THREADS, smem_bytes, st>>>(args..., ts);
     L3C_LAUNCH_CHECK(name);
     return L3C_OK;
 }

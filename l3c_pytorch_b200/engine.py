@@ -109,6 +109,27 @@ def conv_launch_limits(max_sms=0, conv_smem_kb=0):
 
 
 @contextlib.contextmanager
+def conv_tile_schedule(mode):
+    """Test and diagnosis knob (l3c_set_conv_tile_schedule): inside the block the persistent tensor-core
+    convolutions hand out their tiles with schedule `mode`: 0 dynamic (the default), 1 the static stripe, 2 dynamic
+    with odd CTAs starting 500 us late.  Every mode gives the same bits.  Process-wide; the default is restored on
+    exit."""
+    check(lib.l3c_set_conv_tile_schedule(int(mode)))
+    try:
+        yield
+    finally:
+        check(lib.l3c_set_conv_tile_schedule(0))
+
+
+def conv_idle_ctas(reset=False):
+    """l3c_conv_idle_ctas: CTAs of the current device that ran no tile under schedule 2 since the last reset
+    (waits for the device)."""
+    n = ctypes.c_longlong(0)
+    check(lib.l3c_conv_idle_ctas(ctypes.byref(n), int(bool(reset))))
+    return n.value
+
+
+@contextlib.contextmanager
 def decoder_streams_per_cta(spc):
     """Test knob (l3c_set_decoder_streams_per_cta): inside the block the range decoder of alphabets L > 32 packs `spc`
     streams (1, 2 or 4) into one CTA; 0 = the L3C_DEC_SPC / default choice.  Process-wide; the default is restored on
