@@ -59,17 +59,27 @@ def _groups(keys):
 
 
 class Bitcoding(object):
-    def __init__(self, blueprint, times=NoOp, compare_with_theory=False, tile=None):
+    def __init__(self, blueprint, times=NoOp, compare_with_theory=False, tile=None, recursive=0):
         """tile = (th, tw): write TILED containers (codec.ContainerLayout): every channel plane of every scale is
         cut into tiles coded as independent streams -- thousands of streams per batch instead of 18 per image,
         so encode and decode are no longer bound by one warp's serial chain.  Not readable by the reference and a
         few bytes per tile larger; decode() / decode_batch() recognise either layout.  Default: the reference's
-        byte-compatible `.l3c` layout."""
+        byte-compatible `.l3c` layout.
+        recursive = R > 0 (RGB baselines only): write RECURSIVE containers (DESIGN §4.7): the last trained scale
+        codes its own bicubic thumbnails R more times and only the 1 / 2**(num_scales + R) thumbnail is left for
+        the uniform prior; images are padded to multiples of 2**(num_scales + R).  Not readable by the reference;
+        decode() / decode_batch() read R from the file.  ValueError for anything but a non-negative int, and for
+        R > 0 on an L3C model."""
         self.blueprint = blueprint
         self.compare_with_theory = compare_with_theory
         self.times = times
         self.tile = tile
         self.codec = BatchCodec(blueprint)
+        self.recursive = self.codec.check_recursive(recursive)
+
+    def pad_factor(self):
+        """Images are padded to multiples of this: 2**(num_scales + R)."""
+        return 2 ** (self.blueprint.net.config_ms.num_scales + self.recursive)
 
     # ------------------------------------------------------------------------------------------
     def _device(self):
@@ -77,7 +87,7 @@ class Bitcoding(object):
 
     def _prepare(self, img, quiet=False):
         """-> (uint8 [1,3,H',W'] padded, on device; padding tuple)."""
-        factor = 2 ** self.blueprint.net.config_ms.num_scales
+        factor = self.pad_factor()
         if img.dim() == 3:
             img = img.unsqueeze(0)
         _, _, H, W = img.shape
@@ -104,12 +114,12 @@ class Bitcoding(object):
         if all(sh == shapes[0] for sh in shapes):
             batch = torch.cat(imgs, 0) if len(imgs) > 1 else imgs[0]
             pt = pts[0] if all(p == pts[0] for p in pts) else pts
-            return self.codec.encode_begin(batch, pt, tile=self.tile)
+            return self.codec.encode_begin(batch, pt, tile=self.tile, recursive=self.recursive)
         Hb, Wb = max(h for (h, _) in shapes), max(w for (_, w) in shapes)
         batch = torch.zeros(len(imgs), 3, Hb, Wb, dtype=torch.uint8, device=self._device())
         for k, t in enumerate(imgs):
             batch[k, :, :t.shape[2], :t.shape[3]] = t[0]
-        return self.codec.encode_begin(batch, pts, tile=self.tile, extents=shapes)
+        return self.codec.encode_begin(batch, pts, tile=self.tile, extents=shapes, recursive=self.recursive)
 
     def encode(self, img, pout):
         """img: int64 (or uint8) CHW / 1CHW tensor with values 0..255; writes `pout`; returns bpsp."""
@@ -153,13 +163,13 @@ class Bitcoding(object):
             with self.times.run('[-] encode forwardpass'):
                 # without --compare_theory nobody reads the parameter tensors: the probability heads emit the
                 # coding intervals directly (f16 mode; MultiscaleNetwork.forward(intervals_of=...))
-                out = self.blueprint.forward(batch) if self.compare_with_theory else \
-                    self.blueprint.forward_for_coding(batch)
+                out = self.blueprint.forward(batch, self.recursive) if self.compare_with_theory else \
+                    self.blueprint.forward_for_coding(batch, self.recursive)
             if self.compare_with_theory:
                 with self.times.run('[-] get loss'):
                     loss_out = self.blueprint.get_loss(out)
             with self.times.run('[-] entropy coding'):
-                datas, info = self.codec.encode_batch(batch, pt, out=out, tile=self.tile)
+                datas, info = self.codec.encode_batch(batch, pt, out=out, tile=self.tile, recursive=self.recursive)
             num_subpixels = int(np.prod(batch.shape[1:]))
             for k, i in enumerate(idxs):
                 with open(pouts[i], 'wb') as f:
@@ -167,7 +177,8 @@ class Bitcoding(object):
                 bpsps[i] = len(datas[k]) * 8 / num_subpixels
             if self.compare_with_theory:
                 total = sum(len(d) for d in datas) * 8 / (num_subpixels * len(idxs))
-                theory = loss_out.nonrecursive_bpsps
+                # recursive containers code every scale of recursive_bpsps (the last one under the uniform prior)
+                theory = loss_out.recursive_bpsps if self.recursive else loss_out.nonrecursive_bpsps
                 print('Bitrates:\ntheory:  {} => {:.3f}\nactual:  => {:.3f}'.format(
                     ' | '.join('{:.3f}'.format(b) for b in theory), sum(theory), total))
         return bpsps
@@ -218,15 +229,14 @@ class Bitcoding(object):
                 if why is not None and len({tuple(t.shape) for (t, _) in prepared}) > 1:
                     raise NotImplementedError(why)
                 return self._encode_prepared(prepared)
-        factor = 2 ** self.blueprint.net.config_ms.num_scales
-        pt = pad.padding_tuple(imgs_u8.shape[-2], imgs_u8.shape[-1], factor)
+        pt = pad.padding_tuple(imgs_u8.shape[-2], imgs_u8.shape[-1], self.pad_factor())
         stream = stream if stream is not None else torch.cuda.current_stream(self._device())
         with torch.cuda.stream(stream):
             x = imgs_u8.to(self._device(), non_blocking=True)
             if any(pt):
                 x = torch.nn.functional.pad(x, pt, 'constant')
             x = x.contiguous()
-            job = self.codec.encode_begin(x, pt, tile=self.tile)
+            job = self.codec.encode_begin(x, pt, tile=self.tile, recursive=self.recursive)
         N = x.shape[0]
         return _ListEncodeJob([(list(range(N)), job)], [int(np.prod(x.shape[1:]))] * N)
 

@@ -38,13 +38,14 @@ class MultiscaleBlueprint(nn.Module):
         with torch.cuda.device(self.device):          # kernels launch on the CURRENT device
             return self.net(in_batch, auto_recurse, extents=extents)
 
-    def forward_for_coding(self, in_batch) -> Out:
+    def forward_for_coding(self, in_batch, auto_recurse=0) -> Out:
         """forward() for the bit-coder: in f16 mode the DMLL head is fused into the 1x1 convs of the probability
-        classifiers and `Out.IV` holds the coding intervals instead of `Out.P` the parameters."""
+        classifiers and `Out.IV` holds the coding intervals instead of `Out.P` the parameters (recursive scales
+        included)."""
         if self.device.type != 'cuda':
-            return self.net(in_batch, intervals_of=self.losses)
+            return self.net(in_batch, auto_recurse, intervals_of=self.losses)
         with torch.cuda.device(self.device):
-            return self.net(in_batch, intervals_of=self.losses)
+            return self.net(in_batch, auto_recurse, intervals_of=self.losses)
 
     def get_loss(self, out: Out, num_subpixels_before_pad=None) -> MultiscaleLoss:
         """Theoretical bpsp per scale, incl. the uniform-prior final scale

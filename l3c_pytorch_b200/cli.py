@@ -3,6 +3,7 @@
 
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt enc IMG OUT.l3c [--overwrite]
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png
+    python -m l3c_pytorch_b200.cli --config cr_rgb_shared --ckpt CKPT.pt enc IMG OUT.l3c --recursive auto
 
 `--ckpt` is a checkpoint as written by the reference's Saver (`torch.save({'net': state_dict})`,
 helpers/saver.py:168); the module tree here has the same parameter names, so it loads strict.
@@ -83,7 +84,13 @@ def decode(bc, pin, png_out):
     print('Decoded {} -> {}'.format(pin, png_out))
 
 
-def main(argv=None):
+def recursive_of(args, config_ms):
+    """R of `enc --recursive N|auto` (harness.parse_recursive_flag: 0 for L3C configs); 0 for `dec`."""
+    from .harness import parse_recursive_flag
+    return parse_recursive_flag(getattr(args, 'recursive', '0'), config_ms) if args.mode == 'enc' else 0
+
+
+def build_parser():
     p = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     p.add_argument('--config', default='cr', help='cr | cr_rgb_shared | cr_rgb or a path to a .cf file')
     p.add_argument('--ckpt', default=None, help="checkpoint with {'net': state_dict}")
@@ -94,12 +101,20 @@ def main(argv=None):
     e.add_argument('img')
     e.add_argument('out')
     e.add_argument('--overwrite', action='store_true')
+    e.add_argument('--recursive', default='0', metavar='N|auto',
+                   help='RGB baselines: code the last scale N more times on its own thumbnails (auto: 3 for '
+                        'cr_rgb_shared); a recursive file, not readable by the reference.  Ignored for L3C.')
     d = sub.add_parser('dec')
     d.add_argument('inp')
     d.add_argument('out_png')
-    a = p.parse_args(argv)
+    return p
+
+
+def main(argv=None):
+    a = build_parser().parse_args(argv)
     from .bitcoding import Bitcoding
-    bc = Bitcoding(load_blueprint(a.config, a.ckpt, a.precision))
+    bp = load_blueprint(a.config, a.ckpt, a.precision)
+    bc = Bitcoding(bp, recursive=recursive_of(a, bp.net.config_ms))      # dec: R is read from the file
     try:
         if a.mode == 'enc':
             encode(bc, a.img, a.out, a.overwrite)

@@ -273,12 +273,25 @@ class BatchCodec(object):
         self._const = {}
 
     # ------------------------------------------------------------------------------------------
-    def iter_scale_dmll(self):
-        """coarse -> fine: (scale, dmll, uniform) -- bitcoding.py:163-169."""
+    def iter_scale_dmll(self, recursive=0):
+        """coarse -> fine: (scale, dmll, uniform) -- bitcoding.py:163-169.  recursive = R: a recursive container
+        (DESIGN §4.7) with R more scales num_scales .. num_scales + R - 1 between the trained ones and the
+        uniform-prior thumbnail (scale num_scales + R)."""
         losses = self.blueprint.losses
-        for scale in reversed(range(self.net.scales + 1)):
-            yield (scale, losses.loss_dmol_rgb if scale == 0 else losses.loss_dmol_n,
-                   scale == self.net.scales)
+        n = self.net.scales + recursive
+        for scale in reversed(range(n + 1)):
+            yield (scale, losses.loss_dmol_rgb if scale == 0 else losses.loss_dmol_n, scale == n)
+
+    def check_recursive(self, recursive):
+        """-> R as an int: the number of extra applications of the last trained scale (a recursive container,
+        DESIGN §4.7).  ValueError unless it is a non-negative int, and for R > 0 on a model that is not an RGB
+        baseline: the learned bottlenecks of L3C are not images that its last scale could code again."""
+        if isinstance(recursive, bool) or not isinstance(recursive, (int, np.integer)) or recursive < 0:
+            raise ValueError('recursive must be a non-negative int, got %r' % (recursive,))
+        if recursive and not self.net._rgb:
+            raise ValueError('recursive=%d: only the RGB baselines code recursively (their scales are bicubic '
+                             'thumbnails); the L3C bottlenecks cannot be coded by the last scale again' % recursive)
+        return int(recursive)
 
     def _uniform(self, L, device):
         key = ('uniform', L, str(device))
@@ -302,14 +315,16 @@ class BatchCodec(object):
         return self.net.nets[0].enc._consts(device)[1]
 
     # ------------------------------------------------------------------------------------------
-    def encode_batch(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, to_host=True, tile=None, extents=None):
+    def encode_batch(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, to_host=True, tile=None, extents=None,
+                     recursive=0):
         """imgs_u8: uint8 [N,3,H,W] on the GPU, H and W multiples of 2**num_scales.  pad_tuple: the padding
         tuple written into every container, or a list of one per image.
         Returns a list of N container byte strings (or, with to_host=False, the device blob,
         per-image sizes and offsets, leaving the bytes in HBM).  `out`: a precomputed network Out.
         tile = (th, tw): tiled containers (ContainerLayout).
-        extents = [(h_n, w_n)]: a ragged batch (encode_begin)."""
-        return self.encode_begin(imgs_u8, pad_tuple, out, tile, extents).finish(to_host)
+        extents = [(h_n, w_n)]: a ragged batch (encode_begin).
+        recursive = R: recursive containers (encode_begin)."""
+        return self.encode_begin(imgs_u8, pad_tuple, out, tile, extents, recursive).finish(to_host)
 
     def ragged_unsupported(self, tile=None):
         """Why this codec cannot code a ragged batch (a message naming it), or None when it can."""
@@ -339,7 +354,7 @@ class BatchCodec(object):
         return ext
 
     @_on_device
-    def encode_begin(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, tile=None, extents=None):
+    def encode_begin(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, tile=None, extents=None, recursive=0):
         """First half of encode_batch: enqueues the whole GPU side of an encode (networks, intervals,
         the range-coder launch, the copy of the stream lengths to pinned memory) on the CURRENT stream
         and returns without waiting.  EncodeJob.finish() completes it.  Lets a caller overlap the
@@ -349,10 +364,18 @@ class BatchCodec(object):
         extents = [(h_n, w_n)]: a ragged batch (DESIGN §4.6): image n is the top-left h_n x w_n of imgs_u8[n]
         (zero elsewhere; multiples of 2**num_scales), and every container is byte-identical to the one of that
         image encoded on its own -- one network pass and one range-coder launch for the batch.  f16, learned
-        bottlenecks, reference layout only.  Extents that all equal the tensor are the equal-size call."""
+        bottlenecks, reference layout only.  Extents that all equal the tensor are the equal-size call.
+        recursive = R > 0 (RGB baselines, DESIGN §4.7): the last trained scale codes its own thumbnails R more
+        times (forward(auto_recurse=R)); H and W must be multiples of 2**(num_scales + R); every stream of the
+        batch is still coded in one range-coder launch.  `out`, if given, must come from forward(auto_recurse=R)."""
         assert imgs_u8.dtype == torch.uint8 and imgs_u8.dim() == 4 and imgs_u8.shape[1] == 3
+        recursive = self.check_recursive(recursive)
         dev = imgs_u8.device
         N, _, Hb, Wb = imgs_u8.shape
+        if recursive:
+            fac = 2 ** (self.net.scales + recursive)
+            if Hb % fac or Wb % fac:
+                raise ValueError('recursive=%d needs H and W divisible by %d, got %dx%d' % (recursive, fac, Hb, Wb))
         ext = self._ragged_extents(extents, N, Hb, Wb, tile)
         if len(pad_tuple) and isinstance(pad_tuple[0], (tuple, list)):
             pads = [tuple(int(v) for v in p) for p in pad_tuple]
@@ -364,11 +387,14 @@ class BatchCodec(object):
             tile = (int(tile[0]), int(tile[1]))
         if out is None:
             # f16 mode: DMLL head fused into the convs
-            out = self.net(imgs_u8, intervals_of=self.blueprint.losses, extents=ext)
+            out = self.net(imgs_u8, recursive, intervals_of=self.blueprint.losses, extents=ext)
+        elif recursive and len(out.S_u8) != self.net.scales + recursive + 1:
+            raise ValueError('the network output has %d scales, recursive=%d needs %d'
+                             % (len(out.S_u8), recursive, self.net.scales + recursive + 1))
 
         # ---- per-symbol intervals, scale by scale (coarse -> fine = container order), as stream planes
         shapes, shapes_of, ivs = [], [[] for _ in range(N)], []
-        for (scale, C, H, W), iv in self._scale_intervals(out, dev):
+        for (scale, C, H, W), iv in self._scale_intervals(out, dev, recursive):
             f = Hb // H
             es = [(H, W)] * N if ext is None else [(h // f, w // f) for (h, w) in ext]
             if ext is not None:
@@ -396,11 +422,11 @@ class BatchCodec(object):
         desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
         return EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, (imgs_u8, ivs, slots))
 
-    def _scale_intervals(self, out, dev):
+    def _scale_intervals(self, out, dev, recursive=0):
         """Coding intervals of every scale, coarse -> fine: [(shape (scale, C, H, W), int32 [N][C][H*W])]."""
         K = self.net.config_ms.prob.K
         res = []
-        for scale, dmll, uniform in self.iter_scale_dmll():
+        for scale, dmll, uniform in self.iter_scale_dmll(recursive):
             S = out.S_u8[scale]
             _, C, H, W = S.shape
             if uniform:
@@ -585,10 +611,11 @@ class BatchCodec(object):
             why = self.ragged_unsupported(tile)
             if why is not None:
                 raise NotImplementedError(why)
-        for sh in {tuple(sh): sh for sh in shapes_of}.values():               # every distinct shape list once
-            if len(sh) != self.net.scales + 1:
-                raise ValueError('container has %d scales, model expects %d' % (len(sh), self.net.scales + 1))
-            self._check_shapes(sh)
+        # every distinct shape list once; R (recursive scales) is what the scale count says beyond the model's own
+        Rs = {self._check_shapes(sh) for sh in {tuple(sh): sh for sh in shapes_of}.values()}
+        if len(Rs) != 1:
+            raise ValueError('containers with different numbers of scales in one batch')
+        recursive = Rs.pop()
         if tile is not None:
             tile = (int(tile[0]), int(tile[1]))
         si, elem, n_sym, planes = stream_layout(shapes_of, tile)
@@ -597,7 +624,7 @@ class BatchCodec(object):
         K = self.net.config_ms.prob.K
         bn8, F_prev, S = None, None, None
         self._mark('start')
-        for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll()):
+        for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll(recursive)):
             C = shapes_of[0][idx][0]
             H, W = max(sh[idx][1] for sh in shapes_of), max(sh[idx][2] for sh in shapes_of)
             plane = int(planes[idx])
@@ -616,8 +643,11 @@ class BatchCodec(object):
                 d['row_pitch'][:] = 0
                 self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
             else:
-                l, F_prev = self.net.get_P_nhwc(scale, bn8, F_prev if self.net._fuse_feat else None, extents=fin)
-                self._mark('net%d' % scale)
+                # MultiscaleNetwork._forward's fusion rule: no decoder features cross into or out of a recursive
+                # scale, and the coarsest trained scale gets none
+                fuse = self.net._fuse_feat and scale < self.net.scales - 1
+                l, F_prev = self.net.get_P_nhwc(scale, bn8, F_prev if fuse else None, extents=fin)
+                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
                 if tuple(l.shape[1:3]) != (H, W) or non_shared_get_K(l.shape[-1], C) != K:
                     raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
                                      % (scale, C, H, W, tuple(l.shape)))
@@ -661,7 +691,8 @@ class BatchCodec(object):
                 S = E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
             else:
                 S = Sp.view(N, C, H, W)
-            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else 'S%d' % scale))
+            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
+                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
             if scale > 0:
                 bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
         return S
@@ -688,9 +719,17 @@ class BatchCodec(object):
         """C, H, W of every scale come straight from the (untrusted) file, while the kernels index with
         the shapes the MODEL produces (each scale twice the size of the coarser one, C = 3 for the image
         and the RGB baselines, q.C for bottlenecks).  A crafted, truncated or wrong-config container must
-        fail here, before any buffer is sized from it (the reference fails with a torch shape error)."""
+        fail here, before any buffer is sized from it (the reference fails with a torch shape error).
+        -> R, the number of recursive scales (DESIGN §4.7): the scales beyond the model's num_scales + 1, allowed
+        for the RGB baselines only."""
         cfg = self.net.config_ms
         n = len(shapes)
+        R = n - (self.net.scales + 1)
+        if R < 0:
+            raise ValueError('container has %d scales, model expects %d' % (n, self.net.scales + 1))
+        if R > 0 and not self.net._rgb:
+            raise ValueError('container has %d scales, model expects %d: recursive containers are written by the '
+                             'RGB baselines only' % (n, self.net.scales + 1))
         for idx, (C, H, W) in enumerate(shapes):
             scale = n - 1 - idx
             want_C = 3 if (scale == 0 or self.net._rgb) else cfg.q.C
@@ -703,6 +742,7 @@ class BatchCodec(object):
                 if (H, W) != (2 * Hc, 2 * Wc):
                     raise ValueError('container scale %d is %dx%d, expected twice the coarser scale (%dx%d)'
                                      % (scale, H, W, 2 * Hc, 2 * Wc))
+        return R
 
     def _symbol_values(self, scale, dmll, dev):
         """Value of every symbol of bottleneck `scale`: the `levels` LUT of the quantiser that produced

@@ -16,7 +16,9 @@ What it mirrors (flag names and meaning as in /root/reference/src/test.py:44-141
   * default mode: theoretical bpsp per image from the network's own likelihoods, crops of large images
     weighted by their sub-pixel counts (test/multiscale_tester.py:283-345), cached per (test set, itr);
   * --write_to_files: every image through the real coder to `<name>.l3c`, decoded again and compared,
-    real bpsp reported, per-stage times collected (test/multiscale_tester.py:347-373).
+    real bpsp reported, per-stage times collected (test/multiscale_tester.py:347-373).  With --recursive N|auto
+    on an RGB baseline the files are recursive containers (DESIGN §4.7), which the reference cannot write
+    (multiscale_tester.py:187-188 raises); --compare_theory then prints the recursive theory.
 --sample writes the ground truth and three sampled images per test image (row f3).
 
 H100-first difference: in the default mode up to `--batch` images (default 16) share one network pass instead
@@ -265,8 +267,6 @@ class Tester(object):
         (ms_path, _dl_path), _postfix = configs_of_experiment(self.experiment_dir, configs_dir or default_configs_dir())
         self.config_ms = config_parser.parse(ms_path)[0]
         self.recursive = parse_recursive_flag(getattr(flags, 'recursive', '0'), self.config_ms)
-        if flags.write_to_files and self.recursive:
-            raise NotImplementedError('--write_to_file not implemented for --recursive')   # multiscale_tester.py:187-188
         if self.recursive:
             print('--recursive={}'.format(self.recursive))
         if make_blueprint is None:
@@ -289,7 +289,10 @@ class Tester(object):
             if make_bitcoding is None:
                 from .bitcoding import Bitcoding
                 make_bitcoding = Bitcoding
-            self.bc = make_bitcoding(self.blueprint, times=self.times, compare_with_theory=flags.compare_theory)
+            # --write_to_files --recursive: recursive containers (DESIGN §4.7), which the reference cannot write
+            # (multiscale_tester.py:187-188); without --recursive the call is the reference's
+            kw = dict(recursive=self.recursive) if self.recursive else {}
+            self.bc = make_bitcoding(self.blueprint, times=self.times, compare_with_theory=flags.compare_theory, **kw)
 
     # ---- cache of theoretical results: {"<testset id>@<itr>": {"metric": .., "per_img": {..}}}
     def _cache(self):

@@ -484,9 +484,10 @@ class MultiscaleNetwork(nn.Module):
         for i, s in reversed(list(enumerate(forward_scales))):
             # no fusion for: disabled / auto-recursive scales / the final trained scale
             fuse = prev if (self._fuse_feat and s != -1 and s != max(forward_scales)) else None
-            prev = self.nets[s].dec(enc_outs[i].bn_q, fuse, operand_only=(i == 0)).F
+            # the features of scale 0 and of the recursive scales feed nothing but their probability classifier
+            prev = self.nets[s].dec(enc_outs[i].bn_q, fuse, operand_only=(i == 0 or s == -1)).F
             dec_F[i] = prev
-        fuse_iv = (intervals_of is not None and E.f16_mode() and not auto_recurse and
+        fuse_iv = (intervals_of is not None and E.f16_mode() and
                    all(self.prob_clfs[s].atrous.lin.in_channels % 64 == 0 for s in forward_scales))
         if fuse_iv:
             out.IV = []
@@ -556,13 +557,22 @@ class MultiscaleNetwork(nn.Module):
     def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False, extents=None):
         """-> (parameters NHWC, decoder features as engine.Act for the next finer scale).  At scale 0 the
         features feed nothing else (need_F=True keeps their fp32 tensor for the reference-shaped get_P).
-        extents: [(h_n, w_n)] at the FINEST scale -> bn8 is a ragged batch (forward())."""
-        assert 0 <= scale < self.config_ms.num_scales, 'Out of range: {}'.format(scale)
-        self._check_ragged(extents)
+        extents: [(h_n, w_n)] at the FINEST scale -> bn8 is a ragged batch (forward()).
+        scale >= num_scales: a recursive scale of forward(auto_recurse=R) (RGB baselines), num_scales + k the k-th
+        extra application of the last trained scale: nets[-1] / prob_clfs[-1], no features in or out (like scale 0,
+        its features feed nothing but its probability classifier).  The bit-coder decodes recursive scales of the
+        RGB baselines only (codec.BatchCodec)."""
+        ns = self.config_ms.num_scales
+        recursive = scale >= ns
+        assert 0 <= scale, 'Out of range: {}'.format(scale)
+        if recursive and dec_F_prev is not None:
+            raise ValueError('recursive scale %d takes no decoder features' % scale)
+        self._check_ragged(extents, int(recursive))
         f = 2 ** (scale + 1)
+        s = -1 if recursive else scale
         with E.ragged_extents(extents, bn8.shape[1] * f, bn8.shape[2] * f):
-            F = self.nets[scale].dec(bn8, dec_F_prev, operand_only=(scale == 0 and not need_F)).F
-            return self.prob_clfs[scale](F), F
+            F = self.nets[s].dec(bn8, dec_F_prev, operand_only=((scale == 0 or recursive) and not need_F)).F
+            return self.prob_clfs[s](F), F
 
     def get_P(self, scale, bn_q, dec_F_prev=None):
         """multiscale_network.py:308-322 with NCHW-shaped tensors in and out."""
