@@ -181,6 +181,18 @@ int l3c_dmll_build_table_tiled(const float *l_dev, const uint8_t *sym_dev, const
                                uint16_t *table_dev, int pitch, void *stream);
 int l3c_reorder_tiles(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int H, int W, int th,
                       int tw, int to_tiles, void *stream);
+/* Region decode (DESIGN §4.8): l3c_dmll_build_table_tiled for an H x W symbol plane whose parameters are the
+ * rectangle at (oy, ox) of a wider plane, l_dev NHWC [N][Hl][Wl][Kp] (the output of a decoder window); rows and
+ * sym_dev are in the tile order of the H x W plane.  Same rows as l3c_dmll_build_table_tiled on a copy of that
+ * rectangle, without the copy.
+ * l3c_crop_rect: the h x w rectangle at origins_dev[n] = (y, x) (int32 [N][2], inside the plane) of each of the
+ * `planes` planes of image n: src N * planes planes of H x W elements of elem_bytes bytes -> dst N * planes planes
+ * of h x w (NHWC tensors: planes = 1, elem_bytes = bytes per pixel). */
+int l3c_dmll_build_table_window(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev,
+                                const float *targets_dev, int N, int H, int W, int C, int K, int L, int rgb, int c,
+                                int th, int tw, uint16_t *table_dev, int pitch, void *stream);
+int l3c_crop_rect(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
+                  const int *origins_dev, int h, int w, void *stream);
 
 /* Negative log-likelihood (nats) summed per image: nll_dev f64 [N] (overwritten).
  * target value of symbol s is values_dev[s] (logistic_mixture.py:146-207). */

@@ -272,6 +272,21 @@ class Bitcoding(object):
                 outs[i] = img
         return outs
 
+    def decode_region(self, data, region, level=0):
+        """One region of a tiled container (DESIGN §4.8) -> int64 1CHW tensor (GPU), equal bit for bit to the same
+        crop of decode_batch([data])[0].  region = (y, x, h, w): at level 0 in the coordinates decode() returns (the
+        unpadded image); at level k >= 1 (RGB baselines) in those of the stored scale-k thumbnail.  Only the tile
+        streams and decoder windows the region depends on are decoded.  ValueError, before any GPU work, for an
+        untiled container, a container this model did not write, an empty region or one outside the image, and a
+        level that does not exist."""
+        return self.decode_regions([data], [region], [level])[0]
+
+    def decode_regions(self, datas, regions, levels=None):
+        """decode_region for many (container, region[, level]) pairs -> list of int64 1CHW tensors in input order.
+        Pairs whose plans have equal window shapes share one network pass and one range-decoder launch per channel
+        step; the others run one after another."""
+        return [S.long() for S in self.codec.decode_regions(datas, regions, levels)]
+
 
 class _ListEncodeJob:
     """encode_batch_begin: the codec jobs of its passes (one for a batch tensor); finish() -> (containers, bpsps) in

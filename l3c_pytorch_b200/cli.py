@@ -4,6 +4,7 @@
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt enc IMG OUT.l3c [--overwrite]
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png
     python -m l3c_pytorch_b200.cli --config cr_rgb_shared --ckpt CKPT.pt enc IMG OUT.l3c --recursive auto
+    python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png --region Y,X,H,W [--level K]
 
 `--ckpt` is a checkpoint as written by the reference's Saver (`torch.save({'net': state_dict})`,
 helpers/saver.py:168); the module tree here has the same parameter names, so it loads strict.
@@ -107,7 +108,41 @@ def build_parser():
     d = sub.add_parser('dec')
     d.add_argument('inp')
     d.add_argument('out_png')
+    d.add_argument('--region', default=None, type=parse_region, metavar='Y,X,H,W',
+                   help='tiled files: decode only this crop (DESIGN §4.8), decoding only the tiles it depends on')
+    d.add_argument('--level', default=0, type=int, metavar='K',
+                   help='with --region, RGB baselines: the crop is of the stored scale-K thumbnail (0 = the image)')
     return p
+
+
+def parse_region(text):
+    """'Y,X,H,W' -> (y, x, h, w)."""
+    try:
+        vals = tuple(int(v) for v in text.split(','))
+    except ValueError:
+        vals = ()
+    if len(vals) != 4:
+        raise argparse.ArgumentTypeError('--region takes Y,X,H,W (four integers), got %r' % text)
+    return vals
+
+
+def decode_region(bc, pin, png_out, region, level=0):
+    """`dec --region`: one crop of a tiled file.  ValueError for crop files (`.partN`, an image coded in parts) and
+    for what Bitcoding.decode_region refuses."""
+    from . import part_suffix_helper
+    if not os.path.isfile(pin):
+        if os.path.isfile(pin + '.part0'):
+            raise ValueError('{} is stored in parts ({}.part0, ...): region decode of part files is not '
+                             'supported'.format(pin, pin))
+        raise DecodeError('File not found: {}'.format(pin))
+    if part_suffix_helper.contains_part_suffix(pin):
+        raise ValueError('{} is one part of an image coded in parts: region decode of part files is not '
+                         'supported'.format(pin))
+    with open(pin, 'rb') as f:
+        data = f.read()
+    img = bc.decode_region(data, region, level)
+    write_image(img, png_out)
+    print('Decoded region {} (level {}) of {} -> {}'.format(region, level, pin, png_out))
 
 
 def main(argv=None):
@@ -118,6 +153,11 @@ def main(argv=None):
     try:
         if a.mode == 'enc':
             encode(bc, a.img, a.out, a.overwrite)
+        elif a.region is not None:
+            try:
+                decode_region(bc, a.inp, a.out_png, a.region, a.level)
+            except ValueError as err:
+                raise DecodeError(str(err))
         else:
             decode(bc, a.inp, a.out_png)
     except (EncodeError, DecodeError) as err:

@@ -200,6 +200,20 @@ def parse_container(data):
     return pad_tuple, scales
 
 
+def _upload(datas, dev):
+    """One upload of every container: -> (device blob, readable 16 bytes past every container; start of each)."""
+    starts = np.zeros(len(datas), np.int64)
+    pos = 0
+    for n, dta in enumerate(datas):
+        starts[n] = pos
+        pos += (len(dta) + 15) & ~15
+    host = torch.zeros(pos + 16, dtype=torch.uint8, pin_memory=True)
+    hb = host.numpy()
+    for n, dta in enumerate(datas):
+        hb[starts[n]:starts[n] + len(dta)] = np.frombuffer(dta, np.uint8)
+    return host.to(dev, non_blocking=True), starts
+
+
 class DecodeLane(object):
     """Streams of one decode in flight (BatchCodec.lanes)."""
     __slots__ = ('main', 'dec', 'bld', 'partitioned')
@@ -457,17 +471,7 @@ class BatchCodec(object):
             raise ValueError('decode_batch needs containers of identical shape')
         if any(len(sh) != len(shapes_of[0]) for sh in shapes_of):
             raise ValueError('decode_batch: containers with different numbers of scales')
-        # one upload of everything
-        starts = np.zeros(N, np.int64)
-        pos = 0
-        for n, dta in enumerate(datas):
-            starts[n] = pos
-            pos += (len(dta) + 15) & ~15
-        host = torch.zeros(pos + 16, dtype=torch.uint8, pin_memory=True)
-        hb = host.numpy()
-        for n, dta in enumerate(datas):
-            hb[starts[n]:starts[n] + len(dta)] = np.frombuffer(dta, np.uint8)
-        blob = host.to(dev, non_blocking=True)
+        blob, starts = _upload(datas, dev)
         offs = np.array([[starts[n] + o for (_, _, _, st) in parsed[n][1] for (o, _) in st] for n in range(N)],
                         np.int64)
         lens = np.array([[ln for (_, _, _, st) in parsed[n][1] for (_, ln) in st] for n in range(N)], np.int64)
@@ -696,6 +700,149 @@ class BatchCodec(object):
             if scale > 0:
                 bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
         return S
+
+    # ------------------------------------------------------------------------------------------
+    def plan_regions(self, datas, regions, levels=None):
+        """Parse, validate and plan (region.plan_region) every (container, region, level) of a decode_regions call,
+        before any GPU work: -> ([(pad_tuple, scales)] parsed, [RegionPlan]).  ValueError for an untiled
+        container, a container this model cannot have written, an empty region or one outside the image, and a
+        level that does not exist."""
+        from .region import DecoderGeometry, plan_region
+        if len(regions) != len(datas):
+            raise ValueError('%d regions for %d containers' % (len(regions), len(datas)))
+        levels = [0] * len(datas) if levels is None else list(levels)
+        if len(levels) != len(datas):
+            raise ValueError('%d levels for %d containers' % (len(levels), len(datas)))
+        geo = DecoderGeometry(self.net)
+        parsed, plans = [], []
+        for i, (dta, reg, lev) in enumerate(zip(datas, regions, levels)):
+            pt, scales = parse_container(dta)
+            tile = container_tile(dta)
+            if tile is None:
+                raise ValueError('container %d: region decode needs a tiled container (written with '
+                                 'Bitcoding(..., tile=(th, tw))); the streams of the reference layout are serial' % i)
+            shapes = [(C, H, W) for (C, H, W, _) in scales]
+            try:
+                self._check_shapes(shapes)
+            except ValueError as err:
+                raise ValueError('container %d was not written by this model: %s' % (i, err))
+            parsed.append((pt, scales))
+            plans.append(plan_region(shapes, pt, tile, geo, reg, lev))
+        return parsed, plans
+
+    @_on_device
+    def decode_regions(self, datas, regions, levels=None):
+        """Decode one region of each tiled container (DESIGN §4.8): -> [uint8 [1, C, h, w] on the device] in input
+        order, each equal to the same crop of the full decode (at level k >= 1, of the stored scale-k plane).  Only the
+        tile streams and decoder windows the region depends on are decoded.  Pairs whose plans have the same shape
+        (RegionPlan.shape_key) share one network pass and one range-decoder launch per channel step; the groups run
+        one after another.  regions: (y, x, h, w) each; levels: None (all 0) or one int each."""
+        from .region import stream_columns
+        parsed, plans = self.plan_regions(datas, regions, levels)
+        dev = self.blueprint.device
+        blob, starts = _upload(datas, dev)
+        groups = {}
+        for i, p in enumerate(plans):
+            groups.setdefault(p.shape_key(), []).append(i)
+        outs = [None] * len(datas)
+        # streams and symbols handed to the range decoder by this call (decode_region_device adds to them)
+        self.region_counts = {'streams': 0, 'symbols': 0}
+        for idxs in groups.values():
+            offs, lens = [], []
+            for i in idxs:
+                scales = parsed[i][1]
+                cols = stream_columns(plans[i], plans[i].tile)
+                st = [scales[sp.idx][3][c] for sp, cs in zip(plans[i].scales, cols) for c in cs]
+                offs.append([starts[i] + o for (o, _) in st])
+                lens.append([ln for (_, ln) in st])
+            S = self.decode_region_device(blob, np.array(offs, np.int64), np.array(lens, np.int64),
+                                          [plans[i] for i in idxs])
+            for k, i in enumerate(idxs):
+                outs[i] = S[k:k + 1]
+        return outs
+
+    @_on_device
+    def decode_region_device(self, blob, offs, lens, plans):
+        """decode_device for region plans of equal shape_key (DESIGN §4.8): offs / lens int64 [N][planned streams]
+        in the order of region.stream_columns.  Every scale decodes the tiles of its plan's rectangle (a plane that
+        tile_grid cuts like the full one), its decoder network runs on the plan's window of the coarser scale
+        (symbols and, with dec.skip, features cropped by l3c_crop_rect) and its rows are built from the used
+        rectangle of that output in place (l3c_dmll_build_table_window).  -> uint8 [N, C, h, w], the regions."""
+        dev = blob.device
+        N = len(plans)
+        p0 = plans[0]
+        tile = p0.tile
+        rects = [(sp.C, sp.rect[2] - sp.rect[0], sp.rect[3] - sp.rect[1]) for sp in p0.scales]
+        si, elem, n_sym, planes = stream_layout([rects] * N, tile)
+        bounds = np.searchsorted(si[0], np.arange(len(planes) + 1))
+        K = self.net.config_ms.prob.K
+        walk = list(self.iter_scale_dmll(p0.recursive))[:len(p0.scales)]
+
+        def origins(fn):
+            return E._to_device_async(np.array([fn(p) for p in plans], np.int32).reshape(N, 2), dev)
+
+        counts = self.__dict__.setdefault('region_counts', {'streams': 0, 'symbols': 0})
+        bn8, F_win, S = None, None, None
+        self._mark('start')
+        for idx, (scale, dmll, uniform) in enumerate(walk):
+            sp = p0.scales[idx]
+            C, H, W = rects[idx]
+            plane = int(planes[idx])
+            cols = slice(bounds[idx], bounds[idx + 1])
+            T = (cols.stop - cols.start) // C
+            Sp = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # symbols in stream order
+            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
+            d = desc.reshape(N, C, T)
+            d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
+            d['in_len'][:] = lens[:, cols].reshape(N, C, T)
+            d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
+            d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
+            counts['streams'] += desc.shape[0]
+            counts['symbols'] += int(desc['n_sym'].sum())
+            if uniform:
+                d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
+                d['row_pitch'][:] = 0
+                E.ac_decode_streams(desc, dev, dmll.L)
+            else:
+                l, F = self.net.get_P_nhwc(scale, bn8, F_win if sp.fused else None)
+                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
+                wy0, wx0, wy1, wx1 = sp.window
+                if tuple(l.shape[1:3]) != (2 * (wy1 - wy0), 2 * (wx1 - wx0)) or non_shared_get_K(l.shape[-1], C) != K:
+                    raise ValueError('container scale %d (C=%d) does not match the model output %s'
+                                     % (scale, C, tuple(l.shape)))
+                pitch = E.table_pitch(dmll.L)
+                table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
+                d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
+                d['row_pitch'][:] = pitch
+                tg = dmll.targets(dev)
+                oy, ox = sp.out[:2]
+                if dmll.rgb_scale:
+                    for c in range(C):
+                        E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, True, c, table, H, W, tile)
+                        E.ac_decode_streams(np.ascontiguousarray(d[:, c, :]).reshape(-1), dev, dmll.L)
+                else:
+                    E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, False, -1, table, H, W, tile)
+                    E.ac_decode_streams(desc, dev, dmll.L)
+            S = E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
+            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
+                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
+            if idx + 1 == len(walk):
+                break
+            # the finer network's inputs: its window of this scale's symbols, and of this scale's features
+            nxt = p0.scales[idx + 1]
+            wh, ww = nxt.window[2] - nxt.window[0], nxt.window[3] - nxt.window[1]
+            S_win = E.crop_rect(S, origins(lambda p: (p.scales[idx + 1].window[0] - p.scales[idx].rect[0],
+                                                      p.scales[idx + 1].window[1] - p.scales[idx].rect[1])),
+                                wh, ww, nhwc=False)
+            bn8 = E.symbols_to_values(S_win, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
+            F_win = None
+            if nxt.fused:
+                F_win = E.crop_rect(F.f, origins(lambda p: (p.scales[idx + 1].window[0] - 2 * p.scales[idx].window[0],
+                                                            p.scales[idx + 1].window[1] - 2 * p.scales[idx].window[1])),
+                                    wh, ww, nhwc=True)
+        y0, x0, y1, x1 = p0.region
+        return E.crop_rect(S, origins(lambda p: (p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1])),
+                           y1 - y0, x1 - x0, nhwc=False)
 
     # stage timing of a decode (bench.py / tools): set `codec.stage_events = []` before decode_device,
     # synchronise, then read stage_ms()

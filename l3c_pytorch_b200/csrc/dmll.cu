@@ -86,12 +86,15 @@ __host__ __device__ __forceinline__ int tile_order_to_raster(int r, int H, int W
 }
 
 // rows (and the symbols of the already decoded channels, `sym`) are indexed in STREAM order: raster order, or
-// tile order when th > 0; the parameters `l` are always read at the raster pixel.
-template <int K>
+// tile order when th > 0; the parameters `l` are always read at the raster pixel.  WIN: the H x W symbol plane is
+// the rectangle at (oy, ox) of a wider parameter plane of l_hw pixels per image and width Wl (a decoder window,
+// l3c_dmll_build_table_window); otherwise `l` covers exactly the H x W plane and the last four arguments are unused.
+template <int K, bool WIN>
 __global__ void __launch_bounds__(TB_THREADS)
 dmll_table_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
                   const float *__restrict__ targets, int HW, int C, int L, int rgb, int c_first,
-                  int pix0, int npix, uint16_t *__restrict__ table, int pitch, int H, int W, int th, int tw) {
+                  int pix0, int npix, uint16_t *__restrict__ table, int pitch, int H, int W, int th, int tw,
+                  int64_t l_hw, int Wl, int oy, int ox) {
     __shared__ float s_pi[TB_PIX][K];
     __shared__ float s_mu[TB_PIX][K];
     __shared__ float s_is[TB_PIX][K];
@@ -103,7 +106,13 @@ dmll_table_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
     if ((int)threadIdx.x < np) {
         const int p = pix0 + q0 + threadIdx.x;                                     // stream-order index
         const int pr = th > 0 ? tile_order_to_raster(p, H, W, th, tw) : p;         // raster pixel
-        const float *lp = l + ((size_t)n * HW + pr) * Kp;
+        const float *lp;
+        if (WIN) {
+            const int py = pr / W, px = pr - py * W;
+            lp = l + ((size_t)n * l_hw + (size_t)(oy + py) * Wl + ox + px) * Kp;
+        } else {
+            lp = l + ((size_t)n * HW + pr) * Kp;
+        }
         float xr = 0.f, xg = 0.f;
         if (rgb && c >= 1) xr = (float)sym[((size_t)n * C + 0) * HW + p];
         if (rgb && c >= 2) xg = (float)sym[((size_t)n * C + 1) * HW + p];
@@ -480,8 +489,9 @@ extern "C" int l3c_dmll_build_table(const float *l_dev, const uint8_t *sym_dev,
     L3C_REQUIRE(pix0 >= 0 && npix >= 0 && pix0 + npix <= HW, "l3c_dmll_build_table: pixel range");
     if (npix == 0) return L3C_OK;
     dim3 grid(ceil_div(npix, TB_PIX), N, c < 0 ? C : 1);
-    dmll_table_kernel<10><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
-        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, pix0, npix, table_dev, pitch, 0, 0, 0, 0);
+    dmll_table_kernel<10, false><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, pix0, npix, table_dev, pitch, 0, 0, 0, 0, 0, 0, 0,
+        0);
     L3C_LAUNCH_CHECK("dmll_table_kernel");
     return L3C_OK;
 }
@@ -515,8 +525,31 @@ extern "C" int l3c_dmll_build_table_tiled(const float *l_dev, const uint8_t *sym
                 "l3c_dmll_build_table_tiled: pitch=%d must be 32 (L<=32) or 256, L=%d", pitch, L);
     L3C_REQUIRE(th >= 1 && tw >= 1 && H >= 1 && W >= 1, "l3c_dmll_build_table_tiled: tile %dx%d", th, tw);
     dim3 grid(ceil_div(HW, TB_PIX), N, c < 0 ? C : 1);
-    dmll_table_kernel<10><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
-        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, 0, HW, table_dev, pitch, H, W, th, tw);
+    dmll_table_kernel<10, false><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, 0, HW, table_dev, pitch, H, W, th, tw, 0, 0, 0, 0);
+    L3C_LAUNCH_CHECK("dmll_table_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_build_table_window(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev,
+                                           const float *targets_dev, int N, int H, int W, int C, int K, int L, int rgb,
+                                           int c, int th, int tw, uint16_t *table_dev, int pitch, void *stream) {
+    using namespace l3c;
+    const int HW = H * W;
+    if (int e = check_common("l3c_dmll_build_table_window", N, HW, C, K, L, rgb)) return e;
+    L3C_REQUIRE(l_dev && targets_dev && table_dev, "l3c_dmll_build_table_window: null pointer");
+    L3C_REQUIRE(!(rgb && c > 0) || sym_dev, "l3c_dmll_build_table_window: decoded symbols needed for c>0");
+    L3C_REQUIRE(c < C && (c >= 0 || !rgb), "l3c_dmll_build_table_window: c=%d C=%d rgb=%d", c, C, rgb);
+    L3C_REQUIRE((pitch == 32 && L <= 32) || (pitch == 256 && L <= 256 && L > 32),
+                "l3c_dmll_build_table_window: pitch=%d must be 32 (L<=32) or 256, L=%d", pitch, L);
+    L3C_REQUIRE(th >= 1 && tw >= 1 && H >= 1 && W >= 1, "l3c_dmll_build_table_window: tile %dx%d", th, tw);
+    L3C_REQUIRE(oy >= 0 && ox >= 0 && oy + H <= Hl && ox + W <= Wl,
+                "l3c_dmll_build_table_window: %dx%d rectangle at (%d, %d) outside the %dx%d parameter plane", H, W, oy,
+                ox, Hl, Wl);
+    dim3 grid(ceil_div(HW, TB_PIX), N, c < 0 ? C : 1);
+    dmll_table_kernel<10, true><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, 0, HW, table_dev, pitch, H, W, th, tw,
+        (int64_t)Hl * Wl, Wl, oy, ox);
     L3C_LAUNCH_CHECK("dmll_table_kernel");
     return L3C_OK;
 }
@@ -533,7 +566,40 @@ __global__ void reorder_tiles_kernel(const T *__restrict__ src, T *__restrict__ 
     if (to_tiles) dst[base + r] = src[base + p];
     else dst[base + p] = src[base + r];
 }
+
+// the h x w rectangle at origins[n] of every plane of image n (planes H x W of per_elem words or bytes)
+template <typename T>
+__global__ void crop_rect_kernel(const T *__restrict__ src, T *__restrict__ dst, int per_elem, int planes, int H,
+                                 int W, const int *__restrict__ origins, int h, int w) {
+    const int plane = blockIdx.y;
+    const int n = plane / planes;
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= (int64_t)h * w * per_elem) return;
+    const int64_t e = r / per_elem, k = r % per_elem;
+    const int64_t y = origins[2 * n] + e / w, x = origins[2 * n + 1] + e % w;
+    dst[((int64_t)plane * h * w + e) * per_elem + k] = src[(((int64_t)plane * H + y) * W + x) * per_elem + k];
+}
 }  // namespace l3c
+
+extern "C" int l3c_crop_rect(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
+                             const int *origins_dev, int h, int w, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(src_dev && dst_dev && src_dev != dst_dev && origins_dev, "l3c_crop_rect: bad pointers");
+    L3C_REQUIRE(elem_bytes >= 1 && planes >= 1 && N >= 1 && (int64_t)N * planes <= 65535 && h >= 1 && w >= 1 &&
+                    h <= H && w <= W,
+                "l3c_crop_rect: elem_bytes=%d planes=%d N=%d %dx%d of %dx%d", elem_bytes, planes, N, h, w, H, W);
+    const bool words = elem_bytes % 4 == 0;
+    const int per_elem = words ? elem_bytes / 4 : elem_bytes;
+    dim3 grid((unsigned)ceil_div64((int64_t)h * w * per_elem, 256), N * planes);
+    if (words)
+        crop_rect_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
+            (const uint32_t *)src_dev, (uint32_t *)dst_dev, per_elem, planes, H, W, origins_dev, h, w);
+    else
+        crop_rect_kernel<uint8_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
+            (const uint8_t *)src_dev, (uint8_t *)dst_dev, per_elem, planes, H, W, origins_dev, h, w);
+    L3C_LAUNCH_CHECK("crop_rect_kernel");
+    return L3C_OK;
+}
 
 extern "C" int l3c_reorder_tiles(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int H, int W, int th,
                                  int tw, int to_tiles, void *stream) {

@@ -783,6 +783,36 @@ def dmll_build_table_tiled(l, sym, targets, C, K, L, rgb, c, table, tile):
     LAUNCHES['n'] += 1
 
 
+def dmll_build_table_window(l, oy, ox, sym, targets, C, K, L, rgb, c, table, H, W, tile):
+    """dmll_build_table_tiled for the H x W symbol plane whose parameters are the rectangle at (oy, ox) of the
+    wider plane l NHWC [N,Hl,Wl,Kp] (a decoder window's output, DESIGN §4.8); rows and `sym` in tile order."""
+    N, Hl, Wl, _ = l.shape
+    assert l.is_contiguous()
+    check(lib.l3c_dmll_build_table_window(_ptr(l), Hl, Wl, int(oy), int(ox), _ptr(sym), _ptr(targets), N, H, W, C,
+                                          K, L, int(rgb), c, tile[0], tile[1], _ptr(table), table_pitch(L),
+                                          _stream_ptr()))
+    LAUNCHES['n'] += 1
+
+
+def crop_rect(src, origins_dev, h, w, nhwc):
+    """l3c_crop_rect: the h x w rectangle at origins_dev[n] = (y, x) (int32 [N, 2] on the device) of image n, as a
+    new tensor.  nhwc: src is NHWC [N, H, W, C]; otherwise planes [N, P, H, W]."""
+    assert src.is_contiguous() and src.dim() == 4
+    N = origins_dev.shape[0]
+    if nhwc:
+        H, W, planes = src.shape[1], src.shape[2], 1
+        out = torch.empty(N, h, w, src.shape[3], dtype=src.dtype, device=src.device)
+        elem_bytes = src.shape[3] * src.element_size()
+    else:
+        H, W, planes = src.shape[2], src.shape[3], src.shape[1]
+        out = torch.empty(N, planes, h, w, dtype=src.dtype, device=src.device)
+        elem_bytes = src.element_size()
+    check(lib.l3c_crop_rect(_ptr(src), _ptr(out), elem_bytes, planes, N, H, W, _ptr(origins_dev), int(h), int(w),
+                            _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return out
+
+
 def reorder_tiles(src, H, W, tile, to_tiles):
     """[planes..., H*W or H, W] uint8 / int32 tensor: raster <-> tile order (l3c_reorder_tiles); new tensor."""
     assert src.is_contiguous() and src.dtype in (torch.uint8, torch.int32)

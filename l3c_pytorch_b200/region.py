@@ -1,0 +1,228 @@
+"""Region decode of tiled containers (DESIGN §4.8): which tile streams and decoder windows a crop of the image
+depends on.  Pure host code.
+
+Every tile of a tiled container is an independent stream whose symbols depend only on their CDF rows, and a row
+depends on the coarser scale only within the bounded receptive field of the decoder network and the probability
+classifier.  Every conv kernel computes an output pixel the same way wherever it sits in the tensor, so a decoder
+network run on a window of the coarser scale gives, inside the window shrunk by that field, exactly the bits of the
+full run.  `plan_region` walks the scales fine to coarse:
+
+  tiles needed at scale s  ->  their P_s rectangle  ->  widened by the classifier's radius (fine grid), halved
+  (Upsampler x2), widened by the tail, body and head radii (coarse grid) and clipped to the image: the window of
+  bn_{s+1} the decoder of scale s runs on  ->  (with dec.skip) the F_{s+1} region that decoder adds after its
+  head  ->  the union, tile-aligned: the tiles needed at scale s+1  ->  ... up to the uniform-prior scale.
+
+At a clipped edge the window edge is the image edge, so the kernels' zero padding is the image's own.  Rectangles
+are tile-aligned (their start on a tile boundary, their end on one or at the plane's edge), so `tile_grid` cuts them
+into the same tiles, in the same order, as the full plane.
+"""
+import numpy as np
+
+from .codec import tile_grid
+
+
+def _radius(conv):
+    """Pixels a same-size conv reads on each side of its output pixel."""
+    return conv.dilation[0] * (conv.kernel_size[0] - 1) // 2
+
+
+class Radii(object):
+    """Receptive radii of one scale's decoder (head, body, tail: on the coarse grid) and classifier (fine grid)."""
+    __slots__ = ('head', 'body', 'tail', 'clf')
+
+    def __init__(self, dec, clf):
+        self.head = _radius(dec.head)
+        body = list(dec.body)
+        self.body = sum(_radius(m.body[0]) + _radius(m.body[2]) for m in body[:-1]) + _radius(body[-1])
+        self.tail = _radius(dec.tail[0])
+        self.clf = max(_radius(a) for a in clf.atrous.atrous) + _radius(clf.atrous.lin)
+
+
+class DecoderGeometry(object):
+    """What the planner needs of a MultiscaleNetwork, read from its module tree: the radii of every trained
+    scale's decoder and classifier, which scales fuse the coarser decoder's features (dec.skip), and whether the
+    scales are images (RGB baselines)."""
+
+    def __init__(self, net):
+        self.num_scales = net.scales
+        self.rgb = bool(net._rgb)
+        self.skip = bool(net._fuse_feat)
+        self.radii = [Radii(net.nets[s].dec, net.prob_clfs[s]) for s in range(net.scales)]
+
+    def radii_of(self, scale):
+        """Recursive scales (scale >= num_scales) run nets[-1] / prob_clfs[-1]."""
+        return self.radii[min(scale, self.num_scales - 1)]
+
+    def fuses(self, scale):
+        """MultiscaleNetwork._forward's rule: no features into a recursive scale or the coarsest trained one."""
+        return self.skip and scale < self.num_scales - 1
+
+
+def geometry_of(config):
+    return config if isinstance(config, DecoderGeometry) else DecoderGeometry(config)
+
+
+def _expand(r, m):
+    return (r[0] - m, r[1] - m, r[2] + m, r[3] + m)
+
+
+def _clip(r, H, W):
+    return (max(r[0], 0), max(r[1], 0), min(r[2], H), min(r[3], W))
+
+
+def _union(a, b):
+    return (min(a[0], b[0]), min(a[1], b[1]), max(a[2], b[2]), max(a[3], b[3]))
+
+
+def _area(r):
+    return (r[2] - r[0]) * (r[3] - r[1])
+
+
+def _align(r, H, W, tile):
+    th, tw = tile
+    return (r[0] // th * th, r[1] // tw * tw, min(-(-r[2] // th) * th, H), min(-(-r[3] // tw) * tw, W))
+
+
+class ScalePlan(object):
+    """One scale of a region plan.  Rectangles are (y0, x0, y1, x1), half-open.
+    rect: the tile-aligned symbols decoded, in this scale's coordinates; tiles: their indices in the plane's tile
+    grid (tile_grid order).  For a scale with a decoder network: window, the bn_{s+1} rectangle (coarser scale's
+    coordinates) its network runs on; out, the rectangle of that network's output (2x the window) that is exact
+    and used, i.e. rect relative to 2 * window's origin; fused, whether the coarser decoder's features are added.
+    The uniform-prior scale has window = out = None."""
+    __slots__ = ('idx', 'scale', 'C', 'H', 'W', 'rect', 'tiles', 'window', 'out', 'fused')
+
+    def __init__(self, **kw):
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+    @property
+    def streams(self):
+        return self.C * len(self.tiles)
+
+    @property
+    def symbols(self):
+        return self.C * _area(self.rect)
+
+    @property
+    def window_pixels(self):
+        return 0 if self.window is None else _area(self.window)
+
+    def shape_key(self):
+        r, w = self.rect, self.window
+        return (self.C, r[2] - r[0], r[3] - r[1], None if w is None else (w[2] - w[0], w[3] - w[1]), self.out,
+                self.fused, len(self.tiles))
+
+    def __repr__(self):
+        return 'ScalePlan(scale=%d, rect=%s, tiles=%d, window=%s, out=%s, fused=%s)' % (
+            self.scale, self.rect, len(self.tiles), self.window, self.out, self.fused)
+
+
+class RegionPlan(object):
+    """plan_region's result: scales coarse -> fine (the finest is the requested level), the region in that level's
+    plane, and the totals."""
+
+    def __init__(self, scales, region, level, tile, n_scales, recursive):
+        self.scales, self.region, self.level, self.tile = scales, region, level, tile
+        self.n_scales, self.recursive = n_scales, recursive
+
+    @property
+    def tiles(self):
+        return sum(len(s.tiles) for s in self.scales)
+
+    @property
+    def streams(self):
+        return sum(s.streams for s in self.scales)
+
+    @property
+    def symbols(self):
+        return sum(s.symbols for s in self.scales)
+
+    @property
+    def window_pixels(self):
+        return sum(s.window_pixels for s in self.scales)
+
+    def shape_key(self):
+        """Plans with equal keys decode as one batch (BatchCodec.decode_regions): every rectangle has the same size
+        and every network output the same used rectangle, wherever the regions lie."""
+        return (self.tile, self.n_scales, self.level, tuple(s.shape_key() for s in self.scales))
+
+    def __repr__(self):
+        return 'RegionPlan(level=%d, region=%s, tiles=%d, symbols=%d, window_pixels=%d)' % (
+            self.level, self.region, self.tiles, self.symbols, self.window_pixels)
+
+
+def plan_region(shapes, pad_tuple, tile, config, region, level=0):
+    """shapes: [(C, H, W)] of a container's scales, coarse -> fine; pad_tuple: its (left, right, top, bottom);
+    tile: its (th, tw), None for the reference layout; config: a MultiscaleNetwork or its DecoderGeometry;
+    region = (y, x, h, w): at level 0 in unpadded image coordinates, at level k >= 1 (RGB baselines) in the
+    coordinates of the stored scale-k plane.  -> RegionPlan.  ValueError for an untiled container, an empty region
+    or one outside the image, and a level that does not exist."""
+    geo = geometry_of(config)
+    if tile is None:
+        raise ValueError('region decode needs a tiled container (written with Bitcoding(..., tile=(th, tw))): '
+                         'the streams of the reference layout are serial')
+    tile = (int(tile[0]), int(tile[1]))
+    n = len(shapes)
+    recursive = n - geo.num_scales - 1
+    if recursive < 0:
+        raise ValueError('container has %d scales, model expects %d' % (n, geo.num_scales + 1))
+    if isinstance(level, bool) or not isinstance(level, (int, np.integer)) or level < 0 or level >= n:
+        raise ValueError('level %r does not exist: the container stores levels 0 .. %d' % (level, n - 1))
+    level = int(level)
+    if level > 0 and not geo.rgb:
+        raise ValueError('level %d: only the RGB baselines store images at the coarser scales; the L3C bottlenecks '
+                         'are not images' % level)
+    if len(region) != 4:
+        raise ValueError('region must be (y, x, h, w), got %r' % (region,))
+    y, x, h, w = (int(v) for v in region)
+    idx_f = n - 1 - level
+    _, Hf, Wf = shapes[idx_f]
+    if level == 0:
+        left, right, top, bottom = (int(v) for v in pad_tuple)
+        Hu, Wu, oy, ox = Hf - top - bottom, Wf - left - right, top, left
+    else:
+        Hu, Wu, oy, ox = Hf, Wf, 0, 0
+    if h < 1 or w < 1:
+        raise ValueError('empty region %r' % (tuple(region),))
+    if y < 0 or x < 0 or y + h > Hu or x + w > Wu:
+        raise ValueError('region %r lies outside the %dx%d image' % (tuple(region), Hu, Wu))
+    want = (y + oy, x + ox, y + oy + h, x + ox + w)
+    region_px = want
+    plans = []
+    for idx in range(idx_f, -1, -1):
+        C, H, W = shapes[idx]
+        scale = n - 1 - idx
+        rect = _align(want, H, W, tile)
+        th, tw = tile
+        ntx = -(-W // tw)
+        tiles = [ty * ntx + tx for ty in range(rect[0] // th, -(-rect[2] // th))
+                 for tx in range(rect[1] // tw, -(-rect[3] // tw))]
+        if idx == 0:                                                 # the uniform-prior thumbnail
+            plans.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect, tiles=tiles, window=None,
+                                   out=None, fused=False))
+            break
+        r = geo.radii_of(scale)
+        need_F = _clip(_expand(rect, r.clf), H, W)                   # decoder features the classifier reads
+        coarse = (need_F[0] // 2, need_F[1] // 2, -(-need_F[2] // 2), -(-need_F[3] // 2))   # Upsampler x2
+        Hc, Wc = shapes[idx - 1][1:]
+        window = _clip(_expand(coarse, r.tail + r.body + r.head), Hc, Wc)
+        fused = geo.fuses(scale)
+        want = window
+        if fused:                                                    # F_{s+1}, added after the head
+            want = _union(want, _clip(_expand(coarse, r.tail + r.body), Hc, Wc))
+        out = (rect[0] - 2 * window[0], rect[1] - 2 * window[1], rect[2] - 2 * window[0], rect[3] - 2 * window[1])
+        plans.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect, tiles=tiles, window=window, out=out,
+                               fused=fused))
+    plans.reverse()
+    return RegionPlan(plans, region_px, level, tile, n, recursive)
+
+
+def stream_columns(plan, tile):
+    """Indices, in container order, of the planned streams of every scale: [[column in that scale's stream list]]
+    coarse -> fine, channel-major and in tile order within a channel (the order of a tiled container)."""
+    cols = []
+    for sp in plan.scales:
+        T = len(tile_grid(sp.H, sp.W, tile))
+        cols.append([c * T + t for c in range(sp.C) for t in sp.tiles])
+    return cols
