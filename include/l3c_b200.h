@@ -464,7 +464,7 @@ int l3c_cta_trace_launches(char *buf, size_t cap, int64_t *n_records);
 
 /* Test knob for the range decoder of alphabets L > 32, process-wide, from the next launch on: streams per CTA (1, 2
  * or 4) of v3::ac_decode_kernel<FULLROW, SPC>; 0 = the L3C_DEC_SPC environment variable or, without it, the default
- * (1).  Any other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant
+ * (2).  Any other value is L3C_EINVAL.  Lets one process run every variant, including a partial last CTA.  Not meant
  * for production use. */
 int l3c_set_decoder_streams_per_cta(int spc);
 

@@ -514,7 +514,8 @@ class BatchCodec(object):
         uses: `main` (decoder networks, CDF rows of the bottleneck scales), `bld[3]` (CDF-row builders of the
         R, G, B channels), `dec[3]` (the range decoders).  The `dec` streams of all lanes own a group of SMs
         (driver green contexts, l3c_partition_streams) sized for `L3C_DEC_WARPS_PER_SM` decoder-kernel warps
-        per SM (default 4 for one lane = one latency-bound warp per SM sub-partition, 8 for several lanes; a
+        per SM (default 4 for one lane = one latency-bound warp per SM sub-partition, 8 for two or three lanes,
+        16 from four lanes on; a
         decoder warp that shares its scheduler with throughput-bound warps runs ~1.5x slower); everything else -- including the encode
         stream, which has the lowest priority -- runs on the remaining SMs.  Several lanes = several batches
         being decoded side by side: the decode of ONE batch is bound by the serial chain of its range coder
@@ -537,10 +538,11 @@ class BatchCodec(object):
                 want_part = False
             if want_part:
                 n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
-                # one lane: 4 warps per SM (lowest latency); several lanes: 8, from four lanes on 12 (measured at
+                # one lane: 4 warps per SM (lowest latency); several lanes: 8, from four lanes on 16 (measured at
                 # 16 x 512^2: 3 lanes on 36 / 48 / 72 SMs -> 86 / 69 / 63 Mpx/s, 4 lanes on 32 / 48 SMs -> 89 / 80: what
-                # the decoders' group takes is lost to the throughput work)
-                wps = int(os.environ.get('L3C_DEC_WARPS_PER_SM', 4 if n_lanes == 1 else (8 if n_lanes <= 3 else 12)))
+                # the decoders' group takes is lost to the throughput work; 4 lanes with the coarse RGB decoder, 12 vs
+                # 16 warps = 32 vs 24 SMs: 69.2 - 71.6 vs 72.8 - 74.3 Mpx/s, DESIGN §7)
+                wps = int(os.environ.get('L3C_DEC_WARPS_PER_SM', 4 if n_lanes == 1 else (8 if n_lanes <= 3 else 16)))
                 # every stream = decoder warp + helper warp (measured at 16 x 512^2, one lane, 4 warps per SM:
                 # 48 / 24 / 16 SMs -> decode 95 / 86 / 93 ms)
                 want = -(-(2 * n_decoders * n_lanes) // (8 * wps)) * 8
