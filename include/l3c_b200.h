@@ -193,6 +193,23 @@ int l3c_dmll_build_table_window(const float *l_dev, int Hl, int Wl, int oy, int 
                                 int th, int tw, uint16_t *table_dev, int pitch, void *stream);
 int l3c_crop_rect(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
                   const int *origins_dev, int h, int w, void *stream);
+/* One pass over region windows of different shapes (DESIGN §4.8 "Batches").
+ * l3c_dmll_build_table_windows: l3c_dmll_build_table_window with a rectangle per image, geo_dev int32 [N][4] =
+ * (oy, ox, H_n, W_n) (16-byte aligned): image n's rows and symbols are the tile order of its own H_n x W_n plane,
+ * in stream-order planes of `plane` elements ((n * C + c) * plane), max_hw = max_n H_n * W_n.
+ * l3c_crop_rects: l3c_crop_rect with a rectangle per image, rects_dev int32 [N][4] = (y, x, h_n, w_n) (16-byte
+ * aligned).  dst_off_dev null: dst is N * planes planes of hp x wp, image n top-left and +0 elsewhere; otherwise image
+ * n's planes of h_n x w_n follow each other from element dst_off_dev[n] (hp x wp: the largest rectangle).
+ * l3c_reorder_tiles_images: uint8 tile order -> raster for images of different sizes: src N * planes planes of
+ * plane_len bytes, image n's hold the tile order of its extents_dev[n] = (h_n, w_n) plane (int32 [N][2]); dst
+ * N * planes planes of hp x wp, image n top-left and 0 elsewhere. */
+int l3c_dmll_build_table_windows(const float *l_dev, int Hl, int Wl, const int *geo_dev, int max_hw, int plane,
+                                 const uint8_t *sym_dev, const float *targets_dev, int N, int C, int K, int L, int rgb,
+                                 int c, int th, int tw, uint16_t *table_dev, int pitch, void *stream);
+int l3c_crop_rects(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
+                   const int *rects_dev, const int64_t *dst_off_dev, int hp, int wp, void *stream);
+int l3c_reorder_tiles_images(const uint8_t *src_dev, uint8_t *dst_dev, int planes, int N, int plane_len, int hp,
+                             int wp, const int *extents_dev, int th, int tw, void *stream);
 
 /* Negative log-likelihood (nats) summed per image: nll_dev f64 [N] (overwritten).
  * target value of symbol s is values_dev[s] (logistic_mixture.py:146-207). */

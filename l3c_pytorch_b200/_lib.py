@@ -63,6 +63,10 @@ _SIGNATURES = {
     'l3c_dmll_build_table_window': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] * 2 + [c_int] * 10 +
                                     [c_void_p, c_int, c_void_p]),
     'l3c_crop_rect': (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_int, c_int, c_void_p]),
+    'l3c_dmll_build_table_windows': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int] + [c_void_p] * 2 +
+                                     [c_int] * 8 + [c_void_p, c_int, c_void_p]),
+    'l3c_crop_rects': (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    'l3c_reorder_tiles_images': (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_int, c_int, c_void_p]),
     'l3c_dmll_nll': (c_int, [c_void_p] * 3 + [c_int] * 6 + [c_float, c_float, c_void_p, c_void_p, c_void_p]),
     'l3c_dmll_channel_params': (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p] * 4),
     'l3c_dmll_sample': (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p, c_void_p]),

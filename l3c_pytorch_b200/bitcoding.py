@@ -272,20 +272,22 @@ class Bitcoding(object):
                 outs[i] = img
         return outs
 
-    def decode_region(self, data, region, level=0):
+    def decode_region(self, data, region, level=0, lane=None):
         """One region of a tiled container (DESIGN §4.8) -> int64 1CHW tensor (GPU), equal bit for bit to the same
         crop of decode_batch([data])[0].  region = (y, x, h, w): at level 0 in the coordinates decode() returns (the
         unpadded image); at level k >= 1 (RGB baselines) in those of the stored scale-k thumbnail.  Only the tile
         streams and decoder windows the region depends on are decoded.  ValueError, before any GPU work, for an
         untiled container, a container this model did not write, an empty region or one outside the image, and a
-        level that does not exist."""
-        return self.decode_regions([data], [region], [level])[0]
+        level that does not exist.  lane: as in decode_batch (BatchCodec.lanes; the caller has made `lane.main`
+        current)."""
+        return self.decode_regions([data], [region], [level], lane=lane)[0]
 
-    def decode_regions(self, datas, regions, levels=None):
+    def decode_regions(self, datas, regions, levels=None, lane=None):
         """decode_region for many (container, region[, level]) pairs -> list of int64 1CHW tensors in input order.
-        Pairs whose plans have equal window shapes share one network pass and one range-decoder launch per channel
-        step; the others run one after another."""
-        return [S.long() for S in self.codec.decode_regions(datas, regions, levels)]
+        In f16 and f16x2 the pairs of one level and tile size decode in one pass, whatever the shapes of their regions
+        and images; in tf32 / fp32 pairs whose plans have equal window shapes share one pass and the others run one
+        after another (BatchCodec.decode_regions)."""
+        return [S.long() for S in self.codec.decode_regions(datas, regions, levels, lane=lane)]
 
 
 class _ListEncodeJob:

@@ -71,6 +71,10 @@ def _slot_cap(n_sym):
     return ((n_sym * 17 + 7) // 8 + 64 + 3) & ~3
 
 
+# BatchCodec.decode_regions: False runs every group of equal RegionPlan.shape_key on its own, also where one ragged pass
+# per pass key would do (to compare the two)
+REGION_RAGGED_PASS = True
+
 TILED_MAGIC = b'L3CT'                # tiled containers: this tag + u16 tile_h + u16 tile_w follow the padding tuple
 
 
@@ -90,11 +94,14 @@ def tile_grid(H, W, tile):
     return out
 
 
-def stream_layout(shapes_of, tile=None):
+def stream_layout(shapes_of, tile=None, pad_tiles=False):
     """Where every stream of a batch lives (DESIGN §4.6 "Stream order").  shapes_of: [image][(C, h, w)] coarse ->
     fine.  Scale si has the plane length plane[si] = max_n h_n * w_n (H * W when the images are equal), and stream
     (n, si, c, t) covers the elements [(n*C + c) * plane[si] + off_t, ... + n_t) of that scale's [N][C][plane]
     tensor, (off_t, n_t) = tile_grid(h_n, w_n, tile)[t].
+    pad_tiles: images whose planes have different tile counts (a ragged pass of region rectangles, DESIGN §4.8) get
+    their per-channel stream lists padded to the largest count with empty streams (off 0, n_sym 0); otherwise such a
+    batch is refused.
     -> (scale, elem, n_sym, plane): the scale index, first element and symbol count of every stream, int64
     [N][streams per image] in container order (image, scale, channel[, tile]), and plane int64 [scales]."""
     N = len(shapes_of)
@@ -111,8 +118,12 @@ def stream_layout(shapes_of, tile=None):
         for e in distinct - grids.keys():
             grids[e] = np.array(tile_grid(e[0], e[1], tile), np.int64).T      # [offset, n_sym][tile]
         if len({grids[e].shape for e in distinct}) > 1:
-            raise ValueError('images with different numbers of tiles in one batch')
-        g = grids[ext[0]][:, None] if len(distinct) == 1 else np.stack([grids[e] for e in ext], 1)
+            if not pad_tiles:
+                raise ValueError('images with different numbers of tiles in one batch')
+            T = max(grids[e].shape[1] for e in distinct)
+            g = np.stack([np.pad(grids[e], ((0, 0), (0, T - grids[e].shape[1]))) for e in ext], 1)
+        else:
+            g = grids[ext[0]][:, None] if len(distinct) == 1 else np.stack([grids[e] for e in ext], 1)
         off, cnt = g[:, :, None, :]                                          # [N or 1][1][tiles] each
         shape = (N, C, off.shape[-1])
         si.append(np.full(shape, k))
@@ -733,43 +744,63 @@ class BatchCodec(object):
         return parsed, plans
 
     @_on_device
-    def decode_regions(self, datas, regions, levels=None):
+    def decode_regions(self, datas, regions, levels=None, lane=None):
         """Decode one region of each tiled container (DESIGN §4.8): -> [uint8 [1, C, h, w] on the device] in input
         order, each equal to the same crop of the full decode (at level k >= 1, of the stored scale-k plane).  Only the
-        tile streams and decoder windows the region depends on are decoded.  Pairs whose plans have the same shape
-        (RegionPlan.shape_key) share one network pass and one range-decoder launch per channel step; the groups run
-        one after another.  regions: (y, x, h, w) each; levels: None (all 0) or one int each."""
-        from .region import stream_columns
+        tile streams and decoder windows the region depends on are decoded.  In f16 and f16x2, pairs whose plans walk
+        the same scales with the same tile size (RegionPlan.pass_key) share one ragged pass: one network pass per scale
+        on a padded batch of their windows and one range-decoder launch per channel step (decode_region_device_ragged);
+        pairs of equal RegionPlan.shape_key share the equal-shape pass (decode_region_device), and in tf32 / fp32 the
+        groups of equal shape_key run one after another (region.plan_passes; REGION_RAGGED_PASS = False forces that
+        grouping everywhere).  regions: (y, x, h, w) each; levels: None (all 0) or one int each.
+        lane: as in decode_batch -- the caller has made `lane.main` current; the range decoders run on the lane's
+        decoder streams."""
+        from .region import plan_passes, stream_columns
         parsed, plans = self.plan_regions(datas, regions, levels)
         dev = self.blueprint.device
         blob, starts = _upload(datas, dev)
-        groups = {}
-        for i, p in enumerate(plans):
-            groups.setdefault(p.shape_key(), []).append(i)
+        ragged = REGION_RAGGED_PASS and self.net.windows_unsupported() is None
         outs = [None] * len(datas)
         # streams and symbols handed to the range decoder by this call (decode_region_device adds to them)
         self.region_counts = {'streams': 0, 'symbols': 0}
-        for idxs in groups.values():
+        for idxs, is_ragged in plan_passes(plans, ragged):
+            # per scale the largest tile count of the pass: a ragged pass pads every channel's list to it with empty
+            # streams (stream_layout(pad_tiles=True)), which read nothing
+            n_sc = len(plans[idxs[0]].scales)
+            T_max = [max(len(plans[i].scales[k].tiles) for i in idxs) for k in range(n_sc)]
             offs, lens = [], []
             for i in idxs:
                 scales = parsed[i][1]
-                cols = stream_columns(plans[i], plans[i].tile)
-                st = [scales[sp.idx][3][c] for sp, cs in zip(plans[i].scales, cols) for c in cs]
-                offs.append([starts[i] + o for (o, _) in st])
-                lens.append([ln for (_, ln) in st])
-            S = self.decode_region_device(blob, np.array(offs, np.int64), np.array(lens, np.int64),
-                                          [plans[i] for i in idxs])
+                o, ln = [], []
+                for k, (sp, cs) in enumerate(zip(plans[i].scales, stream_columns(plans[i], plans[i].tile))):
+                    T = len(sp.tiles)
+                    for c in range(sp.C):
+                        for col in cs[c * T:(c + 1) * T]:
+                            o.append(starts[i] + scales[sp.idx][3][col][0])
+                            ln.append(scales[sp.idx][3][col][1])
+                        o += [starts[i]] * (T_max[k] - T)
+                        ln += [0] * (T_max[k] - T)
+                offs.append(o)
+                lens.append(ln)
+            offs, lens = np.array(offs, np.int64), np.array(lens, np.int64)
+            sel = [plans[i] for i in idxs]
+            if is_ragged:
+                res = self.decode_region_device_ragged(blob, offs, lens, sel, lane=lane)
+            else:
+                S = self.decode_region_device(blob, offs, lens, sel, lane=lane)
+                res = [S[k:k + 1] for k in range(len(idxs))]
             for k, i in enumerate(idxs):
-                outs[i] = S[k:k + 1]
+                outs[i] = res[k]
         return outs
 
     @_on_device
-    def decode_region_device(self, blob, offs, lens, plans):
+    def decode_region_device(self, blob, offs, lens, plans, lane=None):
         """decode_device for region plans of equal shape_key (DESIGN §4.8): offs / lens int64 [N][planned streams]
         in the order of region.stream_columns.  Every scale decodes the tiles of its plan's rectangle (a plane that
         tile_grid cuts like the full one), its decoder network runs on the plan's window of the coarser scale
         (symbols and, with dec.skip, features cropped by l3c_crop_rect) and its rows are built from the used
-        rectangle of that output in place (l3c_dmll_build_table_window).  -> uint8 [N, C, h, w], the regions."""
+        rectangle of that output in place (l3c_dmll_build_table_window).  -> uint8 [N, C, h, w], the regions.
+        lane: as in decode_device."""
         dev = blob.device
         N = len(plans)
         p0 = plans[0]
@@ -804,7 +835,7 @@ class BatchCodec(object):
             if uniform:
                 d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
                 d['row_pitch'][:] = 0
-                E.ac_decode_streams(desc, dev, dmll.L)
+                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
             else:
                 l, F = self.net.get_P_nhwc(scale, bn8, F_win if sp.fused else None)
                 self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
@@ -821,10 +852,11 @@ class BatchCodec(object):
                 if dmll.rgb_scale:
                     for c in range(C):
                         E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, True, c, table, H, W, tile)
-                        E.ac_decode_streams(np.ascontiguousarray(d[:, c, :]).reshape(-1), dev, dmll.L)
+                        dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
+                        self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
                 else:
                     E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, False, -1, table, H, W, tile)
-                    E.ac_decode_streams(desc, dev, dmll.L)
+                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
             S = E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
             self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
                                                   ('R%d' if scale >= self.net.scales else 'S%d') % scale))
@@ -845,6 +877,101 @@ class BatchCodec(object):
         y0, x0, y1, x1 = p0.region
         return E.crop_rect(S, origins(lambda p: (p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1])),
                            y1 - y0, x1 - x0, nhwc=False)
+
+    @_on_device
+    def decode_region_device_ragged(self, blob, offs, lens, plans, lane=None):
+        """decode_region_device for plans of one pass_key and different shapes, in one pass (DESIGN §4.8 "Batches";
+        f16 / f16x2): offs / lens int64 [N][streams], per scale and channel the plan's tile streams padded with empty
+        ones to the pass's largest tile count (stream_layout(pad_tiles=True)).  Per scale: one range-decoder launch per
+        channel step for every stream of the pass; the decoder network on a padded batch [N][max h][max w] of the
+        windows, window n top-left (get_P_nhwc(windows=)); rows from each plan's used rectangle of its output
+        (l3c_dmll_build_table_windows); the symbols back to raster planes padded alike (l3c_reorder_tiles_images); the
+        next windows and the regions cut by l3c_crop_rects.  -> [uint8 [1, C, h_n, w_n]], the regions."""
+        dev = blob.device
+        N = len(plans)
+        p0 = plans[0]
+        tile = p0.tile
+        rects_of = [[(sp.C, sp.rect[2] - sp.rect[0], sp.rect[3] - sp.rect[1]) for sp in p.scales] for p in plans]
+        si, elem, n_sym, planes = stream_layout(rects_of, tile, pad_tiles=True)
+        bounds = np.searchsorted(si[0], np.arange(len(planes) + 1))
+        K = self.net.config_ms.prob.K
+        walk = list(self.iter_scale_dmll(p0.recursive))[:len(p0.scales)]
+
+        def rows_dev(rows):
+            return E._to_device_async(np.array(rows, np.int32).reshape(N, -1), dev)
+
+        def size(r):
+            return r[2] - r[0], r[3] - r[1]
+
+        counts = self.__dict__.setdefault('region_counts', {'streams': 0, 'symbols': 0})
+        bn8, F_win, S = None, None, None
+        self._mark('start')
+        for idx, (scale, dmll, uniform) in enumerate(walk):
+            sps = [p.scales[idx] for p in plans]
+            C = sps[0].C
+            ext = [size(sp.rect) for sp in sps]
+            Hm, Wm = max(h for h, _ in ext), max(w for _, w in ext)
+            plane = int(planes[idx])
+            cols = slice(bounds[idx], bounds[idx + 1])
+            T = (cols.stop - cols.start) // C
+            Sp = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # symbols in each plan's tile order
+            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
+            d = desc.reshape(N, C, T)
+            d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
+            d['in_len'][:] = lens[:, cols].reshape(N, C, T)
+            d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
+            d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
+            counts['streams'] += int((desc['n_sym'] > 0).sum())
+            counts['symbols'] += int(desc['n_sym'].sum())
+            if uniform:
+                d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
+                d['row_pitch'][:] = 0
+                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
+            else:
+                wins = [size(sp.window) for sp in sps]
+                l, F = self.net.get_P_nhwc(scale, bn8, F_win if sps[0].fused else None,
+                                           windows=wins if len(set(wins)) > 1 else None)
+                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
+                want = (2 * max(h for h, _ in wins), 2 * max(w for _, w in wins))
+                if tuple(l.shape[1:3]) != want or non_shared_get_K(l.shape[-1], C) != K:
+                    raise ValueError('container scale %d (C=%d) does not match the model output %s'
+                                     % (scale, C, tuple(l.shape)))
+                pitch = E.table_pitch(dmll.L)
+                table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
+                d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
+                d['row_pitch'][:] = pitch
+                tg = dmll.targets(dev)
+                geo = rows_dev([(sp.out[0], sp.out[1], h, w) for sp, (h, w) in zip(sps, ext)])
+                max_hw = max(h * w for h, w in ext)
+                if dmll.rgb_scale:
+                    for c in range(C):
+                        E.dmll_build_table_windows(l, geo, max_hw, plane, Sp, tg, C, K, dmll.L, True, c, table, tile)
+                        dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
+                        self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
+                else:
+                    E.dmll_build_table_windows(l, geo, max_hw, plane, Sp, tg, C, K, dmll.L, False, -1, table, tile)
+                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
+            S = E.reorder_tiles_images(Sp, rows_dev(ext), Hm, Wm, tile)            # [N][C][Hm][Wm], zero-padded
+            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
+                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
+            if idx + 1 == len(walk):
+                break
+            # the finer networks' inputs: their windows of this scale's symbols, and of this scale's features
+            nxt = [p.scales[idx + 1] for p in plans]
+            wins = [size(nx.window) for nx in nxt]
+            wh, ww = max(h for h, _ in wins), max(w for _, w in wins)
+            S_win = E.crop_rects(S, rows_dev([(nx.window[0] - sp.rect[0], nx.window[1] - sp.rect[1], h, w)
+                                              for nx, sp, (h, w) in zip(nxt, sps, wins)]), wh, ww, nhwc=False)
+            bn8 = E.symbols_to_values(S_win, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
+            F_win = None
+            if nxt[0].fused:
+                F_win = E.crop_rects(F.f, rows_dev([(nx.window[0] - 2 * sp.window[0], nx.window[1] - 2 * sp.window[1],
+                                                     h, w) for nx, sp, (h, w) in zip(nxt, sps, wins)]),
+                                     wh, ww, nhwc=True)
+        regs = [size(p.region) for p in plans]
+        return E.crop_rects(S, rows_dev([(p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1], h, w)
+                                         for p, (h, w) in zip(plans, regs)]),
+                            max(h for h, _ in regs), max(w for _, w in regs), nhwc=False, sizes=regs)
 
     # stage timing of a decode (bench.py / tools): set `codec.stage_events = []` before decode_device,
     # synchronise, then read stage_ms()

@@ -85,24 +85,40 @@ __host__ __device__ __forceinline__ int tile_order_to_raster(int r, int H, int W
     return (ty * th + rem2 / w) * W + tx * tw + rem2 % w;
 }
 
+// Position of raster pixel (y, x) in the tile order of an H x W plane (the inverse of tile_order_to_raster).
+__host__ __device__ __forceinline__ int raster_to_tile_order(int y, int x, int H, int W, int th, int tw) {
+    const int ty = y / th, tx = x / tw;
+    const int h = min(th, H - ty * th), w = min(tw, W - tx * tw);
+    return ty * th * W + tx * tw * h + (y - ty * th) * w + (x - tx * tw);
+}
+
 // rows (and the symbols of the already decoded channels, `sym`) are indexed in STREAM order: raster order, or
 // tile order when th > 0; the parameters `l` are always read at the raster pixel.  WIN: the H x W symbol plane is
 // the rectangle at (oy, ox) of a wider parameter plane of l_hw pixels per image and width Wl (a decoder window,
 // l3c_dmll_build_table_window); otherwise `l` covers exactly the H x W plane and the last four arguments are unused.
-template <int K, bool WIN>
+// IMG (with WIN): every image n has its own rectangle, geo[n] = (oy, ox, H_n, W_n), cut into its own tile grid;
+// HW is then the stride of the stream-order planes (>= H_n * W_n) and H, W, oy, ox are unused
+// (l3c_dmll_build_table_windows).
+template <int K, bool WIN, bool IMG = false>
 __global__ void __launch_bounds__(TB_THREADS)
 dmll_table_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
                   const float *__restrict__ targets, int HW, int C, int L, int rgb, int c_first,
                   int pix0, int npix, uint16_t *__restrict__ table, int pitch, int H, int W, int th, int tw,
-                  int64_t l_hw, int Wl, int oy, int ox) {
+                  int64_t l_hw, int Wl, int oy, int ox, const int4 *__restrict__ geo) {
     __shared__ float s_pi[TB_PIX][K];
     __shared__ float s_mu[TB_PIX][K];
     __shared__ float s_is[TB_PIX][K];
     const int Kp = (rgb ? 4 : 3) * C * K;
     const int n = blockIdx.y;
     const int c = c_first + blockIdx.z;
+    if (IMG) {
+        const int4 g = geo[n];
+        oy = g.x, ox = g.y, H = g.z, W = g.w;
+        npix = H * W;
+    }
     const int q0 = blockIdx.x * TB_PIX;                // offset inside [pix0, pix0+npix)
     const int np = min(TB_PIX, npix - q0);
+    if (IMG && np <= 0) return;                        // past this image's rectangle (uniform per CTA)
     if ((int)threadIdx.x < np) {
         const int p = pix0 + q0 + threadIdx.x;                                     // stream-order index
         const int pr = th > 0 ? tile_order_to_raster(p, H, W, th, tw) : p;         // raster pixel
@@ -491,7 +507,7 @@ extern "C" int l3c_dmll_build_table(const float *l_dev, const uint8_t *sym_dev,
     dim3 grid(ceil_div(npix, TB_PIX), N, c < 0 ? C : 1);
     dmll_table_kernel<10, false><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, pix0, npix, table_dev, pitch, 0, 0, 0, 0, 0, 0, 0,
-        0);
+        0, nullptr);
     L3C_LAUNCH_CHECK("dmll_table_kernel");
     return L3C_OK;
 }
@@ -526,7 +542,8 @@ extern "C" int l3c_dmll_build_table_tiled(const float *l_dev, const uint8_t *sym
     L3C_REQUIRE(th >= 1 && tw >= 1 && H >= 1 && W >= 1, "l3c_dmll_build_table_tiled: tile %dx%d", th, tw);
     dim3 grid(ceil_div(HW, TB_PIX), N, c < 0 ? C : 1);
     dmll_table_kernel<10, false><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
-        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, 0, HW, table_dev, pitch, H, W, th, tw, 0, 0, 0, 0);
+        l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, 0, HW, table_dev, pitch, H, W, th, tw, 0, 0, 0, 0,
+        nullptr);
     L3C_LAUNCH_CHECK("dmll_table_kernel");
     return L3C_OK;
 }
@@ -549,7 +566,30 @@ extern "C" int l3c_dmll_build_table_window(const float *l_dev, int Hl, int Wl, i
     dim3 grid(ceil_div(HW, TB_PIX), N, c < 0 ? C : 1);
     dmll_table_kernel<10, true><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, HW, C, L, rgb, c < 0 ? 0 : c, 0, HW, table_dev, pitch, H, W, th, tw,
-        (int64_t)Hl * Wl, Wl, oy, ox);
+        (int64_t)Hl * Wl, Wl, oy, ox, nullptr);
+    L3C_LAUNCH_CHECK("dmll_table_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_build_table_windows(const float *l_dev, int Hl, int Wl, const int *geo_dev, int max_hw,
+                                            int plane, const uint8_t *sym_dev, const float *targets_dev, int N, int C,
+                                            int K, int L, int rgb, int c, int th, int tw, uint16_t *table_dev,
+                                            int pitch, void *stream) {
+    using namespace l3c;
+    if (int e = check_common("l3c_dmll_build_table_windows", N, plane, C, K, L, rgb)) return e;
+    L3C_REQUIRE(l_dev && targets_dev && table_dev && geo_dev, "l3c_dmll_build_table_windows: null pointer");
+    L3C_REQUIRE(!(rgb && c > 0) || sym_dev, "l3c_dmll_build_table_windows: decoded symbols needed for c>0");
+    L3C_REQUIRE(c < C && (c >= 0 || !rgb), "l3c_dmll_build_table_windows: c=%d C=%d rgb=%d", c, C, rgb);
+    L3C_REQUIRE((pitch == 32 && L <= 32) || (pitch == 256 && L <= 256 && L > 32),
+                "l3c_dmll_build_table_windows: pitch=%d must be 32 (L<=32) or 256, L=%d", pitch, L);
+    L3C_REQUIRE(th >= 1 && tw >= 1 && Hl >= 1 && Wl >= 1 && max_hw >= 1 && max_hw <= plane,
+                "l3c_dmll_build_table_windows: tile %dx%d, %dx%d parameter plane, max_hw=%d plane=%d", th, tw, Hl, Wl,
+                max_hw, plane);
+    L3C_REQUIRE(((uintptr_t)geo_dev & 15) == 0, "l3c_dmll_build_table_windows: geo must be 16-byte aligned");
+    dim3 grid(ceil_div(max_hw, TB_PIX), N, c < 0 ? C : 1);
+    dmll_table_kernel<10, true, true><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, plane, C, L, rgb, c < 0 ? 0 : c, 0, 0, table_dev, pitch, 0, 0, th, tw,
+        (int64_t)Hl * Wl, Wl, 0, 0, (const int4 *)geo_dev);
     L3C_LAUNCH_CHECK("dmll_table_kernel");
     return L3C_OK;
 }
@@ -579,7 +619,81 @@ __global__ void crop_rect_kernel(const T *__restrict__ src, T *__restrict__ dst,
     const int64_t y = origins[2 * n] + e / w, x = origins[2 * n + 1] + e % w;
     dst[((int64_t)plane * h * w + e) * per_elem + k] = src[(((int64_t)plane * H + y) * W + x) * per_elem + k];
 }
+
+// crop_rect_kernel with a rectangle per image, rects[n] = (y, x, h_n, w_n).  dst_off null: dst is N * planes planes of
+// hp x wp, image n top-left, zero elsewhere; otherwise image n's planes of h_n x w_n start at element dst_off[n].
+template <typename T>
+__global__ void crop_rects_kernel(const T *__restrict__ src, T *__restrict__ dst, int per_elem, int planes, int H,
+                                  int W, const int4 *__restrict__ rects, const int64_t *__restrict__ dst_off, int hp,
+                                  int wp) {
+    const int plane = blockIdx.y;
+    const int n = plane / planes;
+    const int4 rc = rects[n];
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t e = r / per_elem, k = r % per_elem;
+    if (dst_off) {
+        if (r >= (int64_t)rc.z * rc.w * per_elem) return;
+        const int64_t y = rc.x + e / rc.w, x = rc.y + e % rc.w;
+        dst[dst_off[n] + ((int64_t)(plane - n * planes) * rc.z * rc.w + e) * per_elem + k] =
+            src[(((int64_t)plane * H + y) * W + x) * per_elem + k];
+        return;
+    }
+    if (r >= (int64_t)hp * wp * per_elem) return;
+    const int64_t oy = e / wp, ox = e % wp;
+    dst[((int64_t)plane * hp * wp + e) * per_elem + k] =
+        (oy < rc.z && ox < rc.w) ? src[(((int64_t)plane * H + rc.x + oy) * W + rc.y + ox) * per_elem + k] : T(0);
+}
+
+// stream order -> raster for images of different sizes: image n's planes hold the tile order of its own
+// ext[n] = (h_n, w_n) plane in the first h_n * w_n of `plane_len` bytes; dst planes are hp x wp, zero outside h_n x w_n
+__global__ void reorder_tiles_images_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, int planes,
+                                            int64_t plane_len, int hp, int wp, const int *__restrict__ ext, int th,
+                                            int tw) {
+    const int plane = blockIdx.y;
+    const int n = plane / planes;
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= hp * wp) return;
+    const int y = r / wp, x = r - y * wp, h = ext[2 * n], w = ext[2 * n + 1];
+    dst[(int64_t)plane * hp * wp + r] =
+        (y < h && x < w) ? src[plane * plane_len + raster_to_tile_order(y, x, h, w, th, tw)] : (uint8_t)0;
+}
 }  // namespace l3c
+
+extern "C" int l3c_crop_rects(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
+                              const int *rects_dev, const int64_t *dst_off_dev, int hp, int wp, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(src_dev && dst_dev && src_dev != dst_dev && rects_dev, "l3c_crop_rects: bad pointers");
+    L3C_REQUIRE(((uintptr_t)rects_dev & 15) == 0, "l3c_crop_rects: rects must be 16-byte aligned");
+    L3C_REQUIRE(elem_bytes >= 1 && planes >= 1 && N >= 1 && (int64_t)N * planes <= 65535 && hp >= 1 && wp >= 1 &&
+                    hp <= H && wp <= W,
+                "l3c_crop_rects: elem_bytes=%d planes=%d N=%d %dx%d of %dx%d", elem_bytes, planes, N, hp, wp, H, W);
+    const bool words = elem_bytes % 4 == 0;
+    const int per_elem = words ? elem_bytes / 4 : elem_bytes;
+    dim3 grid((unsigned)ceil_div64((int64_t)hp * wp * per_elem, 256), N * planes);
+    if (words)
+        crop_rects_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
+            (const uint32_t *)src_dev, (uint32_t *)dst_dev, per_elem, planes, H, W, (const int4 *)rects_dev,
+            dst_off_dev, hp, wp);
+    else
+        crop_rects_kernel<uint8_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
+            (const uint8_t *)src_dev, (uint8_t *)dst_dev, per_elem, planes, H, W, (const int4 *)rects_dev,
+            dst_off_dev, hp, wp);
+    L3C_LAUNCH_CHECK("crop_rects_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_reorder_tiles_images(const uint8_t *src_dev, uint8_t *dst_dev, int planes, int N, int plane_len,
+                                        int hp, int wp, const int *extents_dev, int th, int tw, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(src_dev && dst_dev && src_dev != dst_dev && extents_dev, "l3c_reorder_tiles_images: bad pointers");
+    L3C_REQUIRE(planes >= 1 && N >= 1 && (int64_t)N * planes <= 65535 && hp >= 1 && wp >= 1 && th >= 1 && tw >= 1 &&
+                    plane_len >= 1, "l3c_reorder_tiles_images: bad arguments");
+    dim3 grid(ceil_div(hp * wp, 256), N * planes);
+    reorder_tiles_images_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src_dev, dst_dev, planes, plane_len, hp, wp,
+                                                                        extents_dev, th, tw);
+    L3C_LAUNCH_CHECK("reorder_tiles_images_kernel");
+    return L3C_OK;
+}
 
 extern "C" int l3c_crop_rect(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,
                              const int *origins_dev, int h, int w, void *stream) {

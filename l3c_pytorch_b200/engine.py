@@ -418,11 +418,11 @@ def conv2d(conv, x, cin=None, relu=False, residual=None, pixel_shuffle=False, ou
     mode = _PRECISION['mode'] if precision is None else precision
     if mode == _lib.PREC_F16:
         return _conv2d_f16(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want)
-    if _RAGGED['v'] is not None:
-        raise NotImplementedError('ragged batches run in precision f16 only, not %s'
-                                  % {v: k for k, v in _lib.PRECISIONS.items()}[mode])
     if mode == _lib.PREC_F16X2:
         return _conv2d_f16x2(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want)
+    if _RAGGED['v'] is not None:
+        raise NotImplementedError('ragged batches run in precision f16 or f16x2 only, not %s'
+                                  % {v: k for k, v in _lib.PRECISIONS.items()}[mode])
     x = xa.f
     require_cuda(x, 'x')
     assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4
@@ -587,6 +587,7 @@ def _conv2d_f16x2(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, w
         if xa.r is None or xa.r.dtype != torch.float16 or xa.r.shape[-1] != 2 * cin_all:
             xa = Act(xa.f, split_f16x2(xa.f))
         w_h, b = pc.get_f16x2()
+        _ragged_guard(kh, dil, xa.r)
         yh_pitch = y_h.shape[-1] if y_h is not None else 0
         d = ConvDesc(x_h=xa.r.data_ptr(), w_h=w_h.data_ptr(), bias=b.data_ptr(),
                      residual=residual.data_ptr() if residual is not None else None,
@@ -613,6 +614,7 @@ def _conv2d_f16x2(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, w
         else:
             assert xa.f is not None, 'an fp32 (CUDA-core) layer needs the fp32 activation'
             w, b = pc.get()
+            _ragged_guard(kh, dil, xa.f)
             d = ConvDesc(x=xa.f.data_ptr(), w=w.data_ptr(), bias=b.data_ptr(),
                          residual=residual.data_ptr() if residual is not None else None, y=y.data_ptr(),
                          N=N, H=H, W=W, Cin=cin, x_pitch=xa.f.shape[-1], Cout=cout, cout_pad=b.shape[0],
@@ -811,6 +813,59 @@ def crop_rect(src, origins_dev, h, w, nhwc):
                             _stream_ptr()))
     LAUNCHES['n'] += 1
     return out
+
+
+def dmll_build_table_windows(l, geo_dev, max_hw, plane, sym, targets, C, K, L, rgb, c, table, tile):
+    """dmll_build_table_window with a rectangle per image (l3c_dmll_build_table_windows): geo_dev int32 [N, 4] =
+    (oy, ox, H_n, W_n) on the device; rows and `sym` in each image's own tile order, in planes of `plane` elements."""
+    N, Hl, Wl, _ = l.shape
+    assert l.is_contiguous() and geo_dev.shape == (N, 4) and geo_dev.dtype == torch.int32
+    check(lib.l3c_dmll_build_table_windows(_ptr(l), Hl, Wl, _ptr(geo_dev), int(max_hw), int(plane), _ptr(sym),
+                                           _ptr(targets), N, C, K, L, int(rgb), c, tile[0], tile[1], _ptr(table),
+                                           table_pitch(L), _stream_ptr()))
+    LAUNCHES['n'] += 1
+
+
+def crop_rects(src, rects_dev, hp, wp, nhwc, sizes=None):
+    """l3c_crop_rects: the rectangle rects_dev[n] = (y, x, h_n, w_n) (int32 [N, 4] on the device) of image n.
+    sizes None: -> one tensor, [N, hp, wp, C] (nhwc) or [N, P, hp, wp], image n top-left and +0 elsewhere.
+    sizes = [(h_n, w_n)] (planes only): -> [tensor [1, P, h_n, w_n]], contiguous views of one buffer."""
+    assert src.is_contiguous() and src.dim() == 4
+    N = rects_dev.shape[0]
+    if nhwc:
+        H, W, planes = src.shape[1], src.shape[2], 1
+        elem_bytes = src.shape[3] * src.element_size()
+        shape = (N, hp, wp, src.shape[3])
+    else:
+        H, W, planes = src.shape[2], src.shape[3], src.shape[1]
+        elem_bytes = src.element_size()
+        shape = (N, planes, hp, wp)
+    off_dev, views = None, None
+    if sizes is None:
+        out = torch.empty(shape, dtype=src.dtype, device=src.device)
+    else:
+        assert not nhwc and len(sizes) == N
+        n_el = [planes * h * w for (h, w) in sizes]
+        offs = np.concatenate([[0], np.cumsum(n_el)]).astype(np.int64)
+        out = torch.empty(int(offs[-1]), dtype=src.dtype, device=src.device)
+        off_dev = _to_device_async(offs[:-1], src.device)
+        views = [out[offs[n]:offs[n + 1]].view(1, planes, h, w) for n, (h, w) in enumerate(sizes)]
+    check(lib.l3c_crop_rects(_ptr(src), _ptr(out), elem_bytes, planes, N, H, W, _ptr(rects_dev), _ptr(off_dev),
+                             int(hp), int(wp), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return out if views is None else views
+
+
+def reorder_tiles_images(src, extents_dev, hp, wp, tile):
+    """uint8 [N, P, plane] in each image's own tile order (extents_dev int32 [N, 2] = (h_n, w_n) on the device) ->
+    raster [N, P, hp, wp], image n top-left and 0 elsewhere (l3c_reorder_tiles_images)."""
+    assert src.is_contiguous() and src.dtype == torch.uint8 and src.dim() == 3
+    N, P, plane = src.shape
+    dst = torch.empty(N, P, hp, wp, dtype=torch.uint8, device=src.device)
+    check(lib.l3c_reorder_tiles_images(_ptr(src), _ptr(dst), P, N, plane, int(hp), int(wp), _ptr(extents_dev),
+                                       tile[0], tile[1], _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return dst
 
 
 def reorder_tiles(src, H, W, tile, to_tiles):

@@ -434,6 +434,14 @@ class MultiscaleNetwork(nn.Module):
             return 'ragged batches run in precision f16 only, not %s' % E.get_conv_precision()
         return None
 
+    def windows_unsupported(self):
+        """Why this network cannot run a decoder on a ragged batch of region windows (get_P_nhwc(windows=)), or None
+        when it can.  Only the decoder and classifier convs run there, so unlike ragged_unsupported this allows the RGB
+        baselines, recursive scales and f16x2."""
+        if not (E.f16_mode() or E.f16x2_mode()):
+            return 'ragged decoder windows run in precision f16 or f16x2 only, not %s' % E.get_conv_precision()
+        return None
+
     def _check_ragged(self, extents, auto_recurse=0):
         why = None if extents is None else self.ragged_unsupported(auto_recurse)
         if why is not None:
@@ -554,10 +562,13 @@ class MultiscaleNetwork(nn.Module):
                 prev_x = loss_dmm.sample(nchw_view(P), C=C)
         return prev_x
 
-    def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False, extents=None):
+    def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False, extents=None, windows=None):
         """-> (parameters NHWC, decoder features as engine.Act for the next finer scale).  At scale 0 the
         features feed nothing else (need_F=True keeps their fp32 tensor for the reference-shaped get_P).
         extents: [(h_n, w_n)] at the FINEST scale -> bn8 is a ragged batch (forward()).
+        windows: [(h_n, w_n)] at bn8's own resolution -> bn8 (and dec_F_prev) is a padded batch of region windows of
+        different sizes (DESIGN §4.8), window n top-left; the outputs inside 2 x window n are bit-identical to a run
+        on that window alone (windows_unsupported).
         scale >= num_scales: a recursive scale of forward(auto_recurse=R) (RGB baselines), num_scales + k the k-th
         extra application of the last trained scale: nets[-1] / prob_clfs[-1], no features in or out (like scale 0,
         its features feed nothing but its probability classifier).  The bit-coder decodes recursive scales of the
@@ -567,8 +578,15 @@ class MultiscaleNetwork(nn.Module):
         assert 0 <= scale, 'Out of range: {}'.format(scale)
         if recursive and dec_F_prev is not None:
             raise ValueError('recursive scale %d takes no decoder features' % scale)
-        self._check_ragged(extents, int(recursive))
         f = 2 ** (scale + 1)
+        if windows is not None:
+            assert extents is None, 'extents and windows exclude each other'
+            why = self.windows_unsupported()
+            if why is not None:
+                raise NotImplementedError(why)
+            extents, f = [(2 * int(h), 2 * int(w)) for (h, w) in windows], 2
+        else:
+            self._check_ragged(extents, int(recursive))
         s = -1 if recursive else scale
         with E.ragged_extents(extents, bn8.shape[1] * f, bn8.shape[2] * f):
             F = self.nets[s].dec(bn8, dec_F_prev, operand_only=((scale == 0 or recursive) and not need_F)).F

@@ -144,8 +144,16 @@ class RegionPlan(object):
 
     def shape_key(self):
         """Plans with equal keys decode as one batch (BatchCodec.decode_regions): every rectangle has the same size
-        and every network output the same used rectangle, wherever the regions lie."""
-        return (self.tile, self.n_scales, self.level, tuple(s.shape_key() for s in self.scales))
+        and every network output the same used rectangle, wherever the regions lie, and the regions have one size
+        (regions of different sizes inside the same tiles plan the same rectangles)."""
+        r = self.region
+        return (self.tile, self.n_scales, self.level, (r[2] - r[0], r[3] - r[1]),
+                tuple(s.shape_key() for s in self.scales))
+
+    def pass_key(self):
+        """Plans with equal keys walk the same scales with the same tile size: where ragged windows are supported they
+        decode in one pass whatever their shape_key (BatchCodec.decode_regions)."""
+        return (self.tile, self.n_scales, self.level)
 
     def __repr__(self):
         return 'RegionPlan(level=%d, region=%s, tiles=%d, symbols=%d, window_pixels=%d)' % (
@@ -226,3 +234,13 @@ def stream_columns(plan, tile):
         T = len(tile_grid(sp.H, sp.W, tile))
         cols.append([c * T + t for c in range(sp.C) for t in sp.tiles])
     return cols
+
+
+def plan_passes(plans, ragged):
+    """How BatchCodec.decode_regions runs a list of plans: -> [(indices into plans, is_ragged)] in order of first
+    appearance.  Plans of one shape_key always share a pass of equal shapes.  ragged (the decoder networks can run
+    padded batches of windows): plans of one pass_key share one ragged pass, unless their shape_keys are all equal."""
+    groups = {}
+    for i, p in enumerate(plans):
+        groups.setdefault(p.pass_key() if ragged else p.shape_key(), []).append(i)
+    return [(idxs, len({plans[i].shape_key() for i in idxs}) > 1) for idxs in groups.values()]
