@@ -16,8 +16,10 @@ Decoding uploads the concatenated containers once and decodes every stream in pl
 Equal-size, tiled and ragged batches share one encode and one decode path: `stream_layout` says where every
 stream's intervals (encode) or symbols and CDF rows (decode) sit in the `[N][C][plane]` tensor of its scale, and
 only the step between those stream planes and the raster planes of the networks differs (a view, l3c_reorder_tiles
-or l3c_ragged_pack).
+or l3c_ragged_pack).  Every decode -- full (`decode_device`) or of regions of tiled containers (`decode_region_pass`,
+DESIGN §4.8) -- is one coarse-to-fine walk, `BatchCodec._decode_scales`, told its geometry by the caller.
 """
+import functools
 import os
 import struct
 
@@ -35,8 +37,6 @@ def _on_device(fn):
     """Run a codec entry point with the blueprint's GPU as the current CUDA device: the kernels of the
     shared library launch on whatever device is current, and `current_stream()` is per device -- a
     Blueprint(device='cuda:1') must not depend on the caller having called torch.cuda.set_device(1)."""
-    import functools
-
     @functools.wraps(fn)
     def wrapped(self, *a, **kw):
         dev = self.codec.blueprint.device if isinstance(self, EncodeJob) else self.blueprint.device
@@ -296,6 +296,9 @@ class BatchCodec(object):
         self.blueprint = blueprint
         self.net = blueprint.net
         self._const = {}
+        self._lane_cache = {}
+        # streams and symbols the last decode_regions call handed to the range decoder (decode_region_pass)
+        self.region_counts = {'streams': 0, 'symbols': 0}
 
     # ------------------------------------------------------------------------------------------
     def iter_scale_dmll(self, recursive=0):
@@ -533,7 +536,7 @@ class BatchCodec(object):
         and keeps only ~1/6 of the GPU busy.  L3C_SM_PARTITION=0, a driver without green contexts or an
         attached profiler give ordinary streams (slower, same bytes)."""
         key = (str(dev), n_decoders, n_lanes)
-        cache = self.__dict__.setdefault('_lane_cache', {})
+        cache = self._lane_cache
         if key not in cache:
             part = None
             # encode streams: an encode is a throughput phase (the networks) followed by a latency-bound one (the
@@ -601,6 +604,94 @@ class BatchCodec(object):
         cur.wait_event(done)
         return out
 
+    def _stream_descs(self, blob, offs, lens, layout, idx, Sp, table, pitch):
+        """Range-decoder descriptors of scale `idx` of a pass whose streams `layout` (stream_layout's result) places:
+        every stream reads its bytes in place in `blob` (offs / lens int64 [N][streams per image], the layout's
+        order), writes its symbols to its elements of the stream planes Sp [N][C][plane] and finds its CDF rows at
+        the same elements of `table` (int16, `pitch` entries per symbol; pitch 0: the one row of a uniform prior).
+        -> (desc [N * C * T], its [N][C][T] view)."""
+        si, elem, n_sym, _ = layout
+        N, C = Sp.shape[:2]
+        lo, hi = np.searchsorted(si[0], [idx, idx + 1])                 # scale idx: columns lo:hi
+        cols, T = slice(lo, hi), (hi - lo) // C
+        desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
+        d = desc.reshape(N, C, T)
+        d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
+        d['in_len'][:] = lens[:, cols].reshape(N, C, T)
+        d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
+        d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
+        d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
+        d['row_pitch'][:] = pitch
+        return desc, d
+
+    def _decode_scales(self, blob, offs, lens, layout, channels, recursive, lane, network, rows, raster,
+                       symbols=lambda idx, S: S, features=lambda idx, F: F,
+                       row_pitch=lambda dmll: E.table_pitch(dmll.L)):
+        """The coarse-to-fine walk of every decode: full decodes of equal-size, tiled and ragged batches
+        (decode_device) and region passes (decode_region_pass).  blob, offs, lens, layout: as in _stream_descs;
+        channels: C of every scale walked, coarse -> fine (a region at level k stops early); recursive: as in
+        iter_scale_dmll; lane: as in decode_device.  -> the raster planes of the last scale.
+        Every scale decodes into stream planes Sp [N][C][plane], where its CDF rows are built too, and then goes back
+        to the raster planes the network of the next scale reads:
+          * the uniform-prior scale is one range-decoder launch on the lane's decoder stream;
+          * any other scale runs its decoder network, checks the output against the container, lays out the row
+            table and runs the channel steps: on an RGB scale channel c's means depend on the decoded channels < c
+            of the same pixel, so R, G, B go one after the other -- the rows of c, then one launch decoding every
+            stream of c -- while a bottleneck scale builds all rows and decodes every stream in one launch;
+          * the symbols become raster planes, and the next scale gets their values and this scale's features.
+        What differs between the passes is geometry, asked of the caller's hooks with the scale's index idx:
+          network(idx, scale, bn8, F) -> (l, F, (H, W)): get_P_nhwc on the coarser scale's values bn8 and features F,
+            and the height and width its output l must have;
+          row_pitch(dmll) -> entries per row of the table (full rows unless the caller's `rows` reads coarse records);
+          rows(idx, dmll, l, Sp, table, d, steps): code the scale -- steps(build) runs the channel steps above with
+            build(c) building the rows of channel c (of every channel for c = -1) -- or decode it some other way
+            from the [N][C][T] descriptors d;
+          raster(idx, Sp) -> S [N][C][H][W]; symbols(idx, S), features(idx, F) -> what of them the next network reads
+            (all of it by default)."""
+        dev = blob.device
+        N = offs.shape[0]
+        K = self.net.config_ms.prob.K
+        bn8, F, S = None, None, None
+        self._mark('start')
+        for idx, ((scale, dmll, uniform), C) in enumerate(zip(self.iter_scale_dmll(recursive), channels)):
+            Sp = torch.empty(N, C, int(layout[3][idx]), dtype=torch.uint8, device=dev)     # symbols in stream order
+
+            def decode(dsc):
+                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(dsc, dev, dmll.L))
+
+            def steps(build):
+                if dmll.rgb_scale:
+                    for c in range(C):
+                        build(c)
+                        decode(np.ascontiguousarray(d[:, c, :]).reshape(-1))
+                else:
+                    build(-1)
+                    decode(desc)
+
+            if uniform:
+                table, pitch = self._uniform(dmll.L, dev)[1], 0
+            else:
+                l, F, want = network(idx, scale, bn8, F)
+                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
+                if tuple(l.shape[1:3]) != want or non_shared_get_K(l.shape[-1], C) != K:
+                    raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
+                                     % (scale, C, want[0], want[1], tuple(l.shape)))
+                pitch = row_pitch(dmll)
+                table = torch.empty(Sp.numel() * pitch, dtype=torch.int16, device=dev)
+            desc, d = self._stream_descs(blob, offs, lens, layout, idx, Sp, table, pitch)
+            if uniform:
+                decode(desc)
+            else:
+                rows(idx, dmll, l, Sp, table, d, steps)
+            S = raster(idx, Sp)
+            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
+                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
+            if idx + 1 < len(channels):
+                bn8 = E.symbols_to_values(symbols(idx, S), self._symbol_values(scale, dmll, dev),
+                                          self._rgb_shift(dev))
+                F = features(idx, F)
+        return S
+
     @_on_device
     def decode_device(self, blob, offs, lens, shapes, lane=None, tile=None):
         """Decode streams that already sit in HBM: `blob` uint8 device buffer (readable 4 bytes past
@@ -613,8 +704,8 @@ class BatchCodec(object):
         streams, so the three RGB channels are simply decoded one after the other, all tiles at once.
         shapes may also be one list per image: a ragged batch (DESIGN §4.6) when they differ; image n then is the
         top-left H_n x W_n of the result, zero elsewhere.
-        Every scale decodes into [N][C][plane] stream planes (stream_layout), where the CDF rows are built too, and
-        then goes back to the raster planes the networks of the next scale read."""
+        The scales are walked by _decode_scales; between stream and raster planes lies a view, l3c_reorder_tiles
+        (tiled) or l3c_ragged_pack (ragged)."""
         dev = blob.device
         N = offs.shape[0]
         if shapes and isinstance(shapes[0][0], (tuple, list)):
@@ -632,87 +723,55 @@ class BatchCodec(object):
         Rs = {self._check_shapes(sh) for sh in {tuple(sh): sh for sh in shapes_of}.values()}
         if len(Rs) != 1:
             raise ValueError('containers with different numbers of scales in one batch')
-        recursive = Rs.pop()
         if tile is not None:
             tile = (int(tile[0]), int(tile[1]))
-        si, elem, n_sym, planes = stream_layout(shapes_of, tile)
-        bounds = np.searchsorted(si[0], np.arange(len(planes) + 1))     # scale idx: columns bounds[idx]:bounds[idx+1]
         fin = [sh[-1][1:] for sh in shapes_of] if ragged else None      # extents at the finest scale
         K = self.net.config_ms.prob.K
-        bn8, F_prev, S = None, None, None
-        self._mark('start')
-        for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll(recursive)):
-            C = shapes_of[0][idx][0]
-            H, W = max(sh[idx][1] for sh in shapes_of), max(sh[idx][2] for sh in shapes_of)
-            plane = int(planes[idx])
-            ext_dev = E._to_device_async(np.array([sh[idx][1:] for sh in shapes_of], np.int32), dev) if ragged else None
-            cols = slice(bounds[idx], bounds[idx + 1])
-            T = (cols.stop - cols.start) // C
-            Sp = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # symbols in stream order
-            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
-            d = desc.reshape(N, C, T)
-            d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
-            d['in_len'][:] = lens[:, cols].reshape(N, C, T)
-            d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
-            d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
-            if uniform:
-                d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
-                d['row_pitch'][:] = 0
-                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            else:
-                # MultiscaleNetwork._forward's fusion rule: no decoder features cross into or out of a recursive
-                # scale, and the coarsest trained scale gets none
-                fuse = self.net._fuse_feat and scale < self.net.scales - 1
-                l, F_prev = self.net.get_P_nhwc(scale, bn8, F_prev if fuse else None, extents=fin)
-                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
-                if tuple(l.shape[1:3]) != (H, W) or non_shared_get_K(l.shape[-1], C) != K:
-                    raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
-                                     % (scale, C, H, W, tuple(l.shape)))
-                # the RGB scale of an equal-size batch in f16 mode decodes from coarse records (parameters + every 8th
-                # CDF entry, 192 instead of 512 B per sub-pixel; the decoder evaluates the bracketed entries itself);
-                # tiled and ragged batches, the bottleneck scales, L < 256 and the other precision modes build full rows
-                coarse = (dmll.rgb_scale and tile is None and not ragged and dmll.L == 256 and K == 10 and
-                          E.f16_mode())
-                pitch = E.COARSE_PITCH if coarse else E.table_pitch(dmll.L)
-                table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
-                d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
-                d['row_pitch'][:] = pitch
-                tg = dmll.targets(dev)
-                if tile is not None:
-                    if dmll.rgb_scale:
-                        # channel c's means depend on the decoded channels < c of the same pixel: R, G, B one
-                        # after the other, every tile of every image at once (N*T streams per launch)
-                        for c in range(C):
-                            E.dmll_build_table_tiled(l, Sp, tg, C, K, dmll.L, True, c, table, tile)
-                            dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
-                            self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
-                    else:
-                        E.dmll_build_table_tiled(l, Sp, tg, C, K, dmll.L, False, -1, table, tile)
-                        self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-                else:
-                    # per-pixel kernels from here on: the stream planes are an N x 1 x plane "image" each
-                    if ragged:
-                        l = E.ragged_pack(l, 1, H, W, ext_dev, plane, True)
-                    l = l.view(N, 1, plane, l.shape[-1])
-                    Sv = Sp.view(N, C, 1, plane)
-                    if dmll.rgb_scale:
-                        self._decode_rgb_pipelined(l, Sv, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane,
-                                                   coarse=coarse)
-                    else:
-                        E.dmll_build_table(l, Sv, tg, C, K, dmll.L, False, -1, table)
-                        self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            # back to raster planes
+        # per scale: H, W of the batch's raster planes and (ragged) every image's extent on the device, uploaded once
+        dims = [tuple(max(sh[idx][k] for sh in shapes_of) for k in (1, 2)) for idx in range(len(shapes_of[0]))]
+        ext_dev = functools.lru_cache(None)(
+            lambda idx: E._to_device_async(np.array([sh[idx][1:] for sh in shapes_of], np.int32), dev))
+
+        def coarse(dmll):
+            # the RGB scale of an equal-size batch in f16 mode decodes from coarse records (parameters + every 8th
+            # CDF entry, 192 instead of 512 B per sub-pixel; the decoder evaluates the bracketed entries itself);
+            # tiled and ragged batches, the bottleneck scales, L < 256 and the other precision modes build full rows
+            return dmll.rgb_scale and tile is None and not ragged and dmll.L == 256 and K == 10 and E.f16_mode()
+
+        def network(idx, scale, bn8, F):
             if ragged:
-                S = E.ragged_pack(Sp, C, H, W, ext_dev, plane, False)          # zero-padded [N][C][H][W]
-            elif tile is not None:
-                S = E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
+                ext_dev(idx)                      # queued ahead of the network: the rows and the raster step read it
+            l, F = self.net.get_P_nhwc(scale, bn8, F if self.net.fuses(scale) else None, extents=fin)
+            return l, F, dims[idx]
+
+        def rows(idx, dmll, l, Sp, table, d, steps):
+            C, plane, (H, W) = Sp.shape[1], Sp.shape[2], dims[idx]
+            tg = dmll.targets(dev)
+            if tile is not None:
+                # every tile of every image at once (N*T streams per launch)
+                return steps(lambda c: E.dmll_build_table_tiled(l, Sp, tg, C, K, dmll.L, c >= 0, c, table, tile))
+            # per-pixel kernels from here on: the stream planes are an N x 1 x plane "image" each
+            if ragged:
+                l = E.ragged_pack(l, 1, H, W, ext_dev(idx), plane, True)
+            l = l.view(N, 1, plane, l.shape[-1])
+            Sv = Sp.view(N, C, 1, plane)
+            if dmll.rgb_scale:
+                self._decode_rgb_pipelined(l, Sv, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane,
+                                           coarse=coarse(dmll))
             else:
-                S = Sp.view(N, C, H, W)
-            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
-                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
-            if scale > 0:
-                bn8 = E.symbols_to_values(S, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
-        return S
+                steps(lambda c: E.dmll_build_table(l, Sv, tg, C, K, dmll.L, False, -1, table))
+
+        def raster(idx, Sp):
+            C, (H, W) = Sp.shape[1], dims[idx]
+            if ragged:
+                return E.ragged_pack(Sp, C, H, W, ext_dev(idx), Sp.shape[2], False)    # zero-padded [N][C][H][W]
+            if tile is not None:
+                return E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
+            return Sp.view(N, C, H, W)
+
+        return self._decode_scales(
+            blob, offs, lens, stream_layout(shapes_of, tile), [s[0] for s in shapes_of[0]], Rs.pop(), lane,
+            network, rows, raster, row_pitch=lambda dmll: E.COARSE_PITCH if coarse(dmll) else E.table_pitch(dmll.L))
 
     # ------------------------------------------------------------------------------------------
     def plan_regions(self, datas, regions, levels=None):
@@ -749,229 +808,113 @@ class BatchCodec(object):
         order, each equal to the same crop of the full decode (at level k >= 1, of the stored scale-k plane).  Only the
         tile streams and decoder windows the region depends on are decoded.  In f16 and f16x2, pairs whose plans walk
         the same scales with the same tile size (RegionPlan.pass_key) share one ragged pass: one network pass per scale
-        on a padded batch of their windows and one range-decoder launch per channel step (decode_region_device_ragged);
-        pairs of equal RegionPlan.shape_key share the equal-shape pass (decode_region_device), and in tf32 / fp32 the
-        groups of equal shape_key run one after another (region.plan_passes; REGION_RAGGED_PASS = False forces that
-        grouping everywhere).  regions: (y, x, h, w) each; levels: None (all 0) or one int each.
+        on a padded batch of their windows and one range-decoder launch per channel step; pairs of equal
+        RegionPlan.shape_key share an equal-shape pass, and in tf32 / fp32 the groups of equal shape_key run one after
+        another (region.plan_passes, decode_region_pass; REGION_RAGGED_PASS = False forces that grouping everywhere).
+        regions: (y, x, h, w) each; levels: None (all 0) or one int each.
         lane: as in decode_batch -- the caller has made `lane.main` current; the range decoders run on the lane's
         decoder streams."""
-        from .region import plan_passes, stream_columns
+        from .region import pass_streams, plan_passes
         parsed, plans = self.plan_regions(datas, regions, levels)
-        dev = self.blueprint.device
-        blob, starts = _upload(datas, dev)
+        blob, starts = _upload(datas, self.blueprint.device)
         ragged = REGION_RAGGED_PASS and self.net.windows_unsupported() is None
         outs = [None] * len(datas)
-        # streams and symbols handed to the range decoder by this call (decode_region_device adds to them)
-        self.region_counts = {'streams': 0, 'symbols': 0}
+        self.region_counts = {'streams': 0, 'symbols': 0}          # of this call: every pass adds to them
         for idxs, is_ragged in plan_passes(plans, ragged):
-            # per scale the largest tile count of the pass: a ragged pass pads every channel's list to it with empty
-            # streams (stream_layout(pad_tiles=True)), which read nothing
-            n_sc = len(plans[idxs[0]].scales)
-            T_max = [max(len(plans[i].scales[k].tiles) for i in idxs) for k in range(n_sc)]
-            offs, lens = [], []
-            for i in idxs:
-                scales = parsed[i][1]
-                o, ln = [], []
-                for k, (sp, cs) in enumerate(zip(plans[i].scales, stream_columns(plans[i], plans[i].tile))):
-                    T = len(sp.tiles)
-                    for c in range(sp.C):
-                        for col in cs[c * T:(c + 1) * T]:
-                            o.append(starts[i] + scales[sp.idx][3][col][0])
-                            ln.append(scales[sp.idx][3][col][1])
-                        o += [starts[i]] * (T_max[k] - T)
-                        ln += [0] * (T_max[k] - T)
-                offs.append(o)
-                lens.append(ln)
-            offs, lens = np.array(offs, np.int64), np.array(lens, np.int64)
             sel = [plans[i] for i in idxs]
-            if is_ragged:
-                res = self.decode_region_device_ragged(blob, offs, lens, sel, lane=lane)
-            else:
-                S = self.decode_region_device(blob, offs, lens, sel, lane=lane)
-                res = [S[k:k + 1] for k in range(len(idxs))]
-            for k, i in enumerate(idxs):
-                outs[i] = res[k]
+            offs, lens = pass_streams(sel, [[st for (_, _, _, st) in parsed[i][1]] for i in idxs], starts[idxs])
+            for i, res in zip(idxs, self.decode_region_pass(blob, offs, lens, sel, is_ragged, lane=lane)):
+                outs[i] = res
         return outs
 
     @_on_device
-    def decode_region_device(self, blob, offs, lens, plans, lane=None):
-        """decode_device for region plans of equal shape_key (DESIGN §4.8): offs / lens int64 [N][planned streams]
-        in the order of region.stream_columns.  Every scale decodes the tiles of its plan's rectangle (a plane that
-        tile_grid cuts like the full one), its decoder network runs on the plan's window of the coarser scale
-        (symbols and, with dec.skip, features cropped by l3c_crop_rect) and its rows are built from the used
-        rectangle of that output in place (l3c_dmll_build_table_window).  -> uint8 [N, C, h, w], the regions.
-        lane: as in decode_device."""
+    def decode_region_pass(self, blob, offs, lens, plans, ragged, lane=None):
+        """_decode_scales for the region plans of one pass (DESIGN §4.8; region.plan_passes): offs / lens int64
+        [N][streams] from region.pass_streams.  Every scale decodes the tiles of each plan's rectangle (a plane that
+        tile_grid cuts like the full one), its decoder network runs on the plans' windows of the coarser scale
+        (symbols and, with dec.skip, features cut out of the coarser scale's) and its rows are built from the used
+        rectangle of that output in place.
+        ragged False: plans of equal shape_key, a batch of equal windows at per-image origins (l3c_crop_rect,
+        l3c_dmll_build_table_window, l3c_reorder_tiles).
+        ragged True ("Batches"; f16 / f16x2): plans of one pass_key and different shapes.  Every tensor is padded to
+        the pass's largest, plan n top-left (get_P_nhwc(windows=)), and the kernels take per-image rectangles
+        (l3c_crop_rects, l3c_dmll_build_table_windows, l3c_reorder_tiles_images); each plan's per-channel tile streams
+        are padded with empty ones to the pass's largest tile count (stream_layout(pad_tiles=True)).
+        -> [uint8 [1, C, h_n, w_n]], the regions.  lane: as in decode_device."""
         dev = blob.device
         N = len(plans)
         p0 = plans[0]
         tile = p0.tile
-        rects = [(sp.C, sp.rect[2] - sp.rect[0], sp.rect[3] - sp.rect[1]) for sp in p0.scales]
-        si, elem, n_sym, planes = stream_layout([rects] * N, tile)
-        bounds = np.searchsorted(si[0], np.arange(len(planes) + 1))
         K = self.net.config_ms.prob.K
-        walk = list(self.iter_scale_dmll(p0.recursive))[:len(p0.scales)]
-
-        def origins(fn):
-            return E._to_device_async(np.array([fn(p) for p in plans], np.int32).reshape(N, 2), dev)
-
-        counts = self.__dict__.setdefault('region_counts', {'streams': 0, 'symbols': 0})
-        bn8, F_win, S = None, None, None
-        self._mark('start')
-        for idx, (scale, dmll, uniform) in enumerate(walk):
-            sp = p0.scales[idx]
-            C, H, W = rects[idx]
-            plane = int(planes[idx])
-            cols = slice(bounds[idx], bounds[idx + 1])
-            T = (cols.stop - cols.start) // C
-            Sp = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # symbols in stream order
-            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
-            d = desc.reshape(N, C, T)
-            d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
-            d['in_len'][:] = lens[:, cols].reshape(N, C, T)
-            d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
-            d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
-            counts['streams'] += desc.shape[0]
-            counts['symbols'] += int(desc['n_sym'].sum())
-            if uniform:
-                d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
-                d['row_pitch'][:] = 0
-                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            else:
-                l, F = self.net.get_P_nhwc(scale, bn8, F_win if sp.fused else None)
-                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
-                wy0, wx0, wy1, wx1 = sp.window
-                if tuple(l.shape[1:3]) != (2 * (wy1 - wy0), 2 * (wx1 - wx0)) or non_shared_get_K(l.shape[-1], C) != K:
-                    raise ValueError('container scale %d (C=%d) does not match the model output %s'
-                                     % (scale, C, tuple(l.shape)))
-                pitch = E.table_pitch(dmll.L)
-                table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
-                d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
-                d['row_pitch'][:] = pitch
-                tg = dmll.targets(dev)
-                oy, ox = sp.out[:2]
-                if dmll.rgb_scale:
-                    for c in range(C):
-                        E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, True, c, table, H, W, tile)
-                        dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
-                        self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
-                else:
-                    E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, False, -1, table, H, W, tile)
-                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            S = E.reorder_tiles(Sp, H, W, tile, False).view(N, C, H, W)
-            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
-                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
-            if idx + 1 == len(walk):
-                break
-            # the finer network's inputs: its window of this scale's symbols, and of this scale's features
-            nxt = p0.scales[idx + 1]
-            wh, ww = nxt.window[2] - nxt.window[0], nxt.window[3] - nxt.window[1]
-            S_win = E.crop_rect(S, origins(lambda p: (p.scales[idx + 1].window[0] - p.scales[idx].rect[0],
-                                                      p.scales[idx + 1].window[1] - p.scales[idx].rect[1])),
-                                wh, ww, nhwc=False)
-            bn8 = E.symbols_to_values(S_win, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
-            F_win = None
-            if nxt.fused:
-                F_win = E.crop_rect(F.f, origins(lambda p: (p.scales[idx + 1].window[0] - 2 * p.scales[idx].window[0],
-                                                            p.scales[idx + 1].window[1] - 2 * p.scales[idx].window[1])),
-                                    wh, ww, nhwc=True)
-        y0, x0, y1, x1 = p0.region
-        return E.crop_rect(S, origins(lambda p: (p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1])),
-                           y1 - y0, x1 - x0, nhwc=False)
-
-    @_on_device
-    def decode_region_device_ragged(self, blob, offs, lens, plans, lane=None):
-        """decode_region_device for plans of one pass_key and different shapes, in one pass (DESIGN §4.8 "Batches";
-        f16 / f16x2): offs / lens int64 [N][streams], per scale and channel the plan's tile streams padded with empty
-        ones to the pass's largest tile count (stream_layout(pad_tiles=True)).  Per scale: one range-decoder launch per
-        channel step for every stream of the pass; the decoder network on a padded batch [N][max h][max w] of the
-        windows, window n top-left (get_P_nhwc(windows=)); rows from each plan's used rectangle of its output
-        (l3c_dmll_build_table_windows); the symbols back to raster planes padded alike (l3c_reorder_tiles_images); the
-        next windows and the regions cut by l3c_crop_rects.  -> [uint8 [1, C, h_n, w_n]], the regions."""
-        dev = blob.device
-        N = len(plans)
-        p0 = plans[0]
-        tile = p0.tile
-        rects_of = [[(sp.C, sp.rect[2] - sp.rect[0], sp.rect[3] - sp.rect[1]) for sp in p.scales] for p in plans]
-        si, elem, n_sym, planes = stream_layout(rects_of, tile, pad_tiles=True)
-        bounds = np.searchsorted(si[0], np.arange(len(planes) + 1))
-        K = self.net.config_ms.prob.K
-        walk = list(self.iter_scale_dmll(p0.recursive))[:len(p0.scales)]
-
-        def rows_dev(rows):
-            return E._to_device_async(np.array(rows, np.int32).reshape(N, -1), dev)
 
         def size(r):
             return r[2] - r[0], r[3] - r[1]
 
-        counts = self.__dict__.setdefault('region_counts', {'streams': 0, 'symbols': 0})
-        bn8, F_win, S = None, None, None
-        self._mark('start')
-        for idx, (scale, dmll, uniform) in enumerate(walk):
-            sps = [p.scales[idx] for p in plans]
-            C = sps[0].C
-            ext = [size(sp.rect) for sp in sps]
-            Hm, Wm = max(h for h, _ in ext), max(w for _, w in ext)
-            plane = int(planes[idx])
-            cols = slice(bounds[idx], bounds[idx + 1])
-            T = (cols.stop - cols.start) // C
-            Sp = torch.empty(N, C, plane, dtype=torch.uint8, device=dev)       # symbols in each plan's tile order
-            desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
-            d = desc.reshape(N, C, T)
-            d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
-            d['in_len'][:] = lens[:, cols].reshape(N, C, T)
-            d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
-            d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
-            counts['streams'] += int((desc['n_sym'] > 0).sum())
-            counts['symbols'] += int(desc['n_sym'].sum())
-            if uniform:
-                d['table'][:] = self._uniform(dmll.L, dev)[1].data_ptr()
-                d['row_pitch'][:] = 0
-                self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            else:
-                wins = [size(sp.window) for sp in sps]
-                l, F = self.net.get_P_nhwc(scale, bn8, F_win if sps[0].fused else None,
-                                           windows=wins if len(set(wins)) > 1 else None)
-                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
-                want = (2 * max(h for h, _ in wins), 2 * max(w for _, w in wins))
-                if tuple(l.shape[1:3]) != want or non_shared_get_K(l.shape[-1], C) != K:
-                    raise ValueError('container scale %d (C=%d) does not match the model output %s'
-                                     % (scale, C, tuple(l.shape)))
-                pitch = E.table_pitch(dmll.L)
-                table = torch.empty(N * C * plane * pitch, dtype=torch.int16, device=dev)
-                d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
-                d['row_pitch'][:] = pitch
-                tg = dmll.targets(dev)
-                geo = rows_dev([(sp.out[0], sp.out[1], h, w) for sp, (h, w) in zip(sps, ext)])
+        def pad(sizes):
+            return max(h for h, _ in sizes), max(w for _, w in sizes)
+
+        def rows_dev(rows):
+            return E._to_device_async(np.array(rows, np.int32).reshape(N, -1), dev)
+
+        def crop(src, origins, sizes, nhwc, split=False):
+            """The sizes[n] rectangle at origins[n] of image n of src; split: one tensor per image."""
+            if ragged:
+                hp, wp = pad(sizes)
+                return E.crop_rects(src, rows_dev([o + s for o, s in zip(origins, sizes)]), hp, wp, nhwc=nhwc,
+                                    sizes=sizes if split else None)
+            h, w = sizes[0]
+            out = E.crop_rect(src, rows_dev(origins), h, w, nhwc=nhwc)
+            return [out[n:n + 1] for n in range(N)] if split else out
+
+        rects_of = [[(sp.C,) + size(sp.rect) for sp in p.scales] for p in plans]
+
+        def network(idx, scale, bn8, F):
+            wins = [size(p.scales[idx].window) for p in plans]
+            l, F = self.net.get_P_nhwc(scale, bn8, F, windows=wins if len(set(wins)) > 1 else None)
+            hm, wm = pad(wins)
+            return l, F, (2 * hm, 2 * wm)
+
+        def rows(idx, dmll, l, Sp, table, d, steps):
+            C, plane = Sp.shape[1:]
+            tg = dmll.targets(dev)
+            ext = [r[idx][1:] for r in rects_of]
+            if ragged:
+                geo = rows_dev([p.scales[idx].out[:2] + e for p, e in zip(plans, ext)])
                 max_hw = max(h * w for h, w in ext)
-                if dmll.rgb_scale:
-                    for c in range(C):
-                        E.dmll_build_table_windows(l, geo, max_hw, plane, Sp, tg, C, K, dmll.L, True, c, table, tile)
-                        dc = np.ascontiguousarray(d[:, c, :]).reshape(-1)
-                        self._on_decoder_stream(lane, lambda dc=dc: E.ac_decode_streams(dc, dev, dmll.L))
-                else:
-                    E.dmll_build_table_windows(l, geo, max_hw, plane, Sp, tg, C, K, dmll.L, False, -1, table, tile)
-                    self._on_decoder_stream(lane, lambda: E.ac_decode_streams(desc, dev, dmll.L))
-            S = E.reorder_tiles_images(Sp, rows_dev(ext), Hm, Wm, tile)            # [N][C][Hm][Wm], zero-padded
-            self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
-                                                  ('R%d' if scale >= self.net.scales else 'S%d') % scale))
-            if idx + 1 == len(walk):
-                break
-            # the finer networks' inputs: their windows of this scale's symbols, and of this scale's features
-            nxt = [p.scales[idx + 1] for p in plans]
-            wins = [size(nx.window) for nx in nxt]
-            wh, ww = max(h for h, _ in wins), max(w for _, w in wins)
-            S_win = E.crop_rects(S, rows_dev([(nx.window[0] - sp.rect[0], nx.window[1] - sp.rect[1], h, w)
-                                              for nx, sp, (h, w) in zip(nxt, sps, wins)]), wh, ww, nhwc=False)
-            bn8 = E.symbols_to_values(S_win, self._symbol_values(scale, dmll, dev), self._rgb_shift(dev))
-            F_win = None
-            if nxt[0].fused:
-                F_win = E.crop_rects(F.f, rows_dev([(nx.window[0] - 2 * sp.window[0], nx.window[1] - 2 * sp.window[1],
-                                                     h, w) for nx, sp, (h, w) in zip(nxt, sps, wins)]),
-                                     wh, ww, nhwc=True)
-        regs = [size(p.region) for p in plans]
-        return E.crop_rects(S, rows_dev([(p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1], h, w)
-                                         for p, (h, w) in zip(plans, regs)]),
-                            max(h for h, _ in regs), max(w for _, w in regs), nhwc=False, sizes=regs)
+                steps(lambda c: E.dmll_build_table_windows(l, geo, max_hw, plane, Sp, tg, C, K, dmll.L, c >= 0, c,
+                                                           table, tile))
+            else:
+                (oy, ox), (H, W) = p0.scales[idx].out[:2], ext[0]
+                steps(lambda c: E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, c >= 0, c, table, H, W,
+                                                          tile))
+
+        def raster(idx, Sp):
+            ext = [r[idx][1:] for r in rects_of]
+            H, W = pad(ext)
+            if ragged:
+                return E.reorder_tiles_images(Sp, rows_dev(ext), H, W, tile)      # [N][C][H][W], zero-padded
+            return E.reorder_tiles(Sp, H, W, tile, False).view(N, Sp.shape[1], H, W)
+
+        # the finer networks' inputs: their windows of this scale's symbols and, where they fuse them, of its features
+        def symbols(idx, S):
+            wins = [p.scales[idx + 1].window for p in plans]
+            return crop(S, [(w[0] - p.scales[idx].rect[0], w[1] - p.scales[idx].rect[1]) for w, p in zip(wins, plans)],
+                        [size(w) for w in wins], nhwc=False)
+
+        def features(idx, F):
+            if not p0.scales[idx + 1].fused:
+                return None
+            wins = [p.scales[idx + 1].window for p in plans]
+            return crop(F.f, [(w[0] - 2 * p.scales[idx].window[0], w[1] - 2 * p.scales[idx].window[1])
+                              for w, p in zip(wins, plans)], [size(w) for w in wins], nhwc=True)
+
+        layout = stream_layout(rects_of, tile, pad_tiles=ragged)
+        self.region_counts['streams'] += int((layout[2] > 0).sum())        # the empty ones that pad a ragged pass aside
+        self.region_counts['symbols'] += int(layout[2].sum())
+        S = self._decode_scales(blob, offs, lens, layout, [r[0] for r in rects_of[0]], p0.recursive, lane,
+                                network, rows, raster, symbols, features)
+        return crop(S, [(p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1]) for p in plans],
+                    [size(p.region) for p in plans], nhwc=False, split=True)
 
     # stage timing of a decode (bench.py / tools): set `codec.stage_events = []` before decode_device,
     # synchronise, then read stage_ms()

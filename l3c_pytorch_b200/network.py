@@ -404,6 +404,12 @@ class MultiscaleNetwork(nn.Module):
     def get_Cin_for_scale(self, scale):
         return self.config_ms.Cf if self.config_ms.enc.feed_F else self.config_ms.q.C
 
+    def fuses(self, scale):
+        """Whether the decoder of `scale` adds the coarser decoder's features (dec.skip), by _forward's rule: no
+        features cross into or out of a recursive scale (scale >= num_scales), and the coarsest trained scale gets
+        none."""
+        return bool(self._fuse_feat) and scale < self.scales - 1
+
     # ------------------------------------------------------------------------------------------
     @staticmethod
     def _as_u8_planes(x):

@@ -46,16 +46,12 @@ class DecoderGeometry(object):
     def __init__(self, net):
         self.num_scales = net.scales
         self.rgb = bool(net._rgb)
-        self.skip = bool(net._fuse_feat)
+        self.fuses = net.fuses
         self.radii = [Radii(net.nets[s].dec, net.prob_clfs[s]) for s in range(net.scales)]
 
     def radii_of(self, scale):
         """Recursive scales (scale >= num_scales) run nets[-1] / prob_clfs[-1]."""
         return self.radii[min(scale, self.num_scales - 1)]
-
-    def fuses(self, scale):
-        """MultiscaleNetwork._forward's rule: no features into a recursive scale or the coarsest trained one."""
-        return self.skip and scale < self.num_scales - 1
 
 
 def geometry_of(config):
@@ -234,6 +230,29 @@ def stream_columns(plan, tile):
         T = len(tile_grid(sp.H, sp.W, tile))
         cols.append([c * T + t for c in range(sp.C) for t in sp.tiles])
     return cols
+
+
+def pass_streams(plans, streams_of, starts):
+    """Where the streams of one pass of plans lie in the uploaded containers, the counterpart of
+    codec.stream_layout(pad_tiles=True): streams_of[n][scale idx] = [(offset, length)] of plan n's container
+    (parse_container), starts[n] = where that container begins.  -> (offs, lens) int64 [N][streams]: per scale and
+    channel the planned streams in the order of stream_columns, every channel's list padded to the pass's largest tile
+    count of that scale with empty streams (the container's start, length 0), which read nothing."""
+    T_max = [max(len(p.scales[k].tiles) for p in plans) for k in range(len(plans[0].scales))]
+    offs, lens = [], []
+    for p, streams, start in zip(plans, streams_of, starts):
+        o, ln = [], []
+        for k, (sp, cs) in enumerate(zip(p.scales, stream_columns(p, p.tile))):
+            T = len(sp.tiles)
+            for c in range(sp.C):
+                for col in cs[c * T:(c + 1) * T]:
+                    o.append(start + streams[sp.idx][col][0])
+                    ln.append(streams[sp.idx][col][1])
+                o += [start] * (T_max[k] - T)
+                ln += [0] * (T_max[k] - T)
+        offs.append(o)
+        lens.append(ln)
+    return np.array(offs, np.int64), np.array(lens, np.int64)
 
 
 def plan_passes(plans, ragged):

@@ -98,3 +98,41 @@ def test_padded_stream_layout_of_different_tile_counts():
     eq = [[(3, 40, 70)], [(3, 64, 70)]]
     for a, b in zip(stream_layout(eq, tile), stream_layout(eq, tile, pad_tiles=True)):
         assert np.array_equal(a, b)
+
+
+def test_pass_streams_follow_the_padded_layout():
+    """region.pass_streams: the planned streams of every channel in stream_columns order, then empty ones up to the
+    pass's largest tile count -- column for column the streams stream_layout(pad_tiles=True) lays out."""
+    from l3c_pytorch_b200.codec import stream_layout, tile_grid
+    from l3c_pytorch_b200.region import pass_streams, stream_columns
+    tile = (32, 32)
+    plans = _plans('cr', [(256, 320, (100, 100, 20, 30), 0, 0), (256, 320, (0, 0, 40, 40), 0, 0),
+                          (128, 192, (30, 60, 90, 30), 0, 0)], tile)
+    # stream `col` of scale idx of container n: offset 100000 * idx + 10 * col (from the container's start), col + 1 bytes
+    streams_of = [[[(100000 * sp.idx + 10 * col, col + 1) for col in range(sp.C * len(tile_grid(sp.H, sp.W, tile)))]
+                   for sp in p.scales] for p in plans]
+    starts = np.array([0, 7000000, 9000000], np.int64)
+    offs, lens = pass_streams(plans, streams_of, starts)
+    rects_of = [[(sp.C, sp.rect[2] - sp.rect[0], sp.rect[3] - sp.rect[1]) for sp in p.scales] for p in plans]
+    si, _, n_sym, _ = stream_layout(rects_of, tile, pad_tiles=True)
+    assert offs.dtype == lens.dtype == np.int64 and offs.shape == lens.shape == n_sym.shape
+    assert ((lens > 0) == (n_sym > 0)).all()                 # empty streams exactly where the layout pads
+    assert (offs[lens == 0] == np.broadcast_to(starts[:, None], offs.shape)[lens == 0]).all()
+    padded = 0
+    for n, p in enumerate(plans):
+        for k, (sp, cs) in enumerate(zip(p.scales, stream_columns(p, tile))):
+            row = np.flatnonzero(si[n] == k)
+            T, Tp = len(sp.tiles), len(row) // sp.C
+            assert Tp == max(len(q.scales[k].tiles) for q in plans)
+            padded += Tp - T
+            for c in range(sp.C):
+                real = row[c * Tp:c * Tp + T]
+                want = cs[c * T:(c + 1) * T]
+                assert (offs[n, real] == starts[n] + 100000 * sp.idx + 10 * np.array(want)).all()
+                assert (lens[n, real] == np.array(want) + 1).all()
+    assert padded > 0
+    # plans of one shape_key: nothing is padded
+    same = _plans('cr', [(2048, 2048, (800, 800, 20, 30), 0, 0), (2048, 2048, (1056, 1312, 20, 30), 0, 0)], tile)
+    so = [[[(10 * col, col + 1) for col in range(sp.C * len(tile_grid(sp.H, sp.W, tile)))] for sp in p.scales]
+          for p in same]
+    assert (pass_streams(same, so, np.array([0, 16], np.int64))[1] > 0).all()
