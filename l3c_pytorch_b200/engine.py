@@ -223,15 +223,17 @@ def require_cuda(t, name):
 # weights
 # ----------------------------------------------------------------------------------------------
 class PackedConv(object):
-    """Device-side repack of one nn.Conv2d: OIHW -> [KH][KW][Cin][cout_pad] (+ padded bias).
-    Re-packed automatically when the parameter is modified (load_state_dict, .to())."""
+    """The device-side weight images of one nn.Conv2d, each built on first use.  `get` checks the parameters' key
+    (weight and bias pointer and version, device) and drops every image when it changed (load_state_dict, .to(),
+    an in-place update).  The getters return the cached tensors themselves, with the padded bias."""
 
     def __init__(self, conv):
         self.conv = conv
         self._key = None
-        self.w = self.b = None
+        self.w = self.b = self.w_tc = self.w_h = self.w_h2 = self.w_im2col = None
 
     def get(self):
+        """FFMA image (conv_ffma.cu): OIHW -> [KH][KW][Cin][cout_pad] fp32, bias padded to cout_pad."""
         w, b = self.conv.weight, self.conv.bias
         key = (w.data_ptr(), w._version, b.data_ptr(), b._version, str(w.device))
         if key != self._key:
@@ -243,13 +245,11 @@ class PackedConv(object):
             bp = torch.zeros(cout_pad, dtype=torch.float32, device=w.device)
             bp[:cout] = b.detach().float()
             self.w, self.b, self._key = wp, bp, key
-            self.w_tc = None
-            self.w_h = None
-            self.w_im2col = None
+            self.w_tc = self.w_h = self.w_h2 = self.w_im2col = None
         return self.w, self.b
 
     def get_tc(self):
-        """Tensor-core operand image: [tap][K-half = Cin/32][Cout padded to 64][32] fp32, K-major rows
+        """TF32 tensor-core image (conv_tf32.cu): [tap][K-half = Cin/32][Cout padded to 64][32] fp32, K-major rows
         of 128 B that TMA drops into 128B-swizzled shared memory; values pre-rounded to TF32 (RN)."""
         _, b = self.get()
         if self.w_tc is None:
@@ -262,28 +262,60 @@ class PackedConv(object):
             self.w_tc = img.contiguous()
         return self.w_tc, b
 
+    def get_f16(self):
+        """F16 tensor-core image (conv_f16.cu): 3x3 / 5x5 -> [taps][cout_pad][64 cin] fp16, 1x1 ->
+        [Cin/64][cout_pad][64] fp16; K-major rows of 128 B; values rounded to FP16 (RN, saturating)."""
+        _, b = self.get()
+        if self.w_h is None:
+            w = self.conv.weight.detach().float().clamp(-65504.0, 65504.0)
+            cout, cin, kh, kw = w.shape
+            cout_pad = (cout + 63) // 64 * 64
+            assert cin % 64 == 0 and kh == kw and kh in (1, 3, 5)
+            if kh in (3, 5):
+                assert cin == 64
+                img = torch.zeros(kh * kh, cout_pad, 64, dtype=torch.float16, device=w.device)
+                img[:, :cout] = w.permute(2, 3, 0, 1).reshape(kh * kh, cout, 64).half()
+            else:
+                img = torch.zeros(cin // 64, cout_pad, 64, dtype=torch.float16, device=w.device)
+                img[:, :cout] = w.reshape(cout, cin // 64, 64).permute(1, 0, 2).half()
+            self.w_h = img.contiguous()
+        return self.w_h, b
 
-def _get_f16(self):
-    """F16 tensor-core operand image (conv_f16.cu): 3x3 / 5x5 -> [taps][cout_pad][64 cin] fp16, 1x1 ->
-    [Cin/64][cout_pad][64] fp16; K-major rows of 128 B; values rounded to FP16 (RN, saturating)."""
-    _, b = self.get()
-    if getattr(self, 'w_h', None) is None:
-        w = self.conv.weight.detach().float().clamp(-65504.0, 65504.0)
-        cout, cin, kh, kw = w.shape
-        cout_pad = (cout + 63) // 64 * 64
-        assert cin % 64 == 0 and kh == kw and kh in (1, 3, 5)
-        if kh in (3, 5):
-            assert cin == 64
-            img = torch.zeros(kh * kh, cout_pad, 64, dtype=torch.float16, device=w.device)
-            img[:, :cout] = w.permute(2, 3, 0, 1).reshape(kh * kh, cout, 64).half()
-        else:
-            img = torch.zeros(cin // 64, cout_pad, 64, dtype=torch.float16, device=w.device)
-            img[:, :cout] = w.reshape(cout, cin // 64, 64).permute(1, 0, 2).half()
-        self.w_h = img.contiguous()
-    return self.w_h, b
+    def get_f16x2(self):
+        """Split image of precision mode 'f16x2' (conv_f16x2.cu): 3x3 -> [9][cout_pad][128] (hi | lo per row),
+        1x1 -> [2 * Cin/64][cout_pad][64] (hi chunks, then lo chunks)."""
+        _, b = self.get()
+        if self.w_h2 is None:
+            w = self.conv.weight.detach().float().clamp(-65504.0, 65504.0)
+            cout, cin, kh, kw = w.shape
+            cout_pad = (cout + 63) // 64 * 64
+            assert cin % 64 == 0 and kh == kw and kh in (1, 3)
+            if kh == 3:
+                assert cin == 64
+                hi, lo = _split_host(w.permute(2, 3, 0, 1).reshape(9, cout, 64))
+                img = torch.zeros(9, cout_pad, 128, dtype=torch.float16, device=w.device)
+                img[:, :cout, :64] = hi
+                img[:, :cout, 64:] = lo
+            else:
+                hi, lo = _split_host(w.reshape(cout, cin // 64, 64).permute(1, 0, 2))
+                img = torch.zeros(2 * (cin // 64), cout_pad, 64, dtype=torch.float16, device=w.device)
+                img[:cin // 64, :cout] = hi
+                img[cin // 64:, :cout] = lo
+            self.w_h2 = img.contiguous()
+        return self.w_h2, b
 
-
-PackedConv.get_f16 = _get_f16
+    def get_im2col(self):
+        """FP16 image of the RGB head's 3 -> Cf 3x3 conv as the K = 64 GEMM over its im2col (rgb_head_f16):
+        [1][cout_pad][64], k = (ky*3 + kx)*3 + c, zero for k >= 27."""
+        _, b = self.get()
+        if self.w_im2col is None:
+            w = self.conv.weight.detach().float().clamp(-65504.0, 65504.0)        # [Cf, 3, 3, 3]
+            cout = w.shape[0]
+            assert tuple(w.shape[1:]) == (3, 3, 3) and cout % 2 == 0 and b.shape[0] <= 256
+            img = torch.zeros(1, b.shape[0], 64, dtype=torch.float16, device=w.device)
+            img[0, :cout, :27] = w.permute(0, 2, 3, 1).reshape(cout, 27).half()
+            self.w_im2col = img.contiguous()
+        return self.w_im2col, b
 
 
 _LO_SCALE = 2048.0
@@ -294,33 +326,6 @@ def _split_host(w):
     hi = w.half()
     lo = ((w - hi.float()) * _LO_SCALE).half()
     return hi, lo
-
-
-def _get_f16x2(self):
-    """Split weight image of precision mode 'f16x2' (conv_f16x2.cu): 3x3 -> [9][cout_pad][128] (hi | lo per row),
-    1x1 -> [2 * Cin/64][cout_pad][64] (hi chunks, then lo chunks)."""
-    _, b = self.get()
-    if getattr(self, 'w_h2', None) is None or self._key_h2 != self._key:
-        w = self.conv.weight.detach().float().clamp(-65504.0, 65504.0)
-        cout, cin, kh, kw = w.shape
-        cout_pad = (cout + 63) // 64 * 64
-        assert cin % 64 == 0 and kh == kw and kh in (1, 3)
-        if kh == 3:
-            assert cin == 64
-            hi, lo = _split_host(w.permute(2, 3, 0, 1).reshape(9, cout, 64))
-            img = torch.zeros(9, cout_pad, 128, dtype=torch.float16, device=w.device)
-            img[:, :cout, :64] = hi
-            img[:, :cout, 64:] = lo
-        else:
-            hi, lo = _split_host(w.reshape(cout, cin // 64, 64).permute(1, 0, 2))
-            img = torch.zeros(2 * (cin // 64), cout_pad, 64, dtype=torch.float16, device=w.device)
-            img[:cin // 64, :cout] = hi
-            img[cin // 64:, :cout] = lo
-        self.w_h2, self._key_h2 = img.contiguous(), self._key
-    return self.w_h2, b
-
-
-PackedConv.get_f16x2 = _get_f16x2
 
 
 def round_to_tf32(t):
@@ -384,254 +389,151 @@ def _packed_obj(conv):
     return pc
 
 
-def packed(conv):
-    return _packed_obj(conv).get()
-
-
-def tc_eligible(conv, x_pitch, y_pitch, y_coff, pixel_shuffle=False):
-    """Layers the wgmma kernel covers: 3x3 (any dilation) with 64 input channels and Cout % 64 == 0,
-    and 1x1 with Cin % 64 == 0 (any Cout); stride 1, dense input pitch.  Everything else (5x5/s2,
-    Cin = 3 or 5) runs on the fp32 FFMA kernel."""
-    k, cin, cout = conv.kernel_size[0], conv.in_channels, conv.out_channels
-    if conv.stride[0] != 1 or x_pitch != cin:
-        return False
-    if k == 3:
-        return cin == 64 and cout % 64 == 0 and y_pitch % 4 == 0 and y_coff % 4 == 0
-    if k == 1:
-        return cin % 64 == 0 and not pixel_shuffle
-    return False
-
-
 # ----------------------------------------------------------------------------------------------
 # conv stack
 # ----------------------------------------------------------------------------------------------
+def on_tensor_cores(mode, conv, cin, x_pitch, y_pitch, y_coff, pixel_shuffle, residual):
+    """The route of a conv2d call: True for a tensor-core kernel, False for the fp32 FFMA kernel.  `conv` gives the
+    geometry (kernel_size, stride, dilation, in_channels, out_channels), `cin` the channels read, `x_pitch` the
+    input's pitch in values (half the split image's in f16x2), `y_pitch` / `y_coff` the output's, `residual` whether
+    one is added.  A tensor-core layer reads all of a dense input, cin == x_pitch == in_channels, and then:
+      fp32   never
+      tf32   stride 1: 3x3 with Cin 64, Cout % 64 == 0, y_pitch and y_coff multiples of 4; or 1x1 with
+             Cin % 64 == 0 and no pixel shuffle
+      f16    3x3/s1 with Cin 64 and Cout % 64 == 0; 5x5/s2 with dilation 1, Cin 64, Cout % 64 == 0 and no pixel
+             shuffle; 1x1/s1 with Cin % 64 == 0, no pixel shuffle, even Cout <= 256 and no residual
+      f16x2  f16's 3x3 except with pixel shuffle and a residual together, and f16's 1x1
+    The rows differ where the modes' kernels do (conv_tf32.cu, conv_f16.cu, conv_f16x2.cu)."""
+    cin_all = conv.in_channels
+    if mode == _lib.PREC_FP32 or cin != cin_all or x_pitch != cin_all:
+        return False
+    k, stride, cout = conv.kernel_size[0], conv.stride[0], conv.out_channels
+    if k == 3:
+        return stride == 1 and cin == 64 and cout % 64 == 0 and (
+            y_pitch % 4 == 0 and y_coff % 4 == 0 if mode == _lib.PREC_TF32 else
+            not (mode == _lib.PREC_F16X2 and pixel_shuffle and residual))
+    if k == 1:
+        return stride == 1 and cin % 64 == 0 and not pixel_shuffle and (
+            mode == _lib.PREC_TF32 or (cout % 2 == 0 and cout <= 256 and not residual))
+    return (k == 5 and mode == _lib.PREC_F16 and stride == 2 and conv.dilation[0] == 1 and cin == 64 and
+            cout % 64 == 0 and not pixel_shuffle)
+
+
 def conv2d(conv, x, cin=None, relu=False, residual=None, pixel_shuffle=False, out=None, out_coff=0,
            precision=None, want='plain'):
-    """y = conv(x) [+ReLU] [+residual] on NHWC tensors, parameters taken from the nn.Conv2d `conv`
-    (never called as a torch op).  `out`/`out_coff` write a channel slice of a wider NHWC buffer
-    (used for the atrous concat, prob_clf.py:71).
+    """y = conv(x) [+ReLU] [+residual] on NHWC tensors, parameters taken from the nn.Conv2d `conv` (never called as
+    a torch op), in precision mode `precision` (default: the process-wide mode).  `cin` < in_channels reads the
+    first `cin` channels of the input; `out` / `out_coff` write a channel slice of a wider NHWC buffer (the atrous
+    concat, prob_clf.py:71).
 
-    x: tensor or Act.  want: 'plain' -> tensor; 'act' -> Act whose `.r` twin is produced when the
-    tensor-core mode is on; 'round' -> Act whose only tensor is the operand image (for activations that
-    feed nothing but a following tensor-core conv; then `out`, if given, is that image's buffer)."""
+    x: tensor or Act.  The layer runs on the tensor cores or on the fp32 FFMA kernel (on_tensor_cores).  An FFMA
+    layer reads `x.f`; a tensor-core layer reads the operand image `x.r`, made for this call's mode when it is
+    missing.  y is the fp32 output, `want` picks what is returned:
+
+      mode   tensor-core layer reads   'plain'  'act'                'round'
+      fp32   -                         y        Act(y, None)         Act(y, None)
+      tf32   x.r, else x.f as it is    y        Act(y, TF32 twin)    Act(y, y), y rounded to TF32 in place
+      f16    x.r, else FP16 of x.f     y        Act(y, FP16 image)   Act(None, FP16 image)
+      f16x2  x.r, else split of x.f    y        Act(y, split image)  Act(None, split image)
+
+    The conv kernel writes the operand image beside y, except the f16x2 FFMA and 1x1 kernels: they write y and
+    split_f16x2 splits it.  With want='round' in f16 / f16x2, `out` is the image's buffer (f16x2: a split buffer
+    [.., 2 * C], channels out_coff.. of both halves, which only the 3x3 kernel can fill); otherwise it is y's."""
     xa = x if isinstance(x, Act) else Act(x)
     mode = _PRECISION['mode'] if precision is None else precision
-    if mode == _lib.PREC_F16:
-        return _conv2d_f16(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want)
-    if mode == _lib.PREC_F16X2:
-        return _conv2d_f16x2(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want)
-    if _RAGGED['v'] is not None:
+    f16 = mode in (_lib.PREC_F16, _lib.PREC_F16X2)
+    split = mode == _lib.PREC_F16X2
+    if _RAGGED['v'] is not None and not f16:
         raise NotImplementedError('ragged batches run in precision f16 or f16x2 only, not %s'
                                   % {v: k for k, v in _lib.PRECISIONS.items()}[mode])
-    x = xa.f
-    require_cuda(x, 'x')
-    assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4
-    N, H, W, xp = x.shape
-    kh = conv.kernel_size[0]
-    stride, dil = conv.stride[0], conv.dilation[0]
-    cin = conv.in_channels if cin is None else cin
-    cout = conv.out_channels
-    pad = kh // 2 if dil == 1 else dil
-    Ho = (H + 2 * pad - dil * (kh - 1) - 1) // stride + 1
-    Wo = (W + 2 * pad - dil * (kh - 1) - 1) // stride + 1
-    flags = (_lib.CONV_RELU if relu else 0) | (_lib.CONV_PIXEL_SHUFFLE2 if pixel_shuffle else 0)
-    if out is None:
-        if pixel_shuffle:
-            out = torch.empty(N, Ho * 2, Wo * 2, cout // 4, dtype=torch.float32, device=x.device)
-        else:
-            out = torch.empty(N, Ho, Wo, cout, dtype=torch.float32, device=x.device)
-    prec = mode
-    x_in = x
-    if mode != _lib.PREC_FP32 and tc_eligible(conv, xp, out.shape[-1], out_coff, pixel_shuffle) and cin == conv.in_channels:
-        w, b = _packed_obj(conv).get_tc()
-        if xa.r is not None:
-            x_in = xa.r                       # TF32-rounded operand image
-    else:
-        prec = _lib.PREC_FP32
-        w, b = packed(conv)
-    out_r = None
-    if mode != _lib.PREC_FP32:
-        if want == 'act':
-            out_r = torch.empty_like(out)
-        elif want == 'round':
-            flags |= _lib.CONV_ROUND_TF32
-    d = ConvDesc(x=x_in.data_ptr(), w=w.data_ptr(), bias=b.data_ptr(),
-                 residual=residual.data_ptr() if residual is not None else None, y=out.data_ptr(),
-                 y_tf32=out_r.data_ptr() if out_r is not None else None,
-                 N=N, H=H, W=W, Cin=cin, x_pitch=xp, Cout=cout, cout_pad=b.shape[0],
-                 y_pitch=out.shape[-1], y_coff=out_coff, ksize=kh, stride=stride, dilation=dil,
-                 flags=flags, precision=prec)
-    if residual is not None:
-        assert residual.shape == out.shape and residual.is_contiguous()
-    check(lib.l3c_conv2d(ctypes.byref(d), _stream_ptr()))
-    LAUNCHES['n'] += 1
-    if want == 'plain':
-        return out
-    if want == 'round':
-        return Act(out, out if mode != _lib.PREC_FP32 else None)
-    return Act(out, out_r)
-
-
-def _conv2d_f16(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want):
-    """conv2d in precision mode 'f16': tensor-core-eligible layers read the FP16 operand image `xa.r` and
-    run conv_f16.cu; the others (Cin = 3 or 5) run the fp32 FFMA kernel on `xa.f`.  Either kernel
-    writes what the consumers need: fp32 (`want` 'plain' / 'act') and / or the FP16 image ('act' / 'round')."""
-    src = xa.f if xa.f is not None else xa.r
+    src = xa.r if f16 and xa.f is None else xa.f
     require_cuda(src, 'x')
-    assert src.is_contiguous() and src.dim() == 4
+    assert (f16 or src.dtype == torch.float32) and src.is_contiguous() and src.dim() == 4
     N, H, W, xp = src.shape
-    kh = conv.kernel_size[0]
-    stride, dil = conv.stride[0], conv.dilation[0]
+    if split and xa.f is None:
+        xp //= 2                                              # hi | lo halves
+    kh, stride, dil = conv.kernel_size[0], conv.stride[0], conv.dilation[0]
     cin = conv.in_channels if cin is None else cin
     cout = conv.out_channels
     pad = kh // 2 if dil == 1 else dil
     Ho = (H + 2 * pad - dil * (kh - 1) - 1) // stride + 1
     Wo = (W + 2 * pad - dil * (kh - 1) - 1) // stride + 1
-    flags = (_lib.CONV_RELU if relu else 0) | (_lib.CONV_PIXEL_SHUFFLE2 if pixel_shuffle else 0)
     shape = (N, Ho * 2, Wo * 2, cout // 4) if pixel_shuffle else (N, Ho, Wo, cout)
-    need_f, need_h = want in ('plain', 'act'), want in ('act', 'round')
-    y = y_h = None
-    if out is not None:                      # caller's buffer for the primary output (channel slice)
-        if want == 'round':
-            assert out.dtype == torch.float16
-            y_h = out
+    flags = (_lib.CONV_RELU if relu else 0) | (_lib.CONV_PIXEL_SHUFFLE2 if pixel_shuffle else 0)
+    tc = on_tensor_cores(mode, conv, cin, xp, shape[3] if out is None else out.shape[-1], out_coff, pixel_shuffle,
+                         residual is not None)
+    assert tc or xa.f is not None, 'an fp32 (CUDA-core) layer needs the fp32 activation'
+
+    # y: the fp32 output; y_r: its operand image, written by the conv kernel when kernel_img
+    kernel_img = mode in (_lib.PREC_TF32, _lib.PREC_F16) or (split and tc and kh == 3)
+    image_out = f16 and want == 'round'
+    y = y_r = None
+    if out is not None:
+        assert out.dtype == (torch.float16 if image_out else torch.float32)
+        if image_out:
+            y_r = out
         else:
-            assert out.dtype == torch.float32
             y = out
-    k = kh
-    tc = (xp == conv.in_channels and cin == conv.in_channels and
-          ((k == 3 and stride == 1 and cin == 64 and cout % 64 == 0) or
-           (k == 5 and stride == 2 and dil == 1 and cin == 64 and cout % 64 == 0 and not pixel_shuffle) or
-           (k == 1 and stride == 1 and cin % 64 == 0 and not pixel_shuffle and cout % 2 == 0 and cout <= 256 and
-            residual is None)))
-    if need_f and y is None:
-        y = torch.empty(shape, dtype=torch.float32, device=src.device)
-    if need_h and y_h is None:
-        y_h = torch.empty(shape, dtype=torch.float16, device=src.device)
-    ref = y if y is not None else y_h
+    # sizes as separate ints: torch.empty takes ~1.5 us longer to parse a tuple, on the thread that feeds the GPU
+    if y is None and not (image_out and tc and kernel_img):
+        y = torch.empty(*shape, dtype=torch.float32, device=src.device)
+    if y_r is None and kernel_img and want in ('act', 'round'):
+        if mode == _lib.PREC_TF32 and want == 'round':
+            y_r, flags = y, flags | _lib.CONV_ROUND_TF32
+        elif mode == _lib.PREC_TF32:
+            y_r = torch.empty_like(y)
+        else:
+            y_r = torch.empty(*shape[:3], shape[3] * (2 if split else 1), dtype=torch.float16, device=src.device)
+    if out is not None and y is not None and y_r is not None:
+        assert split or y.shape == y_r.shape                  # an unsplit image has y's layout
+    y_pitch = y.shape[-1] if y is not None else y_r.shape[-1] // (2 if split else 1)
+    if residual is not None:                  # read in y's layout; the f16x2 3x3 kernel adds it to a new y only
+        assert residual.dtype == torch.float32 and residual.is_contiguous()
+        assert residual.shape == (y.shape if y is not None else y_r.shape[:3] + (y_pitch,))
+        assert out is None or not (split and kernel_img)
+
     pc = _packed_obj(conv)
-    if tc:
-        if xa.r is None or xa.r.dtype != torch.float16:
-            xa = as_operand(xa.f)                     # callers from outside the network (tests, bench)
-        w_h, b = pc.get_f16()
-        _ragged_guard(kh, dil, xa.r)
-        d = ConvDesc(x_h=xa.r.data_ptr(), w_h=w_h.data_ptr(), bias=b.data_ptr(),
-                     residual=residual.data_ptr() if residual is not None else None,
-                     y=_dp(y), y_h=_dp(y_h), N=N, H=H, W=W, Cin=cin, x_pitch=xp, Cout=cout, cout_pad=b.shape[0],
-                     y_pitch=ref.shape[-1], y_coff=out_coff, ksize=kh, stride=stride, dilation=dil,
-                     flags=flags, precision=_lib.PREC_F16)
-    else:
-        assert xa.f is not None, 'an fp32 (CUDA-core) layer needs the fp32 activation'
-        if y is None:                                 # the FFMA kernel always writes fp32
-            y = torch.empty(shape, dtype=torch.float32, device=src.device)
+    if not tc:
+        x_in = xa.f
         w, b = pc.get()
-        _ragged_guard(kh, dil, xa.f)
-        d = ConvDesc(x=xa.f.data_ptr(), w=w.data_ptr(), bias=b.data_ptr(),
-                     residual=residual.data_ptr() if residual is not None else None,
-                     y=_dp(y), y_h=_dp(y_h), N=N, H=H, W=W, Cin=cin, x_pitch=xp, Cout=cout, cout_pad=b.shape[0],
-                     y_pitch=ref.shape[-1], y_coff=out_coff, ksize=kh, stride=stride, dilation=dil,
-                     flags=flags, precision=_lib.PREC_FP32)
-    if residual is not None:
-        assert residual.dtype == torch.float32 and residual.shape == ref.shape and residual.is_contiguous()
-    if y is not None and y_h is not None:
-        assert y.shape == y_h.shape
+    elif mode == _lib.PREC_TF32:
+        x_in = xa.r if xa.r is not None else xa.f
+        w, b = pc.get_tc()
+    elif split:
+        x_in = xa.r
+        if x_in is None or x_in.dtype != torch.float16 or x_in.shape[-1] != 2 * conv.in_channels:
+            x_in = split_f16x2(xa.f)
+        w, b = pc.get_f16x2()
+    else:
+        x_in = xa.r
+        if x_in is None or x_in.dtype != torch.float16:
+            x_in = xa.f.clamp(-65504.0, 65504.0).half()
+        w, b = pc.get_f16()
+    _ragged_guard(kh, dil, x_in)
+    d = ConvDesc(bias=b.data_ptr(), residual=_dp(residual), y=_dp(y), N=N, H=H, W=W, Cin=cin,
+                 x_pitch=2 * xp if split and tc else xp, Cout=cout, cout_pad=b.shape[0], y_pitch=y_pitch,
+                 y_coff=out_coff, ksize=kh, stride=stride, dilation=dil, flags=flags,
+                 precision=mode if tc else _lib.PREC_FP32)
+    if f16 and tc:
+        d.x_h, d.w_h = x_in.data_ptr(), w.data_ptr()
+    else:
+        d.x, d.w = x_in.data_ptr(), w.data_ptr()
+    if kernel_img and y_r is not None and y_r is not y:
+        if mode == _lib.PREC_TF32:
+            d.y_tf32 = y_r.data_ptr()
+        else:
+            d.y_h = y_r.data_ptr()
+            if split:
+                d.yh_pitch, d.yh_lo_off = y_r.shape[-1], y_r.shape[-1] // 2
     check(lib.l3c_conv2d(ctypes.byref(d), _stream_ptr()))
     LAUNCHES['n'] += 1
+
+    if not kernel_img and split and want in ('act', 'round'):
+        assert out is None or want != 'round', 'a CUDA-core layer cannot fill a slice of a split buffer'
+        y_r = split_f16x2(y)
     if want == 'plain':
         return y
-    if want == 'round':
-        return Act(None, y_h)
-    return Act(y, y_h)
-
-
-def _conv2d_f16x2(conv, xa, cin, relu, residual, pixel_shuffle, out, out_coff, want):
-    """conv2d in precision mode 'f16x2' (strict tensor-core mode, conv_f16x2.cu): the 64-channel 3x3 layers and
-    the wide 1x1 layers read SPLIT operand images `xa.r` ([N,H,W,2*Cin] FP16, hi | lo) and accumulate hi*hi and
-    hi*lo + lo*hi separately; the other layers (5x5/s2, Cin = 3 or 5) run the fp32 FFMA kernel on `xa.f`, and
-    their output is split by l3c_split_f16x2 when a tensor-core layer follows ('act' / 'round')."""
-    src = xa.f if xa.f is not None else xa.r
-    require_cuda(src, 'x')
-    assert src.is_contiguous() and src.dim() == 4
-    N, H, W = src.shape[:3]
-    kh = conv.kernel_size[0]
-    stride, dil = conv.stride[0], conv.dilation[0]
-    cin_all = conv.in_channels
-    xp = src.shape[-1] if xa.f is not None else src.shape[-1] // 2
-    cin = cin_all if cin is None else cin
-    cout = conv.out_channels
-    pad = kh // 2 if dil == 1 else dil
-    Ho = (H + 2 * pad - dil * (kh - 1) - 1) // stride + 1
-    Wo = (W + 2 * pad - dil * (kh - 1) - 1) // stride + 1
-    flags = (_lib.CONV_RELU if relu else 0) | (_lib.CONV_PIXEL_SHUFFLE2 if pixel_shuffle else 0)
-    co = cout // 4 if pixel_shuffle else cout
-    shape = (N, Ho * 2, Wo * 2, co) if pixel_shuffle else (N, Ho, Wo, co)
-    need_f, need_h = want in ('plain', 'act'), want in ('act', 'round')
-    y = y_h = None
-    if out is not None:
-        if want == 'round':
-            assert out.dtype == torch.float16      # split buffer [.., 2*Ctot]; this layer fills channels out_coff..
-            y_h = out
-        else:
-            assert out.dtype == torch.float32
-            y = out
-    tc = (xp == cin_all and cin == cin_all and stride == 1 and
-          ((kh == 3 and cin == 64 and cout % 64 == 0 and not (pixel_shuffle and residual is not None)) or
-           (kh == 1 and cin % 64 == 0 and not pixel_shuffle and cout % 2 == 0 and cout <= 256 and residual is None)))
-    k1 = tc and kh == 1
-    pc = _packed_obj(conv)
-    if need_f and y is None:
-        y = torch.empty(shape, dtype=torch.float32, device=src.device)
-    if tc and not k1:
-        if need_h and y_h is None:
-            y_h = torch.empty(shape[:3] + (2 * co,), dtype=torch.float16, device=src.device)
-        if xa.r is None or xa.r.dtype != torch.float16 or xa.r.shape[-1] != 2 * cin_all:
-            xa = Act(xa.f, split_f16x2(xa.f))
-        w_h, b = pc.get_f16x2()
-        _ragged_guard(kh, dil, xa.r)
-        yh_pitch = y_h.shape[-1] if y_h is not None else 0
-        d = ConvDesc(x_h=xa.r.data_ptr(), w_h=w_h.data_ptr(), bias=b.data_ptr(),
-                     residual=residual.data_ptr() if residual is not None else None,
-                     y=_dp(y), y_h=_dp(y_h), N=N, H=H, W=W, Cin=cin, x_pitch=2 * cin_all, Cout=cout,
-                     cout_pad=b.shape[0], y_pitch=y.shape[-1] if y is not None else yh_pitch // 2, y_coff=out_coff,
-                     ksize=kh, stride=stride, dilation=dil, flags=flags, precision=_lib.PREC_F16X2,
-                     yh_pitch=yh_pitch, yh_lo_off=yh_pitch // 2)
-        if residual is not None:
-            assert residual.dtype == torch.float32 and residual.is_contiguous() and out is None and \
-                tuple(residual.shape) == tuple(shape)
-        check(lib.l3c_conv2d(ctypes.byref(d), _stream_ptr()))
-        LAUNCHES['n'] += 1
-    else:
-        if y is None:
-            y = torch.empty(shape, dtype=torch.float32, device=src.device)
-        if k1:
-            if xa.r is None or xa.r.dtype != torch.float16 or xa.r.shape[-1] != 2 * cin_all:
-                xa = Act(xa.f, split_f16x2(xa.f))
-            w_h, b = pc.get_f16x2()
-            d = ConvDesc(x_h=xa.r.data_ptr(), w_h=w_h.data_ptr(), bias=b.data_ptr(), y=y.data_ptr(),
-                         N=N, H=H, W=W, Cin=cin, x_pitch=2 * cin_all, Cout=cout, cout_pad=b.shape[0],
-                         y_pitch=y.shape[-1], y_coff=out_coff, ksize=1, stride=1, dilation=1, flags=flags,
-                         precision=_lib.PREC_F16X2)
-        else:
-            assert xa.f is not None, 'an fp32 (CUDA-core) layer needs the fp32 activation'
-            w, b = pc.get()
-            _ragged_guard(kh, dil, xa.f)
-            d = ConvDesc(x=xa.f.data_ptr(), w=w.data_ptr(), bias=b.data_ptr(),
-                         residual=residual.data_ptr() if residual is not None else None, y=y.data_ptr(),
-                         N=N, H=H, W=W, Cin=cin, x_pitch=xa.f.shape[-1], Cout=cout, cout_pad=b.shape[0],
-                         y_pitch=y.shape[-1], y_coff=out_coff, ksize=kh, stride=stride, dilation=dil, flags=flags,
-                         precision=_lib.PREC_FP32)
-            if residual is not None:
-                assert residual.dtype == torch.float32 and residual.shape == y.shape and residual.is_contiguous()
-        check(lib.l3c_conv2d(ctypes.byref(d), _stream_ptr()))
-        LAUNCHES['n'] += 1
-        if need_h:
-            assert out is None or want != 'round', 'a CUDA-core layer cannot fill a slice of a split buffer'
-            y_h = split_f16x2(y)
-    if want == 'plain':
-        return y
-    if want == 'round':
-        return Act(None, y_h)
-    return Act(y, y_h)
+    return Act(None if image_out else y, y_r)
 
 
 def _dp(t):
@@ -682,18 +584,10 @@ def rgb_head_f16(img_u8, conv1, conv2, head_conv):
         check(lib.l3c_rgb_im2col_f16(_ptr(img_u8), _ptr(A1), _ptr(b1), _ptr(A2), _ptr(b2), N, H, W, _ptr(cols),
                                      _stream_ptr()))
     LAUNCHES['n'] += 1
-    pc = _packed_obj(head_conv)
-    _, b = pc.get()
-    if getattr(pc, 'w_im2col', None) is None:
-        w = head_conv.weight.detach().float().clamp(-65504.0, 65504.0)        # [Cf, 3, 3, 3]
-        cout = w.shape[0]
-        assert tuple(w.shape[1:]) == (3, 3, 3) and cout % 2 == 0 and b.shape[0] <= 256
-        img = torch.zeros(1, b.shape[0], 64, dtype=torch.float16, device=w.device)
-        img[0, :cout, :27] = w.permute(0, 2, 3, 1).reshape(cout, 27).half()   # k = (ky*3 + kx)*3 + c
-        pc.w_im2col = img.contiguous()
+    w_h, b = _packed_obj(head_conv).get_im2col()
     cout = head_conv.out_channels
     y_h = torch.empty(N, H, W, cout, dtype=torch.float16, device=img_u8.device)
-    d = ConvDesc(x_h=cols.data_ptr(), w_h=pc.w_im2col.data_ptr(), bias=b.data_ptr(), y_h=y_h.data_ptr(),
+    d = ConvDesc(x_h=cols.data_ptr(), w_h=w_h.data_ptr(), bias=b.data_ptr(), y_h=y_h.data_ptr(),
                  N=N, H=H, W=W, Cin=64, x_pitch=64, Cout=cout, cout_pad=b.shape[0], y_pitch=cout, y_coff=0,
                  ksize=1, stride=1, dilation=1, flags=0, precision=_lib.PREC_F16)
     check(lib.l3c_conv2d(ctypes.byref(d), _stream_ptr()))

@@ -207,7 +207,7 @@ def test_f16_conv_vs_torch_on_fp16_operands(cout, rate, H, W, kw):
         want = F.relu(want)
     if kw.get('pixel_shuffle'):
         want = F.pixel_shuffle(want, 2)
-    xa = E.as_operand(_nhwc(x)) if E.f16_mode() else E.Act(_nhwc(x), _nhwc(x).clamp(-65504.0, 65504.0).half())
+    xa = E.Act(_nhwc(x))                                           # conv2d makes the FP16 operand image
     cc = conv.cuda()
     got = E.conv2d(cc, xa, precision=_lib.PREC_F16, want='act', residual=res, **kw)
     np.testing.assert_allclose(got.f.cpu().permute(0, 3, 1, 2).numpy(), want.numpy(), rtol=1e-4, atol=1e-4)
@@ -223,6 +223,23 @@ def test_f16_conv_vs_torch_on_fp16_operands(cout, rate, H, W, kw):
         E.conv2d(cc, xa, precision=_lib.PREC_F16, want='round', residual=res, out=buf, out_coff=cout, **kw)
         assert torch.equal(buf[..., cout:2 * cout], got.r)
         assert bool((buf[..., :cout] == 7).all()) and bool((buf[..., 2 * cout:] == 7).all())
+
+
+def test_f16_call_makes_its_operand_image_whatever_the_process_mode():
+    """conv2d(..., precision=f16) on an fp32-only activation reads the FP16 image of it whatever the process-wide
+    mode is: the same bits as when the caller passes that image."""
+    from l3c_pytorch_b200 import engine as E, _lib
+    conv = _conv_module(64, 64, 3).cuda()
+    x = _nhwc(torch.randn(2, 64, 20, 28))
+    want = E.conv2d(conv, E.Act(x, x.clamp(-65504.0, 65504.0).half()), precision=_lib.PREC_F16)
+    old = E.get_conv_precision()
+    try:
+        for mode in ('tf32', 'fp32', 'f16x2'):
+            E.set_conv_precision(mode)
+            got = E.conv2d(conv, E.Act(x), precision=_lib.PREC_F16)
+            assert torch.equal(got, want), mode
+    finally:
+        E.set_conv_precision(old)
 
 
 @pytest.mark.parametrize('cin,cout,H,W', [(192, 120, 9, 31), (192, 150, 16, 16), (64, 64, 8, 16), (192, 120, 64, 64),

@@ -291,7 +291,7 @@ class Recorder(object):
             xa = x if isinstance(x, E.Act) else E.Act(x)
             cin_r = conv.in_channels if cin is None else cin
             route, kernels = _expected_route(mode, conv, cin_r, want)
-            # the operand image the kernel reads (routing of conv2d / _conv2d_f16 / _conv2d_f16x2)
+            # the operand image the kernel reads (engine.conv2d's operand for each mode and route)
             op, opkind = None, None
             if route == 'ffma':
                 op, opkind = xa.f[..., :cin_r].clone(), 'f32'
