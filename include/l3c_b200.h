@@ -491,6 +491,35 @@ int l3c_set_decoder_streams_per_cta(int spc);
  * __device__ functions, so a test can measure what the built library computes.  Not meant for production use. */
 int l3c_dmll_probe_sigmoid(const float *u_dev, float *raw_dev, float *term_dev, int64_t n, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * G. Training (l3c_pytorch_b200.train; reference: criterion/logistic_mixture.py:146-207,
+ *    modules/quantizer.py:62-90): the two per-pixel losses of a training step, forward and
+ *    backward, on the NCHW fp32 tensors nn.Conv2d produces.  A NULL gradient pointer selects the
+ *    forward.  The backward reads the upstream gradient from device memory (no host sync) and
+ *    recomputes everything from the forward's inputs; every gradient element is written once, so
+ *    results are bit-identical from run to run.
+ * ---------------------------------------------------------------------------------------- */
+
+/* DMLL negative log-likelihood of one scale, as train.dmll_nll computes it.
+ *   l_dev  f32 [N][Kp][HW], Kp = (rgb ? 4 : 3) * C * K, channel p*C*K + c*K + k (p: 0 logits, 1 means,
+ *          2 log-scales, 3 RGB coefficients); K = 10
+ *   x_dev  f32 [N][C][HW] targets (RGB: the pixel values; bottleneck: the soft quantiser's values)
+ *   half_bin, x_lower, x_upper: half the bin width and the edge-branch thresholds (x < x_lower: lower branch,
+ *          x > x_upper: upper branch), as fp32.
+ * Forward (grad_dev NULL): nll_dev f64 [N] = the nats of every image, summed per 128 pixels and then per image in a
+ * fixed order (two launches).  Backward: grad_dev f32 [1] the upstream gradient of the summed nats; dl_dev f32 like
+ * l_dev, every plane written; dx_dev f32 like x_dev or NULL (must be NULL when rgb).  One launch. */
+int l3c_dmll_nll_train(const float *l_dev, const float *x_dev, int N, int HW, int C, int K, int rgb, float half_bin,
+                       float x_lower, float x_upper, double *nll_dev, const float *grad_dev, float *dl_dev,
+                       float *dx_dev, void *stream);
+
+/* Soft quantiser of n fp32 values q_dev onto levels_dev f32 [L] (1 <= L <= 256).
+ * Forward (grad_dev NULL): sym_dev int64 [n] = the first l minimising (q - level_l)^2, value_dev f32 [n] =
+ * levels[sym].  Backward: dq_dev f32 [n] = grad_dev[i] * 2 sigma Var_phi(levels), phi = softmax_l(-sigma (q -
+ * level_l)^2) (sigma > 0): the gradient of the soft value sum_l level_l phi_l that the hard value stands in for. */
+int l3c_soft_quantize(const float *q_dev, int64_t n, const float *levels_dev, int L, float sigma, int64_t *sym_dev,
+                      float *value_dev, const float *grad_dev, float *dq_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

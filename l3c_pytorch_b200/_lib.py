@@ -98,6 +98,8 @@ _SIGNATURES = {
     'l3c_dmll_probe_sigmoid': (c_int, [c_void_p] * 3 + [c_int64, c_void_p]),
     'l3c_batch_intervals': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     'l3c_batch_rows': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_uint32, c_void_p, c_void_p]),
+    'l3c_dmll_nll_train': (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_float] * 3 + [c_void_p] * 5),
+    'l3c_soft_quantize': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_float] + [c_void_p] * 5),
 }
 
 EXPORTS = sorted(_SIGNATURES)

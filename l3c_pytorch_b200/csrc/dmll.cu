@@ -397,6 +397,234 @@ __global__ void nll_finish_kernel(const double *__restrict__ partial, int per_im
 }
 
 // ---------------------------------------------------------------------------------------------
+// training (DESIGN §4.9): the DMLL loss of train.dmll_nll and its gradient, and the soft quantiser, on the NCHW fp32
+// tensors nn.Conv2d produces.  l [N][Kp][HW] (channel p*C*K + c*K + k), x [N][C][HW] float targets.  One thread per
+// pixel walks the Kp planes, so every load and store of a warp is one coalesced line per plane.  The backward
+// recomputes everything from l and x: nothing but the two inputs is kept between the passes.
+// ---------------------------------------------------------------------------------------------
+// One mixture component as train.dmll_nll evaluates it in fp32 (logistic_mixture.py:146-207): the sigmoid arguments
+// u+ / u- at the two bin edges, their sigmoids, delta = s+ - s- and the component's log-probability lp (middle branch
+// log(max(delta, 1e-12)); x above x_upper: -softplus(u-); x below x_lower: u+ - softplus(u+), applied last).
+struct TrainTerm {
+    float inv, up, um, sp, sm, delta, lp;
+};
+
+__device__ __forceinline__ TrainTerm train_term(float x, float mu, float ls_raw, float half_bin, bool hi, bool lo) {
+    TrainTerm t;
+    t.inv = expf(-fmaxf(ls_raw, LOG_SCALES_MIN));
+    const float cx = __fsub_rn(x, mu);
+    t.up = __fmul_rn(t.inv, __fadd_rn(cx, half_bin));
+    t.um = __fmul_rn(t.inv, __fsub_rn(cx, half_bin));
+    t.sp = sigmoid_rn(t.up);
+    t.sm = sigmoid_rn(t.um);
+    t.delta = __fsub_rn(t.sp, t.sm);
+    float lp = logf(fmaxf(t.delta, 1e-12f));
+    if (hi) lp = -softplus_f(t.um);
+    if (lo) lp = __fsub_rn(t.up, softplus_f(t.up));
+    t.lp = lp;
+    return t;
+}
+
+// The effective mean of component k of channel c: RGB channels 1 and 2 add sigmoid(coeff) times the targets of the
+// channels before them, in torch's order ((mean + co_br x0) + co_bg x1).  lp: the pixel's plane 0, stride HW.
+template <int K>
+__device__ __forceinline__ float train_mean(const float *__restrict__ lp, int64_t HW, int C, int c, int k, bool rgb,
+                                            float x0, float x1) {
+    float mu = __ldg(lp + (int64_t)(1 * C * K + c * K + k) * HW);
+    const float *co = lp + (int64_t)3 * C * K * HW;
+    if (rgb && c == 1) mu = __fadd_rn(mu, __fmul_rn(sigmoid_rn(__ldg(co + (int64_t)(0 * K + k) * HW)), x0));
+    if (rgb && c == 2) {
+        mu = __fadd_rn(mu, __fmul_rn(sigmoid_rn(__ldg(co + (int64_t)(1 * K + k) * HW)), x0));
+        mu = __fadd_rn(mu, __fmul_rn(sigmoid_rn(__ldg(co + (int64_t)(2 * K + k) * HW)), x1));
+    }
+    return mu;
+}
+
+// Channel c of one pixel: w[k] = lp_k + log_softmax(logits)_k, -> nats = -logsumexp_k w_k; also the logits'
+// log-sum-exp and w's maximum and sum of exponentials, from which the backward takes the two softmaxes.
+template <int K>
+__device__ __forceinline__ float train_channel(const float *__restrict__ lp, int64_t HW, int C, int c, bool rgb,
+                                               float xc, float x0, float x1, float half_bin, bool hi, bool lo,
+                                               float (&w)[K], float &lse_pi, float &wmax, float &wsum) {
+    const float *logit = lp + (int64_t)(c * K) * HW;
+    const float *logs = lp + (int64_t)(2 * C * K + c * K) * HW;
+    float lg[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) lg[k] = __ldg(logit + (int64_t)k * HW);
+    float lmax = lg[0];
+#pragma unroll
+    for (int k = 1; k < K; ++k) lmax = fmaxf(lmax, lg[k]);
+    float lsum = 0.f;
+#pragma unroll
+    for (int k = 0; k < K; ++k) lsum += expf(lg[k] - lmax);
+    lse_pi = lmax + logf(lsum);
+    wmax = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const float mu = train_mean<K>(lp, HW, C, c, k, rgb, x0, x1);
+        const TrainTerm t = train_term(xc, mu, __ldg(logs + (int64_t)k * HW), half_bin, hi, lo);
+        w[k] = t.lp + (lg[k] - lse_pi);
+        wmax = fmaxf(wmax, w[k]);
+    }
+    wsum = 0.f;
+#pragma unroll
+    for (int k = 0; k < K; ++k) wsum += expf(w[k] - wmax);
+    return -(wmax + logf(wsum));
+}
+
+// Forward: the nats of every sub-pixel summed per CTA in f64, in the fixed order of dmll_nll_kernel; the per-image
+// totals then come from nll_finish_kernel.
+template <int K>
+__global__ void __launch_bounds__(NLL_THREADS)
+dmll_train_nll_kernel(const float *__restrict__ l, const float *__restrict__ x, int HW, int C, int rgb, float half_bin,
+                      float x_lower, float x_upper, double *__restrict__ partial /* [N][gridDim.x] */) {
+    const int Kp = (rgb ? 4 : 3) * C * K;
+    const int n = blockIdx.y;
+    const int p = blockIdx.x * NLL_THREADS + threadIdx.x;
+    double mine = 0.0;
+    if (p < HW) {
+        const float *lp = l + (int64_t)n * Kp * HW + p;
+        const float *xp = x + (int64_t)n * C * HW + p;
+        const float x0 = rgb ? __ldg(xp) : 0.f, x1 = rgb ? __ldg(xp + HW) : 0.f;
+        for (int c = 0; c < C; ++c) {
+            const float xc = __ldg(xp + (int64_t)c * HW);
+            float w[K], lse_pi, wmax, wsum;
+            mine += (double)train_channel<K>(lp, HW, C, c, rgb != 0, xc, x0, x1, half_bin, xc > x_upper,
+                                             xc < x_lower, w, lse_pi, wmax, wsum);
+        }
+    }
+    __shared__ double red[NLL_THREADS / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_down_sync(0xFFFFFFFFu, mine, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mine;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int i = 0; i < NLL_THREADS / 32; ++i) t += red[i];
+        partial[(size_t)n * gridDim.x + blockIdx.x] = t;
+    }
+}
+
+// Backward of the summed nats for the upstream gradient *grad: every element of dl (all Kp planes) and of dx (non-RGB,
+// optional) is written once by the thread of its pixel -- no atomics, the same bits on every run.  With r = softmax(w)
+// and pi = softmax(logits): dlogit = g (pi - r); e = -g r is the gradient of lp, which reaches u+ / u- as a+ / a- on
+// the branch taken (0 on the others, and 0 on the middle branch where delta < 1e-12, as torch.clamp's gradient);
+// dmean = -inv (a+ + a-), dlogscale = -(u+ a+ + u- a-) where the raw log-scale is >= -7, dx = sum_k inv (a+ + a-);
+// RGB: dcoeff = dmean of the channel it couples into, times the target it multiplies, times sigmoid'(coeff).
+// sigmoid' is s (1 - s) and the lower branch's slope 1 - s, from the same fp32 s as delta, as torch's autograd
+// forms them: where s+ - s- cancels, the rounding of 1 - s and of delta then go together as in the torch path
+// (sigmoid(u) sigmoid(-u) is closer to float64 per element, but moved the encoder's gradients of a step at
+// initialisation by up to 2 % away from the reference's, as many sub-pixels sit in that regime there).
+template <int K>
+__global__ void __launch_bounds__(NLL_THREADS)
+dmll_train_grad_kernel(const float *__restrict__ l, const float *__restrict__ x, int HW, int C, int rgb,
+                       float half_bin, float x_lower, float x_upper, const float *__restrict__ grad,
+                       float *__restrict__ dl, float *__restrict__ dx) {
+    const int Kp = (rgb ? 4 : 3) * C * K;
+    const int n = blockIdx.y;
+    const int p = blockIdx.x * NLL_THREADS + threadIdx.x;
+    if (p >= HW) return;
+    const float g = __ldg(grad);
+    const float *lp = l + (int64_t)n * Kp * HW + p;
+    float *dlp = dl + (int64_t)n * Kp * HW + p;
+    const float *xp = x + (int64_t)n * C * HW + p;
+    const float x0 = rgb ? __ldg(xp) : 0.f, x1 = rgb ? __ldg(xp + HW) : 0.f;
+    for (int c = 0; c < C; ++c) {
+        const float xc = __ldg(xp + (int64_t)c * HW);
+        const bool hi = xc > x_upper, lo = xc < x_lower;
+        float w[K], lse_pi, wmax, wsum;
+        train_channel<K>(lp, HW, C, c, rgb != 0, xc, x0, x1, half_bin, hi, lo, w, lse_pi, wmax, wsum);
+        float dxc = 0.f;
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            const int64_t i_logit = c * K + k, i_mean = C * K + c * K + k, i_ls = 2 * C * K + c * K + k;
+            const float r = expf(w[k] - wmax) / wsum;
+            const float pi = expf(__ldg(lp + i_logit * HW) - lse_pi);
+            dlp[i_logit * HW] = g * (pi - r);
+            const float e = -g * r;
+            const float ls_raw = __ldg(lp + i_ls * HW);
+            const TrainTerm t = train_term(xc, train_mean<K>(lp, HW, C, c, k, rgb != 0, x0, x1), ls_raw, half_bin,
+                                           hi, lo);
+            float ap = 0.f, am = 0.f;
+            if (lo) {
+                ap = (t.up > 20.f) ? 0.f : e * (1.f - t.sp);                 // d(u - softplus u) = 1 - sigmoid(u)
+            } else if (hi) {
+                am = -e * ((t.um > 20.f) ? 1.f : t.sm);                      // d softplus(u) = sigmoid(u)
+            } else if (t.delta >= 1e-12f) {
+                const float q = e / t.delta;
+                ap = q * (t.sp * (1.f - t.sp));                              // sigmoid' = s (1 - s), as torch
+                am = -q * (t.sm * (1.f - t.sm));
+            }
+            const float s = ap + am;
+            const float dmean = -t.inv * s;
+            dlp[i_mean * HW] = dmean;
+            dlp[i_ls * HW] = (ls_raw >= LOG_SCALES_MIN) ? -(t.up * ap + t.um * am) : 0.f;
+            dxc += t.inv * s;
+            if (rgb && c > 0) {
+                // channel 1 couples through coefficient plane 0 (x0); channel 2 through planes 1 (x0) and 2 (x1)
+                const int64_t j0 = 3 * C * K + (c == 1 ? 0 : 1) * K + k;
+                const float s0 = sigmoid_rn(__ldg(lp + j0 * HW));
+                dlp[j0 * HW] = dmean * x0 * (s0 * (1.f - s0));
+                if (c == 2) {
+                    const int64_t j1 = 3 * C * K + 2 * K + k;
+                    const float s1 = sigmoid_rn(__ldg(lp + j1 * HW));
+                    dlp[j1 * HW] = dmean * x1 * (s1 * (1.f - s1));
+                }
+            }
+        }
+        if (!rgb && dx) dx[((int64_t)n * C + c) * HW + p] = dxc;
+    }
+}
+
+// Soft quantiser (quantizer.py:62-90).  Forward: sym = the first argmin of (q - c_l)^2 (strict <, as torch.min and
+// quantize_head_kernel take it), value = levels[sym].  Backward: d value_soft / dq for value_soft = sum_l c_l phi_l,
+// phi = softmax_l(-sigma (q - c_l)^2), is 2 sigma Var_phi(c), evaluated centred (sum_l phi_l (c_l - cbar)^2).
+constexpr int SQ_THREADS = 256;
+
+__global__ void __launch_bounds__(SQ_THREADS)
+soft_quantize_kernel(const float *__restrict__ q, int64_t n, const float *__restrict__ levels, int L, float sigma,
+                     int64_t *__restrict__ sym, float *__restrict__ value, const float *__restrict__ grad,
+                     float *__restrict__ dq) {
+    extern __shared__ float slev[];
+    for (int i = threadIdx.x; i < L; i += SQ_THREADS) slev[i] = levels[i];
+    __syncthreads();
+    const int64_t i = (int64_t)blockIdx.x * SQ_THREADS + threadIdx.x;
+    if (i >= n) return;
+    const float v = __ldg(q + i);
+    int best = 0;
+    float bd = __fmul_rn(__fsub_rn(v, slev[0]), __fsub_rn(v, slev[0]));
+    for (int j = 1; j < L; ++j) {
+        const float d = __fmul_rn(__fsub_rn(v, slev[j]), __fsub_rn(v, slev[j]));
+        if (d < bd) {
+            bd = d;
+            best = j;
+        }
+    }
+    if (!grad) {
+        sym[i] = best;
+        value[i] = slev[best];
+        return;
+    }
+    // the largest logit -sigma d is the nearest level's (sigma > 0)
+    const float m = -sigma * bd;
+    float s = 0.f, sc = 0.f;
+    for (int j = 0; j < L; ++j) {
+        const float d = __fmul_rn(__fsub_rn(v, slev[j]), __fsub_rn(v, slev[j]));
+        const float ph = expf(-sigma * d - m);
+        s += ph;
+        sc += ph * slev[j];
+    }
+    const float cbar = sc / s;
+    float var = 0.f;
+    for (int j = 0; j < L; ++j) {
+        const float d = __fmul_rn(__fsub_rn(v, slev[j]), __fsub_rn(v, slev[j]));
+        const float dc = slev[j] - cbar;
+        var += expf(-sigma * d - m) * dc * dc;
+    }
+    dq[i] = __ldg(grad + i) * (2.f * sigma * (var / s));
+}
+
+// ---------------------------------------------------------------------------------------------
 // sampling from the mixture (logistic_mixture.py:277-323): Gumbel-max choice of the component, inverse-CDF
 // sample of its logistic, RGB means coupled through the coefficients of the CHOSEN components.  The uniform
 // random numbers are inputs (u_sel [N][C][K][HW], u_x [N][C][HW], both in [1e-5, 1 - 1e-5] as in the
@@ -770,6 +998,53 @@ extern "C" int l3c_dmll_nll_ragged(const float *l_dev, const uint8_t *sym_dev, c
     nll_finish_kernel<<<N, 32, 0, (cudaStream_t)stream>>>(partial, per_image, H, W, extents_dev, nll_dev);
     L3C_LAUNCH_CHECK("nll_finish_kernel");
     L3C_CUDA(cudaFreeAsync(partial, (cudaStream_t)stream));
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_nll_train(const float *l_dev, const float *x_dev, int N, int HW, int C, int K, int rgb,
+                                  float half_bin, float x_lower, float x_upper, double *nll_dev,
+                                  const float *grad_dev, float *dl_dev, float *dx_dev, void *stream) {
+    using namespace l3c;
+    // the alphabet does not enter the loss (the targets are values, the bin width comes as half_bin): any L passes
+    if (int e = check_common("l3c_dmll_nll_train", N, HW, C, K, 256, rgb)) return e;
+    L3C_REQUIRE(l_dev && x_dev, "l3c_dmll_nll_train: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int per_image = ceil_div(HW, NLL_THREADS);
+    dim3 grid(per_image, N);
+    if (grad_dev) {
+        L3C_REQUIRE(dl_dev, "l3c_dmll_nll_train: the backward needs dl_dev");
+        L3C_REQUIRE(!(rgb && dx_dev), "l3c_dmll_nll_train: no dx at an RGB scale (the image is not differentiable)");
+        dmll_train_grad_kernel<10><<<grid, NLL_THREADS, 0, st>>>(l_dev, x_dev, HW, C, rgb, half_bin, x_lower, x_upper,
+                                                                 grad_dev, dl_dev, dx_dev);
+        L3C_LAUNCH_CHECK("dmll_train_grad_kernel");
+        return L3C_OK;
+    }
+    L3C_REQUIRE(nll_dev, "l3c_dmll_nll_train: the forward needs nll_dev");
+    double *partial = nullptr;
+    L3C_CUDA(cudaMallocAsync(&partial, sizeof(double) * (size_t)N * per_image, st));
+    dmll_train_nll_kernel<10><<<grid, NLL_THREADS, 0, st>>>(l_dev, x_dev, HW, C, rgb, half_bin, x_lower, x_upper,
+                                                            partial);
+    L3C_LAUNCH_CHECK("dmll_train_nll_kernel");
+    nll_finish_kernel<<<N, 32, 0, st>>>(partial, per_image, 1, HW, nullptr, nll_dev);
+    L3C_LAUNCH_CHECK("nll_finish_kernel");
+    L3C_CUDA(cudaFreeAsync(partial, st));
+    return L3C_OK;
+}
+
+extern "C" int l3c_soft_quantize(const float *q_dev, int64_t n, const float *levels_dev, int L, float sigma,
+                                 int64_t *sym_dev, float *value_dev, const float *grad_dev, float *dq_dev,
+                                 void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(q_dev && levels_dev && n >= 0, "l3c_soft_quantize: bad arguments");
+    L3C_REQUIRE(L >= 1 && L <= 256, "l3c_soft_quantize: L=%d", L);
+    L3C_REQUIRE(grad_dev ? (dq_dev != nullptr) : (sym_dev && value_dev),
+                "l3c_soft_quantize: the forward needs sym_dev and value_dev, the backward dq_dev");
+    L3C_REQUIRE(!grad_dev || sigma > 0.f, "l3c_soft_quantize: sigma=%g must be positive", (double)sigma);
+    L3C_REQUIRE(ceil_div64(n, SQ_THREADS) <= INT32_MAX, "l3c_soft_quantize: n=%lld", (long long)n);
+    if (n == 0) return L3C_OK;
+    soft_quantize_kernel<<<(unsigned)ceil_div64(n, SQ_THREADS), SQ_THREADS, L * sizeof(float), (cudaStream_t)stream>>>(
+        q_dev, n, levels_dev, L, sigma, sym_dev, value_dev, grad_dev, dq_dev);
+    L3C_LAUNCH_CHECK("soft_quantize_kernel");
     return L3C_OK;
 }
 

@@ -805,6 +805,45 @@ def dmll_nll_ragged(l, sym, values, C, K, L, rgb, x_min, x_max, extents):
     return out
 
 
+def dmll_nll_train(l, x, K, rgb, half_bin, x_lower, x_upper, grad=None, want_dx=False):
+    """The training loss of one scale on NCHW fp32 tensors (l3c_dmll_nll_train): l [N,Kp,H,W], x [N,C,H,W] targets,
+    both contiguous.  grad None -> per-image nats float64 [N] (2 launches).  grad (0-dim f32 on the device, the
+    gradient of the summed nats) -> (dl like l, dx like x or None) (1 launch); want_dx only where not rgb."""
+    N, C, H, W = x.shape
+    assert l.is_contiguous() and x.is_contiguous() and l.dtype == x.dtype == torch.float32
+    assert l.shape[0] == N and l.shape[2:] == x.shape[2:]
+    args = (_ptr(l), _ptr(x), N, H * W, C, K, int(rgb), float(half_bin), float(x_lower), float(x_upper))
+    if grad is None:
+        out = torch.empty(N, dtype=torch.float64, device=l.device)
+        check(lib.l3c_dmll_nll_train(*args, _ptr(out), None, None, None, _stream_ptr()))
+        LAUNCHES['n'] += 2
+        return out
+    dl = torch.empty_like(l)
+    dx = torch.empty_like(x) if want_dx else None
+    check(lib.l3c_dmll_nll_train(*args, None, _ptr(grad), _ptr(dl), _ptr(dx), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return dl, dx
+
+
+def soft_quantize(q, levels, sigma, grad=None):
+    """Soft quantiser of a contiguous fp32 tensor q onto fp32 levels [L] (l3c_soft_quantize).
+    grad None -> (sym int64, value f32), both shaped like q.  grad (like q) -> dq = grad * 2 sigma Var_phi(levels)."""
+    assert q.is_contiguous() and q.dtype == levels.dtype == torch.float32 and levels.is_contiguous()
+    if grad is None:
+        sym = torch.empty(q.shape, dtype=torch.int64, device=q.device)
+        val = torch.empty_like(q)
+        check(lib.l3c_soft_quantize(_ptr(q), q.numel(), _ptr(levels), levels.numel(), float(sigma), _ptr(sym),
+                                    _ptr(val), None, None, _stream_ptr()))
+        LAUNCHES['n'] += 1
+        return sym, val
+    assert grad.shape == q.shape and grad.is_contiguous() and grad.dtype == torch.float32
+    dq = torch.empty_like(q)
+    check(lib.l3c_soft_quantize(_ptr(q), q.numel(), _ptr(levels), levels.numel(), float(sigma), None, None,
+                                _ptr(grad), _ptr(dq), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return dq
+
+
 def dmll_channel_params(l, x_dec, C, K, rgb, c):
     """l NHWC; x_dec f32 [N,C,H,W] contiguous (values of already coded channels) or None.
     -> (softmax pi, mu, log sigma), each [N,K,H,W] f32."""

@@ -1,7 +1,10 @@
-"""Training step of L3C (SURVEY.md section 8 row f4) -- the one part of this package that is NOT hand-written
-CUDA: a plain PyTorch-autograd restatement over the SAME parameter tree (`MultiscaleNetwork`'s nn.Conv2d
-containers), so that what it trains loads into the sm_90a coding path unchanged.  It exists so that a user of the
-reference's `train.py` finds the step here; it is not on the encode/decode hot path and is not benchmarked.
+"""Training step of L3C (SURVEY.md section 8 row f4): PyTorch autograd over the SAME parameter tree
+(`MultiscaleNetwork`'s nn.Conv2d containers), so that what it trains loads into the sm_90a coding path unchanged.
+The convolutions and their backward are torch's (cuDNN on the GPU).  The two per-pixel losses are the library's
+kernels on CUDA tensors (DESIGN §4.9): the DMLL negative log-likelihood of every scale and the soft quantiser, each
+forward and backward in one pass over its inputs, without torch's per-element autograd graph.  CPU tensors, and CUDA
+tensors with FUSED_LOSS = False, take the torch restatements `dmll_nll` and `soft_quantize_torch`, which stay the
+reference the kernels are tested against.  `tools/bench_train.py` measures both paths.
 
 Reference (under /root/reference/src):
   train/multiscale_trainer.py:173-226   train_step: zero_grad, forward, get_loss, backward, optim.step
@@ -11,19 +14,61 @@ Reference (under /root/reference/src):
   criterion/logistic_mixture.py:146-246 discretised-logistic-mixture NLL (+ RGB mean coupling)
   blueprints/multiscale_blueprint.py:64-95  bpsp conversion, loss_pc = sum of the per-scale costs without the
                                             uniform-prior final scale
-Works on CPU tensors as well as CUDA ones (it only uses torch operators).
+Works on CPU tensors as well as CUDA ones.
 """
 import numpy as np
 import torch
 import torch.nn.functional as F
 
+from . import engine as E
 from .dmll import non_shared_get_K
 
 _LOG_SCALES_MIN = -7.
+_K = 10                       # the mixture size the kernels are built for (dmll.cu check_common)
+
+# CUDA tensors: True runs the DMLL loss and the soft quantiser as the library's kernels, False as the torch
+# restatements below (for comparisons on the GPU: tests/test_gpu_train_kernels.py, tools/bench_train.py)
+FUSED_LOSS = True
+
+
+def _require_f32(what, *ts):
+    for t in ts:
+        if t.dtype != torch.float32:
+            raise TypeError('%s: the training kernels take fp32 tensors, got %s' % (what, t.dtype))
+        if not t.is_cuda:
+            raise ValueError('%s: mixed devices (%s); the kernels need every tensor on the GPU' % (what, t.device))
+
+
+class _SoftQuantizeFn(torch.autograd.Function):
+    """(q, levels, sigma) -> (hard values levels[sym] with the soft quantiser's gradient, sym int64)."""
+
+    @staticmethod
+    def forward(ctx, q, levels, sigma):
+        q, levels = q.contiguous(), levels.detach().contiguous()
+        sym, val = E.soft_quantize(q, levels, sigma)
+        ctx.save_for_backward(q, levels)
+        ctx.sigma = sigma
+        ctx.mark_non_differentiable(sym)
+        return val, sym
+
+    @staticmethod
+    def backward(ctx, g_val, g_sym):
+        q, levels = ctx.saved_tensors
+        return E.soft_quantize(q, levels, ctx.sigma, grad=g_val.contiguous()), None, None
 
 
 def soft_quantize(x, levels, sigma):
-    """quantizer.py:62-90 -> (x_soft with hard data and soft gradient, x_hard, symbols)."""
+    """quantizer.py:62-90 -> (x_soft with hard data and soft gradient, x_hard, symbols).  CUDA: the soft quantiser
+    kernels (x_hard shares x_soft's data, as in the torch path); CPU: soft_quantize_torch."""
+    if not (FUSED_LOSS and x.is_cuda):
+        return soft_quantize_torch(x, levels, sigma)
+    _require_f32('soft_quantize', x, levels)
+    x_soft, sym = _SoftQuantizeFn.apply(x, levels, float(sigma))
+    return x_soft, x_soft.detach(), sym
+
+
+def soft_quantize_torch(x, levels, sigma):
+    """quantizer.py:62-90 -> (x_soft with hard data and soft gradient, x_hard, symbols), in torch operators."""
     N, C, H, W = x.shape
     xv = x.view(N, C, H * W, 1)
     d = torch.pow(xv - levels, 2)
@@ -98,6 +143,46 @@ def dmll_nll(dm, x, l):
     return -torch.logsumexp(weighted, dim=2)
 
 
+class _DmllNllFn(torch.autograd.Function):
+    """(l, x, dm) -> the summed nats of dmll_nll as a 0-dim fp32 tensor; saves only l and x."""
+
+    @staticmethod
+    def forward(ctx, l, x, dm):
+        l, x = l.contiguous(), x.contiguous()
+        ctx.save_for_backward(l, x)
+        ctx.dm = dm
+        nll = E.dmll_nll_train(l, x, _K, dm.use_coeffs, dm.bin_width / 2, dm.x_lower_bound, dm.x_upper_bound)
+        return nll.sum().float()
+
+    @staticmethod
+    def backward(ctx, g):
+        l, x = ctx.saved_tensors
+        dm = ctx.dm
+        dl, dx = E.dmll_nll_train(l, x, _K, dm.use_coeffs, dm.bin_width / 2, dm.x_lower_bound, dm.x_upper_bound,
+                                  grad=g.float().contiguous(), want_dx=ctx.needs_input_grad[1])
+        return dl, dx, None
+
+
+def dmll_nll_sum(dm, x, l):
+    """dmll_nll(dm, x, l).sum(): the total nats of one scale as a 0-dim fp32 tensor, with its gradient to l and, at a
+    bottleneck scale, to x.  CUDA: the training kernels (the per-image sums in float64, then their total); CPU: the
+    torch restatement.  An RGB target (dm.use_coeffs) must not require grad: the image is a leaf."""
+    if not (FUSED_LOSS and l.is_cuda):
+        return dmll_nll(dm, x, l).sum()
+    _require_f32('dmll_nll_sum', l, x)
+    if x.dim() != 4 or l.dim() != 4 or l.shape[0] != x.shape[0] or l.shape[2:] != x.shape[2:]:
+        raise ValueError('dmll_nll_sum: l %s and x %s are not NKpHW / NCHW of one batch'
+                         % (tuple(l.shape), tuple(x.shape)))
+    C = x.shape[1]
+    if l.shape[1] != dm._num_params * C * _K:
+        raise ValueError('dmll_nll_sum: l has %d channels; the kernels take Kp = %d x C x K = %d (C = %d, K = %d)'
+                         % (l.shape[1], dm._num_params, dm._num_params * C * _K, C, _K))
+    if dm.use_coeffs and (C != 3 or x.requires_grad):
+        raise ValueError('dmll_nll_sum: an RGB scale needs C = 3 targets that do not require grad (got C = %d, '
+                         'requires_grad = %s)' % (C, x.requires_grad))
+    return _DmllNllFn.apply(l, x, dm)
+
+
 def forward_train(net, x):
     """MultiscaleNetwork.forward in training mode (multiscale_network.py:226-306) for the L3C configurations:
     x NCHW float in [0, 255] -> (targets, predictions) per scale fine -> coarse, plus the symbols of every scale.
@@ -133,7 +218,7 @@ def training_loss(blueprint, x):
     costs = []
     for i, (t, p) in enumerate(zip(targets, preds)):
         dm = losses.loss_dmol_rgb if i == 0 else losses.loss_dmol_n
-        costs.append(dmll_nll(dm, t, p).sum())
+        costs.append(dmll_nll_sum(dm, t, p))
     num_subpixels = int(np.prod(x.shape))
     conversion = np.log(2.) * num_subpixels
     costs_bpsp = [c / conversion for c in costs]
