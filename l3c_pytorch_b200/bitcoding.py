@@ -59,7 +59,7 @@ def _groups(keys):
 
 
 class Bitcoding(object):
-    def __init__(self, blueprint, times=NoOp, compare_with_theory=False, tile=None, recursive=0):
+    def __init__(self, blueprint, times=NoOp, compare_with_theory=False, tile=None, recursive=0, crop=True):
         """tile = (th, tw): write TILED containers (codec.ContainerLayout): every channel plane of every scale is
         cut into tiles coded as independent streams -- thousands of streams per batch instead of 18 per image,
         so encode and decode are no longer bound by one warp's serial chain.  Not readable by the reference and a
@@ -69,7 +69,14 @@ class Bitcoding(object):
         codes its own bicubic thumbnails R more times and only the 1 / 2**(num_scales + R) thumbnail is left for
         the uniform prior; images are padded to multiples of 2**(num_scales + R).  Not readable by the reference;
         decode() / decode_batch() read R from the file.  ValueError for anything but a non-negative int, and for
-        R > 0 on an L3C model."""
+        R > 0 on an L3C model.
+        crop = False (tiled containers only): encode() writes ONE container for an image of any size instead of the
+        reference's auto-crop into `pout.partN` files (DESIGN §4.10); decode() of a large tiled container runs in
+        bands of tile rows, and decode_region() reads any crop of it.  ValueError without tile=: the crops of the
+        reference layout are part of its format, and its serial streams could not be decoded in bands."""
+        if not crop and tile is None:
+            raise ValueError('crop=False needs tile=(th, tw): the reference layout codes large images as crops')
+        self.crop = bool(crop)
         self.blueprint = blueprint
         self.compare_with_theory = compare_with_theory
         self.times = times
@@ -129,7 +136,7 @@ class Bitcoding(object):
         assert len(img.shape) == 4 and img.shape[0] == 1 and img.shape[1] == 3, img.shape
         assert img.dtype in (torch.int64, torch.uint8), img.dtype
 
-        if auto_crop.needs_crop(img):
+        if self.crop and auto_crop.needs_crop(img):
             print('Need to encode individual crops!')
             combinator = auto_crop.CropLossCombinator()
             crops = list(auto_crop.iter_crops(img))

@@ -9,7 +9,10 @@
 `--ckpt` is a checkpoint as written by the reference's Saver (`torch.save({'net': state_dict})`,
 helpers/saver.py:168); the module tree here has the same parameter names, so it loads strict.
 Without `--ckpt` the seed-0 default initialisation is used (only useful for testing).
-Images larger than 2000x1500 are coded as crops into `OUT.l3c.part{i}` exactly as the reference does.
+Images larger than 2000x1500 are coded as crops into `OUT.l3c.part{i}` exactly as the reference does, unless
+`enc --tile TH,TW` writes one tiled file for the whole image (DESIGN §4.10):
+
+    python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt enc BIG.png OUT.l3c --tile 64,64
 """
 import argparse
 import os
@@ -105,6 +108,10 @@ def build_parser():
     e.add_argument('--recursive', default='0', metavar='N|auto',
                    help='RGB baselines: code the last scale N more times on its own thumbnails (auto: 3 for '
                         'cr_rgb_shared); a recursive file, not readable by the reference.  Ignored for L3C.')
+    e.add_argument('--tile', default=None, type=parse_tile, metavar='TH,TW',
+                   help='write ONE tiled file (tiles of TH x TW coded as independent streams) for an image of any '
+                        'size, no .partN crops; `dec` decodes it in bands and `dec --region` reads crops of it.  Not '
+                        'readable by the reference')
     d = sub.add_parser('dec')
     d.add_argument('inp')
     d.add_argument('out_png')
@@ -113,6 +120,17 @@ def build_parser():
     d.add_argument('--level', default=0, type=int, metavar='K',
                    help='with --region, RGB baselines: the crop is of the stored scale-K thumbnail (0 = the image)')
     return p
+
+
+def parse_tile(text):
+    """'TH,TW' -> (th, tw), each 1 .. 65535 (the container stores them as u16)."""
+    try:
+        vals = tuple(int(v) for v in text.split(','))
+    except ValueError:
+        vals = ()
+    if len(vals) != 2 or not all(1 <= v <= 65535 for v in vals):
+        raise argparse.ArgumentTypeError('--tile takes TH,TW (two integers 1..65535), got %r' % text)
+    return vals
 
 
 def parse_region(text):
@@ -149,7 +167,8 @@ def main(argv=None):
     a = build_parser().parse_args(argv)
     from .bitcoding import Bitcoding
     bp = load_blueprint(a.config, a.ckpt, a.precision)
-    bc = Bitcoding(bp, recursive=recursive_of(a, bp.net.config_ms))      # dec: R is read from the file
+    tile = getattr(a, 'tile', None) if a.mode == 'enc' else None        # dec: the layout is read from the file
+    bc = Bitcoding(bp, recursive=recursive_of(a, bp.net.config_ms), tile=tile, crop=tile is None)
     try:
         if a.mode == 'enc':
             encode(bc, a.img, a.out, a.overwrite)

@@ -17,7 +17,8 @@ Equal-size, tiled and ragged batches share one encode and one decode path: `stre
 stream's intervals (encode) or symbols and CDF rows (decode) sit in the `[N][C][plane]` tensor of its scale, and
 only the step between those stream planes and the raster planes of the networks differs (a view, l3c_reorder_tiles
 or l3c_ragged_pack).  Every decode -- full (`decode_device`) or of regions of tiled containers (`decode_region_pass`,
-DESIGN §4.8) -- is one coarse-to-fine walk, `BatchCodec._decode_scales`, told its geometry by the caller.
+DESIGN §4.8) -- is one coarse-to-fine walk, `BatchCodec._decode_scales`, told its geometry by the caller; a large
+scale of a tiled pass is decoded in bands of tile rows (DESIGN §4.10).
 """
 import functools
 import os
@@ -75,6 +76,23 @@ def _slot_cap(n_sym):
 # per pass key would do (to compare the two)
 REGION_RAGGED_PASS = True
 
+# Largest N * H * W of one scale of an equal-size tiled pass that decode_device decodes whole; a larger scale is decoded
+# in bands of tile rows of about this many pixels (DESIGN §4.10).  The rows, mixture parameters and classifier
+# features of a whole-plane decode take about 2.1 KB per pixel (DESIGN §7), so a band of 8 Mpx keeps them near 20 GB.
+TILED_BAND_PIXELS = 32 * 512 * 512
+
+# Largest plane (H * W of one scale of one image) the kernels index: they take a plane's pixel count and the pixel
+# index of a thread as 32-bit ints, so a plane is kept well below 2**31 pixels (DESIGN §4.10, "Index width").
+MAX_PLANE_PIXELS = 2 ** 30
+
+
+def check_plane(H, W, what):
+    """ValueError, before any GPU work, for a plane the kernels cannot index (MAX_PLANE_PIXELS)."""
+    if int(H) * int(W) > MAX_PLANE_PIXELS:
+        raise ValueError('%s: a %dx%d plane has more than %d pixels, the most the kernels index'
+                         % (what, H, W, MAX_PLANE_PIXELS))
+
+
 TILED_MAGIC = b'L3CT'                # tiled containers: this tag + u16 tile_h + u16 tile_w follow the padding tuple
 
 
@@ -130,6 +148,23 @@ def stream_layout(shapes_of, tile=None, pad_tiles=False):
         elem.append((img * C + np.arange(C)[None, :, None]) * plane[k] + off)
         n_sym.append(np.broadcast_to(cnt, shape))
     return tuple(np.concatenate([x.reshape(N, -1) for x in xs], 1) for xs in (si, elem, n_sym)) + (plane,)
+
+
+def band_streams(layout, idx, C, band):
+    """The streams of one band (region.plan_bands) of scale idx of an equal-size tiled pass laid out by stream_layout:
+    -> ((e0, e1), (cols, si, elem, n_sym, plane)).  Its symbols are the elements [e0, e1) of every channel plane of the
+    scale; cols are the band's columns of the pass's [N][streams] arrays, and the rest is a stream_layout of one scale
+    that places them in band planes [N][C][e1 - e0]."""
+    si, elem, n_sym, plane = layout
+    lo, hi = np.searchsorted(si[0], [idx, idx + 1])
+    T = (hi - lo) // C
+    t0, t1 = band.tiles[0], band.tiles[-1] + 1
+    cols = lo + (np.arange(C)[:, None] * T + np.arange(t0, t1)[None, :]).reshape(-1)
+    e0, e1 = band.rect[0] * band.W, band.rect[2] * band.W
+    el = elem[:, cols]
+    nc = el // plane[idx]                                                    # n * C + c of every stream
+    local = nc * (e1 - e0) + (el - nc * plane[idx]) - e0
+    return (int(e0), int(e1)), (cols, np.zeros_like(local), local, n_sym[:, cols], np.array([e1 - e0], np.int64))
 
 
 class ContainerLayout(object):
@@ -297,6 +332,7 @@ class BatchCodec(object):
         self.net = blueprint.net
         self._const = {}
         self._lane_cache = {}
+        self._geo = None
         # streams and symbols the last decode_regions call handed to the range decoder (decode_region_pass)
         self.region_counts = {'streams': 0, 'symbols': 0}
 
@@ -400,6 +436,7 @@ class BatchCodec(object):
         recursive = self.check_recursive(recursive)
         dev = imgs_u8.device
         N, _, Hb, Wb = imgs_u8.shape
+        check_plane(Hb, Wb, 'encode')
         if recursive:
             fac = 2 ** (self.net.scales + recursive)
             if Hb % fac or Wb % fac:
@@ -485,6 +522,9 @@ class BatchCodec(object):
             raise ValueError('decode_batch needs containers of identical shape')
         if any(len(sh) != len(shapes_of[0]) for sh in shapes_of):
             raise ValueError('decode_batch: containers with different numbers of scales')
+        for sh in shapes_of:
+            for (_, H, W) in sh:
+                check_plane(H, W, 'decode_batch')
         blob, starts = _upload(datas, dev)
         offs = np.array([[starts[n] + o for (_, _, _, st) in parsed[n][1] for (o, _) in st] for n in range(N)],
                         np.int64)
@@ -626,7 +666,7 @@ class BatchCodec(object):
 
     def _decode_scales(self, blob, offs, lens, layout, channels, recursive, lane, network, rows, raster,
                        symbols=lambda idx, S: S, features=lambda idx, F: F,
-                       row_pitch=lambda dmll: E.table_pitch(dmll.L)):
+                       row_pitch=lambda dmll: E.table_pitch(dmll.L), bands=lambda idx: None):
         """The coarse-to-fine walk of every decode: full decodes of equal-size, tiled and ragged batches
         (decode_device) and region passes (decode_region_pass).  blob, offs, lens, layout: as in _stream_descs;
         channels: C of every scale walked, coarse -> fine (a region at level k stops early); recursive: as in
@@ -647,7 +687,12 @@ class BatchCodec(object):
             build(c) building the rows of channel c (of every channel for c = -1) -- or decode it some other way
             from the [N][C][T] descriptors d;
           raster(idx, Sp) -> S [N][C][H][W]; symbols(idx, S), features(idx, F) -> what of them the next network reads
-            (all of it by default)."""
+            (all of it by default);
+          bands(idx) -> None, or the bands (region.plan_bands) the scale is decoded in (DESIGN §4.10): then per band
+            network(..., band) runs on the band's window of the whole coarser scale, rows(..., band) builds the band's
+            rows into a table of the band's own stream planes, the band's streams decode into those planes and their
+            symbols are copied to their elements of Sp; the F the walk hands on is what network returned for the last
+            band."""
         dev = blob.device
         N = offs.shape[0]
         K = self.net.config_ms.prob.K
@@ -668,21 +713,40 @@ class BatchCodec(object):
                     build(-1)
                     decode(desc)
 
-            if uniform:
-                table, pitch = self._uniform(dmll.L, dev)[1], 0
-            else:
-                l, F, want = network(idx, scale, bn8, F)
-                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
+            def run_net(F_in, *band):
+                l, F_out, want = network(idx, scale, bn8, F_in, *band)
                 if tuple(l.shape[1:3]) != want or non_shared_get_K(l.shape[-1], C) != K:
                     raise ValueError('container scale %d (%dx%dx%d) does not match the model output %s'
                                      % (scale, C, want[0], want[1], tuple(l.shape)))
+                return l, F_out
+
+            band_list = None if uniform else bands(idx)
+            if uniform:
+                table, pitch = self._uniform(dmll.L, dev)[1], 0
+                desc, d = self._stream_descs(blob, offs, lens, layout, idx, Sp, table, pitch)
+                decode(desc)
+            elif band_list is None:
+                l, F = run_net(F)
+                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
                 pitch = row_pitch(dmll)
                 table = torch.empty(Sp.numel() * pitch, dtype=torch.int16, device=dev)
-            desc, d = self._stream_descs(blob, offs, lens, layout, idx, Sp, table, pitch)
-            if uniform:
-                decode(desc)
-            else:
+                desc, d = self._stream_descs(blob, offs, lens, layout, idx, Sp, table, pitch)
                 rows(idx, dmll, l, Sp, table, d, steps)
+            else:
+                # banded (DESIGN §4.10): per band its network window, its rows and its streams; only one band's
+                # parameters and rows are alive at a time, and its symbols go to their elements of Sp
+                pitch, F_in = row_pitch(dmll), F
+                for band in band_list:
+                    l, F = run_net(F_in, band)
+                    (e0, e1), b_layout = band_streams(layout, idx, C, band)
+                    Sb = torch.empty(N, C, e1 - e0, dtype=torch.uint8, device=dev)
+                    table = torch.empty(Sb.numel() * pitch, dtype=torch.int16, device=dev)
+                    desc, d = self._stream_descs(blob, offs[:, b_layout[0]], lens[:, b_layout[0]], b_layout[1:], 0,
+                                                 Sb, table, pitch)
+                    rows(idx, dmll, l, Sb, table, d, steps, band)
+                    Sp[:, :, e0:e1].copy_(Sb)
+                    del l, table
+                self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
             S = raster(idx, Sp)
             self._mark('uniform' if uniform else ('rgb' if dmll.rgb_scale and scale == 0 else
                                                   ('R%d' if scale >= self.net.scales else 'S%d') % scale))
@@ -738,15 +802,50 @@ class BatchCodec(object):
             # tiled and ragged batches, the bottleneck scales, L < 256 and the other precision modes build full rows
             return dmll.rgb_scale and tile is None and not ragged and dmll.L == 256 and K == 10 and E.f16_mode()
 
-        def network(idx, scale, bn8, F):
+        def bands(idx):
+            # an equal-size tiled pass whose plane at this scale exceeds the budget: bands of whole tile rows
+            H, W = dims[idx]
+            if tile is None or ragged or N * H * W <= TILED_BAND_PIXELS:
+                return None
+            from .region import plan_bands
+            return plan_bands(shapes_of[0], tile, self._geometry(), idx, max(1, TILED_BAND_PIXELS // (N * tile[0] * W)))
+
+        whole_F = [None]                  # the features of the scale being banded, assembled band by band
+
+        def band_network(idx, scale, bn8, F, band):
+            # the band's window of the whole coarser scale: its symbol values and, fused, the coarser decoder's features
+            (wy0, _, wy1, _), Wc = band.window, bn8.shape[2]
+            org = E._to_device_async(np.tile(np.array([wy0, 0], np.int32), (N, 1)), dev)
+            win = E.crop_rect(bn8, org, wy1 - wy0, Wc, nhwc=True)
+            Fw = None
+            if self.net.fuses(scale):
+                Fw = E.crop_rect(F if torch.is_tensor(F) else F.f, org, wy1 - wy0, Wc, nhwc=True)
+            l, Fo = self.net.get_P_nhwc(scale, win, Fw)
+            if idx + 1 < len(dims) and scale >= 1 and self.net.fuses(scale - 1):
+                # the next scale adds these features: the band's rows of them go to one whole plane
+                (y0, _, y1, _), oy = band.rect, band.out[0]
+                if y0 == 0:
+                    whole_F[0] = torch.empty(N, dims[idx][0], dims[idx][1], Fo.f.shape[-1], dtype=Fo.f.dtype,
+                                             device=dev)
+                whole_F[0][:, y0:y1].copy_(Fo.f[:, oy:oy + y1 - y0])
+                return l, whole_F[0], (2 * (wy1 - wy0), 2 * Wc)
+            return l, None, (2 * (wy1 - wy0), 2 * Wc)
+
+        def network(idx, scale, bn8, F, band=None):
+            if band is not None:
+                return band_network(idx, scale, bn8, F, band)
             if ragged:
                 ext_dev(idx)                      # queued ahead of the network: the rows and the raster step read it
             l, F = self.net.get_P_nhwc(scale, bn8, F if self.net.fuses(scale) else None, extents=fin)
             return l, F, dims[idx]
 
-        def rows(idx, dmll, l, Sp, table, d, steps):
+        def rows(idx, dmll, l, Sp, table, d, steps, band=None):
             C, plane, (H, W) = Sp.shape[1], Sp.shape[2], dims[idx]
             tg = dmll.targets(dev)
+            if band is not None:
+                (oy, ox), h = band.out[:2], band.rect[2] - band.rect[0]
+                return steps(lambda c: E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, c >= 0, c, table, h,
+                                                                 W, tile))
             if tile is not None:
                 # every tile of every image at once (N*T streams per launch)
                 return steps(lambda c: E.dmll_build_table_tiled(l, Sp, tg, C, K, dmll.L, c >= 0, c, table, tile))
@@ -771,7 +870,15 @@ class BatchCodec(object):
 
         return self._decode_scales(
             blob, offs, lens, stream_layout(shapes_of, tile), [s[0] for s in shapes_of[0]], Rs.pop(), lane,
-            network, rows, raster, row_pitch=lambda dmll: E.COARSE_PITCH if coarse(dmll) else E.table_pitch(dmll.L))
+            network, rows, raster, row_pitch=lambda dmll: E.COARSE_PITCH if coarse(dmll) else E.table_pitch(dmll.L),
+            bands=bands)
+
+    def _geometry(self):
+        """region.DecoderGeometry of this codec's network, built once."""
+        if self._geo is None:
+            from .region import DecoderGeometry
+            self._geo = DecoderGeometry(self.net)
+        return self._geo
 
     # ------------------------------------------------------------------------------------------
     def plan_regions(self, datas, regions, levels=None):
@@ -956,6 +1063,7 @@ class BatchCodec(object):
                 raise ValueError('container scale %d has %d channels, model expects %d' % (scale, C, want_C))
             if H < 1 or W < 1:
                 raise ValueError('container scale %d has an empty shape %dx%d' % (scale, H, W))
+            check_plane(H, W, 'container scale %d' % scale)
             if idx > 0:
                 Hc, Wc = shapes[idx - 1][1:]
                 if (H, W) != (2 * Hc, 2 * Wc):

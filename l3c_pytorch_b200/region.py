@@ -206,20 +206,55 @@ def plan_region(shapes, pad_tuple, tile, config, region, level=0):
             plans.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect, tiles=tiles, window=None,
                                    out=None, fused=False))
             break
-        r = geo.radii_of(scale)
-        need_F = _clip(_expand(rect, r.clf), H, W)                   # decoder features the classifier reads
-        coarse = (need_F[0] // 2, need_F[1] // 2, -(-need_F[2] // 2), -(-need_F[3] // 2))   # Upsampler x2
         Hc, Wc = shapes[idx - 1][1:]
-        window = _clip(_expand(coarse, r.tail + r.body + r.head), Hc, Wc)
-        fused = geo.fuses(scale)
-        want = window
-        if fused:                                                    # F_{s+1}, added after the head
-            want = _union(want, _clip(_expand(coarse, r.tail + r.body), Hc, Wc))
-        out = (rect[0] - 2 * window[0], rect[1] - 2 * window[1], rect[2] - 2 * window[0], rect[3] - 2 * window[1])
+        window, out, fused, want = _window(geo, scale, rect, H, W, Hc, Wc)
         plans.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect, tiles=tiles, window=window, out=out,
                                fused=fused))
     plans.reverse()
     return RegionPlan(plans, region_px, level, tile, n, recursive)
+
+
+def _window(geo, scale, rect, H, W, Hc, Wc):
+    """The decoder window of the symbols `rect` of an H x W plane at `scale`, on the Hc x Wc coarser plane: -> (window,
+    out, fused, want), `want` being the coarser rectangle the window and (fused) the coarser decoder's features need."""
+    r = geo.radii_of(scale)
+    need_F = _clip(_expand(rect, r.clf), H, W)                   # decoder features the classifier reads
+    coarse = (need_F[0] // 2, need_F[1] // 2, -(-need_F[2] // 2), -(-need_F[3] // 2))   # Upsampler x2
+    window = _clip(_expand(coarse, r.tail + r.body + r.head), Hc, Wc)
+    fused = geo.fuses(scale)
+    want = window
+    if fused:                                                    # F_{s+1}, added after the head
+        want = _union(want, _clip(_expand(coarse, r.tail + r.body), Hc, Wc))
+    out = (rect[0] - 2 * window[0], rect[1] - 2 * window[1], rect[2] - 2 * window[0], rect[3] - 2 * window[1])
+    return window, out, fused, want
+
+
+def plan_bands(shapes, tile, config, idx, rows):
+    """Banded decode of scale `idx` of a tiled container (DESIGN §4.10): its H x W plane cut into horizontal bands of
+    `rows` tile rows (the last one partial), each decoded from its own decoder window of the whole coarser scale.
+    shapes, tile, config: as in plan_region.  -> [ScalePlan] top to bottom; band b's rect is (y0, 0, y1, W) and its
+    tiles are consecutive in container order, so its symbols are the elements [y0 * W, y1 * W) of every channel plane in
+    stream order.  Every window and `out` is what plan_region plans for the same rectangle."""
+    geo = geometry_of(config)
+    n = len(shapes)
+    if not 1 <= idx < n:
+        raise ValueError('scale index %d has no decoder network (a container of %d scales)' % (idx, n))
+    th, tw = (int(tile[0]), int(tile[1]))
+    rows = int(rows)
+    if rows < 1:
+        raise ValueError('a band needs at least one tile row, got %d' % rows)
+    C, H, W = shapes[idx]
+    Hc, Wc = shapes[idx - 1][1:]
+    scale = n - 1 - idx
+    ntx, nty = -(-W // tw), -(-H // th)
+    bands = []
+    for ty0 in range(0, nty, rows):
+        ty1 = min(ty0 + rows, nty)
+        rect = (ty0 * th, 0, min(ty1 * th, H), W)
+        window, out, fused, _ = _window(geo, scale, rect, H, W, Hc, Wc)
+        bands.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect,
+                               tiles=list(range(ty0 * ntx, ty1 * ntx)), window=window, out=out, fused=fused))
+    return bands
 
 
 def stream_columns(plan, tile):
