@@ -287,6 +287,22 @@ int l3c_lin_dmll_intervals(const void *x_h, const void *w_h, const float *bias, 
                            const float *targets_dev, int N, int HW, int Cin, int C, int K, int L, int rgb,
                            uint32_t *intervals_dev, void *stream);
 
+/* The intervals of one band of a banded encode (DESIGN §4.10): the symbols of rows [y0, y0 + h) of the whole
+ * symbol plane sym_dev uint8 [N][C][Hs][W], their intervals written in the tile order (th x tw) of an h x W plane to
+ * band stream planes intervals_dev uint32 [N][C][h * W].
+ * l3c_lin_dmll_intervals_band (f16): as l3c_lin_dmll_intervals on rows [oy, oy + h) of x_h, the FP16 concat buffer
+ *   [N][Hl][W][Cin] of a full-width decoder window.
+ * l3c_dmll_intervals_band (any mode): as l3c_dmll_intervals on the h x W rectangle at (oy, ox) of the parameters
+ *   l_dev f32 NHWC [N][Hl][Wl][Kp].
+ * Both are bit-identical to the whole-plane kernel followed by l3c_reorder_tiles, restricted to the band. */
+int l3c_lin_dmll_intervals_band(const void *x_h, int Hl, int oy, const void *w_h, const float *bias,
+                                const uint8_t *sym_dev, int Hs, int y0, int h, int W, const float *targets_dev, int N,
+                                int Cin, int C, int K, int L, int rgb, int th, int tw, uint32_t *intervals_dev,
+                                void *stream);
+int l3c_dmll_intervals_band(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev, int Hs,
+                            int y0, int h, int W, const float *targets_dev, int N, int C, int K, int L, int rgb,
+                            int th, int tw, uint32_t *intervals_dev, void *stream);
+
 /* sub_rgb_mean + first MeanShift of RGBHead as one per-pixel 3x3 affine pair
  * (multiscale_network.py:181-183, head.py:31-33): img uint8 [N][3][HW] planes ->
  * x_sub f32 NHWC [N][HW][3] (= A1 img + b1)  and  t f32 NHWC [N][HW][4] (= A2 x_sub + b2, ch 3 = 0).

@@ -72,6 +72,10 @@ _SIGNATURES = {
     'l3c_dmll_sample': (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p, c_void_p]),
     'l3c_conv2d': (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
     'l3c_lin_dmll_intervals': (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p, c_void_p]),
+    'l3c_lin_dmll_intervals_band': (c_int, [c_void_p, c_int, c_int] + [c_void_p] * 3 + [c_int] * 4 + [c_void_p] +
+                                    [c_int] * 8 + [c_void_p, c_void_p]),
+    'l3c_dmll_intervals_band': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 7 +
+                                [c_void_p, c_void_p]),
     'l3c_rgb_prep': (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_split_f16x2': (c_int, [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p]),
     'l3c_rgb_im2col_f16': (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p, c_void_p]),

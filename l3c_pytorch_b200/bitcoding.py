@@ -167,11 +167,14 @@ class Bitcoding(object):
         for idxs in _groups((tuple(t.shape), pt) for (t, pt) in prepared):
             batch = torch.cat([prepared[i][0] for i in idxs], 0)
             pt = prepared[idxs[0]][1]
+            # a large tiled batch is encoded in bands (DESIGN §4.10), which needs encode_begin to run the networks;
+            # compare_with_theory needs every scale's parameters and keeps the whole-image forward
+            banded = not self.compare_with_theory and self.codec.encode_banded(batch.shape, self.tile)
             with self.times.run('[-] encode forwardpass'):
                 # without --compare_theory nobody reads the parameter tensors: the probability heads emit the
                 # coding intervals directly (f16 mode; MultiscaleNetwork.forward(intervals_of=...))
-                out = self.blueprint.forward(batch, self.recursive) if self.compare_with_theory else \
-                    self.blueprint.forward_for_coding(batch, self.recursive)
+                out = None if banded else self.blueprint.forward(batch, self.recursive) if self.compare_with_theory \
+                    else self.blueprint.forward_for_coding(batch, self.recursive)
             if self.compare_with_theory:
                 with self.times.run('[-] get loss'):
                     loss_out = self.blueprint.get_loss(out)

@@ -21,6 +21,8 @@ import sys
 import numpy as np
 import torch
 
+from . import codec
+
 
 class EncodeError(Exception):
     pass
@@ -45,10 +47,19 @@ def load_blueprint(config_name, ckpt=None, precision=None, device='cuda:0'):
     return bp
 
 
-def read_image(path):
-    """PIL -> int64 1CHW, alpha dropped (multiscale_tester.py:411-422)."""
+def read_image(path, max_pixels=None):
+    """PIL -> int64 1CHW, alpha dropped (multiscale_tester.py:411-422).  max_pixels: Pillow's decompression-bomb
+    limit (Image.MAX_IMAGE_PIXELS) while reading; None keeps Pillow's default."""
     from PIL import Image
-    img = np.array(Image.open(path))
+    if max_pixels is None:
+        img = np.array(Image.open(path))
+    else:
+        old = Image.MAX_IMAGE_PIXELS
+        Image.MAX_IMAGE_PIXELS = max_pixels
+        try:
+            img = np.array(Image.open(path))
+        finally:
+            Image.MAX_IMAGE_PIXELS = old
     if img.ndim == 2:
         img = np.stack([img] * 3, -1)
     img = img[..., :3]
@@ -71,7 +82,8 @@ def encode(bc, img_p, pout, overwrite=False):
                 os.remove(q)
             elif q != pout:
                 break
-    img = read_image(img_p)
+    # a tiled file holds one image of any size (DESIGN §4.10): read up to the largest plane the kernels index
+    img = read_image(img_p, codec.MAX_PLANE_PIXELS if bc.tile is not None else None)
     bpsp = bc.encode(img, pout)
     print('Encoded {} -> {}: {:.4f} bpsp'.format(img_p, pout, bpsp))
     return bpsp

@@ -81,6 +81,12 @@ REGION_RAGGED_PASS = True
 # features of a whole-plane decode take about 2.1 KB per pixel (DESIGN §7), so a band of 8 Mpx keeps them near 20 GB.
 TILED_BAND_PIXELS = 32 * 512 * 512
 
+# Largest N * H * W of the image batch of an equal-size tiled encode that encode_begin runs whole; a larger one is
+# encoded in bands (DESIGN §4.10): the encoder fine to coarse in bands of output rows, then the coding coarse to fine in
+# the bands of tile rows of the banded decode, each band at most about this many pixels.  The whole-image encode takes
+# about 750 B per pixel (DESIGN §7); the budget keeps bench.py's 16 x 512^2 tiled batch on that path.
+TILED_ENCODE_BAND_PIXELS = 32 * 512 * 512
+
 # Largest plane (H * W of one scale of one image) the kernels index: they take a plane's pixel count and the pixel
 # index of a thread as 32-bit ints, so a plane is kept well below 2**31 pixels (DESIGN §4.10, "Index width").
 MAX_PLANE_PIXELS = 2 ** 30
@@ -450,6 +456,8 @@ class BatchCodec(object):
             pads = [tuple(int(v) for v in pad_tuple)] * N
         if tile is not None:
             tile = (int(tile[0]), int(tile[1]))
+        if self.encode_banded(imgs_u8.shape, tile, ext, out):
+            return self._encode_banded(imgs_u8, pads, tile, recursive)
         if out is None:
             # f16 mode: DMLL head fused into the convs
             out = self.net(imgs_u8, recursive, intervals_of=self.blueprint.losses, extents=ext)
@@ -486,6 +494,183 @@ class BatchCodec(object):
         desc['out'] = slots.data_ptr() + slot_off[:-1]
         desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
         return EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, (imgs_u8, ivs, slots))
+
+    @staticmethod
+    def encode_banded(shape, tile, extents=None, out=None):
+        """Whether encode_begin encodes a batch of this shape (N, 3, H, W) in bands (DESIGN §4.10): a tiled,
+        equal-size batch (extents None) without a precomputed `out` whose image planes exceed
+        TILED_ENCODE_BAND_PIXELS (the image is the largest scale)."""
+        N, _, H, W = (int(v) for v in shape)
+        return tile is not None and extents is None and out is None and N * H * W > TILED_ENCODE_BAND_PIXELS
+
+    def _encode_banded(self, imgs, pads, tile, recursive):
+        """encode_begin of a large tiled batch in bands (DESIGN §4.10), same containers as the whole-image encode.
+        Encoder phase, fine to coarse: every scale's encoder runs band by band on its window of the whole input
+        (region.plan_encoder_bands) and writes its rows of the whole symbol planes, bottleneck values and F.  Coding
+        phase, coarse to fine: per band of tile rows (region.plan_bands, the banded decode's bands) the decoder network
+        runs on its window (_band_window), the band's intervals go straight to band stream planes and one range-coder
+        launch codes the band's streams.  All launches share one slot buffer and one descriptor array, in launch
+        order; the lengths are put back in container order for EncodeJob."""
+        from .region import EncoderGeometry, plan_bands, plan_encoder_bands
+        dev, net = imgs.device, self.net
+        N = imgs.shape[0]
+        K = net.config_ms.prob.K
+        budget = TILED_ENCODE_BAND_PIXELS
+        # ---- encoder phase: S[s] the symbol planes [N][C][H][W], bn[s] their values NHWC (s >= 1)
+        S, bn = [imgs], [None]
+        if net._rgb:
+            for s in list(range(net.scales)) + [-1] * recursive:        # the bicubic x0.5 runs whole
+                eo = net.nets[s].enc(S[-1])
+                S.append(eo.S)
+                bn.append(eo.bn_q)
+        else:
+            geo = EncoderGeometry(net)
+            x = imgs                            # scale-s input: the image, then the operand heads[s] reads of F_s
+            for s in range(net.scales):
+                H, W = (x.shape[2], x.shape[3]) if s == 0 else (x.shape[1], x.shape[2])
+                C = net.config_ms.q.C
+                Sn = torch.empty(N, C, H // 2, W // 2, dtype=torch.uint8, device=dev)
+                bq = torch.empty(N, H // 2, W // 2, 8, dtype=torch.float32, device=dev)
+                Fn = None
+                for band in plan_encoder_bands(geo, s, H, max(1, budget // (2 * N * W))):
+                    (a, b), (r0, r1), o = band.window, band.rows, band.out
+                    org = E._to_device_async(np.tile(np.array([a, 0], np.int32), (N, 1)), dev)
+                    if s == 0:
+                        inp = net._rgb_head_input(E.crop_rect(x, org, b - a, W, nhwc=False))
+                        h = inp if isinstance(inp, E.Act) else net.heads[0](inp)
+                    else:
+                        h = net.heads[s](self._operand_act(E.crop_rect(x, org, b - a, W, nhwc=True)))
+                    eo = net.nets[s].enc(h)
+                    Sn[:, :, r0:r1].copy_(eo.S[:, :, o:o + r1 - r0])
+                    bq[:, r0:r1].copy_(eo.bn_q[:, o:o + r1 - r0])
+                    if s + 1 < net.scales:                  # F_{s+1} feeds heads[s + 1]: keep what that conv reads
+                        op = eo.F.r if E.tensor_core_mode() else eo.F.f
+                        if Fn is None:
+                            Fn = torch.empty(N, H // 2, W // 2, op.shape[-1], dtype=op.dtype, device=dev)
+                        Fn[:, r0:r1].copy_(op[:, o:o + r1 - r0])
+                    del eo, h
+                S.append(Sn)
+                bn.append(bq)
+                x = Fn
+            del x
+
+        # ---- coding phase: the streams, the bands of every scale, the descriptors in launch order
+        scales = list(self.iter_scale_dmll(recursive))
+        shapes = [(scale, S[scale].shape[1], S[scale].shape[2], S[scale].shape[3]) for (scale, _, _) in scales]
+        shapes_of = [list(shapes) for _ in range(N)]
+        layout = stream_layout([[sh[1:] for sh in shapes]] * N, tile)
+        si, elem, n_sym, _ = layout
+        per_img = si.shape[1]
+        caps = _slot_cap(n_sym)
+        slot_off = np.concatenate([[0], np.cumsum(caps)])
+        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
+        geo_d = self._geometry()
+        plans = []                                     # per scale: None (uniform) or [(band, (e0, e1), band layout)]
+        scratch_n = 0
+        for idx, (scale, C, H, W) in enumerate(shapes):
+            if scales[idx][2]:
+                plans.append(None)
+                continue
+            bands = plan_bands([sh[1:] for sh in shapes], tile, geo_d, idx, max(1, budget // (N * tile[0] * W)))
+            plans.append([(band,) + band_streams(layout, idx, C, band) for band in bands])
+            scratch_n = max([scratch_n] + [N * C * (e1 - e0) for (_, (e0, e1), _) in plans[-1]])
+        # the band intervals of every launch go to one scratch buffer: a band's range coder reads it before the next
+        # band's interval kernel writes it (one stream)
+        scratch = torch.empty(max(scratch_n, 1), dtype=torch.int32, device=dev)
+        u_idx = [i for i, p in enumerate(plans) if p is None][0]
+        scale_u, dm_u, _ = scales[u_idx]
+        iv_u = E.reorder_tiles(E.lut_intervals(S[scale_u], self._uniform(dm_u.L, dev)[0]), shapes[u_idx][2],
+                               shapes[u_idx][3], tile, True)
+        desc = np.zeros(caps.size, dtype=_lib.ENC_STREAM_DTYPE).reshape(N, per_img)
+        desc['n_sym'] = n_sym
+        desc['out_cap'] = caps
+        desc['out'] = slots.data_ptr() + slot_off[:-1].reshape(N, per_img)
+        img = np.arange(N)[:, None] * per_img
+        groups = []                                    # launch order: [container indices] per launch
+        for idx, p in enumerate(plans):
+            if p is None:
+                cols = np.flatnonzero(si[0] == idx)
+                desc['intervals'][:, cols] = iv_u.data_ptr() + elem[:, cols] * 4
+                groups.append((img + cols[None, :]).reshape(-1))
+                continue
+            for (_, _, (cols, _, local, _, _)) in p:
+                desc['intervals'][:, cols] = scratch.data_ptr() + local * 4
+                groups.append((img + cols[None, :]).reshape(-1))
+        order = np.concatenate(groups)
+        desc = desc.reshape(-1)
+        desc_l = E._desc_to_device(desc[order], dev)
+        desc_c = E._desc_to_device(desc, dev)
+        lens_l = torch.empty(order.size, dtype=torch.int32, device=dev)
+        starts = np.concatenate([[0], np.cumsum([g.size for g in groups])])
+
+        g = 0
+        bn8, F = None, None
+        dims = [sh[2:] for sh in shapes]
+        whole_F = [None]
+        for idx, ((scale, dmll, uniform), p) in enumerate(zip(scales, plans)):
+            C = shapes[idx][1]
+            if uniform:
+                E.ac_encode_slice(desc_l, lens_l, starts[g], starts[g + 1] - starts[g])
+                g += 1
+            else:
+                fuse = (E.f16_mode() and net.prob_clfs[min(scale, net.scales - 1)].atrous.lin.in_channels % 64 == 0
+                        and C == (3 if dmll.rgb_scale else 5))
+                tg = dmll.targets(dev)
+                F_in = F
+                for (band, (e0, e1), _) in p:
+                    ivb = scratch[:N * C * (e1 - e0)]
+                    y0, h = band.rect[0], band.rect[2] - band.rect[0]
+                    if fuse:
+                        _, F, _ = self._band_window(idx, scale, bn8, F_in, band, dims, whole_F,
+                                                    fused=(S[scale], dmll, (band.out[0], y0, h, tile, ivb)))
+                    else:
+                        l, F, _ = self._band_window(idx, scale, bn8, F_in, band, dims, whole_F)
+                        E.dmll_intervals_band(l, band.out[0], band.out[1], S[scale], y0, h, tg, C, K, dmll.L,
+                                              dmll.rgb_scale, tile, out=ivb)
+                        del l
+                    E.ac_encode_slice(desc_l, lens_l, starts[g], starts[g + 1] - starts[g])
+                    g += 1
+                del F_in
+            if idx + 1 < len(scales):
+                bn8 = bn[scale]                        # what the next finer decoder runs on
+        inv = np.empty_like(order)
+        inv[order] = np.arange(order.size)
+        lens_c = lens_l[E._to_device_async(inv, dev)]
+        return EncodeJob(self, shapes, shapes_of, pads, tile, None, caps, desc_c, lens_c,
+                         (imgs, S, scratch, slots, iv_u, desc_l, lens_l))
+
+    @staticmethod
+    def _operand_act(op):
+        """The engine.Act through which a conv reads the cropped operand `op` of an activation (fp32 in fp32, the TF32
+        twin in tf32, the FP16 or split image in f16 / f16x2): what the conv reads of the whole activation."""
+        if not E.tensor_core_mode():
+            return E.Act(op)
+        if E.f16_mode() or E.f16x2_mode():
+            return E.Act(None, op)
+        return E.Act(op, op)
+
+    def _band_window(self, idx, scale, bn8, F, band, dims, whole_F, fused=None):
+        """The decoder network of one band (region.plan_bands) of scale index idx, run on the band's window of the whole
+        coarser scale, for the banded decode and the banded encode: its symbol values bn8 and (dec.skip) the coarser
+        decoder's features F are cropped from the whole planes, and where the next finer scale adds this decoder's
+        features the band's rows of them go to the whole plane whole_F[0] (allocated at the first band).  dims: (H, W)
+        of every scale walked; fused: get_P_nhwc's.  -> (get_P_nhwc's first result, whole_F[0] or None, its size)."""
+        N, dev = bn8.shape[0], bn8.device
+        (wy0, _, wy1, _), Wc = band.window, bn8.shape[2]
+        org = E._to_device_async(np.tile(np.array([wy0, 0], np.int32), (N, 1)), dev)
+        win = E.crop_rect(bn8, org, wy1 - wy0, Wc, nhwc=True)
+        Fw = None
+        if self.net.fuses(scale):
+            Fw = E.crop_rect(F if torch.is_tensor(F) else F.f, org, wy1 - wy0, Wc, nhwc=True)
+        l, Fo = self.net.get_P_nhwc(scale, win, Fw, fused=fused)
+        if idx + 1 < len(dims) and scale >= 1 and self.net.fuses(scale - 1):
+            # the next scale adds these features: the band's rows of them go to one whole plane
+            (y0, _, y1, _), oy = band.rect, band.out[0]
+            if y0 == 0:
+                whole_F[0] = torch.empty(N, dims[idx][0], dims[idx][1], Fo.f.shape[-1], dtype=Fo.f.dtype, device=dev)
+            whole_F[0][:, y0:y1].copy_(Fo.f[:, oy:oy + y1 - y0])
+            return l, whole_F[0], (2 * (wy1 - wy0), 2 * Wc)
+        return l, None, (2 * (wy1 - wy0), 2 * Wc)
 
     def _scale_intervals(self, out, dev, recursive=0):
         """Coding intervals of every scale, coarse -> fine: [(shape (scale, C, H, W), int32 [N][C][H*W])]."""
@@ -812,28 +997,9 @@ class BatchCodec(object):
 
         whole_F = [None]                  # the features of the scale being banded, assembled band by band
 
-        def band_network(idx, scale, bn8, F, band):
-            # the band's window of the whole coarser scale: its symbol values and, fused, the coarser decoder's features
-            (wy0, _, wy1, _), Wc = band.window, bn8.shape[2]
-            org = E._to_device_async(np.tile(np.array([wy0, 0], np.int32), (N, 1)), dev)
-            win = E.crop_rect(bn8, org, wy1 - wy0, Wc, nhwc=True)
-            Fw = None
-            if self.net.fuses(scale):
-                Fw = E.crop_rect(F if torch.is_tensor(F) else F.f, org, wy1 - wy0, Wc, nhwc=True)
-            l, Fo = self.net.get_P_nhwc(scale, win, Fw)
-            if idx + 1 < len(dims) and scale >= 1 and self.net.fuses(scale - 1):
-                # the next scale adds these features: the band's rows of them go to one whole plane
-                (y0, _, y1, _), oy = band.rect, band.out[0]
-                if y0 == 0:
-                    whole_F[0] = torch.empty(N, dims[idx][0], dims[idx][1], Fo.f.shape[-1], dtype=Fo.f.dtype,
-                                             device=dev)
-                whole_F[0][:, y0:y1].copy_(Fo.f[:, oy:oy + y1 - y0])
-                return l, whole_F[0], (2 * (wy1 - wy0), 2 * Wc)
-            return l, None, (2 * (wy1 - wy0), 2 * Wc)
-
         def network(idx, scale, bn8, F, band=None):
             if band is not None:
-                return band_network(idx, scale, bn8, F, band)
+                return self._band_window(idx, scale, bn8, F, band, dims, whole_F)
             if ragged:
                 ext_dev(idx)                      # queued ahead of the network: the rows and the raster step read it
             l, F = self.net.get_P_nhwc(scale, bn8, F if self.net.fuses(scale) else None, extents=fin)

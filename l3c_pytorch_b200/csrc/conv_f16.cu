@@ -210,10 +210,12 @@ struct Params1 {
 
 // Producer of a 1x1 pipe: pipe 0 first loads the resident weights (PLANES x kunits K chunks of npad rows), then
 // each tile t (pixel tile t / nch) stages its kunits K chunks of 64 pixels, in KIND 2 with their lo plane.
-template <int KIND>
+// tpi > 0 (a band, lin_dmll_f16_kernel): map_x is 3-D [N][pixels][channels] and pixel tile pt is tile pt % tpi of
+// image pt / tpi.
+template <int KIND, bool BAND = false>
 __device__ __forceinline__ void produce_1x1(Ring &ring, const CUtensorMap *map_x, const CUtensorMap *map_w,
                                             TileQueue &tiles, uint32_t w_base, uint32_t wbar, int k, int kunits,
-                                            int npad, int nch, int lo_ch) {
+                                            int npad, int nch, int lo_ch, int tpi = 0) {
     constexpr int PLANES = (KIND == 2) ? 2 : 1;
     constexpr int CH = (KIND == 0) ? 32 : 64;           // channels per K chunk
     if (k == 0) {
@@ -225,8 +227,12 @@ __device__ __forceinline__ void produce_1x1(Ring &ring, const CUtensorMap *map_x
         const int pt = t / nch;
         for (int u = 0; u < kunits; ++u) {
             const Slot s = ring.acquire(PLANES * K1_A_BYTES);
-            tma_load_2d(s.dst, map_x, s.bar, u * CH, pt * 64);
-            if (KIND == 2) tma_load_2d(s.dst + K1_A_BYTES, map_x, s.bar, lo_ch + u * CH, pt * 64);
+            if constexpr (BAND) {
+                tma_load_3d(s.dst, map_x, s.bar, u * CH, (pt % tpi) * 64, pt / tpi);
+            } else {
+                tma_load_2d(s.dst, map_x, s.bar, u * CH, pt * 64);
+                if (KIND == 2) tma_load_2d(s.dst + K1_A_BYTES, map_x, s.bar, lo_ch + u * CH, pt * 64);
+            }
         }
     });
 }
@@ -376,12 +382,46 @@ struct ParamsLD {
     long long M;                // pixels = N * HW
     int HW, L;
     int kchunks, npad;
+    static constexpr bool BAND = false;
 };
 
-template <int C, bool RGB, int NB>
+// A band of a banded encode (l3c_lin_dmll_intervals_band): x is the band's rows of a window's concat buffer, a 3-D
+// TMA map [N][g.h * g.W][Cin] with the window's image stride, tpi pixel tiles per image (HW = 64 tpi, M = N HW: the
+// tile numbering); sym is the whole symbol plane and the intervals go to band stream planes in tile order (BandGeom).
+struct ParamsLDBand : ParamsLD {
+    BandGeom g;
+    int tpi;
+    static constexpr bool BAND = true;
+};
+
+// A band's element of the symbol of channel c of pixel q of image n (its row of the whole symbol plane), and of its
+// interval (its tile-order position in the band stream planes); the whole-plane kernel uses element (n C + c) HW + q
+// for both.  The ParamsLD overloads are never called.
+template <int C>
+__device__ __forceinline__ size_t sym_elem(const ParamsLD &, int, int, int) { return 0; }
+template <int C>
+__device__ __forceinline__ size_t iv_elem(const ParamsLD &, int, int, int) { return 0; }
+template <int C>
+__device__ __forceinline__ size_t sym_elem(const ParamsLDBand &p, int n, int c, int q) {
+    const int y = q / p.g.W;
+    return ((size_t)n * C + c) * p.g.sym_hw + (long long)(p.g.y0 + y) * p.g.W + (q - y * p.g.W);
+}
+template <int C>
+__device__ __forceinline__ size_t iv_elem(const ParamsLDBand &p, int n, int c, int q) {
+    const int y = q / p.g.W;
+    return ((size_t)n * C + c) * ((size_t)p.g.h * p.g.W) +
+           raster_to_tile_order(y, q - y * p.g.W, p.g.h, p.g.W, p.g.th, p.g.tw);
+}
+// a band's images are tpi * 64 pixels apart in the tile numbering (p.HW), of which the first h * W are the band's
+__device__ __forceinline__ bool in_band(const ParamsLD &, long long) { return true; }
+__device__ __forceinline__ bool in_band(const ParamsLDBand &p, long long pix) {
+    return pix % p.HW < (long long)p.g.h * p.g.W;
+}
+
+template <int C, bool RGB, int NB, class P = ParamsLD>
 __global__ void __launch_bounds__(THREADS, 1)
 lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
-                    const ParamsLD p, const int n_stages, const int n_tiles, const TileSchedule ts) {
+                    const P p, const int n_stages, const int n_tiles, const TileSchedule ts) {
     L3C_TRACE_BEGIN;
     constexpr int K = 10;
     constexpr int KP = (RGB ? 4 : 3) * C * K;            // parameters per pixel (the bias has KP entries)
@@ -401,7 +441,13 @@ lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     TileQueue tiles(bars, k, 2, n_tiles, ts);
 
     if (warp >= CONSUMER_WARPS) {
-        if (lane == 0) produce_1x1<1>(ring, &map_x, &map_w, tiles, w_base, weight_bar(bars), k, p.kchunks, NPAD, 1, 0);
+        if constexpr (P::BAND) {
+            if (lane == 0)
+                produce_1x1<1, true>(ring, &map_x, &map_w, tiles, w_base, weight_bar(bars), k, p.kchunks, NPAD, 1, 0,
+                                     p.tpi);
+        } else {
+            if (lane == 0) produce_1x1<1>(ring, &map_x, &map_w, tiles, w_base, weight_bar(bars), k, p.kchunks, NPAD, 1, 0);
+        }
         return;
     }
 
@@ -426,13 +472,13 @@ lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
         // thread = (pixel tid % 64, channels of parity tid / 64)
         const int r = tid & 63, par = tid >> 6;
         const long long pix = (long long)t * 64 + r;
-        const bool valid = pix < p.M;
+        const bool valid = pix < p.M && in_band(p, pix);
         const int n = valid ? (int)(pix / p.HW) : 0;
         const int q = valid ? (int)(pix % p.HW) : 0;
         const float *row = stg + r * S;
         // the RGB coefficients condition channels 1 and 2 on the symbols of channels 0 and 1
-        const float xr = (RGB && valid) ? (float)p.sym[((size_t)n * C + 0) * p.HW + q] : 0.f;
-        const float xg = (RGB && valid) ? (float)p.sym[((size_t)n * C + 1) * p.HW + q] : 0.f;
+        const float xr = (RGB && valid) ? (float)p.sym[P::BAND ? sym_elem<C>(p, n, 0, q) : ((size_t)n * C + 0) * p.HW + q] : 0.f;
+        const float xg = (RGB && valid) ? (float)p.sym[P::BAND ? sym_elem<C>(p, n, 1, q) : ((size_t)n * C + 1) * p.HW + q] : 0.f;
 #pragma unroll
         for (int c = 0; c < C; ++c) {
             if ((c & 1) != par) continue;
@@ -451,13 +497,13 @@ lin_dmll_f16_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
             }
             ChanParams<K> cp;
             channel_params_core<K>(logit, mean, logs, co0, co1, c, RGB, xr, xg, cp);
-            const size_t so = ((size_t)n * C + c) * p.HW + q;
+            const size_t so = P::BAND ? sym_elem<C>(p, n, c, q) : ((size_t)n * C + c) * p.HW + q;
             const int s = valid ? (int)p.sym[so] : 0;
             const uint32_t lo = mixture_cdf_u16<K>(cp.pi, cp.mu, cp.inv_s, __ldg(p.targets + s), scale, s);
             const uint32_t hi = (s == p.L - 1) ? 0x10000u
                                                : mixture_cdf_u16<K>(cp.pi, cp.mu, cp.inv_s, __ldg(p.targets + s + 1),
                                                                     scale, s + 1);
-            if (valid) p.intervals[so] = lo | ((hi - 1u) << 16);
+            if (valid) p.intervals[P::BAND ? iv_elem<C>(p, n, c, q) : so] = lo | ((hi - 1u) << 16);
         }
         wg_sync(k);                                      // staging is rewritten by the next tile
     });
@@ -637,4 +683,59 @@ extern "C" int l3c_lin_dmll_intervals(const void *x_h, const void *w_h, const fl
                                                           r.n_stages, n_tiles);
     return launch_tc<lin_dmll_f16_kernel<5, false, 3>>("lin_dmll_f16_kernel", grid, r.smem_bytes, st, map_x, map_w, q,
                                                        r.n_stages, n_tiles);
+}
+
+// l3c_lin_dmll_intervals for a band of a banded encode: rows [oy, oy + h) of the FP16 concat buffer x_h
+// [N][Hl][W][Cin] of a full-width decoder window, the symbols of rows [y0, y0 + h) of the whole Hs x W plane sym_dev,
+// the intervals in tile order to band stream planes [N][C][h * W]
+extern "C" int l3c_lin_dmll_intervals_band(const void *x_h, int Hl, int oy, const void *w_h, const float *bias,
+                                           const uint8_t *sym_dev, int Hs, int y0, int h, int W,
+                                           const float *targets_dev, int N, int Cin, int C, int K, int L, int rgb,
+                                           int th, int tw, uint32_t *intervals_dev, void *stream) {
+    using namespace l3c;
+    using namespace l3c::f16;
+    L3C_REQUIRE(x_h && w_h && bias && sym_dev && targets_dev && intervals_dev,
+                "l3c_lin_dmll_intervals_band: null pointer");
+    L3C_REQUIRE(N >= 1 && N <= 65535 && Cin % 64 == 0 && Cin >= 64 && th >= 1 && tw >= 1,
+                "l3c_lin_dmll_intervals_band: N=%d Cin=%d tile %dx%d", N, Cin, th, tw);
+    L3C_REQUIRE(K == 10 && L >= 2 && L <= 256, "l3c_lin_dmll_intervals_band: K=%d L=%d (only K=10 is built)", K, L);
+    L3C_REQUIRE((rgb && C == 3) || (!rgb && C == 5), "l3c_lin_dmll_intervals_band: built for RGB (C=3) and C=5 "
+                                                     "bottlenecks, got C=%d rgb=%d", C, rgb);
+    L3C_REQUIRE(h >= 1 && W >= 1 && (long long)h * W < (1ll << 31) && oy >= 0 && oy + h <= Hl && y0 >= 0 &&
+                    y0 + h <= Hs,
+                "l3c_lin_dmll_intervals_band: rows [%d, %d) of a %d-row window, [%d, %d) of a %d-row plane", oy,
+                oy + h, Hl, y0, y0 + h, Hs);
+    const int Kp = (rgb ? 4 : 3) * C * K;
+    const int npad = (Kp + 63) / 64 * 64;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int kchunks = Cin / 64;
+    const int HW = h * W;
+    const int tpi = (HW + 63) / 64;
+    const long long n_tiles64 = (long long)N * tpi;
+    L3C_REQUIRE(n_tiles64 < (1ll << 31), "l3c_lin_dmll_intervals_band: band too large");
+    const int w_bytes = kchunks * npad * 128;
+    const int stg_bytes = 2 * 64 * (npad + 1) * 4 + 64;
+    const RingPlan r = plan_ring(conv_smem_cap(), w_bytes + stg_bytes + SMEM_RESERVE, K1_A_BYTES, MAX_STAGES);
+    L3C_REQUIRE(r.n_stages >= 1, "l3c_lin_dmll_intervals_band: weights do not fit in shared memory (Cin=%d)", Cin);
+    const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    const __half *x0 = reinterpret_cast<const __half *>(x_h) + (long long)oy * W * Cin;
+    alignas(64) CUtensorMap map_x, map_w;
+    if (!encode_tmap(&map_x, "l3c_lin_dmll_intervals_band", "x", dt, x0, {Cin, HW, N},
+                     {2LL * Cin, 2LL * Cin * Hl * W}, {64, 64, 1}) ||
+        !encode_tmap(&map_w, "l3c_lin_dmll_intervals_band", "w", dt, w_h, {64, (long long)kchunks * npad}, {128},
+                     {64, npad}))
+        return L3C_EINVAL;
+    ParamsLDBand q;
+    q.bias = bias; q.sym = sym_dev; q.targets = targets_dev; q.intervals = intervals_dev;
+    q.M = (long long)N * tpi * 64; q.HW = tpi * 64; q.L = L; q.kchunks = kchunks; q.npad = npad;
+    q.g.sym_hw = (long long)Hs * W; q.g.l_hw = (long long)Hl * W;
+    q.g.y0 = y0; q.g.h = h; q.g.W = W; q.g.Wl = W; q.g.oy = oy; q.g.ox = 0; q.g.th = th; q.g.tw = tw;
+    q.tpi = tpi;
+    const int n_tiles = (int)n_tiles64;
+    const int grid = grid_1x1(st, n_tiles);
+    if (rgb)
+        return launch_tc<lin_dmll_f16_kernel<3, true, 2, ParamsLDBand>>("lin_dmll_band_f16_kernel", grid, r.smem_bytes,
+                                                                        st, map_x, map_w, q, r.n_stages, n_tiles);
+    return launch_tc<lin_dmll_f16_kernel<5, false, 3, ParamsLDBand>>("lin_dmll_band_f16_kernel", grid, r.smem_bytes,
+                                                                     st, map_x, map_w, q, r.n_stages, n_tiles);
 }

@@ -30,19 +30,29 @@ namespace l3c {
 // ---------------------------------------------------------------------------------------------
 constexpr int IV_PIX = 64;   // pixels (= threads) per CTA
 
-template <int K>
+// BAND: the pixels are the band `g` (BandGeom, dmll_math.cuh) of a banded encode, HW = g.h * g.W; `l` is the window
+// plane the band sits in, the symbols are read from the whole plane and the intervals written in tile order.
+template <int K, bool BAND = false>
 __global__ void __launch_bounds__(IV_PIX)
 dmll_intervals_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
                       const float *__restrict__ targets, int HW, int C, int L, int rgb,
-                      uint32_t *__restrict__ intervals) {
+                      uint32_t *__restrict__ intervals, const BandGeom g = BandGeom()) {
     extern __shared__ float sm[];
     const int Kp = (rgb ? 4 : 3) * C * K;
     const int pitch = Kp + 1;                       // odd pitch: conflict-free column walks
     const int n = blockIdx.y;
     const int p0 = blockIdx.x * IV_PIX;
     const int np = min(IV_PIX, HW - p0);
-    const float *src = l + ((size_t)n * HW + p0) * Kp;
-    for (int i = threadIdx.x; i < np * Kp; i += IV_PIX) sm[(i / Kp) * pitch + (i % Kp)] = src[i];
+    if constexpr (BAND) {
+        for (int i = threadIdx.x; i < np * Kp; i += IV_PIX) {
+            const int j = i / Kp, pb = p0 + j, py = pb / g.W;
+            const int64_t px = (int64_t)n * g.l_hw + (int64_t)(g.oy + py) * g.Wl + g.ox + (pb - py * g.W);
+            sm[j * pitch + (i - j * Kp)] = l[px * Kp + (i - j * Kp)];
+        }
+    } else {
+        const float *src = l + ((size_t)n * HW + p0) * Kp;
+        for (int i = threadIdx.x; i < np * Kp; i += IV_PIX) sm[(i / Kp) * pitch + (i % Kp)] = src[i];
+    }
     __syncthreads();
     if ((int)threadIdx.x >= np) return;
     const int p = p0 + threadIdx.x;
@@ -52,13 +62,21 @@ dmll_intervals_kernel(const float *__restrict__ l, const uint8_t *__restrict__ s
     for (int c = 0; c < C; ++c) {
         ChanParams<K> cp;
         channel_params<K>(lp, 1, C, c, rgb != 0, xr, xg, cp);
-        const int s = sym[((size_t)n * C + c) * HW + p];
+        int64_t si, oi;
+        if constexpr (BAND) {
+            const int py = p / g.W, px = p - py * g.W;
+            si = ((int64_t)n * C + c) * g.sym_hw + (int64_t)(g.y0 + py) * g.W + px;
+            oi = ((int64_t)n * C + c) * HW + raster_to_tile_order(py, px, g.h, g.W, g.th, g.tw);
+        } else {
+            si = oi = ((size_t)n * C + c) * HW + p;
+        }
+        const int s = sym[si];
         const uint32_t lo = mixture_cdf_u16<K>(cp.pi, cp.mu, cp.inv_s, __ldg(targets + s), scale, s);
         const uint32_t hi = (s == L - 1)
                                 ? 0x10000u
                                 : mixture_cdf_u16<K>(cp.pi, cp.mu, cp.inv_s, __ldg(targets + s + 1),
                                                      scale, s + 1);
-        intervals[((size_t)n * C + c) * HW + p] = lo | ((hi - 1u) << 16);
+        intervals[oi] = lo | ((hi - 1u) << 16);
         if (c == 0) xr = (float)s;
         if (c == 1) xg = (float)s;
     }
@@ -71,26 +89,7 @@ constexpr int TB_PIX = 256;      // pixels per CTA = threads: every warp takes p
                                  // (with 64 pixels per CTA, 6 of 8 warps idled through it and it dominated the kernel)
 constexpr int TB_THREADS = 256;
 
-// Tiled stream order (the throughput mode of the codec, codec.py): a plane of H x W symbols is cut into tiles
-// of th x tw (smaller at the right / bottom edge); the tiles follow each other in row-major tile order, the
-// symbols of a tile in row-major order -- every tile is one coded stream.  Position r in that order -> raster
-// pixel index.  All tiles of a tile row have the same height, so the row starts at ty*th*W.
-__host__ __device__ __forceinline__ int tile_order_to_raster(int r, int H, int W, int th, int tw) {
-    const int ty = r / (th * W);
-    const int h = min(th, H - ty * th);
-    const int rem = r - ty * th * W;
-    const int tx = rem / (tw * h);
-    const int w = min(tw, W - tx * tw);
-    const int rem2 = rem - tx * tw * h;
-    return (ty * th + rem2 / w) * W + tx * tw + rem2 % w;
-}
-
-// Position of raster pixel (y, x) in the tile order of an H x W plane (the inverse of tile_order_to_raster).
-__host__ __device__ __forceinline__ int raster_to_tile_order(int y, int x, int H, int W, int th, int tw) {
-    const int ty = y / th, tx = x / tw;
-    const int h = min(th, H - ty * th), w = min(tw, W - tx * tw);
-    return ty * th * W + tx * tw * h + (y - ty * th) * w + (x - tx * tw);
-}
+// tile_order_to_raster, raster_to_tile_order (the tiled stream order): dmll_math.cuh
 
 // rows (and the symbols of the already decoded channels, `sym`) are indexed in STREAM order: raster order, or
 // tile order when th > 0; the parameters `l` are always read at the raster pixel.  WIN: the H x W symbol plane is
@@ -716,6 +715,32 @@ extern "C" int l3c_dmll_intervals(const float *l_dev, const uint8_t *sym_dev,
     dmll_intervals_kernel<10><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, HW, C, L, rgb, intervals_dev);
     L3C_LAUNCH_CHECK("dmll_intervals_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_intervals_band(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev,
+                                       int Hs, int y0, int h, int W, const float *targets_dev, int N, int C, int K,
+                                       int L, int rgb, int th, int tw, uint32_t *intervals_dev, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(h >= 1 && W >= 1 && (int64_t)h * W < (1ll << 31), "l3c_dmll_intervals_band: %dx%d band", h, W);
+    if (int e = check_common("l3c_dmll_intervals_band", N, h * W, C, K, L, rgb)) return e;
+    L3C_REQUIRE(l_dev && sym_dev && targets_dev && intervals_dev, "l3c_dmll_intervals_band: null pointer");
+    L3C_REQUIRE(th >= 1 && tw >= 1, "l3c_dmll_intervals_band: tile %dx%d", th, tw);
+    L3C_REQUIRE(oy >= 0 && ox >= 0 && oy + h <= Hl && ox + W <= Wl,
+                "l3c_dmll_intervals_band: %dx%d rectangle at (%d, %d) outside the %dx%d parameter plane", h, W, oy, ox,
+                Hl, Wl);
+    L3C_REQUIRE(y0 >= 0 && y0 + h <= Hs, "l3c_dmll_intervals_band: rows [%d, %d) outside the %d-row symbol plane", y0,
+                y0 + h, Hs);
+    const int Kp = (rgb ? 4 : 3) * C * K;
+    const size_t smem = (size_t)IV_PIX * (Kp + 1) * sizeof(float);
+    L3C_REQUIRE(smem <= 48 * 1024, "l3c_dmll_intervals_band: Kp=%d too large", Kp);
+    BandGeom g;
+    g.sym_hw = (long long)Hs * W; g.l_hw = (long long)Hl * Wl;
+    g.y0 = y0; g.h = h; g.W = W; g.Wl = Wl; g.oy = oy; g.ox = ox; g.th = th; g.tw = tw;
+    dim3 grid(ceil_div(h * W, IV_PIX), N);
+    dmll_intervals_kernel<10, true><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, h * W, C, L, rgb, intervals_dev, g);
+    L3C_LAUNCH_CHECK("dmll_intervals_band_kernel");
     return L3C_OK;
 }
 

@@ -1431,11 +1431,15 @@ extern "C" int l3c_pack_streams(const l3c_enc_stream_t *streams_dev, const uint3
                                 void *stream) {
     using namespace l3c;
     if (n_streams == 0) return L3C_OK;
-    L3C_REQUIRE(streams_dev && len_dev && dst_off_dev && blob_dev && n_streams > 0 && n_streams <= 65535,
-                "l3c_pack_streams: bad arguments");
-    dim3 grid(PACK_GRID_X, n_streams);
-    pack_streams_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(streams_dev, len_dev, dst_off_dev, blob_dev);
-    L3C_LAUNCH_CHECK("pack_streams_kernel");
+    L3C_REQUIRE(streams_dev && len_dev && dst_off_dev && blob_dev && n_streams > 0, "l3c_pack_streams: bad arguments");
+    // one stream per grid row: a container of more streams than grid.y holds (a large tiled image) takes several
+    // launches of at most 65535 streams each
+    for (int first = 0; first < n_streams; first += 65535) {
+        dim3 grid(PACK_GRID_X, n_streams - first < 65535 ? n_streams - first : 65535);
+        pack_streams_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(streams_dev + first, len_dev + first,
+                                                                     dst_off_dev + first, blob_dev);
+        L3C_LAUNCH_CHECK("pack_streams_kernel");
+    }
     return L3C_OK;
 }
 

@@ -869,6 +869,46 @@ def lin_dmll_intervals(conv, cat_h, sym, targets, C, K, L, rgb):
     return iv
 
 
+def _band_out(out, N, C, n, device):
+    if out is None:
+        return torch.empty(N, C, n, dtype=torch.int32, device=device)
+    assert out.dtype == torch.int32 and out.is_contiguous() and out.numel() == N * C * n
+    return out.view(N, C, n)
+
+
+def lin_dmll_intervals_band(conv, cat_h, oy, sym, y0, h, targets, C, K, L, rgb, tile, out=None):
+    """lin_dmll_intervals for one band of a banded encode (l3c_lin_dmll_intervals_band): rows [oy, oy + h) of the FP16
+    concat buffer cat_h [N,Hl,W,Cin] of a full-width decoder window, coding the symbols of rows [y0, y0 + h) of the
+    whole planes sym uint8 [N,C,Hs,W] -> intervals int32 [N,C,h*W] in the tile order of an h x W plane (written to
+    `out` when given: an int32 tensor of as many elements)."""
+    N, Hl, W, cin = cat_h.shape
+    assert cat_h.dtype == torch.float16 and cat_h.is_contiguous() and cin == conv.in_channels
+    assert conv.kernel_size[0] == 1 and conv.out_channels == (4 if rgb else 3) * C * K
+    assert sym.dtype == torch.uint8 and sym.is_contiguous() and tuple(sym.shape[:2]) == (N, C) and sym.shape[3] == W
+    w_h, b = _packed_obj(conv).get_f16()
+    iv = _band_out(out, N, C, h * W, cat_h.device)
+    check(lib.l3c_lin_dmll_intervals_band(_ptr(cat_h), Hl, int(oy), _ptr(w_h), _ptr(b), _ptr(sym), sym.shape[2],
+                                          int(y0), int(h), W, _ptr(targets), N, cin, C, K, L, int(rgb), tile[0],
+                                          tile[1], _ptr(iv), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return iv
+
+
+def dmll_intervals_band(l, oy, ox, sym, y0, h, targets, C, K, L, rgb, tile, out=None):
+    """dmll_intervals for one band of a banded encode (l3c_dmll_intervals_band): the parameters of the h x W rectangle
+    at (oy, ox) of l NHWC [N,Hl,Wl,Kp], coding the symbols of rows [y0, y0 + h) of the whole planes sym uint8
+    [N,C,Hs,W] -> intervals int32 [N,C,h*W] in the tile order of an h x W plane (to `out` when given)."""
+    N, Hl, Wl, _ = l.shape
+    W = sym.shape[3]
+    assert l.is_contiguous() and l.dtype == torch.float32
+    assert sym.dtype == torch.uint8 and sym.is_contiguous() and tuple(sym.shape[:2]) == (N, C)
+    iv = _band_out(out, N, C, h * W, l.device)
+    check(lib.l3c_dmll_intervals_band(_ptr(l), Hl, Wl, int(oy), int(ox), _ptr(sym), sym.shape[2], int(y0), int(h), W,
+                                      _ptr(targets), N, C, K, L, int(rgb), tile[0], tile[1], _ptr(iv), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return iv
+
+
 def dmll_sample(l, u_sel, u_x, C, K, rgb):
     """l NHWC [N,H,W,Kp]; u_sel f32 [N,C,K,H,W]; u_x f32 [N,C,H,W] -> sampled values f32 [N,C,H,W]."""
     N, H, W, _ = l.shape
@@ -904,10 +944,19 @@ def ac_encode_streams(desc_np, device):
     return desc, lens
 
 
+def ac_encode_slice(desc_dev, lens_dev, first, n):
+    """l3c_ac_encode_streams on descriptors [first, first + n) of an uploaded array (as ac_encode_streams' desc_dev),
+    their lengths to the same elements of lens_dev (int32)."""
+    first, size = int(first), np.dtype(_lib.ENC_STREAM_DTYPE).itemsize
+    check(lib.l3c_ac_encode_streams(ctypes.c_void_p(desc_dev.data_ptr() + first * size), int(n),
+                                    ctypes.c_void_p(lens_dev.data_ptr() + first * 4), _stream_ptr()))
+    LAUNCHES['n'] += 1
+
+
 def pack_streams(desc_dev, lens_dev, dst_off_np, n, blob):
     off = _to_device_async(dst_off_np.astype(np.int64), blob.device)
     check(lib.l3c_pack_streams(_ptr(desc_dev), _ptr(lens_dev), _ptr(off), n, _ptr(blob), _stream_ptr()))
-    LAUNCHES['n'] += 1
+    LAUNCHES['n'] += -(-n // 65535)                 # one launch per 65535 streams
 
 
 COARSE_PITCH = 96     # uint16 per coarse record (l3c_dmll_build_coarse)

@@ -240,7 +240,9 @@ class StackedAtrousConvs(nn.Module):
 
     def forward(self, x, fused=None):
         """x: engine.Act -> NHWC parameter tensor; or, with fused = (sym uint8 planes, dmll) in f16 mode, the
-        coding intervals of `sym` (the DMLL head runs in the 1x1 conv's epilogue: engine.lin_dmll_intervals)."""
+        coding intervals of `sym` (the DMLL head runs in the 1x1 conv's epilogue: engine.lin_dmll_intervals); with
+        fused = (sym, dmll, (oy, y0, h, tile, out)) those of one band of a banded encode, x being the band's decoder
+        window (engine.lin_dmll_intervals_band)."""
         src = x.f if x.f is not None else x.r
         N, H, W = src.shape[:3]
         Cin = self.atrous[0].in_channels
@@ -253,10 +255,14 @@ class StackedAtrousConvs(nn.Module):
             # tensor cores are on
             E.conv2d(a, x, out=cat, out_coff=i * Cin, want='round')
         if fused is not None:
-            sym, dm = fused
+            sym, dm = fused[:2]
             C = sym.shape[1]
-            return E.lin_dmll_intervals(self.lin, cat, sym, dm.targets(cat.device), C,
-                                        self.lin.out_channels // ((4 if dm.rgb_scale else 3) * C), dm.L, dm.rgb_scale)
+            K = self.lin.out_channels // ((4 if dm.rgb_scale else 3) * C)
+            if len(fused) > 2:
+                oy, y0, h, tile, out = fused[2]
+                return E.lin_dmll_intervals_band(self.lin, cat, oy, sym, y0, h, dm.targets(cat.device), C, K, dm.L,
+                                                 dm.rgb_scale, tile, out=out)
+            return E.lin_dmll_intervals(self.lin, cat, sym, dm.targets(cat.device), C, K, dm.L, dm.rgb_scale)
         return E.conv2d(self.lin, E.Act(None, cat) if f16 else cat)
 
 
@@ -568,7 +574,7 @@ class MultiscaleNetwork(nn.Module):
                 prev_x = loss_dmm.sample(nchw_view(P), C=C)
         return prev_x
 
-    def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False, extents=None, windows=None):
+    def get_P_nhwc(self, scale, bn8, dec_F_prev=None, need_F=False, extents=None, windows=None, fused=None):
         """-> (parameters NHWC, decoder features as engine.Act for the next finer scale).  At scale 0 the
         features feed nothing else (need_F=True keeps their fp32 tensor for the reference-shaped get_P).
         extents: [(h_n, w_n)] at the FINEST scale -> bn8 is a ragged batch (forward()).
@@ -578,7 +584,9 @@ class MultiscaleNetwork(nn.Module):
         scale >= num_scales: a recursive scale of forward(auto_recurse=R) (RGB baselines), num_scales + k the k-th
         extra application of the last trained scale: nets[-1] / prob_clfs[-1], no features in or out (like scale 0,
         its features feed nothing but its probability classifier).  The bit-coder decodes recursive scales of the
-        RGB baselines only (codec.BatchCodec)."""
+        RGB baselines only (codec.BatchCodec).
+        fused: the probability classifier's `fused` argument (StackedAtrousConvs.forward): the first result is then the
+        coding intervals instead of the parameters."""
         ns = self.config_ms.num_scales
         recursive = scale >= ns
         assert 0 <= scale, 'Out of range: {}'.format(scale)
@@ -596,7 +604,7 @@ class MultiscaleNetwork(nn.Module):
         s = -1 if recursive else scale
         with E.ragged_extents(extents, bn8.shape[1] * f, bn8.shape[2] * f):
             F = self.nets[s].dec(bn8, dec_F_prev, operand_only=((scale == 0 or recursive) and not need_F)).F
-            return self.prob_clfs[s](F), F
+            return self.prob_clfs[s](F, fused), F
 
     def get_P(self, scale, bn_q, dec_F_prev=None):
         """multiscale_network.py:308-322 with NCHW-shaped tensors in and out."""

@@ -298,3 +298,66 @@ def plan_passes(plans, ragged):
     for i, p in enumerate(plans):
         groups.setdefault(p.pass_key() if ragged else p.shape_key(), []).append(i)
     return [(idxs, len({plans[i].shape_key() for i in idxs}) > 1) for idxs in groups.values()]
+
+
+class EncoderGeometry(object):
+    """What plan_encoder_bands needs of a MultiscaleNetwork, read from its module tree: per trained scale the radii
+    of heads[s] (3x3; the RGB head at scale 0), enc.down (5x5/s2), the encoder body and to_q (1x1).  The RGB
+    baselines have no encoder network (their bicubic x0.5 runs whole): radii is empty then."""
+
+    def __init__(self, net):
+        self.num_scales = net.scales
+        self.rgb = bool(net._rgb)
+        self.radii = []
+        if self.rgb:
+            return
+        for s in range(net.scales):
+            enc = net.nets[s].enc
+            head = net.heads[0].head[1].head if s == 0 else net.heads[s].head
+            body = list(enc.body)
+            self.radii.append(dict(
+                head=_radius(head), down=enc.down.dilation[0] * (enc.down.kernel_size[0] - 1) // 2,
+                body=sum(_radius(m.body[0]) + _radius(m.body[2]) for m in body[:-1]) + _radius(body[-1]),
+                to_q=_radius(enc.to_q[0])))
+
+
+class EncoderBand(object):
+    """One band of the encoder of a scale: rows = [r0, r1) of the scale-(s+1) planes it writes (S, bottleneck values,
+    F); window = [a, b) the rows of the full-width scale-s input (the image or F_s) it runs on, a even; out = r0 - a/2,
+    where its rows start in the window's output."""
+    __slots__ = ('scale', 'rows', 'window', 'out')
+
+    def __init__(self, scale, rows, window):
+        self.scale, self.rows, self.window = scale, rows, window
+        self.out = rows[0] - window[0] // 2
+
+    def __repr__(self):
+        return 'EncoderBand(scale=%d, rows=%s, window=%s)' % (self.scale, self.rows, self.window)
+
+
+def encoder_window(geo, scale, r0, r1, H):
+    """The rows of the H-row input of scale `scale`'s encoder that its output rows [r0, r1) depend on (DESIGN §4.10):
+    widened by the body (and to_q) radius, doubled, widened by the down conv's and the head's radii, clipped to the
+    plane and started on an even row (the stride-2 grid of the full run).  -> (a, b)."""
+    r = geo.radii[scale]
+    m = r['body'] + r['to_q']
+    a, b = 2 * (r0 - m) - r['down'] - r['head'], 2 * (r1 + m) + r['down'] + r['head']
+    a, b = max(a, 0), min(b, H)
+    return a - a % 2, b
+
+
+def plan_encoder_bands(config, scale, H, rows):
+    """Banded encoder of trained scale `scale` (0 .. num_scales - 1) of an L3C network whose input plane has H rows:
+    its H / 2 output rows cut into bands of `rows` rows (the last one partial), top to bottom.  config: a
+    MultiscaleNetwork or its EncoderGeometry.  -> [EncoderBand]."""
+    geo = config if isinstance(config, EncoderGeometry) else EncoderGeometry(config)
+    if geo.rgb:
+        raise ValueError('the RGB baselines have no encoder network to band (their bicubic x0.5 runs whole)')
+    if not 0 <= scale < geo.num_scales:
+        raise ValueError('scale %d has no encoder (the network has %d scales)' % (scale, geo.num_scales))
+    rows = int(rows)
+    if rows < 1:
+        raise ValueError('a band needs at least one row, got %d' % rows)
+    Ho = H // 2
+    return [EncoderBand(scale, (r0, min(r0 + rows, Ho)), encoder_window(geo, scale, r0, min(r0 + rows, Ho), H))
+            for r0 in range(0, Ho, rows)]

@@ -1,13 +1,14 @@
 #!/usr/bin/env python
 """bench_large.py -- large images as one tiled container (DESIGN §4.10) against the reference's crop parts, one GPU.
 
-  python tools/bench_large.py [--sizes 4096x3072,6000x4000,8000x6000] [--tile 64] [--mode f16] [--runs 2]
-                              [--no-unbanded]
+  python tools/bench_large.py [--sizes 4096x3072,6000x4000,8000x6000,16384x16384] [--tile 64] [--mode f16]
+                              [--runs 2] [--no-unbanded] [--no-parts]
 
 Workload: one uint8 noise image per size (default about 12, 24 and 48 Mpx), `cr.cf` with seed-0 default-init weights.
 Per size, three ways to store it, run alternated `--runs` times after one warm-up of each:
-  * whole: one tiled container (tiles of --tile), its decode banded (codec.TILED_BAND_PIXELS);
-  * unbanded: the same container decoded with banding switched off, where that fits on the card;
+  * whole: one tiled container (tiles of --tile), its encode and decode banded;
+  * unbanded: the same container encoded and decoded with banding switched off (codec.TILED_ENCODE_BAND_PIXELS,
+    codec.TILED_BAND_PIXELS), where that fits on the card;
   * parts: the image cut by auto_crop into the reference's crops (2000 x 1500 px at most), each a tiled container.
 Every figure is a host clock around work that ends in a device synchronise; peak device memory is
 torch.cuda.max_memory_allocated above what was allocated before the call.  Every decode is checked lossless.  Also a
@@ -32,6 +33,7 @@ def main():
     ap.add_argument('--mode', default='f16')
     ap.add_argument('--runs', type=int, default=2)
     ap.add_argument('--no-unbanded', action='store_true')
+    ap.add_argument('--no-parts', action='store_true')
     args = ap.parse_args()
 
     import numpy as np
@@ -46,7 +48,7 @@ def main():
     E.set_conv_precision(args.mode)
     tile = (args.tile, args.tile)
     bc = l3c.Bitcoding(bp, tile=tile, crop=False)
-    budget = codec.TILED_BAND_PIXELS
+    budget, enc_budget = codec.TILED_BAND_PIXELS, codec.TILED_ENCODE_BAND_PIXELS
     try:
         power = subprocess.run(['nvidia-smi', '-i', '0', '--query-gpu=power.limit', '--format=csv,noheader'],
                                capture_output=True, text=True, timeout=30).stdout.strip() or None
@@ -77,8 +79,12 @@ def main():
         x = img.unsqueeze(0).to(dev)
         crops = [c[0] for c in auto_crop.iter_crops(x)]
 
-        def enc_whole():
-            return bc.codec.encode_batch(x, tile=tile)[0]
+        def enc_whole(band=True):
+            codec.TILED_ENCODE_BAND_PIXELS = enc_budget if band else 1 << 62
+            try:
+                return bc.codec.encode_batch(x, tile=tile)[0]
+            finally:
+                codec.TILED_ENCODE_BAND_PIXELS = enc_budget
 
         def dec_whole(datas, band):
             codec.TILED_BAND_PIXELS = budget if band else 1 << 62
@@ -94,9 +100,11 @@ def main():
             got = auto_crop.stitch(out)[0] if name == 'parts' else out[0]
             return torch.equal(got, x[0].to(got.dtype))
 
-        variants = {'whole': (enc_whole, lambda d: dec_whole(d, True)), 'parts': (enc_parts, bc.decode_batch)}
+        variants = {'whole': (enc_whole, lambda d: dec_whole(d, True))}
+        if not args.no_parts:
+            variants['parts'] = (enc_parts, bc.decode_batch)
         if not args.no_unbanded:
-            variants['unbanded'] = (enc_whole, lambda d: dec_whole(d, False))
+            variants['unbanded'] = (lambda: enc_whole(False), lambda d: dec_whole(d, False))
         res = {k: {'enc_ms': [], 'enc_peak_mb': [], 'dec_ms': [], 'dec_peak_mb': []} for k in variants}
         datas_of = {}
         for run in range(args.runs + 1):                  # run 0 warms every shape up and checks the result
@@ -122,10 +130,10 @@ def main():
             reg = ((H - 512) // 2, (W - 512) // 2, 512, 512)
             bc.decode_region(d, reg)
             region = [measured(lambda: bc.decode_region(d, reg))[:2] for _ in range(max(args.runs, 3))]
-        line = {'metric': 'large image: one tiled container (banded decode) vs unbanded vs crop parts',
+        line = {'metric': 'large image: one tiled container (banded encode and decode) vs unbanded vs crop parts',
                 'config': {'workload': 'cr.cf seed-0 weights, one 3x%dx%d uint8 noise image (%.1f Mpx), tile %dx%d'
                                        % (H, W, H * W / 1e6, tile[0], tile[1]), 'mode': args.mode, 'runs': args.runs,
-                           'band_pixels': budget, 'parts': len(crops)},
+                           'band_pixels': budget, 'encode_band_pixels': enc_budget, 'parts': len(crops)},
                 'bytes': {k: (sum(len(v) for v in datas_of[k]) if datas_of.get(k) else None) for k in variants},
                 'results': res, 'region_512': {'ms_and_peak_mb': region},
                 'gpu': torch.cuda.get_device_name(0), 'power_limit': power}
