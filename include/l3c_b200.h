@@ -536,6 +536,36 @@ int l3c_dmll_nll_train(const float *l_dev, const float *x_dev, int N, int HW, in
 int l3c_soft_quantize(const float *q_dev, int64_t n, const float *levels_dev, int L, float sigma, int64_t *sym_dev,
                       float *value_dev, const float *grad_dev, float *dq_dev, void *stream);
 
+/* Backward of the 3x3, stride-1, 64-input-channel convolutions (padding = dilation = d in {1, 2, 4}, Cout in {64,
+ * 256}) on the TF32 tensor cores, fp32 accumulation.  Tensors are NHWC fp32: x [N][H][W][64], dy [N][H][W][Cout],
+ * dx [N][H][W][64].  Every call checks its arguments before any GPU work and refuses (L3C_EINVAL) null pointers,
+ * Cin != 64, Cout not in {64, 256}, d not in {1, 2, 4}, N not in [1, 65535], H * W above 2^30 (MAX_PLANE_PIXELS)
+ * and pointers that are not 16-byte aligned (so an element offset that is not a multiple of 64 bits is refused).
+ * Every output element is written once, in a fixed order: the same inputs give the same bits on every run. */
+
+/* y_dev[i] = x_dev[i] rounded to TF32 (cvt.rna), n values; y_dev may be x_dev.  The operand image the TF32 kernels
+ * read (the tensor cores would otherwise truncate). */
+int l3c_round_tf32(const float *x_dev, float *y_dev, int64_t n, void *stream);
+
+/* Data gradient: dx = the 3x3 conv of dy with the weights flipped spatially and Cin / Cout swapped, no bias, run by
+ * the forward TF32 kernel (conv3x3_tf32_kernel).  dy_dev must hold TF32-rounded values (l3c_round_tf32).
+ * w_dev: the flipped image [Cout / 64][9 taps][2 K-halves][64 ci][32 co] fp32, TF32-rounded; slice s reads the
+ * channels 64s..64s+63 of dy, and the Cout / 64 slices are added in order 0, 1, ... through the kernel's residual
+ * epilogue (Cout / 64 launches). */
+int l3c_conv3x3_dgrad(const float *dy_dev, const float *w_dev, int N, int H, int W, int Cin, int Cout, int dilation,
+                      float *dx_dev, void *stream);
+
+/* Bytes of the workspace l3c_conv3x3_wgrad needs for this shape (0 for an invalid one). */
+int64_t l3c_conv3x3_wgrad_workspace(int N, int H, int W, int Cout);
+
+/* Weight and bias gradient: dw_dev [Cout][64][3][3] (OIHW, as nn.Conv2d's weight) = sum over n, y, x of
+ * dy[n, y, x, co] * x[n, y + d (ky - 1), x + d (kx - 1), ci] (x = 0 outside the image); db_dev [Cout] = sum of dy.
+ * The pixels are split into chunks of whole 8x16 tiles, one chunk per CTA (the split depends on the shape only);
+ * each CTA accumulates its chunk with mma.sync m16n8k8 TF32 on operands rounded to TF32 (RN) and writes its partial
+ * sums to work_dev, then a second launch adds the chunks in chunk order.  No atomics. */
+int l3c_conv3x3_wgrad(const float *x_dev, const float *dy_dev, int N, int H, int W, int Cin, int Cout, int dilation,
+                      float *dw_dev, float *db_dev, float *work_dev, int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,10 @@ _SIGNATURES = {
     'l3c_batch_rows': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_uint32, c_void_p, c_void_p]),
     'l3c_dmll_nll_train': (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_float] * 3 + [c_void_p] * 5),
     'l3c_soft_quantize': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_float] + [c_void_p] * 5),
+    'l3c_round_tf32': (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
+    'l3c_conv3x3_dgrad': (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_void_p]),
+    'l3c_conv3x3_wgrad_workspace': (c_int64, [c_int] * 4),
+    'l3c_conv3x3_wgrad': (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p] * 3 + [c_int64, c_void_p]),
 }
 
 EXPORTS = sorted(_SIGNATURES)

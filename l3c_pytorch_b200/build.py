@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, 'csrc')
 SO = os.path.join(HERE, 'libl3c_b200.so')
 SO_TRACE = os.path.join(HERE, 'libl3c_b200_trace.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-SOURCES = ['capi.cu', 'range_coder.cu', 'dmll.cu', 'conv_ffma.cu', 'conv_tf32.cu', 'conv_f16.cu', 'conv_f16x2.cu', 'bicubic.cu', 'partition.cu', 'ragged.cu', 'torchac_batch.cu']
+SOURCES = ['capi.cu', 'range_coder.cu', 'dmll.cu', 'conv_ffma.cu', 'conv_tf32.cu', 'conv_train.cu', 'conv_f16.cu', 'conv_f16x2.cu', 'bicubic.cu', 'partition.cu', 'ragged.cu', 'torchac_batch.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--fmad=true',
               '-DL3C_BUILDING_DSO']

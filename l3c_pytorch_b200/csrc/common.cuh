@@ -5,6 +5,8 @@
 #include <stdio.h>
 #include <stdarg.h>
 
+#include <initializer_list>
+
 #include "../../include/l3c_b200.h"
 
 namespace l3c {
@@ -43,6 +45,11 @@ void count_launch(const char *kernel_name);   // per-kernel launch counters (l3c
 
 // 1x1 layers with Cin % 64 == 0 on the tensor cores, all three tensor-core precisions (conv_f16.cu)
 int conv1x1_tc(const l3c_conv_t &p, cudaStream_t st);
+
+// Argument checks of the 3x3 backward passes (conv_train.cu): every pointer non-null and 16-byte aligned, Cin 64,
+// Cout 64 or 256, dilation 1, 2 or 4, N in [1, 65535], H * W <= 2^30.  L3C_EINVAL with the message otherwise.
+int conv3x3_backward_args(const char *fn, std::initializer_list<const void *> ptrs, int N, int H, int W, int Cin,
+                          int Cout, int dilation);
 
 int sm_count();                          // SMs of the current device
 int stream_sm_count(cudaStream_t st);    // SMs available to kernels launched into `st` (partition.cu)

@@ -23,6 +23,8 @@
 // host side, activations by the producing layer's epilogue, which writes a second, rounded copy (`y_tf32`) next
 // to the fp32 tensor that residual adds and the fp32 layers keep using.
 // (The faster FP16-operand variant of this path is conv_f16.cu, precision L3C_PREC_F16.)
+#include <mutex>
+
 #include "tc_conv.cuh"
 
 namespace l3c {
@@ -150,26 +152,8 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     });
 }
 
-}  // namespace tc
-
-int conv2d_tf32(const l3c_conv_t &p, cudaStream_t st) {
-    using namespace tc;
-    if (p.precision != L3C_PREC_TF32) {
-        set_error("l3c_conv2d: precision mode %d is not built (available: fp32, tf32, f16, f16x2)", p.precision);
-        return L3C_EINVAL;
-    }
-    // The tensor-core kernels cover the 3x3 / 64-input-channel layers (> 92 % of the FLOPs of a round trip) and
-    // the 1x1 layers with Cin % 64 == 0.  The host mirror routes the other layers (5x5/s2 down-sampling,
-    // Cin != 64) to L3C_PREC_FP32 explicitly (engine.conv2d); nothing falls back silently here.
-    const bool k3 = p.ksize == 3 && p.stride == 1 && p.Cin == 64 && p.x_pitch == 64;
-    const bool k1 = p.ksize == 1 && p.stride == 1 && p.Cin % 64 == 0 && p.x_pitch == p.Cin &&
-                    !(p.flags & L3C_CONV_PIXEL_SHUFFLE2);
-    const bool eligible = (k3 || k1) && p.cout_pad % 64 == 0 && p.cout_pad >= p.Cout &&
-                          (k1 || ((p.Cout % 64 == 0) && (p.y_pitch % 4 == 0) && (p.y_coff % 4 == 0)));
-    L3C_REQUIRE(eligible, "l3c_conv2d: tf32 tensor-core path needs 3x3/Cin=64 or 1x1/Cin%%64==0, stride 1 "
-                          "(got k=%d s=%d Cin=%d pitch=%d Cout=%d)", p.ksize, p.stride, p.Cin, p.x_pitch, p.Cout);
-    if (k1) return conv1x1_tc(p, st);
-
+// A checked 3x3 layer: p.x is read as N x H x W pixels of p.Cin = 64 channels, p.x_pitch apart
+static int launch_3x3(const l3c_conv_t &p, cudaStream_t st) {
     const int d = p.dilation;
     const int a_rows = TH + 2 * d;
     const int a_bytes = a_rows * TW * 128;
@@ -189,4 +173,67 @@ int conv2d_tf32(const l3c_conv_t &p, cudaStream_t st) {
                                           st, map_x, map_w, q, r.n_pipes, r.n_stages, a_bytes, ptiles);
 }
 
+}  // namespace tc
+
+int conv2d_tf32(const l3c_conv_t &p, cudaStream_t st) {
+    using namespace tc;
+    if (p.precision != L3C_PREC_TF32) {
+        set_error("l3c_conv2d: precision mode %d is not built (available: fp32, tf32, f16, f16x2)", p.precision);
+        return L3C_EINVAL;
+    }
+    // The tensor-core kernels cover the 3x3 / 64-input-channel layers (> 92 % of the FLOPs of a round trip) and
+    // the 1x1 layers with Cin % 64 == 0.  The host mirror routes the other layers (5x5/s2 down-sampling,
+    // Cin != 64) to L3C_PREC_FP32 explicitly (engine.conv2d); nothing falls back silently here.
+    const bool k3 = p.ksize == 3 && p.stride == 1 && p.Cin == 64 && p.x_pitch == 64;
+    const bool k1 = p.ksize == 1 && p.stride == 1 && p.Cin % 64 == 0 && p.x_pitch == p.Cin &&
+                    !(p.flags & L3C_CONV_PIXEL_SHUFFLE2);
+    const bool eligible = (k3 || k1) && p.cout_pad % 64 == 0 && p.cout_pad >= p.Cout &&
+                          (k1 || ((p.Cout % 64 == 0) && (p.y_pitch % 4 == 0) && (p.y_coff % 4 == 0)));
+    L3C_REQUIRE(eligible, "l3c_conv2d: tf32 tensor-core path needs 3x3/Cin=64 or 1x1/Cin%%64==0, stride 1 "
+                          "(got k=%d s=%d Cin=%d pitch=%d Cout=%d)", p.ksize, p.stride, p.Cin, p.x_pitch, p.Cout);
+    if (k1) return conv1x1_tc(p, st);
+    return tc::launch_3x3(p, st);
+}
+
+// The zero bias of the data-gradient launches: 64 floats per device, made once
+static int zero_bias(const float **out) {
+    static std::mutex mu;
+    static float *buf[64] = {};
+    std::lock_guard<std::mutex> lk(mu);
+    float *&b = buf[current_device_slot()];
+    if (!b) {
+        L3C_CUDA(cudaMalloc(&b, 64 * sizeof(float)));
+        L3C_CUDA(cudaMemset(b, 0, 64 * sizeof(float)));
+        L3C_CUDA(cudaDeviceSynchronize());
+    }
+    *out = b;
+    return L3C_OK;
+}
+
 }  // namespace l3c
+
+using namespace l3c;
+
+extern "C" int l3c_conv3x3_dgrad(const float *dy_dev, const float *w_dev, int N, int H, int W, int Cin, int Cout,
+                                 int dilation, float *dx_dev, void *stream) {
+    if (int e = conv3x3_backward_args("l3c_conv3x3_dgrad", {dy_dev, w_dev, dx_dev}, N, H, W, Cin, Cout, dilation))
+        return e;
+    const float *zero = nullptr;
+    if (int e = zero_bias(&zero)) return e;
+    // slice s: the 64 channels 64s.. of dy (pitch Cout) against image slice s, added to dx through the residual
+    for (int s = 0; s < Cout / 64; ++s) {
+        l3c_conv_t p = {};
+        p.x = dy_dev + 64 * s;
+        p.w = w_dev + (size_t)s * 9 * 2 * 64 * 32;
+        p.bias = zero;
+        p.residual = s ? dx_dev : nullptr;
+        p.y = dx_dev;
+        p.N = N; p.H = H; p.W = W;
+        p.Cin = 64; p.x_pitch = Cout;
+        p.Cout = 64; p.cout_pad = 64; p.y_pitch = 64; p.y_coff = 0;
+        p.ksize = 3; p.stride = 1; p.dilation = dilation;
+        p.flags = 0; p.precision = L3C_PREC_TF32;
+        if (int e = tc::launch_3x3(p, (cudaStream_t)stream)) return e;
+    }
+    return L3C_OK;
+}

@@ -230,28 +230,42 @@ class PackedConv(object):
     def __init__(self, conv):
         self.conv = conv
         self._key = None
-        self.w = self.b = self.w_tc = self.w_h = self.w_h2 = self.w_im2col = None
+        self.w = self.b = self.w_tc = self.w_h = self.w_h2 = self.w_im2col = self.w_dgrad = None
 
-    def get(self):
-        """FFMA image (conv_ffma.cu): OIHW -> [KH][KW][Cin][cout_pad] fp32, bias padded to cout_pad."""
+    def _sync(self):
+        """Drops every image when the parameters' key changed."""
         w, b = self.conv.weight, self.conv.bias
         key = (w.data_ptr(), w._version, b.data_ptr(), b._version, str(w.device))
         if key != self._key:
             require_cuda(w, 'conv weight')
+            self.w = self.b = self.w_tc = self.w_h = self.w_h2 = self.w_im2col = self.w_dgrad = None
+            self._key = key
+
+    def _bias(self):
+        """the bias padded to cout_pad"""
+        self._sync()
+        if self.b is None:
+            b = self.conv.bias
+            bp = torch.zeros((b.shape[0] + 63) // 64 * 64, dtype=torch.float32, device=b.device)
+            bp[:b.shape[0]] = b.detach().float()
+            self.b = bp
+        return self.b
+
+    def get(self):
+        """FFMA image (conv_ffma.cu): OIHW -> [KH][KW][Cin][cout_pad] fp32, bias padded to cout_pad."""
+        b = self._bias()
+        if self.w is None:
+            w = self.conv.weight
             cout, cin, kh, kw = w.shape
-            cout_pad = (cout + 63) // 64 * 64
-            wp = torch.zeros(kh, kw, cin, cout_pad, dtype=torch.float32, device=w.device)
+            wp = torch.zeros(kh, kw, cin, b.shape[0], dtype=torch.float32, device=w.device)
             wp[..., :cout] = w.detach().float().permute(2, 3, 1, 0)
-            bp = torch.zeros(cout_pad, dtype=torch.float32, device=w.device)
-            bp[:cout] = b.detach().float()
-            self.w, self.b, self._key = wp, bp, key
-            self.w_tc = self.w_h = self.w_h2 = self.w_im2col = None
-        return self.w, self.b
+            self.w = wp
+        return self.w, b
 
     def get_tc(self):
         """TF32 tensor-core image (conv_tf32.cu): [tap][K-half = Cin/32][Cout padded to 64][32] fp32, K-major rows
         of 128 B that TMA drops into 128B-swizzled shared memory; values pre-rounded to TF32 (RN)."""
-        _, b = self.get()
+        b = self._bias()
         if self.w_tc is None:
             w = round_to_tf32(self.conv.weight.detach().float())
             cout, cin, kh, kw = w.shape
@@ -261,6 +275,22 @@ class PackedConv(object):
             img[:, :, :cout] = w.permute(2, 3, 0, 1).reshape(kh * kw, cout, cin // 32, 32).permute(0, 2, 1, 3)
             self.w_tc = img.contiguous()
         return self.w_tc, b
+
+    def get_dgrad(self):
+        """Data-gradient image of a 3x3 layer with Cin 64 (l3c_conv3x3_dgrad): the weights flipped spatially with Cin
+        and Cout swapped, as Cout / 64 forward images of 64 -> 64 convs, [Cout/64][tap][K-half][64 ci][32 co] fp32,
+        values rounded to TF32 (RN).  Rebuilt with the other images when the parameters change."""
+        self._sync()
+        if self.w_dgrad is None:
+            w = self.conv.weight.detach().float()                              # [Cout, 64, 3, 3]
+            cout, cin, kh, kw = w.shape
+            assert cin == 64 and kh == kw == 3 and cout % 64 == 0
+            # img[s][tap][kh][ci][j] = w[64 s + 32 kh + j][ci][2 - ky][2 - kx]
+            img = w.flip(2, 3).reshape(cout // 64, 2, 32, 64, 9).permute(0, 4, 1, 3, 2).contiguous()
+            check(lib.l3c_round_tf32(_ptr(img), _ptr(img), img.numel(), _stream_ptr()))
+            LAUNCHES['n'] += 1
+            self.w_dgrad = img
+        return self.w_dgrad
 
     def get_f16(self):
         """F16 tensor-core image (conv_f16.cu): 3x3 / 5x5 -> [taps][cout_pad][64 cin] fp16, 1x1 ->
@@ -842,6 +872,61 @@ def soft_quantize(q, levels, sigma, grad=None):
                                 _ptr(grad), _ptr(dq), _stream_ptr()))
     LAUNCHES['n'] += 1
     return dq
+
+
+def round_tf32(x):
+    """l3c_round_tf32: a new tensor of the contiguous fp32 CUDA tensor x rounded to TF32 (RN), the operand image the
+    TF32 kernels read."""
+    require_cuda(x, 'x')
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    out = torch.empty_like(x)
+    check(lib.l3c_round_tf32(_ptr(x), _ptr(out), x.numel(), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return out
+
+
+def _nhwc_args(t, what):
+    require_cuda(t, what)
+    assert t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 4, (what, t.dtype, tuple(t.shape))
+
+
+def conv3x3_train(conv, x):
+    """Forward of a 3x3 / Cin 64 layer of the training step: x NHWC fp32 [N,H,W,64] -> y NHWC [N,H,W,Cout] in TF32
+    (conv3x3_tf32_kernel on the TF32-rounded x, bias added, no epilogue)."""
+    _nhwc_args(x, 'x')
+    return conv2d(conv, Act(x, round_tf32(x)), precision=_lib.PREC_TF32)
+
+
+def conv3x3_dgrad(conv, dy):
+    """Data gradient of a 3x3 / Cin 64 layer (l3c_conv3x3_dgrad): dy NHWC fp32 [N,H,W,Cout] -> dx NHWC [N,H,W,64],
+    dy rounded to TF32 first.  Cout / 64 launches of the forward TF32 kernel on PackedConv.get_dgrad."""
+    _nhwc_args(dy, 'dy')
+    N, H, W, cout = dy.shape
+    assert cout == conv.out_channels
+    dyr = round_tf32(dy)
+    w = _packed_obj(conv).get_dgrad()
+    dx = torch.empty(N, H, W, conv.in_channels, dtype=torch.float32, device=dy.device)
+    check(lib.l3c_conv3x3_dgrad(_ptr(dyr), _ptr(w), N, H, W, conv.in_channels, cout, conv.dilation[0], _ptr(dx),
+                                _stream_ptr()))
+    LAUNCHES['n'] += cout // 64
+    return dx
+
+
+def conv3x3_wgrad(conv, x, dy):
+    """Weight and bias gradient of a 3x3 / Cin 64 layer (l3c_conv3x3_wgrad): x NHWC fp32 [N,H,W,64] (the layer's
+    input), dy NHWC [N,H,W,Cout] -> (dW [Cout,64,3,3] like conv.weight, db [Cout]).  Two launches, no atomics."""
+    _nhwc_args(x, 'x')
+    _nhwc_args(dy, 'dy')
+    N, H, W, cout = dy.shape
+    assert tuple(x.shape) == (N, H, W, conv.in_channels) and cout == conv.out_channels
+    work = torch.empty(max(1, lib.l3c_conv3x3_wgrad_workspace(N, H, W, cout) // 4), dtype=torch.float32,
+                       device=dy.device)
+    dw = torch.empty(cout, conv.in_channels, 3, 3, dtype=torch.float32, device=dy.device)
+    db = torch.empty(cout, dtype=torch.float32, device=dy.device)
+    check(lib.l3c_conv3x3_wgrad(_ptr(x), _ptr(dy), N, H, W, conv.in_channels, cout, conv.dilation[0], _ptr(dw),
+                                _ptr(db), _ptr(work), work.numel() * 4, _stream_ptr()))
+    LAUNCHES['n'] += 2
+    return dw, db
 
 
 def dmll_channel_params(l, x_dec, C, K, rgb, c):

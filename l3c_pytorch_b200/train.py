@@ -1,6 +1,7 @@
 """Training step of L3C (SURVEY.md section 8 row f4): PyTorch autograd over the SAME parameter tree
 (`MultiscaleNetwork`'s nn.Conv2d containers), so that what it trains loads into the sm_90a coding path unchanged.
-The convolutions and their backward are torch's (cuDNN on the GPU).  The two per-pixel losses are the library's
+The convolutions and their backward are torch's (cuDNN on the GPU), except with FUSED_CONV, where the 3x3 layers with
+64 input channels run the library's TF32 kernels forward and backward (DESIGN §4.11).  The two per-pixel losses are the library's
 kernels on CUDA tensors (DESIGN §4.9): the DMLL negative log-likelihood of every scale and the soft quantiser, each
 forward and backward in one pass over its inputs, without torch's per-element autograd graph.  CPU tensors, and CUDA
 tensors with FUSED_LOSS = False, take the torch restatements `dmll_nll` and `soft_quantize_torch`, which stay the
@@ -29,6 +30,11 @@ _K = 10                       # the mixture size the kernels are built for (dmll
 # CUDA tensors: True runs the DMLL loss and the soft quantiser as the library's kernels, False as the torch
 # restatements below (for comparisons on the GPU: tests/test_gpu_train_kernels.py, tools/bench_train.py)
 FUSED_LOSS = True
+
+# CUDA tensors: True runs every 3x3 / stride-1 / 64-input-channel layer of forward_train (Cout 64 or 256, dilation 1,
+# 2 or 4) as _Conv3x3Fn, forward and backward on the library's TF32 kernels (DESIGN §4.11); False, and every other
+# layer (the RGB head, the 5x5/s2 down conv, the 1x1s), calls the nn.Conv2d itself (cuDNN)
+FUSED_CONV = False
 
 
 def _require_f32(what, *ts):
@@ -81,12 +87,58 @@ def soft_quantize_torch(x, levels, sigma):
     return x_soft, x_hard, sym
 
 
+def conv3x3_in_scope(conv):
+    """The layers _Conv3x3Fn runs: 3x3, stride 1, padding = dilation in {1, 2, 4}, 64 -> 64 or 256, with bias."""
+    d = conv.dilation[0]
+    return (tuple(conv.kernel_size) == (3, 3) and tuple(conv.stride) == (1, 1) and conv.in_channels == 64 and
+            conv.out_channels in (64, 256) and conv.groups == 1 and conv.bias is not None and d in (1, 2, 4) and
+            tuple(conv.dilation) == (d, d) and tuple(conv.padding) == (d, d) and conv.padding_mode == 'zeros')
+
+
+def _nhwc(t):
+    """NCHW-shaped tensor -> its NHWC view, copied to channels_last memory first where it is not already"""
+    return t.contiguous(memory_format=torch.channels_last).permute(0, 2, 3, 1)
+
+
+class _Conv3x3Fn(torch.autograd.Function):
+    """(x NCHW, weight, bias, conv) -> conv(x) NCHW-shaped in channels_last memory: forward conv3x3_tf32_kernel, backward
+    l3c_conv3x3_dgrad / l3c_conv3x3_wgrad.  Saves only x and the weight."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, conv):
+        ctx.save_for_backward(x, weight)
+        ctx.conv = conv
+        return E.conv3x3_train(conv, _nhwc(x)).permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, _ = ctx.saved_tensors
+        dy = _nhwc(gy)
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = E.conv3x3_dgrad(ctx.conv, dy).permute(0, 3, 1, 2)
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            dw, db = E.conv3x3_wgrad(ctx.conv, _nhwc(x), dy)
+        return dx, dw, db, None
+
+
+def _conv(conv, x):
+    """conv(x) for forward_train: _Conv3x3Fn for an in-scope layer on CUDA tensors with FUSED_CONV, else the
+    nn.Conv2d."""
+    if not (FUSED_CONV and x.is_cuda and conv3x3_in_scope(conv)):
+        return conv(x)
+    if x.dtype != torch.float32 or conv.weight.dtype != torch.float32 or conv.bias.dtype != torch.float32:
+        raise TypeError('conv3x3: the training kernels take fp32 tensors, got x %s, weight %s'
+                        % (x.dtype, conv.weight.dtype))
+    return _Conv3x3Fn.apply(x, conv.weight, conv.bias, conv)
+
+
 def _res_body(body, x):
     """Sequential of ResBlocks + final conv with the outer skip (net.py:144,181; edsr.py:83-86)."""
     y = x
     for m in list(body)[:-1]:
-        y = m.body[2](F.relu(m.body[0](y))) + y
-    return body[-1](y) + x
+        y = _conv(m.body[2], F.relu(_conv(m.body[0], y))) + y
+    return _conv(body[-1], y) + x
 
 
 def _enc_forward(enc, x):
@@ -104,12 +156,12 @@ def _dec_forward(dec, bn, fuse):
     if fuse is not None:
         x = x + fuse
     x = _res_body(dec.body, x)
-    return F.pixel_shuffle(dec.tail[0](x), 2)
+    return F.pixel_shuffle(_conv(dec.tail[0], x), 2)
 
 
 def _prob_clf(clf, x):
     a = clf.atrous
-    return a.lin(torch.cat([c(x) for c in a.atrous], dim=1))
+    return a.lin(torch.cat([_conv(c, x) for c in a.atrous], dim=1))
 
 
 def dmll_nll(dm, x, l):
@@ -195,7 +247,7 @@ def forward_train(net, x):
     encs = []
     for s in range(net.scales):
         head = net.heads[s]
-        inp = head.head[1].head(head.head[0](inp)) if s == 0 else head.head(inp)
+        inp = head.head[1].head(head.head[0](inp)) if s == 0 else _conv(head.head, inp)
         bn, bn_q, sym, feat = _enc_forward(net.nets[s].enc, inp)
         encs.append((bn, bn_q))
         syms.append(sym)
