@@ -360,9 +360,13 @@ def _split_host(w):
 
 def round_to_tf32(t):
     """fp32 tensor -> nearest TF32-representable fp32 (10-bit mantissa, ties away from zero like
-    `cvt.rna.tf32.f32`).  Host-side preparation of the tensor-core weight image."""
+    `cvt.rna.tf32.f32`).  Host-side preparation of the tensor-core weight image.  As the instruction does on sm_90a,
+    only finite values are rounded; an inf or NaN keeps its upper 19 bits, so a NaN whose payload lies wholly in the
+    low 13 bits becomes inf there and here.  (Adding the half ulp to a NaN could carry its payload into the sign bit
+    and give +-0.)"""
     bits = t.contiguous().view(torch.int32)
-    return ((bits + 0x1000) & -8192).view(torch.float32)
+    finite = (bits & 0x7F800000) != 0x7F800000
+    return (torch.where(finite, bits + 0x1000, bits) & -8192).view(torch.float32)
 
 
 class Act(object):
@@ -880,8 +884,9 @@ def round_tf32(x):
     require_cuda(x, 'x')
     assert x.dtype == torch.float32 and x.is_contiguous()
     out = torch.empty_like(x)
-    check(lib.l3c_round_tf32(_ptr(x), _ptr(out), x.numel(), _stream_ptr()))
-    LAUNCHES['n'] += 1
+    if x.numel():                 # an empty tensor has no storage: a null pointer the C entry point refuses
+        check(lib.l3c_round_tf32(_ptr(x), _ptr(out), x.numel(), _stream_ptr()))
+        LAUNCHES['n'] += 1
     return out
 
 

@@ -20,6 +20,7 @@ Works on CPU tensors as well as CUDA ones.
 import numpy as np
 import torch
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from . import engine as E
 from .dmll import non_shared_get_K
@@ -96,8 +97,12 @@ def conv3x3_in_scope(conv):
 
 
 def _nhwc(t):
-    """NCHW-shaped tensor -> its NHWC view, copied to channels_last memory first where it is not already"""
-    return t.contiguous(memory_format=torch.channels_last).permute(0, 2, 3, 1)
+    """NCHW-shaped tensor -> its NHWC view, copied to channels_last memory first where it is not already, or where
+    it does not start on a 16-byte boundary (a view at an element offset; the kernels read float4s)"""
+    t = t.contiguous(memory_format=torch.channels_last)
+    if t.data_ptr() % 16:
+        t = t.clone(memory_format=torch.channels_last)
+    return t.permute(0, 2, 3, 1)
 
 
 class _Conv3x3Fn(torch.autograd.Function):
@@ -111,6 +116,7 @@ class _Conv3x3Fn(torch.autograd.Function):
         return E.conv3x3_train(conv, _nhwc(x)).permute(0, 3, 1, 2)
 
     @staticmethod
+    @once_differentiable        # the kernels' outputs carry no graph: a double backward must raise, not drop them
     def backward(ctx, gy):
         x, _ = ctx.saved_tensors
         dy = _nhwc(gy)
