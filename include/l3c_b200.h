@@ -303,6 +303,17 @@ int l3c_dmll_intervals_band(const float *l_dev, int Hl, int Wl, int oy, int ox, 
                             int y0, int h, int W, const float *targets_dev, int N, int C, int K, int L, int rgb,
                             int th, int tw, uint32_t *intervals_dev, void *stream);
 
+/* The intervals of one tile-aligned rectangle of a region update (DESIGN §4.12): as l3c_dmll_intervals_band for the
+ * h x w rectangle at (y0, x0) of the symbol window sym_dev uint8 [N][C][Hs][Ws], which sits at (sy, sx) of the
+ * container's Hf x Wf plane, with the parameters at (oy, ox) of l_dev f32 NHWC [N][Hl][Wl][Kp]; intervals in the tile
+ * order (th x tw) of an h x w plane to intervals_dev uint32 [N][C][h * w].  In the Hf x Wf plane the rectangle starts
+ * on a tile boundary and ends on one or at the plane's edge (else an error), so its tile order is that of the plane's
+ * own tiles.  A band is the rectangle x0 = 0, w = Ws of a whole plane (sy = sx = 0, Hf x Wf = Hs x Ws). */
+int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev, int Hs, int Ws,
+                            int y0, int x0, int h, int w, int sy, int sx, int Hf, int Wf, const float *targets_dev,
+                            int N, int C, int K, int L, int rgb, int th, int tw, uint32_t *intervals_dev,
+                            void *stream);
+
 /* sub_rgb_mean + first MeanShift of RGBHead as one per-pixel 3x3 affine pair
  * (multiscale_network.py:181-183, head.py:31-33): img uint8 [N][3][HW] planes ->
  * x_sub f32 NHWC [N][HW][3] (= A1 img + b1)  and  t f32 NHWC [N][HW][4] (= A2 x_sub + b2, ch 3 = 0).

@@ -76,6 +76,8 @@ _SIGNATURES = {
                                     [c_int] * 8 + [c_void_p, c_void_p]),
     'l3c_dmll_intervals_band': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 7 +
                                 [c_void_p, c_void_p]),
+    'l3c_dmll_intervals_rect': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 10 + [c_void_p] + [c_int] * 7 +
+                                [c_void_p, c_void_p]),
     'l3c_rgb_prep': (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_split_f16x2': (c_int, [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p]),
     'l3c_rgb_im2col_f16': (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p, c_void_p]),

@@ -299,6 +299,15 @@ class Bitcoding(object):
         after another (BatchCodec.decode_regions)."""
         return [S.long() for S in self.codec.decode_regions(datas, regions, levels, lane=lane)]
 
+    def update_region(self, data, pos, patch):
+        """A tiled container with the pixels at pos = (y, x) replaced by `patch` (DESIGN §4.12) -> the new container
+        bytes, byte-identical to encoding the edited image.  pos is in the coordinates decode() returns (the unpadded
+        image); patch: uint8 or int64 [3, h, w] or [1, 3, h, w], values 0..255, on any device.  Only the tile streams
+        the edit can change are re-encoded, from a bounded window of the image (BatchCodec.update_region).
+        ValueError, before any GPU work, for the reference layout, a container this model did not write, the RGB
+        baselines, an empty patch or one not in the image, and a patch that is not 3-channel."""
+        return self.codec.update_region(data, pos, patch)
+
 
 class _ListEncodeJob:
     """encode_batch_begin: the codec jobs of its passes (one for a batch tensor); finish() -> (containers, bpsps) in

@@ -5,6 +5,7 @@
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png
     python -m l3c_pytorch_b200.cli --config cr_rgb_shared --ckpt CKPT.pt enc IMG OUT.l3c --recursive auto
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png --region Y,X,H,W [--level K]
+    python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt upd IN.l3c PATCH.png Y,X OUT.l3c [--overwrite]
 
 `--ckpt` is a checkpoint as written by the reference's Saver (`torch.save({'net': state_dict})`,
 helpers/saver.py:168); the module tree here has the same parameter names, so it loads strict.
@@ -131,7 +132,25 @@ def build_parser():
                    help='tiled files: decode only this crop (DESIGN §4.8), decoding only the tiles it depends on')
     d.add_argument('--level', default=0, type=int, metavar='K',
                    help='with --region, RGB baselines: the crop is of the stored scale-K thumbnail (0 = the image)')
+    u = sub.add_parser('upd', help='tiled L3C files: write OUT.l3c, IN.l3c with the pixels at Y,X replaced by '
+                                   'PATCH.png (DESIGN §4.12), re-encoding only the tiles the edit can change')
+    u.add_argument('inp')
+    u.add_argument('patch')
+    u.add_argument('pos', type=parse_pos, metavar='Y,X')
+    u.add_argument('out')
+    u.add_argument('--overwrite', action='store_true')
     return p
+
+
+def parse_pos(text):
+    """'Y,X' -> (y, x)."""
+    try:
+        vals = tuple(int(v) for v in text.split(','))
+    except ValueError:
+        vals = ()
+    if len(vals) != 2:
+        raise argparse.ArgumentTypeError('the position takes Y,X (two integers), got %r' % text)
+    return vals
 
 
 def parse_tile(text):
@@ -175,6 +194,29 @@ def decode_region(bc, pin, png_out, region, level=0):
     print('Decoded region {} (level {}) of {} -> {}'.format(region, level, pin, png_out))
 
 
+def update_region(bc, pin, patch_p, pos, pout, overwrite=False):
+    """`upd`: IN.l3c with the pixels at pos replaced by the image PATCH, written to OUT.  ValueError for crop files
+    (`.partN`, an image coded in parts), an existing OUT without --overwrite and what Bitcoding.update_region
+    refuses."""
+    from . import part_suffix_helper
+    if not os.path.isfile(pin):
+        if os.path.isfile(pin + '.part0'):
+            raise ValueError('{} is stored in parts ({}.part0, ...): region update of part files is not '
+                             'supported'.format(pin, pin))
+        raise DecodeError('File not found: {}'.format(pin))
+    if part_suffix_helper.contains_part_suffix(pin):
+        raise ValueError('{} is one part of an image coded in parts: region update of part files is not '
+                         'supported'.format(pin))
+    if os.path.isfile(pout) and not overwrite:
+        raise ValueError('{} exists. Consider --overwrite.'.format(pout))
+    with open(pin, 'rb') as f:
+        data = f.read()
+    out = bc.update_region(data, pos, read_image(patch_p))
+    with open(pout, 'wb') as f:
+        f.write(out)
+    print('Updated {} at {} with {} -> {}'.format(pin, pos, patch_p, pout))
+
+
 def main(argv=None):
     a = build_parser().parse_args(argv)
     from .bitcoding import Bitcoding
@@ -184,6 +226,11 @@ def main(argv=None):
     try:
         if a.mode == 'enc':
             encode(bc, a.img, a.out, a.overwrite)
+        elif a.mode == 'upd':
+            try:
+                update_region(bc, a.inp, a.patch, a.pos, a.out, a.overwrite)
+            except ValueError as err:
+                raise EncodeError(str(err))
         elif a.region is not None:
             try:
                 decode_region(bc, a.inp, a.out_png, a.region, a.level)

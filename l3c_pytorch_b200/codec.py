@@ -341,6 +341,9 @@ class BatchCodec(object):
         self._geo = None
         # streams and symbols the last decode_regions call handed to the range decoder (decode_region_pass)
         self.region_counts = {'streams': 0, 'symbols': 0}
+        # what the last update_region call did: streams re-encoded, streams in the container, pixels of the window it
+        # encoded and whether it took the whole-image path
+        self.update_counts = {'streams': 0, 'total': 0, 'window_pixels': 0, 'whole': False}
 
     # ------------------------------------------------------------------------------------------
     def iter_scale_dmll(self, recursive=0):
@@ -1188,6 +1191,181 @@ class BatchCodec(object):
                                 network, rows, raster, symbols, features)
         return crop(S, [(p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1]) for p in plans],
                     [size(p.region) for p in plans], nhwc=False, split=True)
+
+    # ------------------------------------------------------------------------------------------
+    def _update_patch(self, patch):
+        """The patch of update_region as uint8 [1, 3, h, w] on the codec's device; ValueError for anything else."""
+        if not torch.is_tensor(patch) or patch.dtype not in (torch.uint8, torch.int64):
+            raise ValueError('patch must be a uint8 or int64 tensor, got %s' % (
+                patch.dtype if torch.is_tensor(patch) else type(patch).__name__))
+        if patch.dim() == 4 and patch.shape[0] == 1:
+            patch = patch[0]
+        if patch.dim() != 3 or patch.shape[0] != 3:
+            raise ValueError('patch must be [3, h, w] or [1, 3, h, w] (3 channels), got %s' % (tuple(patch.shape),))
+        if patch.shape[1] < 1 or patch.shape[2] < 1:
+            raise ValueError('empty patch %s' % (tuple(patch.shape),))
+        if patch.dtype != torch.uint8 and (int(patch.min()) < 0 or int(patch.max()) > 255):
+            raise ValueError('patch values must lie in 0..255')
+        return patch.to(self.blueprint.device, torch.uint8).contiguous().unsqueeze(0)
+
+    @_on_device
+    def update_region(self, data, pos, patch):
+        """A tiled L3C container with the pixels at pos = (y, x) (unpadded image coordinates) replaced by `patch`
+        (uint8 / int64 [3, h, w] or [1, 3, h, w], 0..255, any device) -> the new container bytes, byte-identical to
+        encoding the edited image (DESIGN §4.12).  Only the tile streams the edit can change are re-encoded
+        (region.plan_update): the old pixels of the plan's window P_0 come from decode_regions, the encoder runs on
+        its planned window of every scale, the decoder networks on their windows, the intervals of every re-encoded
+        rectangle come from l3c_dmll_intervals_rect, and one range-coder launch codes every new stream; the host
+        splices them into the old container.  A window of more than TILED_ENCODE_BAND_PIXELS pixels takes the whole
+        path instead: decode the container, paste, encode the image (both banded where large).  update_counts says
+        what ran.  ValueError, before any GPU work, for the reference layout, a container this model did not write,
+        the RGB baselines, an empty patch or one not in the unpadded image, and a patch that is not 3-channel."""
+        from .region import plan_update
+        tile = container_tile(data)
+        if tile is None:
+            raise ValueError('region update needs a tiled container (written with Bitcoding(..., tile=(th, tw))): '
+                             'the streams of the reference layout are serial')
+        pad_tuple, parsed = parse_container(data)
+        shapes = [(C, H, W) for (C, H, W, _) in parsed]
+        try:
+            self._check_shapes(shapes)
+        except ValueError as err:
+            raise ValueError('the container was not written by this model: %s' % err)
+        if len(pos) != 2:
+            raise ValueError('pos must be (y, x), got %r' % (pos,))
+        patch = self._update_patch(patch)
+        y, x = (int(v) for v in pos)
+        h, w = patch.shape[2:]
+        plan = plan_update(shapes, pad_tuple, tile, self.net, (y, x, h, w))
+        left, _, top, _ = pad_tuple
+        if plan.window_pixels > TILED_ENCODE_BAND_PIXELS:
+            img, _ = self.decode_batch([data], to_host=False)
+            img[:, :, top + y:top + y + h, left + x:left + x + w] = patch
+            out = self.encode_batch(img, pad_tuple, tile=tile)[0][0]
+            self.update_counts = {'streams': plan.total_streams, 'total': plan.total_streams,
+                                  'window_pixels': img.shape[2] * img.shape[3], 'whole': True}
+            return out
+        return self._update_window(data, parsed, pad_tuple, tile, plan, patch)
+
+    def _update_window(self, data, parsed, pad_tuple, tile, plan, patch):
+        """update_region's window path (DESIGN §4.12)."""
+        dev, net = self.blueprint.device, self.net
+        K = net.config_ms.prob.K
+        sc = {sp.scale: sp for sp in plan.scales}
+        left, right, top, bottom = pad_tuple
+        _, Hf, Wf = parsed[-1][:3]
+
+        def org(y0, x0):
+            return E._to_device_async(np.array([[y0, x0]], np.int32), dev)
+
+        def crop(src, at, r, nhwc):
+            """rectangle r (y0, x0, y1, x1) of the plane whose origin is `at`, as a new tensor"""
+            return E.crop_rect(src, org(r[0] - at[0], r[1] - at[1]), r[2] - r[0], r[3] - r[1], nhwc=nhwc)
+
+        # ---- the pixels of P_0: the old ones (the padding is zero), the patch pasted in
+        P = plan.window
+        img = torch.zeros(1, 3, P[2] - P[0], P[3] - P[1], dtype=torch.uint8, device=dev)
+        u = (max(P[0], top), max(P[1], left), min(P[2], Hf - bottom), min(P[3], Wf - right))
+        old = self.decode_regions([data], [(u[0] - top, u[1] - left, u[2] - u[0], u[3] - u[1])])[0]
+        img[:, :, u[0] - P[0]:u[2] - P[0], u[1] - P[1]:u[3] - P[1]] = old
+        e = plan.edit
+        img[:, :, e[0] - P[0]:e[2] - P[0], e[1] - P[1]:e[3] - P[1]] = patch
+        del old
+
+        # ---- encoder phase, fine to coarse: every scale's encoder on its planned window of the finer outputs
+        sym = {0: ((P[0], P[1]), img)}                          # scale -> (origin, symbol window [1][C][h][w])
+        bq = {}                                                 # scale -> (origin, bottleneck values NHWC)
+        x, at = img, (P[0], P[1])
+        for s in range(net.scales):
+            a = sc[s].enc
+            if s == 0:
+                inp = net._rgb_head_input(crop(x, at, a, nhwc=False))
+                hd = inp if isinstance(inp, E.Act) else net.heads[0](inp)
+            else:
+                hd = net.heads[s](self._operand_act(crop(x, at, a, nhwc=True)))
+            eo = net.nets[s].enc(hd)
+            o = (a[0] // 2, a[1] // 2)
+            sym[s + 1] = (o, eo.S.contiguous())
+            bq[s + 1] = (o, eo.bn_q.contiguous())
+            if s + 1 < net.scales:                  # F_{s+1} feeds heads[s + 1]: keep what that conv reads
+                x, at = (eo.F.r if E.tensor_core_mode() else eo.F.f).contiguous(), o
+            del eo, hd
+        del x
+
+        # ---- coding phase, coarse to fine: the intervals of every R_s in its tile order, then one range-coder launch
+        ivs, cols, n_sym, ptrs = [], [], [], []
+        base, F, fwin = 0, None, None
+        for sp, (scale, dmll, uniform) in zip(plan.scales, self.iter_scale_dmll()):
+            r, C = sp.rect, sp.C
+            h, w = r[2] - r[0], r[3] - r[1]
+            o, S = sym[scale]
+            if uniform:
+                iv = E.reorder_tiles(E.lut_intervals(crop(S, o, r, nhwc=False), self._uniform(dmll.L, dev)[0]), h, w,
+                                     tile, True)
+            else:
+                win = sp.window
+                ob, b = bq[scale + 1]
+                Fw = None
+                if sp.fused:
+                    Fw = crop(F.f, (2 * fwin[0], 2 * fwin[1]), win, nhwc=True)
+                l, F = net.get_P_nhwc(scale, crop(b, ob, win, nhwc=True), Fw)
+                fwin = win
+                iv = E.dmll_intervals_rect(l, sp.out[0], sp.out[1], S, (r[0] - o[0], r[1] - o[1], h, w),
+                                           dmll.targets(dev), C, K, dmll.L, dmll.rgb_scale, tile, origin=o,
+                                           plane=(sp.H, sp.W))
+                del l
+            ivs.append(iv)
+            T = len(tile_grid(sp.H, sp.W, tile))
+            grid = np.array(tile_grid(h, w, tile), np.int64)                 # the rectangle's tiles, in sp.tiles order
+            for c in range(C):
+                cols.append(base + c * T + np.asarray(sp.tiles, np.int64))
+                n_sym.append(grid[:, 1])
+                ptrs.append(iv.data_ptr() + (c * h * w + grid[:, 0]) * 4)
+            base += C * T
+        del F
+        cols, n_sym, ptrs = np.concatenate(cols), np.concatenate(n_sym), np.concatenate(ptrs)
+        caps = _slot_cap(n_sym)
+        slot_off = np.concatenate([[0], np.cumsum(caps)])
+        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
+        desc = np.zeros(cols.size, dtype=_lib.ENC_STREAM_DTYPE)
+        desc['intervals'] = ptrs
+        desc['n_sym'] = n_sym
+        desc['out_cap'] = caps
+        desc['out'] = slots.data_ptr() + slot_off[:-1]
+        _, lens_dev = E.ac_encode_streams(desc, dev)
+        lens_h = torch.empty(lens_dev.shape, dtype=lens_dev.dtype, pin_memory=True)
+        slots_h = torch.empty(slots.shape, dtype=torch.uint8, pin_memory=True)
+        lens_h.copy_(lens_dev, non_blocking=True)
+        slots_h.copy_(slots, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        del ivs
+        lens = lens_h.numpy().astype(np.int64)
+        if (lens > caps).any():
+            raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
+
+        # ---- splice: the old streams' bytes, the new ones in their places, laid out afresh
+        old_off = np.array([o for (_, _, _, st) in parsed for (o, _) in st], np.int64)
+        old_len = np.array([n for (_, _, _, st) in parsed for (_, n) in st], np.int64)
+        new_len = old_len.copy()
+        new_len[cols] = lens
+        layout = ContainerLayout([(i, C, H, W) for i, (C, H, W, _) in enumerate(parsed)], tile)
+        total, pieces, new_off = layout.header_and_offsets(new_len, pad_tuple)
+        new_off = np.asarray(new_off, np.int64)
+        buf = np.empty(total, np.uint8)
+        for o, b in pieces:
+            buf[o:o + len(b)] = np.frombuffer(b, np.uint8)
+        src = np.frombuffer(data, np.uint8)
+        changed = np.sort(cols)
+        # a run of unchanged streams keeps its bytes and the headers between them: one copy per run
+        for a, b in zip(np.concatenate([[0], changed + 1]), np.concatenate([changed, [old_len.size]])):
+            if b > a:
+                buf[new_off[a]:new_off[b - 1] + new_len[b - 1]] = src[old_off[a]:old_off[b - 1] + old_len[b - 1]]
+        sl = slots_h.numpy()
+        for k, col in enumerate(cols):
+            buf[new_off[col]:new_off[col] + lens[k]] = sl[slot_off[k]:slot_off[k] + lens[k]]
+        self.update_counts = {'streams': int(cols.size), 'total': plan.total_streams,
+                              'window_pixels': plan.window_pixels, 'whole': False}
+        return buf.tobytes()
 
     # stage timing of a decode (bench.py / tools): set `codec.stage_events = []` before decode_device,
     # synchronise, then read stage_ms()

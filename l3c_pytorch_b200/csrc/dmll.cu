@@ -30,13 +30,14 @@ namespace l3c {
 // ---------------------------------------------------------------------------------------------
 constexpr int IV_PIX = 64;   // pixels (= threads) per CTA
 
-// BAND: the pixels are the band `g` (BandGeom, dmll_math.cuh) of a banded encode, HW = g.h * g.W; `l` is the window
-// plane the band sits in, the symbols are read from the whole plane and the intervals written in tile order.
-template <int K, bool BAND = false>
+// BAND: the pixels are the band `g` (BandGeom, dmll_math.cuh) of a banded encode, or the tile-aligned rectangle `g`
+// (RectGeom) of a region update, HW = g.h * g.W; `l` is the window plane the band sits in, the symbols are read from
+// the whole plane and the intervals written in tile order.
+template <int K, bool BAND = false, class G = BandGeom>
 __global__ void __launch_bounds__(IV_PIX)
 dmll_intervals_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
                       const float *__restrict__ targets, int HW, int C, int L, int rgb,
-                      uint32_t *__restrict__ intervals, const BandGeom g = BandGeom()) {
+                      uint32_t *__restrict__ intervals, const G g = G()) {
     extern __shared__ float sm[];
     const int Kp = (rgb ? 4 : 3) * C * K;
     const int pitch = Kp + 1;                       // odd pitch: conflict-free column walks
@@ -65,7 +66,7 @@ dmll_intervals_kernel(const float *__restrict__ l, const uint8_t *__restrict__ s
         int64_t si, oi;
         if constexpr (BAND) {
             const int py = p / g.W, px = p - py * g.W;
-            si = ((int64_t)n * C + c) * g.sym_hw + (int64_t)(g.y0 + py) * g.W + px;
+            si = ((int64_t)n * C + c) * g.sym_hw + sym_row(g, py) + px;
             oi = ((int64_t)n * C + c) * HW + raster_to_tile_order(py, px, g.h, g.W, g.th, g.tw);
         } else {
             si = oi = ((size_t)n * C + c) * HW + p;
@@ -741,6 +742,43 @@ extern "C" int l3c_dmll_intervals_band(const float *l_dev, int Hl, int Wl, int o
     dmll_intervals_kernel<10, true><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, h * W, C, L, rgb, intervals_dev, g);
     L3C_LAUNCH_CHECK("dmll_intervals_band_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev,
+                                       int Hs, int Ws, int y0, int x0, int h, int w, int sy, int sx, int Hf, int Wf,
+                                       const float *targets_dev, int N, int C, int K, int L, int rgb, int th, int tw,
+                                       uint32_t *intervals_dev, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(h >= 1 && w >= 1 && (int64_t)h * w < (1ll << 31), "l3c_dmll_intervals_rect: %dx%d rectangle", h, w);
+    if (int e = check_common("l3c_dmll_intervals_rect", N, h * w, C, K, L, rgb)) return e;
+    L3C_REQUIRE(l_dev && sym_dev && targets_dev && intervals_dev, "l3c_dmll_intervals_rect: null pointer");
+    L3C_REQUIRE(th >= 1 && tw >= 1, "l3c_dmll_intervals_rect: tile %dx%d", th, tw);
+    L3C_REQUIRE(oy >= 0 && ox >= 0 && (int64_t)oy + h <= Hl && (int64_t)ox + w <= Wl,
+                "l3c_dmll_intervals_rect: %dx%d rectangle at (%d, %d) outside the %dx%d parameter plane", h, w, oy, ox,
+                Hl, Wl);
+    L3C_REQUIRE(y0 >= 0 && x0 >= 0 && (int64_t)y0 + h <= Hs && (int64_t)x0 + w <= Ws,
+                "l3c_dmll_intervals_rect: %dx%d rectangle at (%d, %d) outside the %dx%d symbol plane", h, w, y0, x0, Hs,
+                Ws);
+    L3C_REQUIRE(sy >= 0 && sx >= 0 && (int64_t)sy + Hs <= Hf && (int64_t)sx + Ws <= Wf,
+                "l3c_dmll_intervals_rect: %dx%d symbol window at (%d, %d) outside the %dx%d plane", Hs, Ws, sy, sx, Hf, Wf);
+    // tile-aligned in the whole plane: starts on a tile boundary, ends on one or at the plane's edge, so the
+    // rectangle's tile order is that of the plane's own tiles
+    const int ry = sy + y0, rx = sx + x0;
+    L3C_REQUIRE(ry % th == 0 && rx % tw == 0 && ((ry + h) % th == 0 || ry + h == Hf) && ((rx + w) % tw == 0 || rx + w == Wf),
+                "l3c_dmll_intervals_rect: %dx%d rectangle at (%d, %d) of a %dx%d plane is not aligned to %dx%d tiles",
+                h, w, ry, rx, Hf, Wf, th, tw);
+    const int Kp = (rgb ? 4 : 3) * C * K;
+    const size_t smem = (size_t)IV_PIX * (Kp + 1) * sizeof(float);
+    L3C_REQUIRE(smem <= 48 * 1024, "l3c_dmll_intervals_rect: Kp=%d too large", Kp);
+    RectGeom g;
+    g.sym_hw = (long long)Hs * Ws; g.l_hw = (long long)Hl * Wl;
+    g.y0 = y0; g.h = h; g.W = w; g.Wl = Wl; g.oy = oy; g.ox = ox; g.th = th; g.tw = tw;
+    g.x0 = x0; g.Ws = Ws;
+    dim3 grid(ceil_div(h * w, IV_PIX), N);
+    dmll_intervals_kernel<10, true, RectGeom><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, h * w, C, L, rgb, intervals_dev, g);
+    L3C_LAUNCH_CHECK("dmll_intervals_rect_kernel");
     return L3C_OK;
 }
 

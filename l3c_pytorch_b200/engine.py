@@ -999,6 +999,26 @@ def dmll_intervals_band(l, oy, ox, sym, y0, h, targets, C, K, L, rgb, tile, out=
     return iv
 
 
+def dmll_intervals_rect(l, oy, ox, sym, rect, targets, C, K, L, rgb, tile, origin=(0, 0), plane=None, out=None):
+    """dmll_intervals for one tile-aligned rectangle of a region update (l3c_dmll_intervals_rect): the parameters of
+    the h x w rectangle at (oy, ox) of l NHWC [N,Hl,Wl,Kp], coding the symbols of rect = (y0, x0, h, w) of the window
+    sym uint8 [N,C,Hs,Ws] -> intervals int32 [N,C,h*w] in the tile order of an h x w plane (to `out` when given).
+    The window sits at `origin` of the container's plane of (H, W) = `plane` (default: sym is the whole plane), in
+    which the rectangle must be tile-aligned."""
+    N, Hl, Wl, _ = l.shape
+    y0, x0, h, w = (int(v) for v in rect)
+    Hs, Ws = sym.shape[2], sym.shape[3]
+    Hf, Wf = (Hs, Ws) if plane is None else (int(plane[0]), int(plane[1]))
+    assert l.is_contiguous() and l.dtype == torch.float32
+    assert sym.dtype == torch.uint8 and sym.is_contiguous() and tuple(sym.shape[:2]) == (N, C)
+    iv = _band_out(out, N, C, h * w, l.device)
+    check(lib.l3c_dmll_intervals_rect(_ptr(l), Hl, Wl, int(oy), int(ox), _ptr(sym), Hs, Ws, y0, x0, h, w,
+                                      int(origin[0]), int(origin[1]), Hf, Wf, _ptr(targets), N, C, K, L, int(rgb),
+                                      tile[0], tile[1], _ptr(iv), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return iv
+
+
 def dmll_sample(l, u_sel, u_x, C, K, rgb):
     """l NHWC [N,H,W,Kp]; u_sel f32 [N,C,K,H,W]; u_x f32 [N,C,H,W] -> sampled values f32 [N,C,H,W]."""
     N, H, W, _ = l.shape

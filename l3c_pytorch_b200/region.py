@@ -214,11 +214,15 @@ def plan_region(shapes, pad_tuple, tile, config, region, level=0):
     return RegionPlan(plans, region_px, level, tile, n, recursive)
 
 
-def _window(geo, scale, rect, H, W, Hc, Wc):
+def _window(geo, scale, rect, H, W, Hc, Wc, features=None):
     """The decoder window of the symbols `rect` of an H x W plane at `scale`, on the Hc x Wc coarser plane: -> (window,
-    out, fused, want), `want` being the coarser rectangle the window and (fused) the coarser decoder's features need."""
+    out, fused, want), `want` being the coarser rectangle the window and (fused) the coarser decoder's features need.
+    features: a rectangle of this decoder's own output features that must come out exact as well (the ones a finer
+    decoder adds, plan_update)."""
     r = geo.radii_of(scale)
     need_F = _clip(_expand(rect, r.clf), H, W)                   # decoder features the classifier reads
+    if features is not None:
+        need_F = _union(need_F, features)
     coarse = (need_F[0] // 2, need_F[1] // 2, -(-need_F[2] // 2), -(-need_F[3] // 2))   # Upsampler x2
     window = _clip(_expand(coarse, r.tail + r.body + r.head), Hc, Wc)
     fused = geo.fuses(scale)
@@ -361,3 +365,140 @@ def plan_encoder_bands(config, scale, H, rows):
     Ho = H // 2
     return [EncoderBand(scale, (r0, min(r0 + rows, Ho)), encoder_window(geo, scale, r0, min(r0 + rows, Ho), H))
             for r0 in range(0, Ho, rows)]
+
+
+def encoder_rect(geo, scale, rect, H, W):
+    """encoder_window on both axes: the rectangle of the H x W input of scale `scale`'s encoder that its output
+    rectangle `rect` (y0, x0, y1, x1) depends on, clipped to the plane and started on an even row and column."""
+    a0, a1 = encoder_window(geo, scale, rect[0], rect[2], H)
+    b0, b1 = encoder_window(geo, scale, rect[1], rect[3], W)
+    return (a0, b0, a1, b1)
+
+
+def _encoder_reach(geo, scale, r, Ho, Wo):
+    """The outputs of scale `scale`'s encoder (an Ho x Wo plane) that the input rectangle r can change: output pixel p
+    reads the inputs [2 (p - m) - k, 2 (p + m) + k] (m: body and to_q radius, k: down conv and head radii), on both
+    axes.  The inverse of encoder_rect."""
+    g = geo.radii[scale]
+    m, k = g['body'] + g['to_q'], g['down'] + g['head']
+
+    def axis(e0, e1, n):
+        return max(-((k - e0) // 2) - m, 0), min((e1 - 1 + k) // 2 + m + 1, n)
+    (y0, y1), (x0, x1) = axis(r[0], r[2], Ho), axis(r[1], r[3], Wo)
+    return (y0, x0, y1, x1)
+
+
+class UpdateScale(ScalePlan):
+    """One scale of an update plan (plan_update), in that scale's coordinates.  rect / tiles: the tile-aligned
+    rectangle R_s re-encoded and its tiles; window / out / fused: as in ScalePlan, the decoder window that codes rect
+    (None at the uniform-prior scale); need: what the walk reads of this scale's encoder outputs (its symbols, values
+    and F), at scale 0 the pixel window P_0; enc: the window of this scale's plane its encoder reads (None at the
+    uniform-prior scale)."""
+    __slots__ = ('need', 'enc')
+
+    def __repr__(self):
+        return 'UpdateScale(scale=%d, rect=%s, tiles=%d, window=%s, need=%s, enc=%s)' % (
+            self.scale, self.rect, len(self.tiles), self.window, self.need, self.enc)
+
+
+class UpdatePlan(object):
+    """plan_update's result: scales coarse -> fine, the edit in padded image coordinates, the pixel window P_0 and the
+    totals: streams re-encoded, streams in the container and the pixels of P_0."""
+
+    def __init__(self, scales, edit, tile, total_streams):
+        self.scales, self.edit, self.tile, self.total_streams = scales, edit, tile, total_streams
+
+    @property
+    def window(self):
+        return self.scales[-1].need
+
+    @property
+    def streams(self):
+        return sum(s.streams for s in self.scales)
+
+    @property
+    def window_pixels(self):
+        return _area(self.window)
+
+    def __repr__(self):
+        return 'UpdatePlan(edit=%s, window=%s, streams=%d of %d)' % (self.edit, self.window, self.streams,
+                                                                    self.total_streams)
+
+
+def plan_update(shapes, pad_tuple, tile, config, rect):
+    """Update of the region rect = (y, x, h, w) (unpadded image coordinates) of a tiled L3C container (DESIGN §4.12).
+    shapes, pad_tuple, tile: as in plan_region; config: a MultiscaleNetwork (its DecoderGeometry and EncoderGeometry
+    are read from it).  -> UpdatePlan.
+    Forward pass, fine to coarse: the edited pixels E_0 change the scale-(s+1) symbols and F where the encoder of scale
+    s reads E_s (_encoder_reach), and the scale-s CDFs where the decoder of scale s reads changed symbols of scale s+1
+    (head, body and tail radii, x2, the classifier's radius) or, with dec.skip, adds changed coarser decoder features;
+    R_s is the tile-aligned bounding rectangle of both (of the symbols alone at the uniform-prior scale).
+    Backward pass: fine to coarse the decoder windows that code every R_s (_window; with dec.skip they also give the
+    features the finer decoder adds), then coarse to fine the encoder windows that produce every symbol a window or R_s
+    reads (encoder_rect), down to the pixel window P_0.
+    ValueError for an untiled container, the RGB baselines, a container of the wrong scale count, and an empty
+    region or one outside the image."""
+    if tile is None:
+        raise ValueError('region update needs a tiled container (written with Bitcoding(..., tile=(th, tw))): '
+                         'the streams of the reference layout are serial')
+    geo = geometry_of(config)
+    egeo = config if isinstance(config, EncoderGeometry) else EncoderGeometry(config)
+    if geo.rgb:
+        raise ValueError('region update is not supported by the RGB baselines: their bicubic encoder has no planned '
+                         'windows')
+    tile = (int(tile[0]), int(tile[1]))
+    n = len(shapes)
+    S = geo.num_scales
+    if n != S + 1:
+        raise ValueError('container has %d scales, model expects %d' % (n, S + 1))
+    if len(rect) != 4:
+        raise ValueError('region must be (y, x, h, w), got %r' % (rect,))
+    y, x, h, w = (int(v) for v in rect)
+    left, right, top, bottom = (int(v) for v in pad_tuple)
+    _, Hf, Wf = shapes[-1]
+    Hu, Wu = Hf - top - bottom, Wf - left - right
+    if h < 1 or w < 1:
+        raise ValueError('empty region %r' % (tuple(rect),))
+    if y < 0 or x < 0 or y + h > Hu or x + w > Wu:
+        raise ValueError('region %r lies outside the %dx%d image' % (tuple(rect), Hu, Wu))
+    dims = [shapes[n - 1 - s][1:] for s in range(n)]                     # (H, W) by scale, fine -> coarse
+    # forward pass: changed symbols E_s, fine -> coarse
+    E = [(y + top, x + left, y + top + h, x + left + w)]
+    for s in range(S):
+        E.append(_encoder_reach(egeo, s, E[s], *dims[s + 1]))
+    # changed decoder features G_s (scale-s grid) and CDFs, coarse -> fine
+    R, G = [None] * n, [None] * n
+    R[S] = _align(E[S], dims[S][0], dims[S][1], tile)
+    for s in range(S - 1, -1, -1):
+        r = geo.radii_of(s)
+        Hc, Wc = dims[s + 1]
+        q = _clip(_expand(E[s + 1], r.head + r.body + r.tail), Hc, Wc)
+        if geo.fuses(s):
+            q = _union(q, _clip(_expand(G[s + 1], r.body + r.tail), Hc, Wc))
+        G[s] = (2 * q[0], 2 * q[1], 2 * q[2], 2 * q[3])                 # Upsampler x2
+        cdf = _clip(_expand(G[s], r.clf), *dims[s])
+        R[s] = _align(_union(E[s], cdf), dims[s][0], dims[s][1], tile)
+    # decoder windows, fine -> coarse: R_s and, with dec.skip, the features the finer decoder adds
+    win, out, fused, need = [None] * n, [None] * n, [False] * n, [None] * n
+    want = None
+    for s in range(S):
+        win[s], out[s], fused[s], want = _window(geo, s, R[s], dims[s][0], dims[s][1], *dims[s + 1], features=want)
+        if not fused[s]:
+            want = None
+    # encoder windows, coarse -> fine: scale s's encoder produces what scale s + 1 needs
+    enc = [None] * n
+    need[S] = _union(R[S], win[S - 1])
+    for s in range(S - 1, -1, -1):
+        enc[s] = encoder_rect(egeo, s, need[s + 1], *dims[s])
+        need[s] = _union(enc[s], R[s] if s == 0 else _union(R[s], win[s - 1]))
+    scales = []
+    for s in range(S, -1, -1):
+        H, W = dims[s]
+        th, tw = tile
+        ntx = -(-W // tw)
+        rr = R[s]
+        tiles = [ty * ntx + tx for ty in range(rr[0] // th, -(-rr[2] // th)) for tx in range(rr[1] // tw, -(-rr[3] // tw))]
+        scales.append(UpdateScale(idx=n - 1 - s, scale=s, C=shapes[n - 1 - s][0], H=H, W=W, rect=rr, tiles=tiles,
+                                  window=win[s], out=out[s], fused=fused[s], need=need[s], enc=enc[s]))
+    total = sum(C * len(tile_grid(H, W, tile)) for (C, H, W) in shapes)
+    return UpdatePlan(scales, E[0], tile, total)
