@@ -1,14 +1,20 @@
 // bicubic.cu -- Pillow-compatible bicubic x0.5 down-sampling of uint8 planes (RGB baselines only).
 //
 // The reference's "encoder" for cr_rgb_shared.cf / cr_rgb.cf is PIL.Image.resize(.., BICUBIC) on the
-// CPU (/root/reference/src/dataloaders/images_loader.py:277-293, called from modules/net.py:75).
+// CPU (the reference's src/dataloaders/images_loader.py:277-293, called from modules/net.py:75).
 // Pillow is a third-party, un-pinned dependency of the reference; this file restates the published
 // algorithm of Pillow's two-pass resampler (src/libImaging/Resample.c: precompute_coeffs,
-// normalize_coeffs_8bpc, ImagingResampleHorizontal_8bpc / Vertical_8bpc): separable, horizontal pass
-// first with an 8-bit intermediate, Keys cubic a=-0.5, support scaled by the down-scale factor,
-// coefficients normalised then rounded to 22-bit fixed point, accumulation started at 2^21,
-// arithmetic shift and clamp to [0,255].  Validated bit-for-bit against the installed Pillow by
-// tests/test_bicubic.py (CPU restatement) and on the GPU against that restatement.
+// normalize_coeffs_8bpc, ImagingResampleHorizontal_8bpc / Vertical_8bpc): separable, Keys cubic a=-0.5,
+// support scaled by the down-scale factor, coefficients normalised then rounded to 22-bit fixed point,
+// accumulation started at 2^21, arithmetic shift and clamp to [0,255], an 8-bit intermediate between the
+// passes.  The horizontal pass runs first, except on images more than 100 times taller than wide
+// (H > 100 * W), which Pillow 12 resizes vertically first.
+//
+// tests/test_bicubic_host.py pins an int64 restatement of that algorithm bit for bit to the installed
+// Pillow (every H, W in 2..40, tall, flat and multi-megapixel shapes, content that drives both passes past
+// both clamps) and shows that plausible mis-restatements differ from Pillow.  tests/test_gpu_bicubic.py
+// checks this kernel bit for bit against both: the sweep, block edges of the x grid, batches, the grid
+// limits below, large images, side streams, and every call the codec makes on every RGB-baseline path.
 #include <math.h>
 
 #include <vector>
@@ -114,16 +120,25 @@ extern "C" int l3c_bicubic_half_u8(const uint8_t *in_dev, int N, int H, int W, u
     L3C_CUDA(cudaMallocAsync(&d_kh, kh.size() * 4, st));
     L3C_CUDA(cudaMallocAsync(&d_bv, bv.size() * 4, st));
     L3C_CUDA(cudaMallocAsync(&d_kv, kv.size() * 4, st));
-    L3C_CUDA(cudaMallocAsync(&tmp, (size_t)planes * H * Wo, st));
+    // Pillow 12's pass order: vertical first only for images more than 100x taller than wide
+    const bool v_first = (long long)H > 100LL * W;
+    L3C_CUDA(cudaMallocAsync(&tmp, (size_t)planes * (v_first ? (size_t)Ho * W : (size_t)H * Wo), st));
     L3C_CUDA(cudaMemcpyAsync(d_bh, bh.data(), bh.size() * 4, cudaMemcpyHostToDevice, st));
     L3C_CUDA(cudaMemcpyAsync(d_kh, kh.data(), kh.size() * 4, cudaMemcpyHostToDevice, st));
     L3C_CUDA(cudaMemcpyAsync(d_bv, bv.data(), bv.size() * 4, cudaMemcpyHostToDevice, st));
     L3C_CUDA(cudaMemcpyAsync(d_kv, kv.data(), kv.size() * 4, cudaMemcpyHostToDevice, st));
     // the pageable host vectors above are consumed synchronously by cudaMemcpyAsync (staged copy)
-    resample_h_kernel<<<dim3(ceil_div(Wo, 128), H, planes), 128, 0, st>>>(in_dev, H, W, Wo, d_bh, d_kh, ksh, tmp);
-    L3C_LAUNCH_CHECK("resample_h_kernel");
-    resample_v_kernel<<<dim3(ceil_div(Wo, 128), Ho, planes), 128, 0, st>>>(tmp, H, Ho, Wo, d_bv, d_kv, ksv, out_dev);
-    L3C_LAUNCH_CHECK("resample_v_kernel");
+    if (v_first) {
+        resample_v_kernel<<<dim3(ceil_div(W, 128), Ho, planes), 128, 0, st>>>(in_dev, H, Ho, W, d_bv, d_kv, ksv, tmp);
+        L3C_LAUNCH_CHECK("resample_v_kernel");
+        resample_h_kernel<<<dim3(ceil_div(Wo, 128), Ho, planes), 128, 0, st>>>(tmp, Ho, W, Wo, d_bh, d_kh, ksh, out_dev);
+        L3C_LAUNCH_CHECK("resample_h_kernel");
+    } else {
+        resample_h_kernel<<<dim3(ceil_div(Wo, 128), H, planes), 128, 0, st>>>(in_dev, H, W, Wo, d_bh, d_kh, ksh, tmp);
+        L3C_LAUNCH_CHECK("resample_h_kernel");
+        resample_v_kernel<<<dim3(ceil_div(Wo, 128), Ho, planes), 128, 0, st>>>(tmp, H, Ho, Wo, d_bv, d_kv, ksv, out_dev);
+        L3C_LAUNCH_CHECK("resample_v_kernel");
+    }
     L3C_CUDA(cudaFreeAsync(d_bh, st));
     L3C_CUDA(cudaFreeAsync(d_kh, st));
     L3C_CUDA(cudaFreeAsync(d_bv, st));
