@@ -287,28 +287,23 @@ int l3c_lin_dmll_intervals(const void *x_h, const void *w_h, const float *bias, 
                            const float *targets_dev, int N, int HW, int Cin, int C, int K, int L, int rgb,
                            uint32_t *intervals_dev, void *stream);
 
-/* The intervals of one band of a banded encode (DESIGN §4.10): the symbols of rows [y0, y0 + h) of the whole
- * symbol plane sym_dev uint8 [N][C][Hs][W], their intervals written in the tile order (th x tw) of an h x W plane to
- * band stream planes intervals_dev uint32 [N][C][h * W].
- * l3c_lin_dmll_intervals_band (f16): as l3c_lin_dmll_intervals on rows [oy, oy + h) of x_h, the FP16 concat buffer
- *   [N][Hl][W][Cin] of a full-width decoder window.
- * l3c_dmll_intervals_band (any mode): as l3c_dmll_intervals on the h x W rectangle at (oy, ox) of the parameters
- *   l_dev f32 NHWC [N][Hl][Wl][Kp].
- * Both are bit-identical to the whole-plane kernel followed by l3c_reorder_tiles, restricted to the band. */
+/* The intervals of one band of a banded encode in f16 (DESIGN §4.10): as l3c_lin_dmll_intervals on rows [oy, oy + h)
+ * of x_h, the FP16 concat buffer [N][Hl][W][Cin] of a full-width decoder window, coding the symbols of rows
+ * [y0, y0 + h) of the whole symbol plane sym_dev uint8 [N][C][Hs][W]; their intervals written in the tile order
+ * (th x tw) of an h x W plane to band stream planes intervals_dev uint32 [N][C][h * W].  Bit-identical to the
+ * whole-plane kernel followed by l3c_reorder_tiles, restricted to the band. */
 int l3c_lin_dmll_intervals_band(const void *x_h, int Hl, int oy, const void *w_h, const float *bias,
                                 const uint8_t *sym_dev, int Hs, int y0, int h, int W, const float *targets_dev, int N,
                                 int Cin, int C, int K, int L, int rgb, int th, int tw, uint32_t *intervals_dev,
                                 void *stream);
-int l3c_dmll_intervals_band(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev, int Hs,
-                            int y0, int h, int W, const float *targets_dev, int N, int C, int K, int L, int rgb,
-                            int th, int tw, uint32_t *intervals_dev, void *stream);
 
-/* The intervals of one tile-aligned rectangle of a region update (DESIGN §4.12): as l3c_dmll_intervals_band for the
- * h x w rectangle at (y0, x0) of the symbol window sym_dev uint8 [N][C][Hs][Ws], which sits at (sy, sx) of the
- * container's Hf x Wf plane, with the parameters at (oy, ox) of l_dev f32 NHWC [N][Hl][Wl][Kp]; intervals in the tile
- * order (th x tw) of an h x w plane to intervals_dev uint32 [N][C][h * w].  In the Hf x Wf plane the rectangle starts
- * on a tile boundary and ends on one or at the plane's edge (else an error), so its tile order is that of the plane's
- * own tiles.  A band is the rectangle x0 = 0, w = Ws of a whole plane (sy = sx = 0, Hf x Wf = Hs x Ws). */
+/* The intervals of one tile-aligned rectangle of a banded encode (a band: x0 = 0, w = Ws of a whole plane) or of a
+ * region update (DESIGN §4.10, §4.12): as l3c_dmll_intervals for the h x w rectangle at (y0, x0) of the symbol window
+ * sym_dev uint8 [N][C][Hs][Ws], which sits at (sy, sx) of the container's Hf x Wf plane, with the parameters at
+ * (oy, ox) of l_dev f32 NHWC [N][Hl][Wl][Kp]; intervals in the tile order (th x tw) of an h x w plane to
+ * intervals_dev uint32 [N][C][h * w].  In the Hf x Wf plane the rectangle starts on a tile boundary and ends on one
+ * or at the plane's edge (else an error), so its tile order is that of the plane's own tiles.  Bit-identical to the
+ * whole-plane kernel followed by l3c_reorder_tiles, restricted to the rectangle. */
 int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev, int Hs, int Ws,
                             int y0, int x0, int h, int w, int sy, int sx, int Hf, int Wf, const float *targets_dev,
                             int N, int C, int K, int L, int rgb, int th, int tw, uint32_t *intervals_dev,

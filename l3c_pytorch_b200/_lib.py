@@ -74,8 +74,6 @@ _SIGNATURES = {
     'l3c_lin_dmll_intervals': (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p, c_void_p]),
     'l3c_lin_dmll_intervals_band': (c_int, [c_void_p, c_int, c_int] + [c_void_p] * 3 + [c_int] * 4 + [c_void_p] +
                                     [c_int] * 8 + [c_void_p, c_void_p]),
-    'l3c_dmll_intervals_band': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 7 +
-                                [c_void_p, c_void_p]),
     'l3c_dmll_intervals_rect': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 10 + [c_void_p] + [c_int] * 7 +
                                 [c_void_p, c_void_p]),
     'l3c_rgb_prep': (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),

@@ -18,7 +18,10 @@ stream's intervals (encode) or symbols and CDF rows (decode) sit in the `[N][C][
 only the step between those stream planes and the raster planes of the networks differs (a view, l3c_reorder_tiles
 or l3c_ragged_pack).  Every decode -- full (`decode_device`) or of regions of tiled containers (`decode_region_pass`,
 DESIGN §4.8) -- is one coarse-to-fine walk, `BatchCodec._decode_scales`, told its geometry by the caller; a large
-scale of a tiled pass is decoded in bands of tile rows (DESIGN §4.10).
+scale of a tiled pass is decoded in bands of tile rows (DESIGN §4.10).  The encodes on windows -- a large tiled batch in
+bands (DESIGN §4.10) and a region update (DESIGN §4.12) -- share two walks told their rectangles by the caller:
+`BatchCodec._encode_windows`, the encoders fine to coarse, and `BatchCodec._code_rects`, the intervals of tile-aligned
+rectangles coarse to fine, whose streams `region.rect_streams` finds and `_enc_descs` gives slots and descriptors.
 """
 import functools
 import os
@@ -70,6 +73,54 @@ def _under_injection_tool():
 def _slot_cap(n_sym):
     """worst case: every symbol has probability 2^-16 -> 17 bits, plus termination."""
     return ((n_sym * 17 + 7) // 8 + 64 + 3) & ~3
+
+
+def _enc_descs(ptrs, n_sym, dev):
+    """Range-coder descriptors of the streams whose intervals start at the device addresses ptrs and hold n_sym symbols
+    (int64 arrays of one shape), each given a slot of _slot_cap(n_sym) bytes in one new slot buffer.
+    -> (caps, slots, desc): caps of ptrs' shape, desc flat in the arrays' order."""
+    caps = _slot_cap(n_sym)
+    slot_off = np.concatenate([[0], np.cumsum(caps)])
+    slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
+    desc = np.zeros(caps.size, dtype=_lib.ENC_STREAM_DTYPE)
+    desc['intervals'] = ptrs.reshape(-1)
+    desc['n_sym'] = n_sym.reshape(-1)
+    desc['out_cap'] = caps.reshape(-1)
+    desc['out'] = slots.data_ptr() + slot_off[:-1]
+    return caps, slots, desc
+
+
+def _check_lens(lens, caps):
+    if (lens > caps).any():
+        raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
+
+
+def _crop(src, at, r, nhwc):
+    """Rectangle r (y0, x0, y1, x1) of every image of the plane src whose element (0, 0) sits at `at`, as a new tensor
+    (l3c_crop_rect).  nhwc: src is NHWC [N, H, W, C]; otherwise planes [N, P, H, W]."""
+    org = np.tile(np.array([r[0] - at[0], r[1] - at[1]], np.int32), (src.shape[0], 1))
+    return E.crop_rect(src, E._to_device_async(org, src.device), r[2] - r[0], r[3] - r[1], nhwc=nhwc)
+
+
+def _put(dst, D, K, src, at, nhwc):
+    """Rectangle K (y0, x0, y1, x1) of the plane src, whose element (0, 0) sits at `at`, to its place in the destination
+    plane of rectangle D: dst, allocated at the first piece written into it (dst None).  A first piece that is all of D
+    becomes the destination itself, without a copy.  nhwc as in _crop.  -> the destination."""
+    y, x = (1, 2) if nhwc else (2, 3)
+    h, w = D[2] - D[0], D[3] - D[1]
+    if dst is None:
+        if tuple(K) == tuple(D) and tuple(at) == tuple(D[:2]) and (src.shape[y], src.shape[x]) == (h, w):
+            return src.contiguous()
+        shape = list(src.shape)
+        shape[y], shape[x] = h, w
+        dst = torch.empty(shape, dtype=src.dtype, device=src.device)
+
+    def part(t, o):
+        idx = [slice(None)] * t.dim()
+        idx[y], idx[x] = slice(K[0] - o[0], K[2] - o[0]), slice(K[1] - o[1], K[3] - o[1])
+        return t[tuple(idx)]
+    part(dst, D).copy_(part(src, at))
+    return dst
 
 
 # BatchCodec.decode_regions: False runs every group of equal RegionPlan.shape_key on its own, also where one ragged pass
@@ -154,23 +205,6 @@ def stream_layout(shapes_of, tile=None, pad_tiles=False):
         elem.append((img * C + np.arange(C)[None, :, None]) * plane[k] + off)
         n_sym.append(np.broadcast_to(cnt, shape))
     return tuple(np.concatenate([x.reshape(N, -1) for x in xs], 1) for xs in (si, elem, n_sym)) + (plane,)
-
-
-def band_streams(layout, idx, C, band):
-    """The streams of one band (region.plan_bands) of scale idx of an equal-size tiled pass laid out by stream_layout:
-    -> ((e0, e1), (cols, si, elem, n_sym, plane)).  Its symbols are the elements [e0, e1) of every channel plane of the
-    scale; cols are the band's columns of the pass's [N][streams] arrays, and the rest is a stream_layout of one scale
-    that places them in band planes [N][C][e1 - e0]."""
-    si, elem, n_sym, plane = layout
-    lo, hi = np.searchsorted(si[0], [idx, idx + 1])
-    T = (hi - lo) // C
-    t0, t1 = band.tiles[0], band.tiles[-1] + 1
-    cols = lo + (np.arange(C)[:, None] * T + np.arange(t0, t1)[None, :]).reshape(-1)
-    e0, e1 = band.rect[0] * band.W, band.rect[2] * band.W
-    el = elem[:, cols]
-    nc = el // plane[idx]                                                    # n * C + c of every stream
-    local = nc * (e1 - e0) + (el - nc * plane[idx]) - e0
-    return (int(e0), int(e1)), (cols, np.zeros_like(local), local, n_sym[:, cols], np.array([e1 - e0], np.int64))
 
 
 class ContainerLayout(object):
@@ -293,8 +327,7 @@ class EncodeJob:
         N, per_img = self.caps.shape
         self.coded.synchronize()                                                   # sync #1 (tiny)
         lens = self.lens_host.numpy().astype(np.int64).reshape(N, per_img)
-        if (lens > self.caps).any():
-            raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
+        _check_lens(lens, self.caps)
         with torch.cuda.stream(self.stream):
             # ---- container layout + gather + single D2H
             sizes, pieces_all, dst = [], [], np.zeros((N, per_img), np.int64)
@@ -486,15 +519,8 @@ class BatchCodec(object):
 
         # ---- one range-coder launch for all streams, each with its own slot
         si, elem, n_sym, _ = stream_layout([[s[1:] for s in sh] for sh in shapes_of], tile)
-        caps = _slot_cap(n_sym)
-        slot_off = np.concatenate([[0], np.cumsum(caps)])
-        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
-        desc = np.zeros(caps.size, dtype=_lib.ENC_STREAM_DTYPE)
         bases = np.array([iv.data_ptr() for iv in ivs], np.int64)
-        desc['intervals'] = (bases[si] + elem * 4).reshape(-1)
-        desc['n_sym'] = n_sym.reshape(-1)
-        desc['out_cap'] = caps.reshape(-1)
-        desc['out'] = slots.data_ptr() + slot_off[:-1]
+        caps, slots, desc = _enc_descs(bases[si] + elem * 4, n_sym, dev)
         desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
         return EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, (imgs_u8, ivs, slots))
 
@@ -508,139 +534,135 @@ class BatchCodec(object):
 
     def _encode_banded(self, imgs, pads, tile, recursive):
         """encode_begin of a large tiled batch in bands (DESIGN §4.10), same containers as the whole-image encode.
-        Encoder phase, fine to coarse: every scale's encoder runs band by band on its window of the whole input
-        (region.plan_encoder_bands) and writes its rows of the whole symbol planes, bottleneck values and F.  Coding
-        phase, coarse to fine: per band of tile rows (region.plan_bands, the banded decode's bands) the decoder network
-        runs on its window (_band_window), the band's intervals go straight to band stream planes and one range-coder
-        launch codes the band's streams.  All launches share one slot buffer and one descriptor array, in launch
-        order; the lengths are put back in container order for EncodeJob."""
-        from .region import EncoderGeometry, plan_bands, plan_encoder_bands
+        Encoder phase (_encode_windows): every scale's encoder runs band by band on its window of the whole input
+        (region.plan_encoder_bands), each band writing its rows of the whole planes.  Coding phase (_code_rects): the
+        uniform-prior scale whole, then the bands of tile rows of the banded decode (region.plan_bands); the intervals
+        of every piece go to one scratch buffer and one range-coder launch codes the piece's streams.  All launches
+        share one slot buffer and one descriptor array, in launch order; the lengths are put back in container order
+        for EncodeJob."""
+        from .region import EncoderGeometry, ScalePlan, plan_bands, plan_encoder_bands, rect_streams
         dev, net = imgs.device, self.net
-        N = imgs.shape[0]
-        K = net.config_ms.prob.K
+        N, _, Hb, Wb = imgs.shape
         budget = TILED_ENCODE_BAND_PIXELS
-        # ---- encoder phase: S[s] the symbol planes [N][C][H][W], bn[s] their values NHWC (s >= 1)
-        S, bn = [imgs], [None]
         if net._rgb:
+            enc = [((0, 0), imgs, None)]
             for s in list(range(net.scales)) + [-1] * recursive:        # the bicubic x0.5 runs whole
-                eo = net.nets[s].enc(S[-1])
-                S.append(eo.S)
-                bn.append(eo.bn_q)
+                eo = net.nets[s].enc(enc[-1][1])
+                enc.append(((0, 0), eo.S, eo.bn_q))
         else:
-            geo = EncoderGeometry(net)
-            x = imgs                            # scale-s input: the image, then the operand heads[s] reads of F_s
+            geo, walk = EncoderGeometry(net), []
             for s in range(net.scales):
-                H, W = (x.shape[2], x.shape[3]) if s == 0 else (x.shape[1], x.shape[2])
-                C = net.config_ms.q.C
-                Sn = torch.empty(N, C, H // 2, W // 2, dtype=torch.uint8, device=dev)
-                bq = torch.empty(N, H // 2, W // 2, 8, dtype=torch.float32, device=dev)
-                Fn = None
-                for band in plan_encoder_bands(geo, s, H, max(1, budget // (2 * N * W))):
-                    (a, b), (r0, r1), o = band.window, band.rows, band.out
-                    org = E._to_device_async(np.tile(np.array([a, 0], np.int32), (N, 1)), dev)
-                    if s == 0:
-                        inp = net._rgb_head_input(E.crop_rect(x, org, b - a, W, nhwc=False))
-                        h = inp if isinstance(inp, E.Act) else net.heads[0](inp)
-                    else:
-                        h = net.heads[s](self._operand_act(E.crop_rect(x, org, b - a, W, nhwc=True)))
-                    eo = net.nets[s].enc(h)
-                    Sn[:, :, r0:r1].copy_(eo.S[:, :, o:o + r1 - r0])
-                    bq[:, r0:r1].copy_(eo.bn_q[:, o:o + r1 - r0])
-                    if s + 1 < net.scales:                  # F_{s+1} feeds heads[s + 1]: keep what that conv reads
-                        op = eo.F.r if E.tensor_core_mode() else eo.F.f
-                        if Fn is None:
-                            Fn = torch.empty(N, H // 2, W // 2, op.shape[-1], dtype=op.dtype, device=dev)
-                        Fn[:, r0:r1].copy_(op[:, o:o + r1 - r0])
-                    del eo, h
-                S.append(Sn)
-                bn.append(bq)
-                x = Fn
-            del x
+                H, W = Hb >> s, Wb >> s
+                bands = plan_encoder_bands(geo, s, H, max(1, budget // (2 * N * W)))
+                walk.append(((0, 0, H // 2, W // 2),
+                             [((b.window[0], 0, b.window[1], W), (b.rows[0], 0, b.rows[1], W // 2)) for b in bands]))
+            enc = self._encode_windows(imgs, (0, 0), walk)
 
-        # ---- coding phase: the streams, the bands of every scale, the descriptors in launch order
+        # ---- coding phase: the pieces of every scale, their streams and the descriptors in launch order
         scales = list(self.iter_scale_dmll(recursive))
-        shapes = [(scale, S[scale].shape[1], S[scale].shape[2], S[scale].shape[3]) for (scale, _, _) in scales]
-        shapes_of = [list(shapes) for _ in range(N)]
+        shapes = [(scale,) + tuple(enc[scale][1].shape[1:]) for (scale, _, _) in scales]
         layout = stream_layout([[sh[1:] for sh in shapes]] * N, tile)
-        si, elem, n_sym, _ = layout
-        per_img = si.shape[1]
-        caps = _slot_cap(n_sym)
-        slot_off = np.concatenate([[0], np.cumsum(caps)])
-        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
-        geo_d = self._geometry()
-        plans = []                                     # per scale: None (uniform) or [(band, (e0, e1), band layout)]
-        scratch_n = 0
-        for idx, (scale, C, H, W) in enumerate(shapes):
-            if scales[idx][2]:
-                plans.append(None)
-                continue
-            bands = plan_bands([sh[1:] for sh in shapes], tile, geo_d, idx, max(1, budget // (N * tile[0] * W)))
-            plans.append([(band,) + band_streams(layout, idx, C, band) for band in bands])
-            scratch_n = max([scratch_n] + [N * C * (e1 - e0) for (_, (e0, e1), _) in plans[-1]])
-        # the band intervals of every launch go to one scratch buffer: a band's range coder reads it before the next
-        # band's interval kernel writes it (one stream)
-        scratch = torch.empty(max(scratch_n, 1), dtype=torch.int32, device=dev)
-        u_idx = [i for i, p in enumerate(plans) if p is None][0]
-        scale_u, dm_u, _ = scales[u_idx]
-        iv_u = E.reorder_tiles(E.lut_intervals(S[scale_u], self._uniform(dm_u.L, dev)[0]), shapes[u_idx][2],
-                               shapes[u_idx][3], tile, True)
-        desc = np.zeros(caps.size, dtype=_lib.ENC_STREAM_DTYPE).reshape(N, per_img)
-        desc['n_sym'] = n_sym
-        desc['out_cap'] = caps
-        desc['out'] = slots.data_ptr() + slot_off[:-1].reshape(N, per_img)
-        img = np.arange(N)[:, None] * per_img
-        groups = []                                    # launch order: [container indices] per launch
-        for idx, p in enumerate(plans):
-            if p is None:
-                cols = np.flatnonzero(si[0] == idx)
-                desc['intervals'][:, cols] = iv_u.data_ptr() + elem[:, cols] * 4
-                groups.append((img + cols[None, :]).reshape(-1))
-                continue
-            for (_, _, (cols, _, local, _, _)) in p:
-                desc['intervals'][:, cols] = scratch.data_ptr() + local * 4
-                groups.append((img + cols[None, :]).reshape(-1))
+        rects = []
+        for idx, ((scale, C, H, W), (_, _, uniform)) in enumerate(zip(shapes, scales)):
+            if uniform:
+                whole = ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=(0, 0, H, W),
+                                  tiles=list(range(len(tile_grid(H, W, tile)))), window=None, out=None, fused=False)
+                rects.append((None, [(whole, None)]))
+            else:
+                bands = plan_bands([sh[1:] for sh in shapes], tile, self._geometry(), idx,
+                                   max(1, budget // (N * tile[0] * W)))
+                rects.append(((0, 0, H, W), [(b, b.rect) for b in bands]))
+        streams = [rect_streams(layout, idx, sp) for idx, (_, pieces) in enumerate(rects) for sp, _ in pieces]
+        # the intervals of every piece go to one scratch buffer: a piece's range coder reads it before the next piece's
+        # interval kernel writes it (one stream)
+        scratch = torch.empty(max(int(n.sum()) for _, n, _ in streams), dtype=torch.int32, device=dev)
+        ptrs = np.zeros_like(layout[2])
+        for cols, _, elem in streams:
+            ptrs[:, cols] = scratch.data_ptr() + elem * 4
+        caps, slots, desc = _enc_descs(ptrs, layout[2], dev)
+        groups = [(np.arange(N)[:, None] * caps.shape[1] + cols[None, :]).reshape(-1) for cols, _, _ in streams]
         order = np.concatenate(groups)
-        desc = desc.reshape(-1)
         desc_l = E._desc_to_device(desc[order], dev)
         desc_c = E._desc_to_device(desc, dev)
         lens_l = torch.empty(order.size, dtype=torch.int32, device=dev)
-        starts = np.concatenate([[0], np.cumsum([g.size for g in groups])])
-
-        g = 0
-        bn8, F = None, None
-        dims = [sh[2:] for sh in shapes]
-        whole_F = [None]
-        for idx, ((scale, dmll, uniform), p) in enumerate(zip(scales, plans)):
-            C = shapes[idx][1]
-            if uniform:
-                E.ac_encode_slice(desc_l, lens_l, starts[g], starts[g + 1] - starts[g])
-                g += 1
-            else:
-                fuse = (E.f16_mode() and net.prob_clfs[min(scale, net.scales - 1)].atrous.lin.in_channels % 64 == 0
-                        and C == (3 if dmll.rgb_scale else 5))
-                tg = dmll.targets(dev)
-                F_in = F
-                for (band, (e0, e1), _) in p:
-                    ivb = scratch[:N * C * (e1 - e0)]
-                    y0, h = band.rect[0], band.rect[2] - band.rect[0]
-                    if fuse:
-                        _, F, _ = self._band_window(idx, scale, bn8, F_in, band, dims, whole_F,
-                                                    fused=(S[scale], dmll, (band.out[0], y0, h, tile, ivb)))
-                    else:
-                        l, F, _ = self._band_window(idx, scale, bn8, F_in, band, dims, whole_F)
-                        E.dmll_intervals_band(l, band.out[0], band.out[1], S[scale], y0, h, tg, C, K, dmll.L,
-                                              dmll.rgb_scale, tile, out=ivb)
-                        del l
-                    E.ac_encode_slice(desc_l, lens_l, starts[g], starts[g + 1] - starts[g])
-                    g += 1
-                del F_in
-            if idx + 1 < len(scales):
-                bn8 = bn[scale]                        # what the next finer decoder runs on
+        first = 0
+        for _, group in zip(self._code_rects(rects, enc, tile, scratch, fuse=True), groups):
+            E.ac_encode_slice(desc_l, lens_l, first, group.size)
+            first += group.size
         inv = np.empty_like(order)
         inv[order] = np.arange(order.size)
         lens_c = lens_l[E._to_device_async(inv, dev)]
-        return EncodeJob(self, shapes, shapes_of, pads, tile, None, caps, desc_c, lens_c,
-                         (imgs, S, scratch, slots, iv_u, desc_l, lens_l))
+        return EncodeJob(self, shapes, [list(shapes) for _ in range(N)], pads, tile, None, caps, desc_c, lens_c,
+                         (imgs, enc, scratch, slots, desc_l, lens_l))
+
+    def _encode_windows(self, img, at, walk):
+        """The encoder of every trained scale of an L3C network, fine to coarse, on windows of its input (the banded
+        encode and region updates, DESIGN §4.10 and §4.12).  img: the pixels uint8 [N][3][h][w], whose element (0, 0)
+        sits at `at` of the image plane.  walk: per trained scale s, (D, [(A, K)]): the rectangle D (y0, x0, y1, x1) of
+        the scale-(s+1) planes produced and the pieces written into it (_put), each the input rectangle A of scale s
+        (even origin) the head and encoder run on and the rectangle K of their output that goes to D.
+        -> [(origin, symbols [N][C][h][w], bottleneck values NHWC)] by scale: scale 0 the pixels (values None), every
+        other scale its D."""
+        net = self.net
+        out = [(at, img, None)]
+        x = img                               # scale-s input: the image, then the operand heads[s] reads of F_s
+        for s, (D, pieces) in enumerate(walk):
+            S = bq = F = None
+            for A, K in pieces:
+                inp = _crop(x, at, A, nhwc=s > 0)
+                if s == 0:
+                    inp = net._rgb_head_input(inp)
+                    hd = inp if isinstance(inp, E.Act) else net.heads[0](inp)
+                else:
+                    hd = net.heads[s](self._operand_act(inp))
+                eo = net.nets[s].enc(hd)
+                o = (A[0] // 2, A[1] // 2)
+                S = _put(S, D, K, eo.S, o, nhwc=False)
+                bq = _put(bq, D, K, eo.bn_q, o, nhwc=True)
+                if s + 1 < net.scales:                  # F_{s+1} feeds heads[s + 1]: keep what that conv reads
+                    F = _put(F, D, K, eo.F.r if E.tensor_core_mode() else eo.F.f, o, nhwc=True)
+                del eo, hd, inp
+            out.append((D[:2], S, bq))
+            x, at = F, D[:2]
+        return out
+
+    def _code_rects(self, rects, enc, tile, out=None, fuse=False):
+        """The coding phase of an encode on windows (the banded encode and region updates, DESIGN §4.10 and §4.12),
+        coarse to fine.  rects: per scale walked (iter_scale_dmll), (D, [(sp, K)]): the tile-aligned rectangles sp
+        (region.ScalePlan) coded and, where the next finer scale adds this scale's decoder features, the rectangle D
+        they are assembled in and the rectangle K of each piece's that goes there (_band_window).  enc: by scale, as
+        _encode_windows returns.  Per rectangle the decoder network runs on its window of the coarser scale and the
+        intervals of its symbols go, in its own tile order, to `out` (an int32 buffer every rectangle reuses; None: a
+        new tensor each).  fuse: in f16 a band's intervals come from the classifier's 1x1 conv fused with the interval
+        kernel, where that kernel is built (lin_dmll_intervals_band).
+        Yields (idx, sp, intervals int32 [N][C][h * w]) once a rectangle's intervals are queued."""
+        net, K = self.net, self.net.config_ms.prob.K
+        F = None                              # (origin, features) the next finer decoder adds
+        for idx, ((scale, dmll, uniform), (D, pieces)) in enumerate(
+                zip(self.iter_scale_dmll(len(rects) - 1 - net.scales), rects)):
+            o, S, _ = enc[scale]
+            dev, dst = S.device, None
+            for sp, Kr in pieces:
+                r, C = sp.rect, sp.C
+                h, w = r[2] - r[0], r[3] - r[1]
+                ivb = None if out is None else out[:S.shape[0] * C * h * w]
+                if uniform:
+                    sym = S if r == (0, 0, sp.H, sp.W) else _crop(S, o, r, nhwc=False)
+                    iv = E.reorder_tiles(E.lut_intervals(sym, self._uniform(dmll.L, dev)[0]), h, w, tile, True, out=ivb)
+                    yield idx, sp, iv
+                    continue
+                bn8, keep = (enc[scale + 1][0], enc[scale + 1][2]), (D, Kr, dst)
+                if fuse and E.f16_mode() and net.prob_clfs[min(scale, net.scales - 1)].atrous.lin.in_channels % 64 == 0 \
+                        and C == (3 if dmll.rgb_scale else 5):
+                    iv, dst = self._band_window(sp, bn8, F, keep, fused=(S, dmll, (sp.out[0], r[0], h, tile, ivb)))
+                else:
+                    l, dst = self._band_window(sp, bn8, F, keep)
+                    iv = E.dmll_intervals_rect(l, sp.out[0], sp.out[1], S, (r[0] - o[0], r[1] - o[1], h, w),
+                                               dmll.targets(dev), C, K, dmll.L, dmll.rgb_scale, tile, origin=o,
+                                               plane=(sp.H, sp.W), out=ivb)
+                    del l
+                yield idx, sp, iv
+            F = None if dst is None else (D[:2], dst)
 
     @staticmethod
     def _operand_act(op):
@@ -652,28 +674,23 @@ class BatchCodec(object):
             return E.Act(None, op)
         return E.Act(op, op)
 
-    def _band_window(self, idx, scale, bn8, F, band, dims, whole_F, fused=None):
-        """The decoder network of one band (region.plan_bands) of scale index idx, run on the band's window of the whole
-        coarser scale, for the banded decode and the banded encode: its symbol values bn8 and (dec.skip) the coarser
-        decoder's features F are cropped from the whole planes, and where the next finer scale adds this decoder's
-        features the band's rows of them go to the whole plane whole_F[0] (allocated at the first band).  dims: (H, W)
-        of every scale walked; fused: get_P_nhwc's.  -> (get_P_nhwc's first result, whole_F[0] or None, its size)."""
-        N, dev = bn8.shape[0], bn8.device
-        (wy0, _, wy1, _), Wc = band.window, bn8.shape[2]
-        org = E._to_device_async(np.tile(np.array([wy0, 0], np.int32), (N, 1)), dev)
-        win = E.crop_rect(bn8, org, wy1 - wy0, Wc, nhwc=True)
+    def _band_window(self, sp, bn8, F, keep, fused=None):
+        """The decoder network of one tile-aligned rectangle sp (region.ScalePlan: a band of region.plan_bands, an
+        update's R_s) run on its window sp.window of the coarser scale, for the banded decode and _code_rects.
+        bn8 = (origin, symbol values NHWC) and F = (origin, decoder features NHWC or their engine.Act) are planes of the
+        coarser scale whose element (0, 0) sits at origin; the window is cut out of both (of F where dec.skip adds them).
+        keep = (D, K, dst): where the next finer scale adds this decoder's features, their rectangle K goes to the
+        destination dst of rectangle D (_put).  fused: get_P_nhwc's.
+        -> (get_P_nhwc's first result, the destination, or None where the finer scale adds no features)."""
+        win = _crop(bn8[1], bn8[0], sp.window, nhwc=True)
         Fw = None
-        if self.net.fuses(scale):
-            Fw = E.crop_rect(F if torch.is_tensor(F) else F.f, org, wy1 - wy0, Wc, nhwc=True)
-        l, Fo = self.net.get_P_nhwc(scale, win, Fw, fused=fused)
-        if idx + 1 < len(dims) and scale >= 1 and self.net.fuses(scale - 1):
-            # the next scale adds these features: the band's rows of them go to one whole plane
-            (y0, _, y1, _), oy = band.rect, band.out[0]
-            if y0 == 0:
-                whole_F[0] = torch.empty(N, dims[idx][0], dims[idx][1], Fo.f.shape[-1], dtype=Fo.f.dtype, device=dev)
-            whole_F[0][:, y0:y1].copy_(Fo.f[:, oy:oy + y1 - y0])
-            return l, whole_F[0], (2 * (wy1 - wy0), 2 * Wc)
-        return l, None, (2 * (wy1 - wy0), 2 * Wc)
+        if self.net.fuses(sp.scale):
+            Fw = _crop(F[1] if torch.is_tensor(F[1]) else F[1].f, F[0], sp.window, nhwc=True)
+        l, Fo = self.net.get_P_nhwc(sp.scale, win, Fw, fused=fused)
+        if sp.scale < 1 or not self.net.fuses(sp.scale - 1):
+            return l, None
+        D, K, dst = keep
+        return l, _put(dst, D, K, Fo.f, (2 * sp.window[0], 2 * sp.window[1]), nhwc=True)
 
     def _scale_intervals(self, out, dev, recursive=0):
         """Coding intervals of every scale, coarse -> fine: [(shape (scale, C, H, W), int32 [N][C][H*W])]."""
@@ -832,23 +849,20 @@ class BatchCodec(object):
         cur.wait_event(done)
         return out
 
-    def _stream_descs(self, blob, offs, lens, layout, idx, Sp, table, pitch):
-        """Range-decoder descriptors of scale `idx` of a pass whose streams `layout` (stream_layout's result) places:
-        every stream reads its bytes in place in `blob` (offs / lens int64 [N][streams per image], the layout's
-        order), writes its symbols to its elements of the stream planes Sp [N][C][plane] and finds its CDF rows at
-        the same elements of `table` (int16, `pitch` entries per symbol; pitch 0: the one row of a uniform prior).
-        -> (desc [N * C * T], its [N][C][T] view)."""
-        si, elem, n_sym, _ = layout
+    def _stream_descs(self, blob, offs, lens, n_sym, elem, Sp, table, pitch):
+        """Range-decoder descriptors of the streams of one scale, or of one band of it (offs / lens / n_sym / elem int64
+        [N][C * T], channel-major): every stream reads its bytes in place in `blob`, writes its symbols to its elements
+        of the stream planes Sp [N][C][plane] and finds its CDF rows at the same elements of `table` (int16, `pitch`
+        entries per symbol; pitch 0: the one row of a uniform prior).  -> (desc [N * C * T], its [N][C][T] view)."""
         N, C = Sp.shape[:2]
-        lo, hi = np.searchsorted(si[0], [idx, idx + 1])                 # scale idx: columns lo:hi
-        cols, T = slice(lo, hi), (hi - lo) // C
+        T = n_sym.shape[1] // C
         desc = np.zeros(N * C * T, dtype=_lib.DEC_STREAM_DTYPE)
         d = desc.reshape(N, C, T)
-        d['in'][:] = (blob.data_ptr() + offs[:, cols]).reshape(N, C, T)
-        d['in_len'][:] = lens[:, cols].reshape(N, C, T)
-        d['n_sym'][:] = n_sym[:, cols].reshape(N, C, T)
-        d['sym_out'][:] = (Sp.data_ptr() + elem[:, cols]).reshape(N, C, T)
-        d['table'][:] = (table.data_ptr() + elem[:, cols] * (pitch * 2)).reshape(N, C, T)
+        d['in'][:] = (blob.data_ptr() + offs).reshape(N, C, T)
+        d['in_len'][:] = lens.reshape(N, C, T)
+        d['n_sym'][:] = n_sym.reshape(N, C, T)
+        d['sym_out'][:] = (Sp.data_ptr() + elem).reshape(N, C, T)
+        d['table'][:] = (table.data_ptr() + elem * (pitch * 2)).reshape(N, C, T)
         d['row_pitch'][:] = pitch
         return desc, d
 
@@ -856,7 +870,8 @@ class BatchCodec(object):
                        symbols=lambda idx, S: S, features=lambda idx, F: F,
                        row_pitch=lambda dmll: E.table_pitch(dmll.L), bands=lambda idx: None):
         """The coarse-to-fine walk of every decode: full decodes of equal-size, tiled and ragged batches
-        (decode_device) and region passes (decode_region_pass).  blob, offs, lens, layout: as in _stream_descs;
+        (decode_device) and region passes (decode_region_pass).  blob: the uploaded containers; offs / lens int64
+        [N][streams per image] in the order of the stream_layout `layout`, where every stream reads its bytes in place;
         channels: C of every scale walked, coarse -> fine (a region at level k stops early); recursive: as in
         iter_scale_dmll; lane: as in decode_device.  -> the raster planes of the last scale.
         Every scale decodes into stream planes Sp [N][C][plane], where its CDF rows are built too, and then goes back
@@ -909,28 +924,32 @@ class BatchCodec(object):
                 return l, F_out
 
             band_list = None if uniform else bands(idx)
+            cols = slice(*np.searchsorted(layout[0][0], [idx, idx + 1]))          # the scale's streams
             if uniform:
                 table, pitch = self._uniform(dmll.L, dev)[1], 0
-                desc, d = self._stream_descs(blob, offs, lens, layout, idx, Sp, table, pitch)
+                desc, d = self._stream_descs(blob, offs[:, cols], lens[:, cols], layout[2][:, cols], layout[1][:, cols],
+                                             Sp, table, pitch)
                 decode(desc)
             elif band_list is None:
                 l, F = run_net(F)
                 self._mark(('rnet%d' if scale >= self.net.scales else 'net%d') % scale)
                 pitch = row_pitch(dmll)
                 table = torch.empty(Sp.numel() * pitch, dtype=torch.int16, device=dev)
-                desc, d = self._stream_descs(blob, offs, lens, layout, idx, Sp, table, pitch)
+                desc, d = self._stream_descs(blob, offs[:, cols], lens[:, cols], layout[2][:, cols], layout[1][:, cols],
+                                             Sp, table, pitch)
                 rows(idx, dmll, l, Sp, table, d, steps)
             else:
                 # banded (DESIGN §4.10): per band its network window, its rows and its streams; only one band's
                 # parameters and rows are alive at a time, and its symbols go to their elements of Sp
+                from .region import rect_streams
                 pitch, F_in = row_pitch(dmll), F
                 for band in band_list:
                     l, F = run_net(F_in, band)
-                    (e0, e1), b_layout = band_streams(layout, idx, C, band)
+                    b_cols, n_sym, elem = rect_streams(layout, idx, band)
+                    e0, e1 = band.rect[0] * band.W, band.rect[2] * band.W
                     Sb = torch.empty(N, C, e1 - e0, dtype=torch.uint8, device=dev)
                     table = torch.empty(Sb.numel() * pitch, dtype=torch.int16, device=dev)
-                    desc, d = self._stream_descs(blob, offs[:, b_layout[0]], lens[:, b_layout[0]], b_layout[1:], 0,
-                                                 Sb, table, pitch)
+                    desc, d = self._stream_descs(blob, offs[:, b_cols], lens[:, b_cols], n_sym, elem, Sb, table, pitch)
                     rows(idx, dmll, l, Sb, table, d, steps, band)
                     Sp[:, :, e0:e1].copy_(Sb)
                     del l, table
@@ -1002,7 +1021,10 @@ class BatchCodec(object):
 
         def network(idx, scale, bn8, F, band=None):
             if band is not None:
-                return self._band_window(idx, scale, bn8, F, band, dims, whole_F)
+                # the features of the next finer scale are assembled in one whole plane, band by band
+                keep = ((0, 0) + dims[idx], band.rect, whole_F[0] if band.rect[0] else None)
+                l, whole_F[0] = self._band_window(band, ((0, 0), bn8), ((0, 0), F), keep)
+                return l, whole_F[0], (2 * (band.window[2] - band.window[0]), 2 * bn8.shape[2])
             if ragged:
                 ext_dev(idx)                      # queued ahead of the network: the rows and the raster step read it
             l, F = self.net.get_P_nhwc(scale, bn8, F if self.net.fuses(scale) else None, extents=fin)
@@ -1249,18 +1271,10 @@ class BatchCodec(object):
 
     def _update_window(self, data, parsed, pad_tuple, tile, plan, patch):
         """update_region's window path (DESIGN §4.12)."""
-        dev, net = self.blueprint.device, self.net
-        K = net.config_ms.prob.K
-        sc = {sp.scale: sp for sp in plan.scales}
+        from .region import rect_streams
+        dev = self.blueprint.device
         left, right, top, bottom = pad_tuple
         _, Hf, Wf = parsed[-1][:3]
-
-        def org(y0, x0):
-            return E._to_device_async(np.array([[y0, x0]], np.int32), dev)
-
-        def crop(src, at, r, nhwc):
-            """rectangle r (y0, x0, y1, x1) of the plane whose origin is `at`, as a new tensor"""
-            return E.crop_rect(src, org(r[0] - at[0], r[1] - at[1]), r[2] - r[0], r[3] - r[1], nhwc=nhwc)
 
         # ---- the pixels of P_0: the old ones (the padding is zero), the patch pasted in
         P = plan.window
@@ -1272,66 +1286,30 @@ class BatchCodec(object):
         img[:, :, e[0] - P[0]:e[2] - P[0], e[1] - P[1]:e[3] - P[1]] = patch
         del old
 
-        # ---- encoder phase, fine to coarse: every scale's encoder on its planned window of the finer outputs
-        sym = {0: ((P[0], P[1]), img)}                          # scale -> (origin, symbol window [1][C][h][w])
-        bq = {}                                                 # scale -> (origin, bottleneck values NHWC)
-        x, at = img, (P[0], P[1])
-        for s in range(net.scales):
-            a = sc[s].enc
-            if s == 0:
-                inp = net._rgb_head_input(crop(x, at, a, nhwc=False))
-                hd = inp if isinstance(inp, E.Act) else net.heads[0](inp)
-            else:
-                hd = net.heads[s](self._operand_act(crop(x, at, a, nhwc=True)))
-            eo = net.nets[s].enc(hd)
-            o = (a[0] // 2, a[1] // 2)
-            sym[s + 1] = (o, eo.S.contiguous())
-            bq[s + 1] = (o, eo.bn_q.contiguous())
-            if s + 1 < net.scales:                  # F_{s+1} feeds heads[s + 1]: keep what that conv reads
-                x, at = (eo.F.r if E.tensor_core_mode() else eo.F.f).contiguous(), o
-            del eo, hd
-        del x
+        # ---- encoder phase, fine to coarse: every scale's encoder on its planned window, all of its output kept
+        walk = []
+        for sp in plan.scales[::-1][:-1]:                       # scales 0 .. num_scales - 1
+            a = sp.enc
+            D = (a[0] // 2, a[1] // 2, -(-a[2] // 2), -(-a[3] // 2))
+            walk.append((D, [(a, D)]))
+        enc = self._encode_windows(img, P[:2], walk)
 
         # ---- coding phase, coarse to fine: the intervals of every R_s in its tile order, then one range-coder launch
+        rects = []
+        for sp in plan.scales:
+            D = None if sp.window is None else tuple(2 * v for v in sp.window)      # the decoder's features: all kept
+            rects.append((D, [(sp, D)]))
+        layout = stream_layout([[s[:3] for s in parsed]], tile)
         ivs, cols, n_sym, ptrs = [], [], [], []
-        base, F, fwin = 0, None, None
-        for sp, (scale, dmll, uniform) in zip(plan.scales, self.iter_scale_dmll()):
-            r, C = sp.rect, sp.C
-            h, w = r[2] - r[0], r[3] - r[1]
-            o, S = sym[scale]
-            if uniform:
-                iv = E.reorder_tiles(E.lut_intervals(crop(S, o, r, nhwc=False), self._uniform(dmll.L, dev)[0]), h, w,
-                                     tile, True)
-            else:
-                win = sp.window
-                ob, b = bq[scale + 1]
-                Fw = None
-                if sp.fused:
-                    Fw = crop(F.f, (2 * fwin[0], 2 * fwin[1]), win, nhwc=True)
-                l, F = net.get_P_nhwc(scale, crop(b, ob, win, nhwc=True), Fw)
-                fwin = win
-                iv = E.dmll_intervals_rect(l, sp.out[0], sp.out[1], S, (r[0] - o[0], r[1] - o[1], h, w),
-                                           dmll.targets(dev), C, K, dmll.L, dmll.rgb_scale, tile, origin=o,
-                                           plane=(sp.H, sp.W))
-                del l
+        for idx, sp, iv in self._code_rects(rects, enc, tile):
+            c, n, elem = rect_streams(layout, idx, sp)
             ivs.append(iv)
-            T = len(tile_grid(sp.H, sp.W, tile))
-            grid = np.array(tile_grid(h, w, tile), np.int64)                 # the rectangle's tiles, in sp.tiles order
-            for c in range(C):
-                cols.append(base + c * T + np.asarray(sp.tiles, np.int64))
-                n_sym.append(grid[:, 1])
-                ptrs.append(iv.data_ptr() + (c * h * w + grid[:, 0]) * 4)
-            base += C * T
-        del F
-        cols, n_sym, ptrs = np.concatenate(cols), np.concatenate(n_sym), np.concatenate(ptrs)
-        caps = _slot_cap(n_sym)
-        slot_off = np.concatenate([[0], np.cumsum(caps)])
-        slots = torch.empty(int(slot_off[-1]), dtype=torch.uint8, device=dev)
-        desc = np.zeros(cols.size, dtype=_lib.ENC_STREAM_DTYPE)
-        desc['intervals'] = ptrs
-        desc['n_sym'] = n_sym
-        desc['out_cap'] = caps
-        desc['out'] = slots.data_ptr() + slot_off[:-1]
+            cols.append(c)
+            n_sym.append(n[0])
+            ptrs.append(iv.data_ptr() + elem[0] * 4)
+        del enc
+        cols = np.concatenate(cols)
+        caps, slots, desc = _enc_descs(np.concatenate(ptrs), np.concatenate(n_sym), dev)
         _, lens_dev = E.ac_encode_streams(desc, dev)
         lens_h = torch.empty(lens_dev.shape, dtype=lens_dev.dtype, pin_memory=True)
         slots_h = torch.empty(slots.shape, dtype=torch.uint8, pin_memory=True)
@@ -1340,8 +1318,8 @@ class BatchCodec(object):
         torch.cuda.current_stream().synchronize()
         del ivs
         lens = lens_h.numpy().astype(np.int64)
-        if (lens > caps).any():
-            raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
+        _check_lens(lens, caps)
+        slot_off = desc['out'].astype(np.int64) - slots.data_ptr()
 
         # ---- splice: the old streams' bytes, the new ones in their places, laid out afresh
         old_off = np.array([o for (_, _, _, st) in parsed for (o, _) in st], np.int64)

@@ -30,14 +30,14 @@ namespace l3c {
 // ---------------------------------------------------------------------------------------------
 constexpr int IV_PIX = 64;   // pixels (= threads) per CTA
 
-// BAND: the pixels are the band `g` (BandGeom, dmll_math.cuh) of a banded encode, or the tile-aligned rectangle `g`
-// (RectGeom) of a region update, HW = g.h * g.W; `l` is the window plane the band sits in, the symbols are read from
-// the whole plane and the intervals written in tile order.
-template <int K, bool BAND = false, class G = BandGeom>
+// BAND: the pixels are the tile-aligned rectangle `g` (RectGeom, dmll_math.cuh) of a banded encode or a region update,
+// HW = g.h * g.W; `l` is the window plane the rectangle sits in, the symbols are read from the symbol window and the
+// intervals written in tile order.
+template <int K, bool BAND = false>
 __global__ void __launch_bounds__(IV_PIX)
 dmll_intervals_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
                       const float *__restrict__ targets, int HW, int C, int L, int rgb,
-                      uint32_t *__restrict__ intervals, const G g = G()) {
+                      uint32_t *__restrict__ intervals, const RectGeom g = RectGeom()) {
     extern __shared__ float sm[];
     const int Kp = (rgb ? 4 : 3) * C * K;
     const int pitch = Kp + 1;                       // odd pitch: conflict-free column walks
@@ -719,32 +719,6 @@ extern "C" int l3c_dmll_intervals(const float *l_dev, const uint8_t *sym_dev,
     return L3C_OK;
 }
 
-extern "C" int l3c_dmll_intervals_band(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev,
-                                       int Hs, int y0, int h, int W, const float *targets_dev, int N, int C, int K,
-                                       int L, int rgb, int th, int tw, uint32_t *intervals_dev, void *stream) {
-    using namespace l3c;
-    L3C_REQUIRE(h >= 1 && W >= 1 && (int64_t)h * W < (1ll << 31), "l3c_dmll_intervals_band: %dx%d band", h, W);
-    if (int e = check_common("l3c_dmll_intervals_band", N, h * W, C, K, L, rgb)) return e;
-    L3C_REQUIRE(l_dev && sym_dev && targets_dev && intervals_dev, "l3c_dmll_intervals_band: null pointer");
-    L3C_REQUIRE(th >= 1 && tw >= 1, "l3c_dmll_intervals_band: tile %dx%d", th, tw);
-    L3C_REQUIRE(oy >= 0 && ox >= 0 && oy + h <= Hl && ox + W <= Wl,
-                "l3c_dmll_intervals_band: %dx%d rectangle at (%d, %d) outside the %dx%d parameter plane", h, W, oy, ox,
-                Hl, Wl);
-    L3C_REQUIRE(y0 >= 0 && y0 + h <= Hs, "l3c_dmll_intervals_band: rows [%d, %d) outside the %d-row symbol plane", y0,
-                y0 + h, Hs);
-    const int Kp = (rgb ? 4 : 3) * C * K;
-    const size_t smem = (size_t)IV_PIX * (Kp + 1) * sizeof(float);
-    L3C_REQUIRE(smem <= 48 * 1024, "l3c_dmll_intervals_band: Kp=%d too large", Kp);
-    BandGeom g;
-    g.sym_hw = (long long)Hs * W; g.l_hw = (long long)Hl * Wl;
-    g.y0 = y0; g.h = h; g.W = W; g.Wl = Wl; g.oy = oy; g.ox = ox; g.th = th; g.tw = tw;
-    dim3 grid(ceil_div(h * W, IV_PIX), N);
-    dmll_intervals_kernel<10, true><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
-        l_dev, sym_dev, targets_dev, h * W, C, L, rgb, intervals_dev, g);
-    L3C_LAUNCH_CHECK("dmll_intervals_band_kernel");
-    return L3C_OK;
-}
-
 extern "C" int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int oy, int ox, const uint8_t *sym_dev,
                                        int Hs, int Ws, int y0, int x0, int h, int w, int sy, int sx, int Hf, int Wf,
                                        const float *targets_dev, int N, int C, int K, int L, int rgb, int th, int tw,
@@ -776,7 +750,7 @@ extern "C" int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int o
     g.y0 = y0; g.h = h; g.W = w; g.Wl = Wl; g.oy = oy; g.ox = ox; g.th = th; g.tw = tw;
     g.x0 = x0; g.Ws = Ws;
     dim3 grid(ceil_div(h * w, IV_PIX), N);
-    dmll_intervals_kernel<10, true, RectGeom><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
+    dmll_intervals_kernel<10, true><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, h * w, C, L, rgb, intervals_dev, g);
     L3C_LAUNCH_CHECK("dmll_intervals_rect_kernel");
     return L3C_OK;

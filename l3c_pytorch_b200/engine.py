@@ -796,11 +796,12 @@ def reorder_tiles_images(src, extents_dev, hp, wp, tile):
     return dst
 
 
-def reorder_tiles(src, H, W, tile, to_tiles):
-    """[planes..., H*W or H, W] uint8 / int32 tensor: raster <-> tile order (l3c_reorder_tiles); new tensor."""
+def reorder_tiles(src, H, W, tile, to_tiles, out=None):
+    """[planes..., H*W or H, W] uint8 / int32 tensor: raster <-> tile order (l3c_reorder_tiles); new tensor, or `out`
+    (a contiguous tensor of src's dtype and size) in src's shape."""
     assert src.is_contiguous() and src.dtype in (torch.uint8, torch.int32)
     planes = src.numel() // (H * W)
-    dst = torch.empty_like(src)
+    dst = torch.empty_like(src) if out is None else out.view(src.shape)
     check(lib.l3c_reorder_tiles(_ptr(src), _ptr(dst), src.element_size(), planes, H, W, tile[0], tile[1],
                                 1 if to_tiles else 0, _stream_ptr()))
     LAUNCHES['n'] += 1
@@ -984,25 +985,10 @@ def lin_dmll_intervals_band(conv, cat_h, oy, sym, y0, h, targets, C, K, L, rgb, 
     return iv
 
 
-def dmll_intervals_band(l, oy, ox, sym, y0, h, targets, C, K, L, rgb, tile, out=None):
-    """dmll_intervals for one band of a banded encode (l3c_dmll_intervals_band): the parameters of the h x W rectangle
-    at (oy, ox) of l NHWC [N,Hl,Wl,Kp], coding the symbols of rows [y0, y0 + h) of the whole planes sym uint8
-    [N,C,Hs,W] -> intervals int32 [N,C,h*W] in the tile order of an h x W plane (to `out` when given)."""
-    N, Hl, Wl, _ = l.shape
-    W = sym.shape[3]
-    assert l.is_contiguous() and l.dtype == torch.float32
-    assert sym.dtype == torch.uint8 and sym.is_contiguous() and tuple(sym.shape[:2]) == (N, C)
-    iv = _band_out(out, N, C, h * W, l.device)
-    check(lib.l3c_dmll_intervals_band(_ptr(l), Hl, Wl, int(oy), int(ox), _ptr(sym), sym.shape[2], int(y0), int(h), W,
-                                      _ptr(targets), N, C, K, L, int(rgb), tile[0], tile[1], _ptr(iv), _stream_ptr()))
-    LAUNCHES['n'] += 1
-    return iv
-
-
 def dmll_intervals_rect(l, oy, ox, sym, rect, targets, C, K, L, rgb, tile, origin=(0, 0), plane=None, out=None):
-    """dmll_intervals for one tile-aligned rectangle of a region update (l3c_dmll_intervals_rect): the parameters of
-    the h x w rectangle at (oy, ox) of l NHWC [N,Hl,Wl,Kp], coding the symbols of rect = (y0, x0, h, w) of the window
-    sym uint8 [N,C,Hs,Ws] -> intervals int32 [N,C,h*w] in the tile order of an h x w plane (to `out` when given).
+    """dmll_intervals for one tile-aligned rectangle (l3c_dmll_intervals_rect), a band of a banded encode or an R_s of a
+    region update: the parameters of the h x w rectangle at (oy, ox) of l NHWC [N,Hl,Wl,Kp], coding the symbols of
+    rect = (y0, x0, h, w) of the window sym uint8 [N,C,Hs,Ws] -> intervals int32 [N,C,h*w] in the tile order of an h x w plane (to `out` when given).
     The window sits at `origin` of the container's plane of (H, W) = `plane` (default: sym is the whole plane), in
     which the rectangle must be tile-aligned."""
     N, Hl, Wl, _ = l.shape

@@ -261,14 +261,32 @@ def plan_bands(shapes, tile, config, idx, rows):
     return bands
 
 
+def rect_columns(sp, T):
+    """Columns of the streams of the tile-aligned rectangle sp (ScalePlan) in the stream list of its scale, which has T
+    tiles per channel (a tiled container's order): channel-major, in tile order within a channel."""
+    return (np.arange(sp.C)[:, None] * T + np.asarray(sp.tiles, np.int64)[None, :]).reshape(-1)
+
+
 def stream_columns(plan, tile):
     """Indices, in container order, of the planned streams of every scale: [[column in that scale's stream list]]
-    coarse -> fine, channel-major and in tile order within a channel (the order of a tiled container)."""
-    cols = []
-    for sp in plan.scales:
-        T = len(tile_grid(sp.H, sp.W, tile))
-        cols.append([c * T + t for c in range(sp.C) for t in sp.tiles])
-    return cols
+    coarse -> fine (rect_columns)."""
+    return [rect_columns(sp, len(tile_grid(sp.H, sp.W, tile))) for sp in plan.scales]
+
+
+def rect_streams(layout, idx, sp):
+    """The streams of the tile-aligned rectangle sp (a ScalePlan: a band, an update's R_s, a whole plane) of scale idx
+    of a pass of equal-size images laid out by codec.stream_layout.  -> (cols, n_sym, elem) int64: its columns of the
+    pass's [N][streams] arrays (rect_columns), their symbol counts [N][cols] and their first elements in the
+    rectangle's own [N][C][h * w] planes in tile order.  tile_grid cuts a tile-aligned rectangle into the plane's tiles,
+    in the plane's order, so a stream starts where the rectangle's earlier tiles of its channel end."""
+    si, _, n_sym, _ = layout
+    lo, hi = np.searchsorted(si[0], [idx, idx + 1])
+    cols = lo + rect_columns(sp, (hi - lo) // sp.C)
+    n = n_sym[:, cols]
+    N = n.shape[0]
+    per_c = n.reshape(N, sp.C, -1)
+    elem = np.arange(N * sp.C).reshape(N, sp.C, 1) * _area(sp.rect) + np.cumsum(per_c, 2) - per_c
+    return cols, n, elem.reshape(N, -1)
 
 
 def pass_streams(plans, streams_of, starts):

@@ -1,7 +1,9 @@
 """CPU: the band planner of the banded decode of large tiled containers (DESIGN §4.10).
 
-* Bands cover every tile of a plane exactly once, in container order, and their streams (codec.band_streams) are the
+* Bands cover every tile of a plane exactly once, in container order, and their streams (region.rect_streams) are the
   plane's stream columns with their elements moved into band planes.
+* The streams rect_streams finds for the rectangles R_s of region updates are stream_columns' columns, cut by tile_grid
+  of the rectangle.
 * Every band's window is plan_region's window for the same rectangle.
 * The NaN dependency check of test_region_plan_host, run on band windows: every planned row stays finite.
 * crop=False needs tile=, and the CLI parses `enc --tile`."""
@@ -16,9 +18,9 @@ from tests.test_region_plan_host import _net, _rect_values, _run_chain, _shapes
 @pytest.mark.parametrize('cfg,H,W,R,tile', [
     ('cr', 200, 312, 0, (16, 16)), ('cr', 200, 312, 0, (32, 48)), ('cr', 64, 72, 0, (7, 5)),
     ('cr_rgb_shared', 96, 80, 2, (16, 24))])
-def test_bands_cover_every_tile_once(cfg, H, W, R, tile):
-    from l3c_pytorch_b200.codec import band_streams, stream_layout, tile_grid
-    from l3c_pytorch_b200.region import plan_bands
+def test_rect_streams_of_bands_cover_every_tile_once(cfg, H, W, R, tile):
+    from l3c_pytorch_b200.codec import stream_layout, tile_grid
+    from l3c_pytorch_b200.region import plan_bands, rect_streams
     net = _net(cfg)
     shapes = _shapes(net, H, W, R)
     N = 3
@@ -35,10 +37,14 @@ def test_bands_cover_every_tile_once(cfg, H, W, R, tile):
             for b in bands:
                 y0, x0, y1, x1 = b.rect
                 assert x0 == 0 and x1 == w and y0 % tile[0] == 0 and (y1 % tile[0] == 0 or y1 == h)
-                (e0, e1), (cols, si, elem, n_sym, plane) = band_streams(layout, idx, C, b)
-                assert (e0, e1) == (y0 * w, y1 * w) and grid[b.tiles[0]][0] == e0
-                assert plane.tolist() == [e1 - e0] and (si == 0).all()
+                cols, n_sym, elem = rect_streams(layout, idx, b)
+                e0, e1 = y0 * w, y1 * w
+                assert grid[b.tiles[0]][0] == e0
                 # the band's columns, channel-major and in tile order, hold the band's symbols of every image
+                lo = np.searchsorted(layout[0][0], idx)
+                T = len(grid)
+                assert (cols == lo + (np.arange(C)[:, None] * T + np.array(b.tiles)[None, :]).reshape(-1)).all()
+                assert (layout[0][:, cols] == idx).all()
                 full_elem, full_n = layout[1][:, cols], layout[2][:, cols]
                 assert (n_sym == full_n).all()
                 nc = full_elem // layout[3][idx]
@@ -51,6 +57,33 @@ def test_bands_cover_every_tile_once(cfg, H, W, R, tile):
                             if base <= col < base + h * w:
                                 seen[n, c, col - base:col - base + cnt] += 1
             assert (seen == 1).all()
+
+
+@pytest.mark.parametrize('H,W,tile,edit', [
+    (520, 392, (16, 16), (253, 175, 30, 41)), (520, 392, (16, 24), (0, 0, 520, 392)),
+    (520, 392, (64, 64), (47, 61, 34, 50)), (1008, 760, (16, 16), (504, 380, 8, 8)),
+    (520, 392, (16, 24), (511, 378, 9, 11))])
+def test_rect_streams_of_update_rectangles(H, W, tile, edit):
+    from l3c_pytorch_b200.codec import stream_layout, tile_grid
+    from l3c_pytorch_b200.region import plan_update, rect_streams, stream_columns
+    net = _net('cr')
+    shapes = _shapes(net, H, W)
+    plan = plan_update(shapes, (0, 0, 0, 0), tile, net, edit)
+    layout = stream_layout([shapes], tile)
+    for idx, sp in enumerate(plan.scales):
+        cols, n_sym, elem = rect_streams(layout, idx, sp)
+        lo = np.searchsorted(layout[0][0], idx)
+        assert (cols == lo + np.asarray(stream_columns(plan, tile)[idx])).all()
+        assert (layout[0][0, cols] == idx).all()
+        # the rectangle's own planes, cut by tile_grid in the plane's tile order
+        h, w = sp.rect[2] - sp.rect[0], sp.rect[3] - sp.rect[1]
+        grid = np.array(tile_grid(h, w, tile), np.int64)
+        assert len(grid) == len(sp.tiles)
+        for c in range(sp.C):
+            part = slice(c * len(grid), (c + 1) * len(grid))
+            assert (n_sym[0, part] == grid[:, 1]).all() and (n_sym[0, part] == layout[2][0, cols[part]]).all()
+            assert (elem[0, part] == c * h * w + grid[:, 0]).all()
+    assert sum(len(rect_streams(layout, idx, sp)[0]) for idx, sp in enumerate(plan.scales)) == plan.streams
 
 
 @pytest.mark.parametrize('cfg,H,W,R,tile', [

@@ -4,7 +4,8 @@
   the banded encode writes the same bytes as the whole-image encode: `cr` in all four precision modes, `cr_rgb_shared`
   with recursive=2 in f16 and f16x2, tiles (16, 16) and (16, 24), one image and a batch of three.  The band kernels
   run, and the containers decode losslessly.  The same bytes when it runs on a side stream beside a decode lane.
-* The band interval kernels equal the whole-plane kernels followed by reorder_tiles, restricted to the band.
+* The band interval kernels (the fused f16 one, and the rectangle kernel on full-width rectangles) equal the
+  whole-plane kernels followed by reorder_tiles, restricted to the band.
 * Every encoder-side kernel the windows rely on is position independent in all four modes.
 * Peak encode memory grows with the band, not with the image height; an 8000 x 6000 image encodes under a 24 GB cap."""
 import contextlib
@@ -40,7 +41,7 @@ def _encode(bc, imgs, budget, monkeypatch):
 
 @pytest.mark.parametrize('cfg,mode,R', [('cr', 'f16', 0), ('cr', 'f16x2', 0), ('cr', 'tf32', 0), ('cr', 'fp32', 0),
                                         ('cr_rgb_shared', 'f16', 2), ('cr_rgb_shared', 'f16x2', 2)])
-def test_banded_encode_equals_unbanded(cfg, mode, R, monkeypatch):
+def test_banded_encode_equals_the_whole_image_encode(cfg, mode, R, monkeypatch):
     from l3c_pytorch_b200 import Bitcoding
     from l3c_pytorch_b200.region import plan_bands
     from l3c_pytorch_b200.codec import parse_container
@@ -58,7 +59,7 @@ def test_banded_encode_equals_unbanded(cfg, mode, R, monkeypatch):
                 bands = plan_bands(shapes, tile, bp.net, len(shapes) - 1, 3)
                 assert len(bands) >= 4 and bands[-1].rect[2] - bands[-1].rect[0] < 3 * tile[0]
                 assert banded == whole, (tile, N)
-                band_kernel = 'lin_dmll_band_f16_kernel' if mode == 'f16' else 'dmll_intervals_band_kernel'
+                band_kernel = 'lin_dmll_band_f16_kernel' if mode == 'f16' else 'dmll_intervals_rect_kernel'
                 assert k_band.get(band_kernel, 0) >= len(bands), k_band
                 assert k_whole.get(band_kernel, 0) == 0
                 outs = bc.decode_batch(banded)
@@ -87,7 +88,7 @@ def test_banded_encode_beside_a_decode_lane(monkeypatch):
 
 @pytest.mark.parametrize('rgb', [True, False])
 @pytest.mark.parametrize('N', [1, 3])
-def test_band_kernels_equal_the_whole_plane_kernels(rgb, N):
+def test_band_interval_kernels_equal_the_whole_plane_kernels(rgb, N):
     from l3c_pytorch_b200 import engine as E
     bp = util.blueprint('cr')
     net, losses, dev = bp.net, bp.losses, bp.device
@@ -115,12 +116,12 @@ def test_band_kernels_equal_the_whole_plane_kernels(rgb, N):
             lw[:, oy:oy + h, ox:ox + W] = l[:, y0:y1]
             with _precision('f16'):
                 a = E.lin_dmll_intervals_band(lin, catw, oy, sym, y0, h, tg, C, K, dm.L, rgb, tile)
-            b = E.dmll_intervals_band(lw, oy, ox, sym, y0, h, tg, C, K, dm.L, rgb, tile)
+            b = E.dmll_intervals_rect(lw, oy, ox, sym, (y0, 0, h, W), tg, C, K, dm.L, rgb, tile)
             assert torch.equal(a, whole_a[:, :, y0 * W:y1 * W]), (y0, y1, oy)
             assert torch.equal(b, whole_b[:, :, y0 * W:y1 * W]), (y0, y1, oy, ox)
 
 
-def test_band_kernels_refuse_bad_rectangles():
+def test_band_interval_kernels_refuse_bad_rectangles():
     from l3c_pytorch_b200 import engine as E
     bp = util.blueprint('cr')
     dev = bp.device
@@ -131,13 +132,13 @@ def test_band_kernels_refuse_bad_rectangles():
     cat = torch.zeros(1, 20, 16, 192, dtype=torch.float16, device=dev)
     for bad in (dict(oy=10, y0=0, h=16), dict(oy=0, y0=20, h=16)):
         with pytest.raises(Exception, match='outside|rows'):
-            E.dmll_intervals_band(l, bad['oy'], 0, sym, bad['y0'], bad['h'], dm.targets(dev), 3, 10, 256, True,
-                                  (16, 16))
+            E.dmll_intervals_rect(l, bad['oy'], 0, sym, (bad['y0'], 0, bad['h'], 16), dm.targets(dev), 3, 10, 256,
+                                  True, (16, 16))
         with pytest.raises(Exception, match='rows'):
             E.lin_dmll_intervals_band(lin, cat, bad['oy'], sym, bad['y0'], bad['h'], dm.targets(dev), 3, 10, 256,
                                       True, (16, 16))
     with pytest.raises(Exception, match='C==3'):
-        E.dmll_intervals_band(l, 0, 0, torch.zeros(1, 4, 32, 16, dtype=torch.uint8, device=dev), 0, 16,
+        E.dmll_intervals_rect(l, 0, 0, torch.zeros(1, 4, 32, 16, dtype=torch.uint8, device=dev), (0, 0, 16, 16),
                               dm.targets(dev), 4, 10, 256, True, (16, 16))
 
 
