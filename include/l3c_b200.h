@@ -133,13 +133,16 @@ typedef struct {
 int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_streams, int L,
                           uint32_t first, uint32_t count, void *stream);
 
-/* Copies the first len_dev[i] bytes of every encoder slot to blob_dev + dst_off_dev[i] (byte
- * offsets: the final .l3c container layout, so ONE device->host copy returns a whole batch). */
+/* Copies the first min(len_dev[i], out_cap) bytes of encoder slot i (a stream that outgrew its slot is truncated as
+ * the slot holds it) to blob_dev + dst_off_dev[i] (byte offsets, any alignment: the final .l3c container layout, so
+ * ONE device->host copy returns a whole batch).  Nothing else of the blob is written.  Any number of streams; more
+ * than 65535 take several launches. */
 int l3c_pack_streams(const l3c_enc_stream_t *streams_dev, const uint32_t *len_dev,
                      const uint64_t *dst_off_dev, int n_streams, uint8_t *blob_dev, void *stream);
 
-/* intervals_dev[i] = lut_dev[sym_dev[i]] -- coding intervals when all pixels share one CDF row
- * (uniform prior of the coarsest scale, bitcoding.py:171-186). lut entry = c_low | (c_high-1)<<16. */
+/* intervals_dev[i] = lut_dev[sym_dev[i]], i < n -- coding intervals when all pixels share one CDF row
+ * (uniform prior of the coarsest scale, bitcoding.py:171-186). lut entry = c_low | (c_high-1)<<16, 256 entries.
+ * intervals_dev must not be sym_dev or lut_dev; n above 2^31 - 1 CTAs of 256 is refused. */
 int l3c_lut_intervals(const uint8_t *sym_dev, const uint32_t *lut_dev, int64_t n,
                       uint32_t *intervals_dev, void *stream);
 
@@ -175,7 +178,8 @@ int l3c_dmll_build_table(const float *l_dev, const uint8_t *sym_dev, const float
  * (smaller at the right / bottom edge), tiles in row-major tile order, symbols row-major inside a tile; each
  * tile is one coded stream.  l3c_dmll_build_table_tiled = l3c_dmll_build_table for ALL pixels with rows and
  * sym_dev indexed in tile order (l_dev stays raster NHWC).  l3c_reorder_tiles converts `planes` planes of
- * 1- or 4-byte elements between raster and tile order (to_tiles != 0: raster -> tiles). */
+ * 1- or 4-byte elements between raster and tile order (to_tiles != 0: raster -> tiles); planes <= 65535 and
+ * H * W < 2^31, else L3C_EINVAL.  A tile larger than the plane is the whole plane in that direction. */
 int l3c_dmll_build_table_tiled(const float *l_dev, const uint8_t *sym_dev, const float *targets_dev,
                                int N, int H, int W, int C, int K, int L, int rgb, int c, int th, int tw,
                                uint16_t *table_dev, int pitch, void *stream);
@@ -199,10 +203,14 @@ int l3c_crop_rect(const void *src_dev, void *dst_dev, int elem_bytes, int planes
  * in stream-order planes of `plane` elements ((n * C + c) * plane), max_hw = max_n H_n * W_n.
  * l3c_crop_rects: l3c_crop_rect with a rectangle per image, rects_dev int32 [N][4] = (y, x, h_n, w_n) (16-byte
  * aligned).  dst_off_dev null: dst is N * planes planes of hp x wp, image n top-left and +0 elsewhere; otherwise image
- * n's planes of h_n x w_n follow each other from element dst_off_dev[n] (hp x wp: the largest rectangle).
+ * n's planes of h_n x w_n follow each other from element dst_off_dev[n] (hp x wp: the largest rectangle); nothing
+ * else of dst is written.  Every rectangle lies inside the H x W plane, and h_n <= hp, w_n <= wp.  Both crops refuse
+ * a destination plane whose elements need more than 2^31 - 1 CTAs of 256 threads (bytes, or 4-byte words when
+ * elem_bytes % 4 == 0).
  * l3c_reorder_tiles_images: uint8 tile order -> raster for images of different sizes: src N * planes planes of
  * plane_len bytes, image n's hold the tile order of its extents_dev[n] = (h_n, w_n) plane (int32 [N][2]); dst
- * N * planes planes of hp x wp, image n top-left and 0 elsewhere. */
+ * N * planes planes of hp x wp, image n top-left and 0 elsewhere; h_n * w_n <= plane_len, and hp * wp < 2^31 (else
+ * L3C_EINVAL). */
 int l3c_dmll_build_table_windows(const float *l_dev, int Hl, int Wl, const int *geo_dev, int max_hw, int plane,
                                  const uint8_t *sym_dev, const float *targets_dev, int N, int C, int K, int L, int rgb,
                                  int c, int th, int tw, uint16_t *table_dev, int pitch, void *stream);
@@ -330,12 +338,15 @@ int l3c_rgb_im2col_f16_ragged(const uint8_t *img_dev, const float *A1, const flo
 
 /* Ragged batches (DESIGN §4.6): padded NHWC / planar tensors in which image n occupies [0,h_n) x [0,w_n);
  * extents_dev int32 [N][2] = (h_n, w_n) at the tensor's resolution.
- * l3c_ragged_zero_halo: sets the band of `halo` pixels right of and below every image (clipped to the tensor) of an
- * NHWC tensor with px_bytes bytes per pixel (a multiple of 4) to +0 -- run on the input of a k x k conv, it gives
- * every output pixel inside its image the operands of the per-image launch.
+ * l3c_ragged_zero_halo: sets the band of `halo` pixels right of and below every image, [h_n, h_n + halo) x
+ * [0, w_n + halo) and [0, h_n) x [w_n, w_n + halo) clipped to the tensor, of an NHWC tensor with px_bytes bytes per
+ * pixel (a multiple of 4) to +0, and nothing else -- run on the input of a k x k conv, it gives every output pixel
+ * inside its image the operands of the per-image launch.
  * l3c_ragged_pack: N * planes planes of H x W elements of elem_bytes bytes (plane n * planes + q belongs to image
  * n); to_compact != 0: padded raster -> compact planes of compact_len elements holding the h_n * w_n elements of
- * the image row-major, then zeros; to_compact == 0: compact -> padded raster with zeros outside the image. */
+ * the image row-major, then zeros; to_compact == 0: compact -> padded raster with zeros outside the image.  Every
+ * extent lies inside H x W and h_n * w_n <= compact_len.  Both refuse a plane (compact_len or H * W elements) that
+ * needs more than 2^31 - 1 CTAs of 256 threads. */
 int l3c_ragged_zero_halo(void *x_dev, int px_bytes, int N, int H, int W, const int *extents_dev, int halo,
                          void *stream);
 int l3c_ragged_pack(const void *src_dev, void *dst_dev, int elem_bytes, int planes, int N, int H, int W,

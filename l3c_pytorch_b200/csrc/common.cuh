@@ -83,4 +83,8 @@ __host__ __device__ static inline int decode_pitch(int L) { return (L <= 32) ? 3
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// n items of `per` threads each, in CTAs of 256 threads, fit in one grid row: at most 2^31 - 1 CTAs (CUDA's
+// grid.x limit; a larger count cast to the launch's unsigned would silently cover only part of the items)
+static inline bool fits_grid_x(int64_t n, int64_t per = 1) { return n >= 0 && n <= 0x7fffffffll * 256 / per; }
+
 }  // namespace l3c

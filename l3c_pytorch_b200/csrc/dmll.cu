@@ -864,10 +864,10 @@ namespace l3c {
 template <typename T>
 __global__ void reorder_tiles_kernel(const T *__restrict__ src, T *__restrict__ dst, int HW, int H, int W, int th,
                                      int tw, int to_tiles) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= HW) return;
     const size_t base = (size_t)blockIdx.y * HW;
-    const int p = tile_order_to_raster(r, H, W, th, tw);
+    const int p = tile_order_to_raster((int)r, H, W, th, tw);
     if (to_tiles) dst[base + r] = src[base + p];
     else dst[base + p] = src[base + r];
 }
@@ -886,7 +886,8 @@ __global__ void crop_rect_kernel(const T *__restrict__ src, T *__restrict__ dst,
 }
 
 // crop_rect_kernel with a rectangle per image, rects[n] = (y, x, h_n, w_n).  dst_off null: dst is N * planes planes of
-// hp x wp, image n top-left, zero elsewhere; otherwise image n's planes of h_n x w_n start at element dst_off[n].
+// hp x wp, image n top-left, zero elsewhere; otherwise image n's planes of h_n x w_n start at element dst_off[n]
+// (elements of per_elem words or bytes, as every other index here).
 template <typename T>
 __global__ void crop_rects_kernel(const T *__restrict__ src, T *__restrict__ dst, int per_elem, int planes, int H,
                                   int W, const int4 *__restrict__ rects, const int64_t *__restrict__ dst_off, int hp,
@@ -899,7 +900,7 @@ __global__ void crop_rects_kernel(const T *__restrict__ src, T *__restrict__ dst
     if (dst_off) {
         if (r >= (int64_t)rc.z * rc.w * per_elem) return;
         const int64_t y = rc.x + e / rc.w, x = rc.y + e % rc.w;
-        dst[dst_off[n] + ((int64_t)(plane - n * planes) * rc.z * rc.w + e) * per_elem + k] =
+        dst[(dst_off[n] + (int64_t)(plane - n * planes) * rc.z * rc.w + e) * per_elem + k] =
             src[(((int64_t)plane * H + y) * W + x) * per_elem + k];
         return;
     }
@@ -916,9 +917,9 @@ __global__ void reorder_tiles_images_kernel(const uint8_t *__restrict__ src, uin
                                             int tw) {
     const int plane = blockIdx.y;
     const int n = plane / planes;
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= hp * wp) return;
-    const int y = r / wp, x = r - y * wp, h = ext[2 * n], w = ext[2 * n + 1];
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= (int64_t)hp * wp) return;
+    const int y = (int)(r / wp), x = (int)(r - (int64_t)y * wp), h = ext[2 * n], w = ext[2 * n + 1];
     dst[(int64_t)plane * hp * wp + r] =
         (y < h && x < w) ? src[plane * plane_len + raster_to_tile_order(y, x, h, w, th, tw)] : (uint8_t)0;
 }
@@ -934,6 +935,8 @@ extern "C" int l3c_crop_rects(const void *src_dev, void *dst_dev, int elem_bytes
                 "l3c_crop_rects: elem_bytes=%d planes=%d N=%d %dx%d of %dx%d", elem_bytes, planes, N, hp, wp, H, W);
     const bool words = elem_bytes % 4 == 0;
     const int per_elem = words ? elem_bytes / 4 : elem_bytes;
+    L3C_REQUIRE(fits_grid_x((int64_t)hp * wp, per_elem), "l3c_crop_rects: %dx%d elements of %d bytes in one launch", hp,
+                wp, elem_bytes);
     dim3 grid((unsigned)ceil_div64((int64_t)hp * wp * per_elem, 256), N * planes);
     if (words)
         crop_rects_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
@@ -953,7 +956,8 @@ extern "C" int l3c_reorder_tiles_images(const uint8_t *src_dev, uint8_t *dst_dev
     L3C_REQUIRE(src_dev && dst_dev && src_dev != dst_dev && extents_dev, "l3c_reorder_tiles_images: bad pointers");
     L3C_REQUIRE(planes >= 1 && N >= 1 && (int64_t)N * planes <= 65535 && hp >= 1 && wp >= 1 && th >= 1 && tw >= 1 &&
                     plane_len >= 1, "l3c_reorder_tiles_images: bad arguments");
-    dim3 grid(ceil_div(hp * wp, 256), N * planes);
+    L3C_REQUIRE((int64_t)hp * wp < (1ll << 31), "l3c_reorder_tiles_images: %dx%d plane", hp, wp);
+    dim3 grid((unsigned)ceil_div64((int64_t)hp * wp, 256), N * planes);
     reorder_tiles_images_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src_dev, dst_dev, planes, plane_len, hp, wp,
                                                                         extents_dev, th, tw);
     L3C_LAUNCH_CHECK("reorder_tiles_images_kernel");
@@ -969,6 +973,8 @@ extern "C" int l3c_crop_rect(const void *src_dev, void *dst_dev, int elem_bytes,
                 "l3c_crop_rect: elem_bytes=%d planes=%d N=%d %dx%d of %dx%d", elem_bytes, planes, N, h, w, H, W);
     const bool words = elem_bytes % 4 == 0;
     const int per_elem = words ? elem_bytes / 4 : elem_bytes;
+    L3C_REQUIRE(fits_grid_x((int64_t)h * w, per_elem), "l3c_crop_rect: %dx%d elements of %d bytes in one launch", h, w,
+                elem_bytes);
     dim3 grid((unsigned)ceil_div64((int64_t)h * w * per_elem, 256), N * planes);
     if (words)
         crop_rect_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
@@ -986,8 +992,13 @@ extern "C" int l3c_reorder_tiles(const void *src_dev, void *dst_dev, int elem_by
     L3C_REQUIRE(src_dev && dst_dev && src_dev != dst_dev, "l3c_reorder_tiles: bad pointers");
     L3C_REQUIRE((elem_bytes == 1 || elem_bytes == 4) && planes >= 1 && planes <= 65535 && H >= 1 && W >= 1 && th >= 1 &&
                     tw >= 1, "l3c_reorder_tiles: bad arguments");
+    L3C_REQUIRE((int64_t)H * W < (1ll << 31), "l3c_reorder_tiles: %dx%d plane", H, W);
+    // a tile that reaches past the plane is the plane's extent in that direction: the same order, and the tile
+    // arithmetic (th * W, tw * th) stays below H * W
+    th = th < H ? th : H;
+    tw = tw < W ? tw : W;
     const int HW = H * W;
-    dim3 grid(ceil_div(HW, 256), planes);
+    dim3 grid((unsigned)ceil_div64(HW, 256), planes);
     if (elem_bytes == 1)
         reorder_tiles_kernel<uint8_t><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t *)src_dev, (uint8_t *)dst_dev,
                                                                               HW, H, W, th, tw, to_tiles);

@@ -19,7 +19,7 @@ __global__ void zero_halo_kernel(uint32_t *__restrict__ x, int words_per_px, int
                                  const int *__restrict__ ext, int halo) {
     const int n = blockIdx.y;
     const int h = min(ext[2 * n], H), w = min(ext[2 * n + 1], W);
-    const int wr = min(w + halo, W), hb = min(h + halo, H);
+    const int wr = (int)min((int64_t)w + halo, (int64_t)W), hb = (int)min((int64_t)h + halo, (int64_t)H);
     const int64_t right = (int64_t)h * (wr - w);                 // [0,h) x [w,wr)
     const int64_t count = right + (int64_t)(hb - h) * wr;         // + [h,hb) x [0,wr)
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -73,8 +73,11 @@ extern "C" int l3c_ragged_zero_halo(void *x_dev, int px_bytes, int N, int H, int
                 "l3c_ragged_zero_halo: px_bytes=%d N=%d H=%d W=%d halo=%d", px_bytes, N, H, W, halo);
     if (halo == 0) return L3C_OK;
     const int wpp = px_bytes / 4;
-    const int64_t band = (int64_t)halo * (H + W) * wpp;          // bound on the band of any image
-    dim3 grid((unsigned)ceil_div64(band, 256), N);
+    halo = halo < (H > W ? H : W) ? halo : (H > W ? H : W);      // a wider band is clipped to the same pixels
+    const int64_t band = (int64_t)halo * ((int64_t)H + W);       // bound on the band of any image, in pixels
+    L3C_REQUIRE(fits_grid_x(band, wpp), "l3c_ragged_zero_halo: a %d-pixel band of %dx%d pixels of %d bytes", halo, H, W,
+                px_bytes);
+    dim3 grid((unsigned)ceil_div64(band * wpp, 256), N);
     zero_halo_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint32_t *)x_dev, wpp, H, W, extents_dev, halo);
     L3C_LAUNCH_CHECK("zero_halo_kernel");
     return L3C_OK;
@@ -91,6 +94,8 @@ extern "C" int l3c_ragged_pack(const void *src_dev, void *dst_dev, int elem_byte
     const bool words = elem_bytes % 4 == 0;
     const int per_elem = words ? elem_bytes / 4 : elem_bytes;
     const int64_t len = to_compact ? (int64_t)compact_len : (int64_t)H * W;
+    L3C_REQUIRE(fits_grid_x(len, per_elem), "l3c_ragged_pack: planes of %lld elements of %d bytes in one launch",
+                (long long)len, elem_bytes);
     dim3 grid((unsigned)ceil_div64(len * per_elem, 256), N * planes);
     if (words)
         ragged_pack_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t)stream>>>(

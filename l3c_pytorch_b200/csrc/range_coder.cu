@@ -1264,8 +1264,9 @@ __global__ void pack_streams_kernel(const l3c_enc_stream_t *__restrict__ streams
     const uint32_t len = min(lens[blockIdx.y], st.out_cap);
     uint8_t *dst = blob + dst_off[blockIdx.y];
     for (uint64_t b0 = (uint64_t)blockIdx.x * PACK_CHUNK; b0 < len; b0 += (uint64_t)gridDim.x * PACK_CHUNK) {
-        const uint32_t b1 = (uint32_t)min(b0 + (uint64_t)PACK_CHUNK, (uint64_t)len);
-        for (uint32_t i = (uint32_t)b0 + threadIdx.x; i < b1; i += blockDim.x) dst[i] = st.out[i];
+        // 64-bit positions: a 32-bit i would wrap past 2^32 - 1 in the last chunk of a slot of almost 4 GiB
+        const uint64_t b1 = min(b0 + (uint64_t)PACK_CHUNK, (uint64_t)len);
+        for (uint64_t i = b0 + threadIdx.x; i < b1; i += blockDim.x) dst[i] = st.out[i];
     }
 }
 
@@ -1446,7 +1447,9 @@ extern "C" int l3c_pack_streams(const l3c_enc_stream_t *streams_dev, const uint3
 extern "C" int l3c_lut_intervals(const uint8_t *sym_dev, const uint32_t *lut_dev, int64_t n,
                                  uint32_t *intervals_dev, void *stream) {
     using namespace l3c;
-    L3C_REQUIRE(sym_dev && lut_dev && intervals_dev && n >= 0, "l3c_lut_intervals: bad arguments");
+    L3C_REQUIRE(sym_dev && lut_dev && intervals_dev && (const void *)sym_dev != (const void *)intervals_dev &&
+                    (const void *)lut_dev != (const void *)intervals_dev && fits_grid_x(n),
+                "l3c_lut_intervals: bad arguments (n=%lld)", (long long)n);
     if (n == 0) return L3C_OK;
     lut_intervals_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(sym_dev, lut_dev, n,
                                                                                        intervals_dev);
