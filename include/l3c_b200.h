@@ -518,6 +518,11 @@ int l3c_cta_trace_launches(char *buf, size_t cap, int64_t *n_records);
  * for production use. */
 int l3c_set_decoder_streams_per_cta(int spc);
 
+/* Test knob: streams per CTA (1, 2 or 4) of ac_encode_kernel<SPC>, each stream a coding warp and an emitter warp;
+ * 0 = the L3C_ENC_SPC environment variable or, without it, the default (4).  Any other value is L3C_EINVAL.  Lets
+ * one process run every variant, including a partial last CTA.  Not meant for production use. */
+int l3c_set_encoder_streams_per_cta(int spc);
+
 /* Test probe of the CDF rows' sigmoid: for the n fp32 values u_dev[i] (device), raw_dev[i] = sigmoid_from_log2(u)
  * (~ 1 / (1 + 2^u), the MUFU.EX2 + MUFU.RCP evaluation every CDF entry uses) and term_dev[i] = mixture_term(0, 1, u)
  * (the same with the saturation shortcuts: exactly 1 for u <= -25, 0 for u >= 40).  Both call the kernels' own

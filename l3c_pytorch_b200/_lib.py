@@ -99,6 +99,7 @@ _SIGNATURES = {
     'l3c_cta_trace_register': (c_int, [c_void_p, c_int64]),
     'l3c_cta_trace_launches': (c_int, [ctypes.c_char_p, c_size_t, ctypes.POINTER(c_int64)]),
     'l3c_set_decoder_streams_per_cta': (c_int, [c_int]),
+    'l3c_set_encoder_streams_per_cta': (c_int, [c_int]),
     'l3c_dmll_probe_sigmoid': (c_int, [c_void_p] * 3 + [c_int64, c_void_p]),
     'l3c_batch_intervals': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     'l3c_batch_rows': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_uint32, c_void_p, c_void_p]),

@@ -1,4 +1,5 @@
-// range_coder.cu -- batched binary arithmetic coder for sm_90a: one warp per stream.
+// range_coder.cu -- batched binary arithmetic coder for sm_90a: one coding warp per stream (decoders of L > 32 and the
+// encoder: plus a helper / emitter warp).
 //
 // Bit-exact re-statement of the reference coder's integer arithmetic
 //   encoder: /root/reference/src/torchac/torchac_backend/torchac.cpp:152-227 (+ bit sink :63-93)
@@ -9,8 +10,8 @@
 //     can only ever visit them in that order, see DESIGN.md section 4.4);
 //   * the encoder consumes pre-computed 32-bit (c_low, c_high-1) intervals (one coalesced load per
 //     32 symbols) instead of indexing a CDF table with the symbol;
-//   * the encoder keeps bit emission off its serial chain: per symbol only (low, k, u) is recorded,
-//     every 32 symbols the warp packs the 32 bit strings in parallel (one packed scan);
+//   * the encoder keeps bit emission off its serial chain and off its warp: per symbol only (low, k, u) is
+//     recorded, every 32 symbols an emitter warp packs the 32 bit strings in parallel (one packed scan);
 //   * the decoder replaces the per-row binary search by a warp-wide comparison of the whole CDF row
 //     against the code value (no division: cdf[m] <= ((value-low+1)*2^16-1)/span  <=>
 //     mulhi(cdf[m] << 16, span) <= value - low) and one warp max-reduction over packed
@@ -32,7 +33,27 @@
 namespace l3c {
 
 constexpr unsigned FULL = 0xFFFFFFFFu;
-constexpr int ENC_WARPS_PER_CTA = 1;
+
+// shared-memory hand-over between the warps of a stream (the encoder's and the decoders' rings)
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done;
+    do {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done)
+            : "r"(bar), "r"(parity)
+            : "memory");
+    } while (!done);
+}
 
 // ---------------------------------------------------------------------------------------------
 // encoder
@@ -80,9 +101,10 @@ struct BitSink {
     }
 };
 
-// Emission is kept OFF the coder's serial dependency chain: the coding loop only records, per symbol,
-// the pre-shift `low` and the two shift counts (k decided bits, u underflow shifts) in lane j's
-// registers; every 32 symbols the warp turns the 32 records into bits IN PARALLEL:
+// Emission is kept OFF the coder's serial dependency chain and off its warp: the coding warp only
+// records, per symbol, the pre-shift `low` and the two shift counts (k decided bits, u underflow shifts)
+// in lane j's registers and hands every 32 records to the stream's emitter warp through a shared-memory
+// ring; the emitter turns the 32 records into bits IN PARALLEL:
 //   pending(j)  = underflow bits owed when symbol j is reached  (segmented sum of u, reset by k > 0)
 //   string(j)   = k(j) > 0 ?  b0, pending(j) x !b0, remaining k-1 bits  :  nothing   (torchac.cpp:186-206)
 //   offset(j)   = exclusive prefix sum of the string lengths
@@ -182,58 +204,67 @@ struct Emitter {
     }
 };
 
-__global__ void __launch_bounds__(32 * ENC_WARPS_PER_CTA)
-ac_encode_kernel(const l3c_enc_stream_t *__restrict__ streams, int n_streams,
-                 uint32_t *__restrict__ out_len) {
-    __shared__ uint32_t s_stage[ENC_WARPS_PER_CTA][STAGE_WORDS];
-    const int sid = blockIdx.x * ENC_WARPS_PER_CTA + (threadIdx.x >> 5);
-    if (sid >= n_streams) return;
-    const int lane = threadIdx.x & 31;
-    const l3c_enc_stream_t st = streams[sid];
-    const uint32_t *__restrict__ iv = st.intervals;
-    const uint32_t n = st.n_sym;
+constexpr int ENC_RING = 4;          // ring slots of 32 records between a stream's coding and emitter warps
 
-    Emitter em;
-    em.stage = s_stage[threadIdx.x >> 5];
-    em.pending = 0u;
-    em.sink.out = reinterpret_cast<uint32_t *>(st.out);
-    em.sink.cap_words = st.out_cap >> 2;
-    em.sink.wpos = 0;
-    em.sink.acc = 0;
-    em.sink.nacc = 0;
-    em.sink.lane = lane;
+// (x << n) >> 32 for a 64-bit x and n <= 32 (the clamp keeps n = 32 exact: the low word)
+__device__ __forceinline__ uint32_t shl64_hi(uint64_t x, uint32_t n) {
+    uint32_t r;
+    asm("shf.l.clamp.b32 %0, %1, %2, %3;" : "=r"(r) : "r"((uint32_t)x), "r"((uint32_t)(x >> 32)), "r"(n));
+    return r;
+}
 
-    // Coder state is (low, r = high - low): `high` itself is never needed.  Every renormalisation
-    // shift -- "equal MSB" (low <<= 1, high = high << 1 | 1) or "underflow" (the same with the MSBs
-    // forced to 0 / 1) -- maps r to 2r + 1 (mod 2^32) and leaves bit 31 of low clear, so
-    //     r' = (width << s) - 1,   low' = (low << s) & 0x7FFFFFFF      with width = r + 1, s = k + u.
-    uint32_t low = 0u, r = 0xFFFFFFFFu;
-
-    // one coding step (torchac.cpp:171-206); lane j keeps the record of symbol j of the batch
-#define L3C_ENC_STEP(j)                                                                            \
-    {                                                                                              \
-        const uint32_t v = __shfl_sync(FULL, mine, (j));                                           \
-        const uint32_t c_lo = v & 0xFFFFu;                                                         \
-        const uint32_t c_hi = (v >> 16) + 1u;                                                      \
-        /* span * c == r * c + c  (span may be 2^32, keep it out of 32-bit registers) */           \
-        const uint32_t hi16 = (uint32_t)(((uint64_t)r * c_hi + c_hi) >> 16);                       \
-        const uint32_t lo16 = (uint32_t)(((uint64_t)r * c_lo + c_lo) >> 16);                       \
-        const uint32_t width = hi16 - lo16;                /* new high - new low + 1 */            \
-        low += lo16;                                                                               \
-        const uint32_t high = low + width - 1u;                                                    \
-        /* renormalisation: k "equal MSB" shifts, then u "underflow" shifts */                     \
-        const uint32_t k = (uint32_t)__clz((int)(low ^ high));                                     \
-        const uint32_t u = clz_nz(~shl_c(shl_c(low & ~high, k), 1u));                              \
-        if (lane == (j)) {                                                                         \
-            rec_low = low;                                                                         \
-            rec_ku = k | (u << 8);                                                                 \
-        }                                                                                          \
-        low = shl_c(shl_c(low, k), u) & 0x7FFFFFFFu;                                               \
-        r = shl_c(shl_c(width, k), u) - 1u;                                                        \
+// Coding warp.  Coder state is (low, r = high - low): `high` itself is never needed.  Every renormalisation
+// shift -- "equal MSB" (low <<= 1, high = high << 1 | 1) or "underflow" (the same with the MSBs forced to 0 / 1)
+// -- maps r to 2r + 1 (mod 2^32) and leaves bit 31 of low clear, so
+//     r' + 1 = width << s,   low' = (low << s) & 0x7FFFFFFF      with width = hi16 - lo16, s = k + u.
+// The next symbol's products span' * c are therefore (width * c) << s: they are formed as soon as width is known,
+// beside the clz chain that yields s, and s only shifts them (one funnel shift each).  The state carried from one
+// symbol to the next is (low before its shift, s, and the two products pre-shifted by 16): the interval bounds are
+// bits 16..47 of product << s, the high word of (product << 16) << s.  A stream starts at span 2^32 = 1 << 32.
+// This equals the r-recurrence of torchac.cpp mod 2^32 whenever the true width << s <= 2^32, i.e. on every valid
+// interval (c_lo < c_hi); a width of 2^32 (c_lo = 0, c_hi = 65536 at span 2^32) is kept as (width - 1) * c + c.
+// The shifted low is not masked to 31 bits on the chain: its bit 31 only flips bit 31 of low and high, which leaves
+// low ^ high (k), the underflow bits below the first differing one (u) and every later low's bits 0..30 unchanged;
+// the record and the terminator clear it.
+__device__ __forceinline__ void encode_records(const uint32_t *__restrict__ iv, uint32_t n, uint2 (*ring)[32],
+                                               uint32_t bar0, int lane) {
+    uint32_t next = (lane < n) ? __ldg(iv + lane) : 0u;
+    uint32_t lowp = 0u, s = 32u;
+    uint64_t xl, xh;
+    {
+        const uint32_t v = __shfl_sync(FULL, next, 0);
+        xl = (uint64_t)(v & 0xFFFFu) << 16;
+        xh = (uint64_t)((v >> 16) + 1u) << 16;
     }
 
-    uint32_t next = (lane < n) ? __ldg(iv + lane) : 0u;
-    for (uint32_t base = 0; base < n; base += 32) {
+    // one coding step (torchac.cpp:171-206); lane j keeps the record of symbol j of the batch
+#define L3C_ENC_STEP(j)                                                                                            \
+    {                                                                                                              \
+        const uint32_t v1 = __shfl_sync(FULL, (j) < 31 ? mine : next, ((j) + 1) & 31);   /* the next symbol */     \
+        const uint32_t c_lo1 = v1 & 0xFFFFu;                                                                       \
+        const uint32_t c_hi1 = (v1 >> 16) + 1u;                                                                    \
+        const uint32_t lo16 = shl64_hi(xl, s);                                                                     \
+        const uint32_t hi16 = shl64_hi(xh, s);                                                                     \
+        const uint32_t lowm = shl_c(lowp, s);                           /* bit 31 unmasked, see above */           \
+        const uint32_t low = lowm + lo16;                                                                          \
+        const uint32_t high = lowm + hi16 - 1u;                                                                    \
+        const uint32_t wm1 = hi16 - lo16 - 1u;                           /* width - 1 */                           \
+        xl = ((uint64_t)wm1 * c_lo1 + c_lo1) << 16;                                                                \
+        xh = ((uint64_t)wm1 * c_hi1 + c_hi1) << 16;                                                                \
+        /* renormalisation: k "equal MSB" shifts, then u "underflow" shifts */                                     \
+        const uint32_t d = low ^ high;                                   /* != 0: a width >= 2^14 */               \
+        const uint32_t k = clz_nz(d);                                                                              \
+        const uint32_t u = clz_nz(~shl_c((d & low) << 1, k));            /* d & low == low & ~high */              \
+        if (lane == (j)) {                                                                                         \
+            rec_low = low ^ (lowm & 0x80000000u);                                                                  \
+            rec_ku = k | (u << 8);                                                                                 \
+        }                                                                                                          \
+        lowp = low;                                                                                                \
+        s = k + u;                                                                                                 \
+    }
+
+    uint32_t b = 0;
+    for (uint32_t base = 0; base < n; base += 32, ++b) {
         const uint32_t mine = next;
         const uint32_t nb = base + 32 + lane;
         next = (nb < n) ? __ldg(iv + nb) : 0u;              // prefetch the next 32 intervals
@@ -246,22 +277,77 @@ ac_encode_kernel(const l3c_enc_stream_t *__restrict__ streams, int n_streams,
 #pragma unroll 1
             for (int j = 0; j < cnt; ++j) L3C_ENC_STEP(j)
         }
-        em.emit(rec_low, rec_ku & 0xFFu, rec_ku >> 8);
+        const uint32_t slot = b % ENC_RING;
+        if (b >= ENC_RING) mbar_wait(bar0 + 8 * (ENC_RING + slot), (b / ENC_RING - 1) & 1u);    // empty[slot]
+        ring[slot][lane] = make_uint2(rec_low, rec_ku);
+        mbar_arrive(bar0 + 8 * slot);                                                           // full[slot]
     }
 #undef L3C_ENC_STEP
 
-    // termination (torchac.cpp:209-219): one more bit + the owed underflow bits, zero-padded --
-    // i.e. a one-bit record met with pending + 1 owed bits
+    // termination (torchac.cpp:209-219): one more bit + the owed underflow bits, zero-padded -- i.e. a one-bit
+    // record (lane 0) that the emitter meets with pending + 1 owed bits
+    const uint32_t low = shl_c(lowp, s) & 0x7FFFFFFFu;
     const uint32_t fin = (low < 0x40000000u) ? 0u : 1u;
-    em.pending += 1u;
-    em.emit(lane == 0 ? (fin << 31) : 0u, lane == 0 ? 1u : 0u, 0u);
+    const uint32_t slot = b % ENC_RING;
+    if (b >= ENC_RING) mbar_wait(bar0 + 8 * (ENC_RING + slot), (b / ENC_RING - 1) & 1u);
+    ring[slot][lane] = lane == 0 ? make_uint2(fin << 31, 1u) : make_uint2(0u, 0u);
+    mbar_arrive(bar0 + 8 * slot);
+}
+
+// Emitter warp: the batches of 32 records in order, then the termination record; writes the words and out_len.
+__device__ __forceinline__ void emit_records(const l3c_enc_stream_t &st, const uint2 (*ring)[32], uint32_t *stage,
+                                             uint32_t bar0, int lane, uint32_t *out_len) {
+    Emitter em;
+    em.stage = stage;
+    em.pending = 0u;
+    em.sink.out = reinterpret_cast<uint32_t *>(st.out);
+    em.sink.cap_words = st.out_cap >> 2;
+    em.sink.wpos = 0;
+    em.sink.acc = 0;
+    em.sink.nacc = 0;
+    em.sink.lane = lane;
+    const uint32_t n_batches = st.n_sym / 32u + (st.n_sym % 32u != 0u);
+    for (uint32_t b = 0; b <= n_batches; ++b) {
+        const uint32_t slot = b % ENC_RING;
+        mbar_wait(bar0 + 8 * slot, (b / ENC_RING) & 1u);                                        // full[slot]
+        const uint2 rec = ring[slot][lane];
+        mbar_arrive(bar0 + 8 * (ENC_RING + slot));                                              // empty[slot]
+        if (b == n_batches) em.pending += 1u;
+        em.emit(rec.x, rec.y & 0xFFu, rec.y >> 8);
+    }
     BitSink &sink = em.sink;
     const uint32_t total = sink.wpos * 4u + (uint32_t)((sink.nacc + 7) >> 3);
     if (sink.nacc > 0) {
         const uint32_t w = (uint32_t)(sink.acc << (32 - sink.nacc));
         if (lane == 0 && sink.wpos < sink.cap_words) sink.out[sink.wpos] = __byte_perm(w, 0, 0x0123);
     }
-    if (lane == 0) out_len[sid] = total;
+    if (lane == 0) *out_len = total;
+}
+
+// SPC = streams per CTA.  Coding warps are warps 0..SPC-1, emitter warps SPC..2*SPC-1 (the decoders' layout).
+template <int SPC>
+__global__ void __launch_bounds__(64 * SPC)
+ac_encode_kernel(const l3c_enc_stream_t *__restrict__ streams, int n_streams, uint32_t *__restrict__ out_len) {
+    __shared__ uint2 s_ring[SPC][ENC_RING][32];
+    __shared__ uint32_t s_stage[SPC][STAGE_WORDS];
+    __shared__ __align__(8) uint64_t s_bar[SPC][2 * ENC_RING];          // full[0..RING), empty[0..RING)
+    const int warp_id = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int sslot = warp_id % SPC;
+    const uint32_t bar0 = smem_u32(s_bar[sslot]);
+    if (warp_id < SPC && lane == 0) {
+#pragma unroll
+        for (int i = 0; i < 2 * ENC_RING; ++i) mbar_init(bar0 + 8 * i, 32);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const int sid = blockIdx.x * SPC + sslot;
+    if (sid >= n_streams) return;
+    const l3c_enc_stream_t st = streams[sid];
+    if (warp_id < SPC)
+        encode_records(st.intervals, st.n_sym, s_ring[sslot], bar0, lane);
+    else
+        emit_records(st, s_ring[sslot], s_stage[sslot], bar0, lane, out_len + sid);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -627,25 +713,6 @@ namespace v3 {
 constexpr int G = 8;            // symbols per group
 constexpr int R = 2 * G;        // ring slots
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-    } while (!done);
-}
 
 // SPC = streams per CTA.  Decoder warps are warps 0..SPC-1, helper warps SPC..2*SPC-1: with SPC = 4 the
 // decoder and the helper of a stream sit on the same SM sub-partition (warp id mod 4) and every scheduler
@@ -874,10 +941,6 @@ namespace coarse {
 
 using v3::G;
 using v3::R;
-using v3::mbar_arrive;
-using v3::mbar_init;
-using v3::mbar_wait;
-using v3::smem_u32;
 
 constexpr int SLOT_WORDS = COARSE_PARAM_WORDS + COARSE_N;     // parameters, then the coarse proposals
 constexpr int RING_BYTES = R * SLOT_WORDS * 4;                 // 4 KB per stream
@@ -1146,10 +1209,6 @@ __device__ __forceinline__ void stage_row(uint32_t dst, const void *src, uint32_
 __global__ void __launch_bounds__(64)
 ac_decode_wide_kernel(const l3c_dec_stream_t *__restrict__ streams, int L, int ring_n, uint32_t first,
                       uint32_t count) {
-    using v3::mbar_arrive;
-    using v3::mbar_init;
-    using v3::mbar_wait;
-    using v3::smem_u32;
     extern __shared__ __align__(16) uint8_t dec_smem[];
     const int warp = threadIdx.x >> 5;                 // 0 = decoder, 1 = helper
     const int lane = threadIdx.x & 31;
@@ -1282,16 +1341,48 @@ __global__ void lut_intervals_kernel(const uint8_t *__restrict__ sym, const uint
 // ---------------------------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------------------------
+namespace l3c {
+// streams per CTA of the helper-warp decoders and of the encoder: a test knob, else an environment variable (read
+// once), else the default
+static int spc_from_env(const char *name, int dflt) {
+    const char *e = getenv(name);
+    const int v = e ? atoi(e) : dflt;
+    return (v == 1 || v == 2 || v == 4) ? v : dflt;
+}
+
+std::atomic<int> g_enc_spc{0};   // l3c_set_encoder_streams_per_cta: 0 = L3C_ENC_SPC / the default
+// 4 streams per CTA: at the 288 streams of a bench batch the fastest in isolation, and in the pipelined step ~5 %
+// faster than 1 (DESIGN §7)
+constexpr int DEFAULT_ENC_SPC = 4;
+static int encoder_spc() {
+    static const int env_spc = spc_from_env("L3C_ENC_SPC", DEFAULT_ENC_SPC);
+    const int forced = g_enc_spc.load(std::memory_order_relaxed);
+    return forced ? forced : env_spc;
+}
+}  // namespace l3c
+
 extern "C" int l3c_ac_encode_streams(const l3c_enc_stream_t *streams_dev, int n_streams,
                                      uint32_t *out_len_dev, void *stream) {
     using namespace l3c;
     L3C_REQUIRE(n_streams >= 0, "l3c_ac_encode_streams: n_streams=%d", n_streams);
     if (n_streams == 0) return L3C_OK;
     L3C_REQUIRE(streams_dev && out_len_dev, "l3c_ac_encode_streams: null pointer");
-    const int grid = ceil_div(n_streams, ENC_WARPS_PER_CTA);
-    ac_encode_kernel<<<grid, 32 * ENC_WARPS_PER_CTA, 0, (cudaStream_t)stream>>>(
-        streams_dev, n_streams, out_len_dev);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int spc = encoder_spc();
+    if (spc == 4)
+        ac_encode_kernel<4><<<ceil_div(n_streams, 4), 256, 0, st>>>(streams_dev, n_streams, out_len_dev);
+    else if (spc == 2)
+        ac_encode_kernel<2><<<ceil_div(n_streams, 2), 128, 0, st>>>(streams_dev, n_streams, out_len_dev);
+    else
+        ac_encode_kernel<1><<<n_streams, 64, 0, st>>>(streams_dev, n_streams, out_len_dev);
     L3C_LAUNCH_CHECK("ac_encode_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_set_encoder_streams_per_cta(int spc) {
+    L3C_REQUIRE(spc == 0 || spc == 1 || spc == 2 || spc == 4,
+                "l3c_set_encoder_streams_per_cta: spc=%d not in {0, 1, 2, 4}", spc);
+    l3c::g_enc_spc.store(spc);
     return L3C_OK;
 }
 
@@ -1304,11 +1395,7 @@ std::atomic<int> g_dec_spc{0};   // l3c_set_decoder_streams_per_cta: 0 = L3C_DEC
 // (DESIGN §7).
 constexpr int DEFAULT_DEC_SPC = 2;
 static int decoder_spc() {
-    static const int env_spc = [] {
-        const char *e = getenv("L3C_DEC_SPC");
-        const int v = e ? atoi(e) : DEFAULT_DEC_SPC;
-        return (v == 1 || v == 2 || v == 4) ? v : DEFAULT_DEC_SPC;
-    }();
+    static const int env_spc = spc_from_env("L3C_DEC_SPC", DEFAULT_DEC_SPC);
     const int forced = g_dec_spc.load(std::memory_order_relaxed);
     return forced ? forced : env_spc;
 }

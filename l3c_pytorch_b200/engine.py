@@ -141,6 +141,18 @@ def decoder_streams_per_cta(spc):
         check(lib.l3c_set_decoder_streams_per_cta(0))
 
 
+@contextlib.contextmanager
+def encoder_streams_per_cta(spc):
+    """Test knob (l3c_set_encoder_streams_per_cta): inside the block the range encoder packs `spc` streams (1, 2 or 4),
+    each a coding warp and an emitter warp, into one CTA; 0 = the L3C_ENC_SPC / default choice.  Process-wide; the
+    default is restored on exit."""
+    check(lib.l3c_set_encoder_streams_per_cta(int(spc)))
+    try:
+        yield
+    finally:
+        check(lib.l3c_set_encoder_streams_per_cta(0))
+
+
 # ----------------------------------------------------------------------------------------------
 # ragged batches (DESIGN §4.6)
 # ----------------------------------------------------------------------------------------------

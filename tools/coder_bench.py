@@ -145,8 +145,63 @@ def run_coarse(n_streams, kind, H=128, W=128):
                           linear_fraction=frac_lin, dec_ns_per_sym=min(times[1:]) * 1e6 / HW, ok=ok)))
 
 
+def run_encoder(n_streams, kind, n_sym=262144, reps=5):
+    """The encoder alone at the size of an RGB plane of bench.py (512 x 512 symbols per stream), every stream its own
+    intervals (one pattern rotated per stream).  kind 'bench': symbols drawn from flat random rows of 256 entries
+    (~8 bits per symbol, as on bench.py's noise images); 'peaked': one dominant entry per row, 80 % of the symbols on
+    it (~1-2 bits per symbol, trained-like).  Reports the median of `reps` launches after one warm-up launch."""
+    dev = torch.device('cuda')
+    rng = np.random.default_rng(1)
+    L, n_rows = 256, 8192
+    w = rng.integers(1, 40, size=(n_rows, L)).astype(np.float64)
+    p = rng.integers(0, L, n_rows)
+    if kind == 'peaked':
+        w[np.arange(n_rows), p] *= 2000
+    w = w / w.sum(1, keepdims=True) * (65536 - L)
+    c = np.floor(np.cumsum(w, 1)).astype(np.int64) + np.arange(1, L + 1)
+    c[:, -1] = 65536
+    cdf = np.concatenate([np.zeros((n_rows, 1), np.int64), c], 1)
+    sym = rng.integers(0, L, n_rows)
+    if kind == 'peaked':
+        sym = np.where(rng.random(n_rows) < 0.8, p, sym)
+    r = np.arange(n_rows)
+    iv1 = torch.from_numpy((cdf[r, sym] | ((cdf[r, sym + 1] - 1) << 16)).astype(np.uint32).view(np.int32))
+    base = iv1.repeat(n_sym // n_rows + 1)[:n_sym].to(dev)
+    iv = torch.stack([torch.roll(base, 977 * i) for i in range(n_streams)])
+    cap = ((n_sym * 17 + 7) // 8 + 64 + 3) & ~3
+    slots = torch.zeros(n_streams * cap, dtype=torch.uint8, device=dev)
+    desc = np.zeros(n_streams, dtype=_lib.ENC_STREAM_DTYPE)
+    desc['intervals'] = iv.data_ptr() + 4 * n_sym * np.arange(n_streams); desc['n_sym'] = n_sym; desc['out_cap'] = cap
+    desc['out'] = slots.data_ptr() + cap * np.arange(n_streams)
+    ddev = E._desc_to_device(desc, dev)
+    lens = torch.empty(n_streams, dtype=torch.int32, device=dev)
+    times = []
+    for _ in range(reps + 1):
+        a = torch.cuda.Event(enable_timing=True); b = torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize(); a.record()
+        E.check(E.lib.l3c_ac_encode_streams(E._ptr(ddev), n_streams, E._ptr(lens), E._stream_ptr()))
+        b.record(); torch.cuda.synchronize(); times.append(a.elapsed_time(b))
+    t = float(np.median(times[1:]))
+    # a digest of every stream's bytes, to compare builds
+    ln = lens.cpu().numpy().astype(np.int64)
+    h = slots.view(n_streams, cap).to(torch.int64)
+    mask = torch.arange(cap, device=dev)[None, :] < torch.from_numpy(ln).to(dev)[:, None]
+    digest = int(((h * mask) * torch.arange(1, cap + 1, device=dev)[None, :]).sum()) & 0xFFFFFFFFFFFF
+    print(json.dumps(dict(encoder=kind, streams=n_streams, n_sym=n_sym, bits_per_sym=float(ln.mean()) * 8 / n_sym,
+                          enc_ms=t, enc_ns_per_sym=t * 1e6 / n_sym, digest=digest)))
+
+
 if __name__ == '__main__':
     only = int(sys.argv[sys.argv.index('--only') + 1]) if '--only' in sys.argv else None
+    if '--encoder' in sys.argv:       # the encoder alone: 1, 48 and 288 streams of an RGB plane of bench.py
+        import subprocess
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', '0'],
+                           capture_output=True, text=True).stdout.strip()
+        print(json.dumps(dict(gpu=torch.cuda.get_device_name(0), nvidia_smi=q)))
+        for kind in ('bench', 'peaked'):
+            for ns in (1, 48, 288):
+                run_encoder(ns, kind)
+        sys.exit(0)
     if '--coarse' in sys.argv:        # the coarse RGB decoder (f16 mode, L = 256), 1 and 48 streams
         import subprocess
         q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', '0'],
