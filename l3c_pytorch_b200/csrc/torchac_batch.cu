@@ -115,8 +115,8 @@ __global__ void __launch_bounds__(BATCH_THREADS)
         const float scale = (float)(65536 - L);
         uint32_t c[8];
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-            c[q] = (e0 + q < L) ? ((uint32_t)(__float2int_rn(__fmul_rn(acc[q], scale)) + e0 + q) & 0xFFFFu) : 0u;
+        for (int q = 0; q < 8; ++q)     // rounded through 64 bits, as plane_cdf_u16
+            c[q] = (e0 + q < L) ? ((uint32_t)(__float2ll_rn(__fmul_rn(acc[q], scale)) + e0 + q) & 0xFFFFu) : 0u;
 #pragma unroll
         for (int q = 0; q < 8; q += 2) w[q / 2] = c[q] | (c[q + 1] << 16);
     }

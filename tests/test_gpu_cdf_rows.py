@@ -10,8 +10,8 @@ sigmoid itself, MUFU.RCP(1 + MUFU.EX2(u)), whose monotonicity the PTX ISA does n
   float64 1 / (1 + 2^u) is within SIG_ABS, the bound the per-entry budget below uses.
 * Restatement: each entry in float64 from the kernel's own fp32 parameters, with an error budget B for the sigmoid,
   the fma chain and the final multiplication.  Outside a band of width B around a half-integer the entry must equal
-  rint(V) + l; an entry whose terms are all saturated must equal the fp32 in-order sum of pi's, bit for bit.  A CPU
-  self-test pushes a numpy float32 emulation of the kernel to both ends of the sigmoid bound and checks that it stays
+  rint(V) + l (rounded to 64 bits, as the reference's lrintf); an entry whose terms are all saturated or at u = 0
+  (sigma exactly 1/2) must equal the fp32 in-order sum of those terms, bit for bit.  A CPU self-test pushes a numpy float32 emulation of the kernel to both ends of the sigmoid bound and checks that it stays
   inside the budget, and that the band holds only a small share of the entries.
 * Every builder is held to the restatement: dmll_table_kernel (pitch 32 and 256, RGB with R/G coupling, non-RGB
   with C = 1 and 5), its pixel chunks, its tiled variant, the coarse records and dmll_intervals_kernel.
@@ -53,30 +53,48 @@ def f2i_rn(x):
     return r.astype(np.int64)
 
 
+def f2ll_rn(x):
+    """the reference's lrintf (torchac_kernel.cu:20-24; on the device lrint of the float as a double, cvt.rni.s64) on
+    float arrays: round half to even to a 64-bit integer, saturating at +-2^63, NaN -> 0 (INT64_MIN, what some
+    conversions give instead, has the same low 16 bits)"""
+    x = np.asarray(x, np.float64)
+    with np.errstate(invalid='ignore'):
+        r = np.rint(np.where(np.isnan(x), 0.0, x))
+        hi, lo = r >= 2.0 ** 63, r < -2.0 ** 63
+        out = np.where(hi | lo, 0.0, r).astype(np.int64)
+    return np.where(hi, np.iinfo(np.int64).max, np.where(lo, np.iinfo(np.int64).min, out))
+
+
 def u32(t, mu, inv_s):
     """u [R, L, K] exactly as the kernels compute it: f32(f32(t - mu) * inv_s)"""
     with np.errstate(invalid='ignore', over='ignore'):
         return (t[None, :, None] - mu[:, None, :]) * inv_s[:, None, :]
 
 
-def restate(pi, mu, inv_s, t, L, u_rel=0.0):
+def restate(pi, mu, inv_s, t, L, u_rel=0.0, scale=None, rnd=f2ll_rn):
     """pi, mu, inv_s float32 [R, K]; t float32 [>= L] bin edges -> dict of int64 [R, L] arrays:
     lo / hi  the acceptable entries (equal outside the rounding band), already + l and mod 2^16
-    band     entry inside the rounding band;  exact  every term saturated (bit-exact fp32 sum)
+    band     entry inside the rounding band;  exact  every term saturated or at u = 0 (bit-exact fp32 sum)
     and V (float64, before + l).  u_rel > 0: inv_s is known only to that relative precision (recomputed from the
-    log-scale), which widens the budget and makes threshold-straddling terms non-exact."""
-    scale = np.float32(65536 - L)
+    log-scale), which widens the budget and makes threshold-straddling terms non-exact.  An entry is
+    rnd(V) + l mod 2^16 with scale (default 65536 - L) and rnd the reference's rounding to 64 bits; a 32-bit one
+    (f2i_rn) gives the same entries while |V| < 2^31, which holds wherever sum(pi) <= 1."""
+    scale = np.float32(65536 - L if scale is None else scale)
     t = np.asarray(t[:L], np.float32)
     u = u32(t, mu, inv_s)
     lo_s, hi_s = u <= SAT_LO, u >= SAT_HI
     mid = ~(lo_s | hi_s)
+    # sigma(0) is exactly 1/2 (test_sigmoid_sweep), and fma(pi, 1/2, acc) = fp32(acc + pi / 2) unless pi / 2 rounds
+    with np.errstate(invalid='ignore'):
+        zero = (u == 0) & ~((pi != 0) & (np.abs(pi) < np.float32(2.0 ** -125)))[:, None, :]
     l_idx = np.arange(L, dtype=np.int64)[None, :]
-    # bit-exact path: in-order fp32 sum of the pi's saturated low
+    # bit-exact path: in-order fp32 sum of the pi's saturated low and the halves of those at u = 0
     acc32 = np.zeros(u.shape[:2], np.float32)
     with np.errstate(invalid='ignore', over='ignore'):
-        for k in range(K):
-            acc32 = np.where(lo_s[..., k], acc32 + pi[:, None, k], acc32)
-        sat_val = f2i_rn(acc32 * scale) + l_idx
+        for k in range(pi.shape[-1]):
+            acc32 = np.where(lo_s[..., k], acc32 + pi[:, None, k],
+                             np.where(zero[..., k], acc32 + pi[:, None, k] * np.float32(0.5), acc32))
+        sat_val = rnd(acc32 * scale) + l_idx
     # float64 value and budget
     pi64 = pi.astype(np.float64)[:, None, :]
     u64 = u.astype(np.float64)
@@ -104,11 +122,11 @@ def restate(pi, mu, inv_s, t, L, u_rel=0.0):
         B = B * 1.01 + 1e-9
         frac = V - np.floor(V)
         band = np.isfinite(V) & (np.abs(frac - 0.5) <= B)
-    assert not (np.isfinite(B) & (B >= 0.25)).any(), 'budget too wide to decide an entry'
-    r = f2i_rn(V)
-    lo = np.where(band, f2i_rn(np.floor(V)), r) + l_idx
-    hi = np.where(band, f2i_rn(np.ceil(V)), r) + l_idx
-    exact = ~mid.any(-1) & ~straddle
+    exact = ~(mid & ~zero).any(-1) & ~straddle
+    assert not (np.isfinite(B) & (B >= 0.25) & ~exact).any(), 'budget too wide to decide an entry'
+    r = rnd(V)
+    lo = np.where(band, rnd(np.floor(V)), r) + l_idx
+    hi = np.where(band, rnd(np.ceil(V)), r) + l_idx
     lo_raw, hi_raw = np.where(exact, sat_val, lo), np.where(exact, sat_val, hi)     # before the 16-bit wrap
     return dict(lo=lo_raw & 0xFFFF, hi=hi_raw & 0xFFFF, lo_raw=lo_raw, hi_raw=hi_raw, band=band & ~exact,
                 exact=exact, V=V, u=u)
@@ -129,25 +147,28 @@ def check_rows(rows, ref, what, l_idx=None):
                                                                   ref['exact'][r, e]))
     unsat = ~ref['exact']
     n_un = max(int(unsat.sum()), 1)
-    off = unsat & (rows != (f2i_rn(ref['V']) + l_idx) & 0xFFFF)
+    off = unsat & (rows != (f2ll_rn(ref['V']) + l_idx) & 0xFFFF)
     return dict(band=float(ref['band'].sum()) / n_un, off_rint=float(off.sum()) / n_un, unsat=int(unsat.sum()))
 
 
-def emulate(pi, mu, inv_s, t, L, sig_push):
-    """numpy float32 model of mixture_cdf_u16 with the sigmoid replaced by sigma64 + sig_push (each term's push in
-    [-1, 1] x SIG_ABS, rounded to fp32 and kept within SIG_ABS of sigma64): [R, L] entries (+ l, mod 2^16)"""
+def emulate(pi, mu, inv_s, t, L, sig_push, rnd=f2i_rn):
+    """numpy float32 model of mixture_cdf_u16 (rnd = f2ll_rn: plane_cdf_u16) with the sigmoid replaced by
+    sigma64 + sig_push (each term's push in [-1, 1] x SIG_ABS, rounded to fp32 and kept within SIG_ABS of sigma64;
+    exactly 1 at u <= -25 and 1/2 at u = 0): [R, L] entries (+ l, mod 2^16)"""
     scale = np.float32(65536 - L)
     u = u32(np.asarray(t[:L], np.float32), mu, inv_s)
     with np.errstate(invalid='ignore', over='ignore'):
         s64 = 1.0 / (1.0 + np.exp2(u.astype(np.float64)))
         s32 = (s64 + sig_push * SIG_ABS).astype(np.float32)
         s32 = np.where(np.abs(s32 - s64) > SIG_ABS, np.nextafter(s32, s64.astype(np.float32)), s32)
-        s32 = np.where(u <= SAT_LO, np.float32(1), s32)
+        s32 = np.where(s32 > 0, s32, s64.astype(np.float32))          # the sigmoid is positive below u = 40
+        s32 = np.where(u <= SAT_LO, np.float32(1), np.where(u == 0, np.float32(0.5), s32))
         acc = np.zeros(u.shape[:2], np.float32)
-        for k in range(K):
+        for k in range(pi.shape[-1]):
             f = (pi[:, None, k].astype(np.float64) * s32[..., k] + acc.astype(np.float64)).astype(np.float32)
+            f = np.where((u[..., k] <= SAT_LO) | (u[..., k] == 0), acc + pi[:, None, k] * s32[..., k], f)
             acc = np.where(u[..., k] >= SAT_HI, acc, f)
-        return (f2i_rn(acc * scale) + np.arange(L)[None, :]) & 0xFFFF
+        return (rnd(acc * scale) + np.arange(L)[None, :]) & 0xFFFF
 
 
 def inv_s_from_logs(logs):
