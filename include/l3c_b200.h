@@ -140,6 +140,22 @@ int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_streams, in
 int l3c_pack_streams(const l3c_enc_stream_t *streams_dev, const uint32_t *len_dev,
                      const uint64_t *dst_off_dev, int n_streams, uint8_t *blob_dev, void *stream);
 
+/* Assembles the containers of region updates (DESIGN §4.12) in ONE launch from segments seg_host int64 [n_seg][4] =
+ * (src, src_off, dst_off, bytes), copying bytes [src_off, src_off + bytes) of a source to out_dev + dst_off:
+ *   src 0: old_dev (old_bytes long, the uploaded old containers): a run of unchanged streams with their length fields
+ *          and the headers and magics between them;
+ *   src 1: slots_dev (slot_bytes long, the encoder slots of the re-encoded streams): one new stream; its length is
+ *          also written, as a little-endian u32, to the 4 bytes at out_dev + dst_off - 4.
+ * One warp copies each 4 KB chunk of a segment.  The segments and each one's first chunk are copied to seg_dev
+ * (device, 8-byte aligned, (5 * n_seg + 1) * 8 bytes) on `stream` before the launch.  Nothing of out_dev outside the
+ * destinations is written.  Refused before any GPU work (L3C_EINVAL): null pointers, a source other than 0 or 1, a
+ * negative size or (src 1) one of 2^32 bytes or more, a segment outside its source or outside out_dev (length field
+ * included), and destinations that overlap (length fields included; an empty segment of src 0 is the point dst_off and
+ * is refused strictly inside another destination).  n_seg = 0 does nothing. */
+int l3c_splice_streams(const uint8_t *old_dev, int64_t old_bytes, const uint8_t *slots_dev, int64_t slot_bytes,
+                       const int64_t *seg_host, int64_t *seg_dev, int n_seg, uint8_t *out_dev, int64_t out_bytes,
+                       void *stream);
+
 /* intervals_dev[i] = lut_dev[sym_dev[i]], i < n -- coding intervals when all pixels share one CDF row
  * (uniform prior of the coarsest scale, bitcoding.py:171-186). lut entry = c_low | (c_high-1)<<16, 256 entries.
  * intervals_dev must not be sym_dev or lut_dev; n above 2^31 - 1 CTAs of 256 is refused. */
@@ -316,6 +332,19 @@ int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int oy, int ox, 
                             int y0, int x0, int h, int w, int sy, int sx, int Hf, int Wf, const float *targets_dev,
                             int N, int C, int K, int L, int rgb, int th, int tw, uint32_t *intervals_dev,
                             void *stream);
+/* l3c_dmll_intervals_rect with one rectangle per image, for a pass of region updates whose windows differ in shape
+ * (DESIGN §4.12, "Batches of updates"): geo_host int32 [N][10] = (oy, ox, y0, x0, h_n, w_n, sy, sx, Hf, Wf) per image:
+ * the rectangle's origin in image n's parameters (l_dev f32 NHWC [N][Hl][Wl][Kp], a padded batch of decoder outputs),
+ * its origin and size in image n's symbol window (sym_dev uint8 [N][C][Hs][Ws], a padded batch), that window's origin
+ * in image n's Hf x Wf plane and the plane's size.  Image n's intervals go, in the tile order (th x tw, shared) of its
+ * own h_n x w_n rectangle, to its stream planes intervals_dev uint32 [N][C][plane] from element (n * C + c) * plane;
+ * nothing past h_n * w_n of a plane is written.  The geometry is copied to geo_dev (device, 4-byte aligned, N * 40 bytes)
+ * on `stream` before the launch.  Refused before any GPU work (L3C_EINVAL), for any image: what l3c_dmll_intervals_rect
+ * refuses (a rectangle outside the parameters, the symbol window or the plane, or not tile-aligned in the plane; C, K,
+ * L; null pointers), and h_n * w_n > plane.  Bit-identical to l3c_dmll_intervals_rect run on every image alone. */
+int l3c_dmll_intervals_rects(const float *l_dev, int Hl, int Wl, const uint8_t *sym_dev, int Hs, int Ws,
+                             const int *geo_host, int *geo_dev, int plane, const float *targets_dev, int N, int C, int K,
+                             int L, int rgb, int th, int tw, uint32_t *intervals_dev, void *stream);
 
 /* sub_rgb_mean + first MeanShift of RGBHead as one per-pixel 3x3 affine pair
  * (multiscale_network.py:181-183, head.py:31-33): img uint8 [N][3][HW] planes ->

@@ -76,6 +76,8 @@ _SIGNATURES = {
                                     [c_int] * 8 + [c_void_p, c_void_p]),
     'l3c_dmll_intervals_rect': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] + [c_int] * 10 + [c_void_p] + [c_int] * 7 +
                                 [c_void_p, c_void_p]),
+    'l3c_dmll_intervals_rects': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
+                                         c_void_p] + [c_int] * 7 + [c_void_p, c_void_p]),
     'l3c_rgb_prep': (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_split_f16x2': (c_int, [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p]),
     'l3c_rgb_im2col_f16': (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p, c_void_p]),
@@ -91,6 +93,8 @@ _SIGNATURES = {
     'l3c_dmll_build_coarse': (c_int, [c_void_p] * 3 + [c_int] * 7 + [c_void_p, c_void_p]),
     'l3c_ac_decode_streams_coarse': (c_int, [c_void_p, c_int, c_void_p, c_uint32, c_uint32, c_void_p]),
     'l3c_pack_streams': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    'l3c_splice_streams': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_int64,
+                                   c_void_p]),
     'l3c_partition_streams': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_partition_streams2': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_set_conv_launch_limits': (c_int, [c_int, c_int]),

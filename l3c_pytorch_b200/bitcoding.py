@@ -308,6 +308,16 @@ class Bitcoding(object):
         baselines, an empty patch or one not in the image, and a patch that is not 3-channel."""
         return self.codec.update_region(data, pos, patch)
 
+    def update_regions(self, datas, edits):
+        """update_region for many containers and many edits each: edits[i] = [(pos, patch)] for datas[i], applied in
+        list order, so a later patch overwrites an earlier one where they overlap -> the new container bytes in input
+        order, each byte-identical to encoding its decoded image with every patch pasted in order.  An empty edit list
+        returns the container unchanged.  Edits whose windows do not meet are re-encoded from their own windows, the
+        others from the window of their bounding rectangle; every container is parsed and uploaded once and spliced on
+        the GPU (BatchCodec.update_regions, which records what ran in updates_counts).  ValueError, before any GPU
+        work, for every refusal of update_region, naming the container and the edit."""
+        return self.codec.update_regions(datas, edits)
+
 
 class _ListEncodeJob:
     """encode_batch_begin: the codec jobs of its passes (one for a batch tensor); finish() -> (containers, bpsps) in

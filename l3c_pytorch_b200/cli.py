@@ -6,6 +6,10 @@
     python -m l3c_pytorch_b200.cli --config cr_rgb_shared --ckpt CKPT.pt enc IMG OUT.l3c --recursive auto
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png --region Y,X,H,W [--level K]
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt upd IN.l3c PATCH.png Y,X OUT.l3c [--overwrite]
+                                                                  [--edit PATCH2.png Y2,X2 ...]
+
+`upd --edit PATCH.png Y,X` (repeatable) applies more edits after the positional one, in order, in one call that
+re-encodes every tile the edits reach once (DESIGN §4.12, "Batches of updates").
 
 `--ckpt` is a checkpoint as written by the reference's Saver (`torch.save({'net': state_dict})`,
 helpers/saver.py:168); the module tree here has the same parameter names, so it loads strict.
@@ -139,6 +143,9 @@ def build_parser():
     u.add_argument('pos', type=parse_pos, metavar='Y,X')
     u.add_argument('out')
     u.add_argument('--overwrite', action='store_true')
+    u.add_argument('--edit', nargs=2, action='append', default=[], metavar=('PATCH.png', 'Y,X'),
+                   help='one more edit, applied after the positional one and the --edit options before it (all in '
+                        'one Bitcoding.update_regions call); may be repeated')
     return p
 
 
@@ -194,10 +201,11 @@ def decode_region(bc, pin, png_out, region, level=0):
     print('Decoded region {} (level {}) of {} -> {}'.format(region, level, pin, png_out))
 
 
-def update_region(bc, pin, patch_p, pos, pout, overwrite=False):
-    """`upd`: IN.l3c with the pixels at pos replaced by the image PATCH, written to OUT.  ValueError for crop files
-    (`.partN`, an image coded in parts), an existing OUT without --overwrite and what Bitcoding.update_region
-    refuses."""
+def update_region(bc, pin, patch_p, pos, pout, overwrite=False, more=()):
+    """`upd`: IN.l3c with the pixels at pos replaced by the image PATCH, written to OUT; more = [(PATCH, 'Y,X')] (the
+    --edit options): edits applied after it, in order, in one Bitcoding.update_regions call.  ValueError for crop files
+    (`.partN`, an image coded in parts), an existing OUT without --overwrite, a malformed --edit position and what
+    Bitcoding.update_region(s) refuses."""
     from . import part_suffix_helper
     if not os.path.isfile(pin):
         if os.path.isfile(pin + '.part0'):
@@ -211,10 +219,21 @@ def update_region(bc, pin, patch_p, pos, pout, overwrite=False):
         raise ValueError('{} exists. Consider --overwrite.'.format(pout))
     with open(pin, 'rb') as f:
         data = f.read()
-    out = bc.update_region(data, pos, read_image(patch_p))
+    if more:
+        edits = [(pos, read_image(patch_p))]
+        for p, text in more:
+            try:
+                edits.append((parse_pos(text), read_image(p)))
+            except argparse.ArgumentTypeError as err:
+                raise ValueError('--edit %s %s: %s' % (p, text, err))
+        out = bc.update_regions([data], [edits])[0]
+    else:
+        out = bc.update_region(data, pos, read_image(patch_p))
     with open(pout, 'wb') as f:
         f.write(out)
     print('Updated {} at {} with {} -> {}'.format(pin, pos, patch_p, pout))
+    for p, text in more:
+        print('  and at {} with {}'.format(text, p))
 
 
 def main(argv=None):
@@ -228,7 +247,7 @@ def main(argv=None):
             encode(bc, a.img, a.out, a.overwrite)
         elif a.mode == 'upd':
             try:
-                update_region(bc, a.inp, a.patch, a.pos, a.out, a.overwrite)
+                update_region(bc, a.inp, a.patch, a.pos, a.out, a.overwrite, a.edit)
             except ValueError as err:
                 raise EncodeError(str(err))
         elif a.region is not None:

@@ -26,6 +26,7 @@ rectangles coarse to fine, whose streams `region.rect_streams` finds and `_enc_d
 import functools
 import os
 import struct
+import time
 
 import numpy as np
 import torch
@@ -242,6 +243,38 @@ class ContainerLayout(object):
             pos += 4
         return pos, pieces, offs
 
+    def offsets(self, lens):
+        """header_and_offsets' total size and stream offsets, without a loop over the streams: lens int64 [streams] in
+        container order -> (total size, int64 [streams]).  Every stream's bytes follow its 4-byte length; a scale's
+        streams follow its 5-byte header, and its 4-byte magic follows them."""
+        th, tw = self.tile if self.tile is not None else (1 << 30, 1 << 30)
+        per_scale = [C * -(-H // th) * -(-W // tw) for (_, C, H, W) in self.shapes]
+        scale_of = np.repeat(np.arange(len(per_scale), dtype=np.int64), per_scale)
+        lens = np.asarray(lens, np.int64)
+        head = 8 if self.tile is None else 16
+        offs = head + 9 * scale_of + 5 + np.cumsum(lens + 4) - lens
+        return head + 9 * len(per_scale) + int((lens + 4).sum()), offs
+
+
+def splice_segments(old_off, old_len, total_old, new_off, cols, lens, slot_off, src0=0, dst0=0):
+    """The segments of l3c_splice_streams that turn one container into its update: old_off / old_len int64 [streams]
+    where its streams lie in the old container of total_old bytes, new_off the offsets of the new layout
+    (ContainerLayout.offsets), cols the ascending columns of the re-encoded streams, lens their new lengths and
+    slot_off where their bytes lie in the slot buffer.  The old container sits at src0 of the source buffer, the new
+    one at dst0 of the output.  -> int64 [segments][4] (src, src_off, dst_off, bytes): src 0 a run of unchanged streams
+    with everything between them (their headers, scale headers and magics), from the end of the previous re-encoded
+    stream to the length field of the next; src 1 a re-encoded stream, whose length field the kernel writes.  Runs of
+    no bytes are left out."""
+    cols = np.asarray(cols, np.int64)
+    lens = np.asarray(lens, np.int64)
+    a = np.concatenate([[0], old_off[cols] + old_len[cols]])           # run starts in the old container
+    b = np.concatenate([old_off[cols] - 4, [total_old]])               # and ends
+    d = np.concatenate([[0], new_off[cols] + lens])                    # their places in the new one
+    seg = np.zeros((2 * cols.size + 1, 4), np.int64)
+    seg[0::2] = np.stack([np.zeros_like(a), src0 + a, dst0 + d, b - a], 1)
+    seg[1::2] = np.stack([np.ones_like(cols), np.asarray(slot_off, np.int64), dst0 + new_off[cols], lens], 1)
+    return seg[(seg[:, 0] == 1) | (seg[:, 3] > 0)]
+
 
 def container_tile(data):
     """tile size (th, tw) of a tiled container, None for the reference layout."""
@@ -365,6 +398,17 @@ class EncodeJob:
         return datas, info
 
 
+class _UpdateJob(object):
+    """One container of an update_regions call (BatchCodec.plan_updates): its bytes, parse_container's result, tile
+    size, the edits as (y, x, h, w) rectangles and their patches (uint8 [1, 3, h, w] on the device) in list order, the
+    merged plans (region.merge_update_plans) and whether it takes the whole path."""
+    __slots__ = ('data', 'pad_tuple', 'parsed', 'tile', 'rects', 'patches', 'plans', 'whole')
+
+    def __init__(self, data, pad_tuple, parsed, tile, rects, patches, plans, whole):
+        self.data, self.pad_tuple, self.parsed, self.tile = data, pad_tuple, parsed, tile
+        self.rects, self.patches, self.plans, self.whole = rects, patches, plans, whole
+
+
 class BatchCodec(object):
     def __init__(self, blueprint):
         self.blueprint = blueprint
@@ -377,6 +421,11 @@ class BatchCodec(object):
         # what the last update_region call did: streams re-encoded, streams in the container, pixels of the window it
         # encoded and whether it took the whole-image path
         self.update_counts = {'streams': 0, 'total': 0, 'window_pixels': 0, 'whole': False}
+        # one dict per container of the last update_regions call: update_counts' keys and `plans`, the plans after merging
+        self.updates_counts = []
+        # host clock of its stages in ms (tools/bench_update.py): parse and plan, upload, GPU (up to the new stream
+        # lengths on the host), splice (layout, splice launch, copy to the host) and whole-path containers
+        self.updates_stage_ms = {}
 
     # ------------------------------------------------------------------------------------------
     def iter_scale_dmll(self, recursive=0):
@@ -1113,15 +1162,20 @@ class BatchCodec(object):
         regions: (y, x, h, w) each; levels: None (all 0) or one int each.
         lane: as in decode_batch -- the caller has made `lane.main` current; the range decoders run on the lane's
         decoder streams."""
-        from .region import pass_streams, plan_passes
         parsed, plans = self.plan_regions(datas, regions, levels)
         blob, starts = _upload(datas, self.blueprint.device)
-        ragged = REGION_RAGGED_PASS and self.net.windows_unsupported() is None
-        outs = [None] * len(datas)
         self.region_counts = {'streams': 0, 'symbols': 0}          # of this call: every pass adds to them
+        return self._decode_planned(blob, starts, [[st for (_, _, _, st) in p[1]] for p in parsed], plans, lane)
+
+    def _decode_planned(self, blob, starts, streams_of, plans, lane=None):
+        """The region plans of containers uploaded to blob (container n at starts[n], its streams streams_of[n] as
+        parse_container lists them per scale) in passes (region.plan_passes) -> the regions in plan order."""
+        from .region import pass_streams, plan_passes
+        ragged = REGION_RAGGED_PASS and self.net.windows_unsupported() is None
+        outs = [None] * len(plans)
         for idxs, is_ragged in plan_passes(plans, ragged):
             sel = [plans[i] for i in idxs]
-            offs, lens = pass_streams(sel, [[st for (_, _, _, st) in parsed[i][1]] for i in idxs], starts[idxs])
+            offs, lens = pass_streams(sel, [streams_of[i] for i in idxs], np.asarray(starts)[idxs])
             for i, res in zip(idxs, self.decode_region_pass(blob, offs, lens, sel, is_ragged, lane=lane)):
                 outs[i] = res
         return outs
@@ -1345,6 +1399,324 @@ class BatchCodec(object):
         self.update_counts = {'streams': int(cols.size), 'total': plan.total_streams,
                               'window_pixels': plan.window_pixels, 'whole': False}
         return buf.tobytes()
+
+    def plan_updates(self, datas, edits):
+        """Parse, validate and plan every container and edit of an update_regions call, before any GPU work: -> one
+        _UpdateJob per container.  ValueError naming the container (and the edit) for every refusal of update_region."""
+        from .region import merge_update_plans, plan_update
+        if len(edits) != len(datas):
+            raise ValueError('%d edit lists for %d containers' % (len(edits), len(datas)))
+        jobs = []
+        for i, (data, ed) in enumerate(zip(datas, edits)):
+            tile = container_tile(data)
+            if tile is None:
+                raise ValueError('container %d: region update needs a tiled container (written with Bitcoding(..., '
+                                 'tile=(th, tw))): the streams of the reference layout are serial' % i)
+            try:
+                pad_tuple, parsed = parse_container(data)
+                shapes = [(C, H, W) for (C, H, W, _) in parsed]
+                self._check_shapes(shapes)
+            except ValueError as err:
+                raise ValueError('container %d was not written by this model: %s' % (i, err))
+            if self.net._rgb:
+                raise ValueError('container %d: region update is not supported by the RGB baselines: their bicubic '
+                                 'encoder has no planned windows' % i)
+            rects, patches = [], []
+            for j, e in enumerate(ed):
+                try:
+                    if len(e) != 2:
+                        raise ValueError('an edit is (pos, patch), got %d items' % len(e))
+                    pos, patch = e
+                    if len(pos) != 2:
+                        raise ValueError('pos must be (y, x), got %r' % (pos,))
+                    patch = self._update_patch(patch)
+                    rect = (int(pos[0]), int(pos[1])) + tuple(patch.shape[2:])
+                    plan_update(shapes, pad_tuple, tile, self.net, rect)        # its refusals, edit by edit
+                except ValueError as err:
+                    raise ValueError('container %d, edit %d: %s' % (i, j, err))
+                rects.append(rect)
+                patches.append(patch)
+            plans = merge_update_plans(shapes, pad_tuple, tile, self.net, rects)
+            whole = any(p.window_pixels > TILED_ENCODE_BAND_PIXELS for p, _ in plans)
+            jobs.append(_UpdateJob(data, pad_tuple, parsed, tile, rects, patches, plans, whole))
+        return jobs
+
+    @_on_device
+    def update_regions(self, datas, edits):
+        """update_region for many containers and many edits each: edits[i] = [(pos, patch)] for datas[i], applied in
+        list order (a later patch overwrites an earlier one where they overlap) -> the new container bytes in input
+        order, result i byte-identical to encoding decode(datas[i]) with every patch pasted in order (DESIGN §4.12,
+        "Batches of updates").  An empty edit list returns the container unchanged.  The edits of one container are
+        planned (region.merge_update_plans); a container whose merged window exceeds TILED_ENCODE_BAND_PIXELS takes the
+        whole path (decode, paste every patch, encode), the others the window path (_update_windows).  updates_counts:
+        one dict per container, update_counts' keys and `plans`, the number of plans after merging.  ValueError,
+        before any GPU work, for every refusal of update_region, naming the container and the edit."""
+        t0 = time.perf_counter()
+        jobs = self.plan_updates(datas, edits)
+        self.updates_stage_ms = {'parse': (time.perf_counter() - t0) * 1e3, 'upload': 0.0, 'gpu': 0.0, 'splice': 0.0,
+                                 'whole': 0.0}
+        outs, counts, window = [None] * len(jobs), [None] * len(jobs), []
+        for i, job in enumerate(jobs):
+            total = job.plans[0][0].total_streams if job.plans else sum(len(st) for (_, _, _, st) in job.parsed)
+            if not job.plans:
+                outs[i] = bytes(job.data)
+                counts[i] = {'streams': 0, 'total': total, 'window_pixels': 0, 'whole': False, 'plans': 0}
+            elif job.whole:
+                t0 = time.perf_counter()
+                left, _, top, _ = job.pad_tuple
+                img, _ = self.decode_batch([job.data], to_host=False)
+                for (y, x, h, w), patch in zip(job.rects, job.patches):
+                    img[:, :, top + y:top + y + h, left + x:left + x + w] = patch
+                outs[i] = self.encode_batch(img, job.pad_tuple, tile=job.tile)[0][0]
+                counts[i] = {'streams': total, 'total': total, 'window_pixels': img.shape[2] * img.shape[3],
+                             'whole': True, 'plans': len(job.plans)}
+                self.updates_stage_ms['whole'] += (time.perf_counter() - t0) * 1e3
+            else:
+                window.append(i)
+        if window:
+            for i, out, c in zip(window, *self._update_windows([jobs[i] for i in window])):
+                outs[i], counts[i] = out, c
+        self.updates_counts = counts
+        return outs
+
+    def _update_windows(self, jobs):
+        """update_regions' window path (DESIGN §4.12, "Batches of updates") for the jobs of one call -> ([bytes],
+        [counts]).  One upload of the containers, read by the old-pixel decodes and the splice.  The plans are grouped
+        into passes of one tile size whose windows fit TILED_ENCODE_BAND_PIXELS (bitcoding.plan_passes).  Per pass: the
+        old pixels of every window from region passes (_decode_planned), the patches pasted in order, then per plan the
+        encoders and the coding on its windows (_encode_windows, _code_rects) and one range-coder launch for every new
+        stream of the pass.  A stream that two separate plans re-encode is coded once (both give the same bytes).  Then
+        one l3c_splice_streams launch assembles every new container and one copy brings them to the host."""
+        from .region import plan_region, plan_update_passes, rect_streams
+        dev = self.blueprint.device
+        stage, t0 = self.updates_stage_ms, time.perf_counter()
+        blob, starts = _upload([job.data for job in jobs], dev)
+        stage['upload'] = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        geo = self._geometry()
+        # ---- host: every plan's streams (duplicates across a container's plans dropped) and its slot in one buffer
+        items = []
+        for k, job in enumerate(jobs):
+            layout = stream_layout([[s[:3] for s in job.parsed]], job.tile)
+            seen = np.zeros(layout[2].shape[1], bool)
+            for plan, _ in job.plans:
+                keep = {}
+                for sp in plan.scales:
+                    cols, n, elem = rect_streams(layout, sp.idx, sp)
+                    new = ~seen[cols]
+                    seen[cols] = True
+                    ch = np.repeat(np.arange(sp.C), len(sp.tiles))
+                    keep[sp.idx] = (cols[new], n[0][new], elem[0][new], ch[new])
+                items.append((k, plan, keep))
+        caps = _slot_cap(np.concatenate([kp[1] for _, _, keep in items for _, kp in sorted(keep.items())]))
+        slot_off = np.concatenate([[0], np.cumsum(caps)])
+        slots = torch.empty(max(int(slot_off[-1]), 1), dtype=torch.uint8, device=dev)
+        passes = plan_update_passes([plan for _, plan, _ in items], TILED_ENCODE_BAND_PIXELS)
+        first = np.zeros(len(items) + 1, np.int64)          # each plan's first stream in the call's stream order
+        first[1:] = np.cumsum([sum(kp[0].size for kp in keep.values()) for _, _, keep in items])
+        lens_parts = []
+        for ps in passes:
+            # ---- old pixels of every window (the padding is zero), then the patches in order
+            imgs, rplans = [], []
+            for t in ps:
+                k, plan, _ = items[t]
+                job, P = jobs[k], plan.window
+                left, right, top, bottom = job.pad_tuple
+                _, Hf, Wf = job.parsed[-1][:3]
+                u = (max(P[0], top), max(P[1], left), min(P[2], Hf - bottom), min(P[3], Wf - right))
+                rplans.append(plan_region([s[:3] for s in job.parsed], job.pad_tuple, job.tile, geo,
+                                          (u[0] - top, u[1] - left, u[2] - u[0], u[3] - u[1])))
+                imgs.append((u, torch.zeros(1, 3, P[2] - P[0], P[3] - P[1], dtype=torch.uint8, device=dev)))
+            olds = self._decode_planned(blob, starts[[items[t][0] for t in ps]],
+                                        [[st for (_, _, _, st) in jobs[items[t][0]].parsed] for t in ps], rplans)
+            for t, (u, img), old in zip(ps, imgs, olds):
+                k, plan, _ = items[t]
+                job, P = jobs[k], plan.window
+                img[:, :, u[0] - P[0]:u[2] - P[0], u[1] - P[1]:u[3] - P[1]] = old
+                left, _, top, _ = job.pad_tuple
+                for (y, x, h, w), patch in zip(job.rects, job.patches):
+                    e = (y + top, x + left, y + top + h, x + left + w)
+                    c = (max(e[0], P[0]), max(e[1], P[1]), min(e[2], P[2]), min(e[3], P[3]))
+                    if c[0] < c[2] and c[1] < c[3]:
+                        img[:, :, c[0] - P[0]:c[2] - P[0], c[1] - P[1]:c[3] - P[1]] = \
+                            patch[:, :, c[0] - e[0]:c[2] - e[0], c[1] - e[1]:c[3] - e[1]]
+            del olds
+            # ---- encoder phase fine to coarse, coding phase coarse to fine: the whole pass as one ragged batch of
+            # windows where the network runs one, else plan after plan as update_region's window path
+            if self.net.ragged_unsupported() is None:
+                coded = self._code_pass_ragged([items[t][1] for t in ps], [img for _, img in imgs], jobs[items[ps[0]][0]].tile)
+            else:
+                coded = self._code_pass_serial([items[t][1] for t in ps], [img for _, img in imgs],
+                                               [jobs[items[t][0]].tile for t in ps])
+            del imgs
+            descs, order, keep_alive, nxt = [], [], [], {t: first[t] for t in ps}
+            for n, idx, sp, iv, plane in coded:
+                t = ps[n]
+                cols, cnt, elem, ch = items[t][2][idx]
+                if plane is not None:           # image n's planes of a [N][C][plane] batch of interval planes
+                    elem = (n * sp.C + ch) * plane + elem - ch * (sp.rect[2] - sp.rect[0]) * (sp.rect[3] - sp.rect[1])
+                s0 = nxt[t]
+                d = np.zeros(cols.size, dtype=_lib.ENC_STREAM_DTYPE)
+                d['intervals'] = iv.data_ptr() + elem * 4
+                d['n_sym'] = cnt
+                d['out_cap'] = caps[s0:s0 + cols.size]
+                d['out'] = slots.data_ptr() + slot_off[s0:s0 + cols.size]
+                nxt[t] = s0 + cols.size
+                descs.append(d)
+                order.append(np.arange(s0, s0 + cols.size))
+                keep_alive.append(iv)
+            # ---- one range-coder launch for every new stream of the pass
+            desc = np.concatenate(descs)
+            if desc.size:
+                lens_parts.append((np.concatenate(order), E.ac_encode_streams(desc, dev)[1]))
+            del keep_alive, coded
+        # ---- the new stream lengths, in the call's stream order, to the host (the layout depends on them)
+        lens_dev = torch.empty(int(first[-1]), dtype=torch.int32, device=dev)
+        for order, ln in lens_parts:
+            lens_dev[E._to_device_async(order, dev)] = ln
+        lens_h = torch.empty(lens_dev.shape, dtype=torch.int32, pin_memory=True)
+        lens_h.copy_(lens_dev, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        lens = lens_h.numpy().astype(np.int64)
+        _check_lens(lens, caps)
+        stage['gpu'] = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        # ---- splice: every container's segments, one launch, one copy to the host
+        segs, sizes, out_starts, counts, pos = [], [], [], [], 0
+        for k, job in enumerate(jobs):
+            mine = [t for t, it in enumerate(items) if it[0] == k]
+            cols = np.concatenate([kp[0] for t in mine for _, kp in sorted(items[t][2].items())])
+            sl = np.concatenate([np.arange(first[t], first[t + 1]) for t in mine])
+            order = np.argsort(cols, kind='stable')
+            cols, sl = cols[order], sl[order]
+            layout = ContainerLayout([(i, C, H, W) for i, (C, H, W, _) in enumerate(job.parsed)], job.tile)
+            old_len = np.concatenate([np.asarray(st, np.int64).reshape(-1, 2)[:, 1] for (_, _, _, st) in job.parsed])
+            _, old_off = layout.offsets(old_len)
+            new_len = old_len.copy()
+            new_len[cols] = lens[sl]
+            total, new_off = layout.offsets(new_len)
+            segs.append(splice_segments(old_off, old_len, len(job.data), new_off, cols, lens[sl], slot_off[sl],
+                                        starts[k], pos))
+            sizes.append(total)
+            out_starts.append(pos)
+            pos += (total + 15) & ~15
+            counts.append({'streams': int(cols.size), 'total': items[mine[0]][1].total_streams,
+                           'window_pixels': sum(items[t][1].window_pixels for t in mine), 'whole': False,
+                           'plans': len(mine)})
+        out = torch.empty(pos, dtype=torch.uint8, device=dev)
+        E.splice_streams(blob, slots, np.concatenate(segs), out)
+        host = torch.empty(out.shape, dtype=torch.uint8, pin_memory=True)
+        host.copy_(out, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        buf = host.numpy()
+        outs = [buf[s:s + n].tobytes() for s, n in zip(out_starts, sizes)]
+        stage['splice'] = (time.perf_counter() - t0) * 1e3
+        return outs, counts
+
+    def _code_pass_serial(self, plans, imgs, tiles):
+        """The encoders and the coding of the update plans of one pass, plan after plan, on their windows as update_region
+        does (_encode_windows, _code_rects).  imgs[n]: the pixels of plans[n]'s P_0, uint8 [1][3][h][w].  Yields (n, idx,
+        sp, intervals int32 [1][C][h * w] of sp.rect in its tile order, None) as each rectangle's intervals are queued."""
+        for n, (plan, img, tile) in enumerate(zip(plans, imgs, tiles)):
+            walk = []
+            for sp in plan.scales[::-1][:-1]:
+                a = sp.enc
+                D = (a[0] // 2, a[1] // 2, -(-a[2] // 2), -(-a[3] // 2))
+                walk.append((D, [(a, D)]))
+            enc = self._encode_windows(img, plan.window[:2], walk)
+            rects = [(None if sp.window is None else tuple(2 * v for v in sp.window),
+                      [(sp, None if sp.window is None else tuple(2 * v for v in sp.window))]) for sp in plan.scales]
+            for idx, sp, iv in self._code_rects(rects, enc, tile):
+                yield n, idx, sp, iv, None
+            del enc
+
+    def _code_pass_ragged(self, plans, imgs, tile):
+        """_code_pass_serial for a pass of plans of one tile size as ONE ragged batch of their windows (f16: the network
+        runs padded batches of differently sized images, ragged_unsupported).  Fine to coarse, each scale's head and
+        encoder run once on a padded batch of the plans' encoder windows, window n top-left, under ragged_extents
+        (l3c_crop_rects cuts them out of the finer scale's padded batch).  Coarse to fine, each decoder runs once on the
+        plans' decoder windows (get_P_nhwc(windows=)) and l3c_dmll_intervals_rects codes every plan's R_s to its own
+        stream planes; the uniform-prior scale codes each plan's rectangle with lut_intervals in its own tile order.
+        Yields (n, idx, sp, intervals, plane): intervals int32 [N][C][plane] shared by the plans of a scale (plane None:
+        [1][C][h * w] of plan n alone)."""
+        net, dev, N = self.net, self.blueprint.device, len(plans)
+        K = net.config_ms.prob.K
+        by = [{sp.scale: sp for sp in p.scales} for p in plans]
+
+        def rows_dev(rows):
+            return E._to_device_async(np.array(rows, np.int32).reshape(N, -1), dev)
+
+        def size(r):
+            return r[2] - r[0], r[3] - r[1]
+
+        # the scale-0 symbols: every P_0, padded, window n top-left
+        P = [p.window for p in plans]
+        X = torch.zeros(N, 3, max(size(r)[0] for r in P), max(size(r)[1] for r in P), dtype=torch.uint8, device=dev)
+        for n, img in enumerate(imgs):
+            X[n, :, :img.shape[2], :img.shape[3]] = img[0]
+        enc = [([r[:2] for r in P], X, None)]                 # by scale: (origin of window n, symbols, values NHWC)
+        x, xo = X, [r[:2] for r in P]
+        for s in range(net.scales):
+            A = [b[s].enc for b in by]
+            # A window that ends on an odd row or column is one longer in the batch, so that every resolution of the
+            # encoder is an exact half of the one before (E.extents_at).  The window starts on an even row and column
+            # (encoder_rect), and where it ends on an odd one that end is not the plane's edge, whose size is even, so it
+            # ends inside the image: the extra row or column is a zero the single-window run also reads there (its
+            # tensor's border), and it reaches only outputs within the window's planned margins, which the plan never
+            # reads.  Every output the plan reads is the same bits as update_region's.
+            ext = [(h + h % 2, w + w % 2) for h, w in map(size, A)]
+            hp, wp = max(h for h, _ in ext), max(w for _, w in ext)
+            Hx, Wx = (x.shape[1], x.shape[2]) if s > 0 else (x.shape[2], x.shape[3])
+            hc, wc = min(hp, Hx), min(wp, Wx)            # a crop is at most its source; a rounded window may be longer
+            inp = E.crop_rects(x, rows_dev([(a[0] - o[0], a[1] - o[1]) + size(a) for a, o in zip(A, xo)]), hc, wc,
+                               nhwc=s > 0)
+            if (hc, wc) != (hp, wp):
+                grown = inp.new_zeros((N, hp, wp, inp.shape[3]) if s > 0 else (N, inp.shape[1], hp, wp))
+                (grown[:, :hc, :wc] if s > 0 else grown[:, :, :hc, :wc]).copy_(inp)
+                inp = grown
+            with E.ragged_extents(ext, hp, wp):
+                if s == 0:
+                    inp = net._rgb_head_input(inp)
+                    hd = inp if isinstance(inp, E.Act) else net.heads[0](inp)
+                else:
+                    hd = net.heads[s](self._operand_act(inp))
+                eo = net.nets[s].enc(hd)
+            xo = [(a[0] // 2, a[1] // 2) for a in A]
+            enc.append((xo, eo.S.contiguous(), eo.bn_q))
+            if s + 1 < net.scales:
+                x = eo.F.r if E.tensor_core_mode() else eo.F.f
+            del eo, hd, inp
+        F = None                                              # (origins, features) the next finer decoder adds
+        for idx, (scale, dmll, uniform) in enumerate(self.iter_scale_dmll(0)):
+            o, Ssym, _ = enc[scale]
+            sps = [b[scale] for b in by]
+            if uniform:
+                for n, sp in enumerate(sps):
+                    h, w = size(sp.rect)
+                    sym = _crop(Ssym[n:n + 1], o[n], sp.rect, nhwc=False)
+                    yield n, idx, sp, E.reorder_tiles(E.lut_intervals(sym, self._uniform(dmll.L, dev)[0]), h, w, tile,
+                                                      True), None
+                continue
+            ob, _, bq = enc[scale + 1]
+            wins = [sp.window for sp in sps]
+            wsz = [size(w) for w in wins]
+            hm, wm = max(h for h, _ in wsz), max(w for _, w in wsz)
+            win = E.crop_rects(bq, rows_dev([(w[0] - b[0], w[1] - b[1]) + sz for w, b, sz in zip(wins, ob, wsz)]), hm,
+                               wm, nhwc=True)
+            Fw = None
+            if net.fuses(scale):
+                Fw = E.crop_rects(F[1], rows_dev([(w[0] - f[0], w[1] - f[1]) + sz for w, f, sz in zip(wins, F[0], wsz)]),
+                                  hm, wm, nhwc=True)
+            l, Fo = net.get_P_nhwc(scale, win, Fw, windows=wsz if len(set(wsz)) > 1 else None)
+            del win, Fw
+            geo = [sp.out[:2] + (sp.rect[0] - on[0], sp.rect[1] - on[1]) + size(sp.rect) + tuple(on) + (sp.H, sp.W)
+                   for sp, on in zip(sps, o)]
+            iv = E.dmll_intervals_rects(l, Ssym, geo, dmll.targets(dev), sps[0].C, K, dmll.L, dmll.rgb_scale, tile)
+            del l
+            for n, sp in enumerate(sps):
+                yield n, idx, sp, iv, iv.shape[2]
+            F = ([(2 * w[0], 2 * w[1]) for w in wins], Fo.f) if scale >= 1 and net.fuses(scale - 1) else None
+            del Fo
 
     # stage timing of a decode (bench.py / tools): set `codec.stage_events = []` before decode_device,
     # synchronise, then read stage_ms()

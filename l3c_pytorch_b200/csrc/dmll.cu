@@ -33,17 +33,30 @@ constexpr int IV_PIX = 64;   // pixels (= threads) per CTA
 // BAND: the pixels are the tile-aligned rectangle `g` (RectGeom, dmll_math.cuh) of a banded encode or a region update,
 // HW = g.h * g.W; `l` is the window plane the rectangle sits in, the symbols are read from the symbol window and the
 // intervals written in tile order.
-template <int K, bool BAND = false>
+// IMG (with BAND): every image n has its own rectangle, geo[n] = (oy, ox, y0, x0, h, w, ...) (RECTS_GEO ints per
+// image), cut into its own tile grid; HW is then the stride of the stream-order planes (>= h * w) and g.oy, g.ox, g.y0,
+// g.x0, g.h, g.W are unused (l3c_dmll_intervals_rects).
+constexpr int RECTS_GEO = 10;
+template <int K, bool BAND = false, bool IMG = false>
 __global__ void __launch_bounds__(IV_PIX)
 dmll_intervals_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
                       const float *__restrict__ targets, int HW, int C, int L, int rgb,
-                      uint32_t *__restrict__ intervals, const RectGeom g = RectGeom()) {
+                      uint32_t *__restrict__ intervals, const RectGeom g_arg = RectGeom(),
+                      const int *__restrict__ geo = nullptr) {
     extern __shared__ float sm[];
     const int Kp = (rgb ? 4 : 3) * C * K;
     const int pitch = Kp + 1;                       // odd pitch: conflict-free column walks
     const int n = blockIdx.y;
     const int p0 = blockIdx.x * IV_PIX;
-    const int np = min(IV_PIX, HW - p0);
+    RectGeom g = g_arg;
+    int npix = HW;
+    if constexpr (IMG) {
+        const int *gn = geo + (size_t)n * RECTS_GEO;
+        g.oy = gn[0], g.ox = gn[1], g.y0 = gn[2], g.x0 = gn[3], g.h = gn[4], g.W = gn[5];
+        npix = g.h * g.W;
+    }
+    const int np = min(IV_PIX, npix - p0);
+    if (IMG && np <= 0) return;                        // past this image's rectangle (uniform per CTA)
     if constexpr (BAND) {
         for (int i = threadIdx.x; i < np * Kp; i += IV_PIX) {
             const int j = i / Kp, pb = p0 + j, py = pb / g.W;
@@ -753,6 +766,59 @@ extern "C" int l3c_dmll_intervals_rect(const float *l_dev, int Hl, int Wl, int o
     dmll_intervals_kernel<10, true><<<grid, IV_PIX, smem, (cudaStream_t)stream>>>(
         l_dev, sym_dev, targets_dev, h * w, C, L, rgb, intervals_dev, g);
     L3C_LAUNCH_CHECK("dmll_intervals_rect_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_intervals_rects(const float *l_dev, int Hl, int Wl, const uint8_t *sym_dev, int Hs, int Ws,
+                                        const int *geo_host, int *geo_dev, int plane, const float *targets_dev, int N,
+                                        int C, int K, int L, int rgb, int th, int tw, uint32_t *intervals_dev,
+                                        void *stream) {
+    using namespace l3c;
+    if (int e = check_common("l3c_dmll_intervals_rects", N, plane, C, K, L, rgb)) return e;
+    L3C_REQUIRE(l_dev && sym_dev && targets_dev && intervals_dev && geo_host && geo_dev,
+                "l3c_dmll_intervals_rects: null pointer");
+    L3C_REQUIRE(th >= 1 && tw >= 1 && Hl >= 1 && Wl >= 1 && Hs >= 1 && Ws >= 1,
+                "l3c_dmll_intervals_rects: tile %dx%d, %dx%d parameter plane, %dx%d symbol plane", th, tw, Hl, Wl, Hs,
+                Ws);
+    L3C_REQUIRE(((uintptr_t)geo_dev & 3) == 0, "l3c_dmll_intervals_rects: geo_dev must be 4-byte aligned");
+    int max_hw = 0;
+    for (int n = 0; n < N; ++n) {
+        const int *g = geo_host + (size_t)n * RECTS_GEO;
+        const int oy = g[0], ox = g[1], y0 = g[2], x0 = g[3], h = g[4], w = g[5], sy = g[6], sx = g[7], Hf = g[8],
+                  Wf = g[9];
+        L3C_REQUIRE(h >= 1 && w >= 1 && (int64_t)h * w <= plane,
+                    "l3c_dmll_intervals_rects: image %d: %dx%d rectangle, planes of %d", n, h, w, plane);
+        L3C_REQUIRE(oy >= 0 && ox >= 0 && (int64_t)oy + h <= Hl && (int64_t)ox + w <= Wl,
+                    "l3c_dmll_intervals_rects: image %d: %dx%d rectangle at (%d, %d) outside the %dx%d parameter plane",
+                    n, h, w, oy, ox, Hl, Wl);
+        L3C_REQUIRE(y0 >= 0 && x0 >= 0 && (int64_t)y0 + h <= Hs && (int64_t)x0 + w <= Ws,
+                    "l3c_dmll_intervals_rects: image %d: %dx%d rectangle at (%d, %d) outside the %dx%d symbol plane", n,
+                    h, w, y0, x0, Hs, Ws);
+        L3C_REQUIRE(sy >= 0 && sx >= 0 && (int64_t)sy + y0 + h <= Hf && (int64_t)sx + x0 + w <= Wf,
+                    "l3c_dmll_intervals_rects: image %d: symbol window at (%d, %d) puts the rectangle outside the %dx%d "
+                    "plane", n, sy, sx, Hf, Wf);
+        const int ry = sy + y0, rx = sx + x0;
+        L3C_REQUIRE(ry % th == 0 && rx % tw == 0 && ((ry + h) % th == 0 || ry + h == Hf) &&
+                        ((rx + w) % tw == 0 || rx + w == Wf),
+                    "l3c_dmll_intervals_rects: image %d: %dx%d rectangle at (%d, %d) of a %dx%d plane is not aligned to "
+                    "%dx%d tiles", n, h, w, ry, rx, Hf, Wf, th, tw);
+        max_hw = h * w > max_hw ? h * w : max_hw;
+    }
+    const int Kp = (rgb ? 4 : 3) * C * K;
+    const size_t smem = (size_t)IV_PIX * (Kp + 1) * sizeof(float);
+    L3C_REQUIRE(smem <= 48 * 1024, "l3c_dmll_intervals_rects: Kp=%d too large", Kp);
+    cudaStream_t st = (cudaStream_t)stream;
+    // from pageable memory: returns once geo_host has been read, so the caller may free it
+    L3C_REQUIRE(cudaMemcpyAsync(geo_dev, geo_host, (size_t)N * RECTS_GEO * sizeof(int), cudaMemcpyHostToDevice, st) ==
+                    cudaSuccess, "l3c_dmll_intervals_rects: geometry upload failed");
+    RectGeom g;
+    g.sym_hw = (long long)Hs * Ws; g.l_hw = (long long)Hl * Wl;
+    g.y0 = 0; g.h = 0; g.W = 0; g.Wl = Wl; g.oy = 0; g.ox = 0; g.th = th; g.tw = tw;
+    g.x0 = 0; g.Ws = Ws;
+    dim3 grid(ceil_div(max_hw, IV_PIX), N);
+    dmll_intervals_kernel<10, true, true><<<grid, IV_PIX, smem, st>>>(
+        l_dev, sym_dev, targets_dev, plane, C, L, rgb, intervals_dev, g, geo_dev);
+    L3C_LAUNCH_CHECK("dmll_intervals_rects_kernel");
     return L3C_OK;
 }
 

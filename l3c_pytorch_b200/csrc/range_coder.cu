@@ -1329,6 +1329,35 @@ __global__ void pack_streams_kernel(const l3c_enc_stream_t *__restrict__ streams
     }
 }
 
+// splice of region updates: one warp per chunk of SPLICE_CHUNK bytes of a segment, so a segment of one short stream
+// takes one warp and a long run of unchanged streams many.  seg = the n_seg segments [n_seg][4] followed by chunk0
+// [n_seg + 1], the first chunk of every segment (a prefix sum; chunk0[n_seg] = all chunks); a segment of src 1 has at
+// least one chunk, whose warp also writes its length field.
+constexpr int SPLICE_CHUNK = 4096;
+constexpr int SPLICE_THREADS = 256;
+__global__ void __launch_bounds__(SPLICE_THREADS)
+splice_streams_kernel(const int64_t *__restrict__ seg, int n_seg, const uint8_t *__restrict__ old,
+                      const uint8_t *__restrict__ slots, uint8_t *__restrict__ out) {
+    const int64_t *chunk0 = seg + 4 * (int64_t)n_seg;
+    const int64_t total = chunk0[n_seg];
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (SPLICE_THREADS / 32);
+    for (int64_t w = (int64_t)blockIdx.x * (SPLICE_THREADS / 32) + (threadIdx.x >> 5); w < total; w += warps) {
+        int lo = 0, hi = n_seg - 1;                    // the segment s with chunk0[s] <= w < chunk0[s + 1]
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (chunk0[mid] <= w) lo = mid; else hi = mid - 1;
+        }
+        const int64_t kind = seg[4 * lo], n = seg[4 * lo + 3];
+        const int64_t b0 = (w - chunk0[lo]) * SPLICE_CHUNK, b1 = min(b0 + SPLICE_CHUNK, n);
+        const uint8_t *src = (kind ? slots : old) + seg[4 * lo + 1];
+        uint8_t *dst = out + seg[4 * lo + 2];
+        if (kind && b0 == 0 && lane < 4)                  // the new stream's u32 length, little-endian
+            dst[lane - 4] = (uint8_t)((uint64_t)n >> (8 * lane));
+        for (int64_t i = b0 + lane; i < b1; i += 32) dst[i] = src[i];
+    }
+}
+
 // intervals from a shared 256-entry LUT (uniform prior: every pixel has the same CDF row)
 __global__ void lut_intervals_kernel(const uint8_t *__restrict__ sym, const uint32_t *__restrict__ lut,
                                      int64_t n, uint32_t *__restrict__ iv) {
@@ -1528,6 +1557,56 @@ extern "C" int l3c_pack_streams(const l3c_enc_stream_t *streams_dev, const uint3
                                                                      dst_off_dev + first, blob_dev);
         L3C_LAUNCH_CHECK("pack_streams_kernel");
     }
+    return L3C_OK;
+}
+
+extern "C" int l3c_splice_streams(const uint8_t *old_dev, int64_t old_bytes, const uint8_t *slots_dev,
+                                  int64_t slot_bytes, const int64_t *seg_host, int64_t *seg_dev, int n_seg,
+                                  uint8_t *out_dev, int64_t out_bytes, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(n_seg >= 0, "l3c_splice_streams: %d segments", n_seg);
+    if (n_seg == 0) return L3C_OK;
+    L3C_REQUIRE(old_dev && slots_dev && seg_host && seg_dev && out_dev, "l3c_splice_streams: null pointer");
+    L3C_REQUIRE(((uintptr_t)seg_dev & 7) == 0, "l3c_splice_streams: seg_dev must be 8-byte aligned");
+    // every destination, a new stream's length field included, as [begin, end) for the overlap check
+    std::vector<std::pair<int64_t, int64_t>> dst(n_seg);
+    for (int s = 0; s < n_seg; ++s) {
+        const int64_t kind = seg_host[4 * s], so = seg_host[4 * s + 1], d = seg_host[4 * s + 2], n = seg_host[4 * s + 3];
+        const int64_t src_bytes = kind ? slot_bytes : old_bytes;
+        L3C_REQUIRE(kind == 0 || kind == 1, "l3c_splice_streams: segment %d has source %lld", s, (long long)kind);
+        L3C_REQUIRE(n >= 0 && (kind == 0 || n <= 0xffffffffll), "l3c_splice_streams: segment %d of %lld bytes", s,
+                    (long long)n);
+        L3C_REQUIRE(so >= 0 && so <= src_bytes - n, "l3c_splice_streams: segment %d reads [%lld, %lld) of a %lld-byte "
+                    "source", s, (long long)so, (long long)(so + n), (long long)src_bytes);
+        L3C_REQUIRE(d - 4 * kind >= 0 && d <= out_bytes - n, "l3c_splice_streams: segment %d writes [%lld, %lld) of a "
+                    "%lld-byte output", s, (long long)(d - 4 * kind), (long long)(d + n), (long long)out_bytes);
+        dst[s] = {d - 4 * kind, d + n};
+    }
+    // chunks of every segment, appended to the segments for the kernel
+    std::vector<int64_t> buf(seg_host, seg_host + 4 * (size_t)n_seg);
+    buf.resize(5 * (size_t)n_seg + 1);
+    int64_t chunks = 0;
+    for (int s = 0; s < n_seg; ++s) {
+        buf[4 * (size_t)n_seg + s] = chunks;
+        const int64_t n = seg_host[4 * s + 3];
+        chunks += n > 0 ? (n + SPLICE_CHUNK - 1) / SPLICE_CHUNK : seg_host[4 * s];
+    }
+    buf[5 * (size_t)n_seg] = chunks;
+    std::sort(dst.begin(), dst.end());
+    for (int s = 1; s < n_seg; ++s)
+        L3C_REQUIRE(dst[s].first >= dst[s - 1].second, "l3c_splice_streams: destinations [%lld, %lld) and [%lld, %lld) "
+                    "overlap", (long long)dst[s - 1].first, (long long)dst[s - 1].second, (long long)dst[s].first,
+                    (long long)dst[s].second);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (chunks == 0) return L3C_OK;                        // every segment empty
+    // from pageable memory: returns once buf has been read, so it may be freed
+    L3C_REQUIRE(cudaMemcpyAsync(seg_dev, buf.data(), buf.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) ==
+                    cudaSuccess, "l3c_splice_streams: segment upload failed");
+    const int64_t blocks = (chunks + SPLICE_THREADS / 32 - 1) / (SPLICE_THREADS / 32);
+    splice_streams_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), SPLICE_THREADS, 0, st>>>(seg_dev, n_seg,
+                                                                                                old_dev, slots_dev,
+                                                                                                out_dev);
+    L3C_LAUNCH_CHECK("splice_streams_kernel");
     return L3C_OK;
 }
 

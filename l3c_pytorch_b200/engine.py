@@ -1017,6 +1017,24 @@ def dmll_intervals_rect(l, oy, ox, sym, rect, targets, C, K, L, rgb, tile, origi
     return iv
 
 
+def dmll_intervals_rects(l, sym, geo, targets, C, K, L, rgb, tile, plane=None, out=None):
+    """dmll_intervals_rect with one rectangle per image (l3c_dmll_intervals_rects): geo int32 [N][10] = (oy, ox, y0, x0,
+    h, w, sy, sx, Hf, Wf) per image, l NHWC [N,Hl,Wl,Kp] and sym uint8 [N,C,Hs,Ws] padded batches -> intervals int32
+    [N,C,plane] (plane default: the largest h * w), image n's in the tile order of its own h x w rectangle."""
+    N, Hl, Wl, _ = l.shape
+    geo = np.ascontiguousarray(geo, np.int32).reshape(N, 10)
+    plane = int((geo[:, 4].astype(np.int64) * geo[:, 5]).max()) if plane is None else int(plane)
+    assert l.is_contiguous() and l.dtype == torch.float32
+    assert sym.dtype == torch.uint8 and sym.is_contiguous() and tuple(sym.shape[:2]) == (N, C)
+    iv = _band_out(out, N, C, plane, l.device)
+    geo_dev = torch.empty(geo.shape, dtype=torch.int32, device=l.device)
+    check(lib.l3c_dmll_intervals_rects(_ptr(l), Hl, Wl, _ptr(sym), sym.shape[2], sym.shape[3],
+                                       geo.ctypes.data_as(ctypes.c_void_p), _ptr(geo_dev), plane, _ptr(targets), N, C,
+                                       K, L, int(rgb), tile[0], tile[1], _ptr(iv), _stream_ptr()))
+    LAUNCHES['n'] += 1
+    return iv
+
+
 def dmll_sample(l, u_sel, u_x, C, K, rgb):
     """l NHWC [N,H,W,Kp]; u_sel f32 [N,C,K,H,W]; u_x f32 [N,C,H,W] -> sampled values f32 [N,C,H,W]."""
     N, H, W, _ = l.shape
@@ -1065,6 +1083,17 @@ def pack_streams(desc_dev, lens_dev, dst_off_np, n, blob):
     off = _to_device_async(dst_off_np.astype(np.int64), blob.device)
     check(lib.l3c_pack_streams(_ptr(desc_dev), _ptr(lens_dev), _ptr(off), n, _ptr(blob), _stream_ptr()))
     LAUNCHES['n'] += -(-n // 65535)                 # one launch per 65535 streams
+
+
+def splice_streams(old, slots, seg, out):
+    """l3c_splice_streams: the segments seg int64 [n][4] (codec.splice_segments) from the uint8 device buffers old and
+    slots into out, in one launch."""
+    seg = np.ascontiguousarray(seg, np.int64).reshape(-1, 4)
+    seg_dev = torch.empty(5 * seg.shape[0] + 1, dtype=torch.int64, device=out.device)
+    check(lib.l3c_splice_streams(_ptr(old), old.numel(), _ptr(slots), slots.numel(),
+                                 seg.ctypes.data_as(ctypes.c_void_p), _ptr(seg_dev), seg.shape[0], _ptr(out),
+                                 out.numel(), _stream_ptr()))
+    LAUNCHES['n'] += int(seg.shape[0] > 0)
 
 
 COARSE_PITCH = 96     # uint16 per coarse record (l3c_dmll_build_coarse)

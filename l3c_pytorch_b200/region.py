@@ -520,3 +520,54 @@ def plan_update(shapes, pad_tuple, tile, config, rect):
                                   window=win[s], out=out[s], fused=fused[s], need=need[s], enc=enc[s]))
     total = sum(C * len(tile_grid(H, W, tile)) for (C, H, W) in shapes)
     return UpdatePlan(scales, E[0], tile, total)
+
+
+def _meets(a, b):
+    return a[0] < b[2] and b[0] < a[2] and a[1] < b[3] and b[1] < a[3]
+
+
+def plans_conflict(a, b):
+    """Whether two update plans of one container must be merged (DESIGN §4.12, "Batches of updates"): the edit E_0 of
+    one meets the pixel window P_0 of the other, so the pixels one plan encodes are not the old ones."""
+    return _meets(a.edit, b.window) or _meets(b.edit, a.window)
+
+
+def merge_update_plans(shapes, pad_tuple, tile, config, rects):
+    """The update plans of several edits rects = [(y, x, h, w)] of one container (plan_update's arguments otherwise):
+    one plan per edit, then any two conflicting plans (plans_conflict) replaced by the plan of the bounding rectangle of
+    their edits, until no two conflict.  -> [(UpdatePlan, [indices into rects, ascending])], ordered by their first
+    edit.  Plans that stay separate are exact on their own: a plan's streams depend only on the pixels of its P_0, which
+    no other plan's edit touches."""
+    left, _, top, _ = (int(v) for v in pad_tuple)
+    plans = [(plan_update(shapes, pad_tuple, tile, config, r), [i]) for i, r in enumerate(rects)]
+    merged = True
+    while merged:
+        merged = False
+        for a in range(len(plans)):
+            for b in range(a + 1, len(plans)):
+                if plans_conflict(plans[a][0], plans[b][0]):
+                    e = _union(plans[a][0].edit, plans[b][0].edit)
+                    plan = plan_update(shapes, pad_tuple, tile, config,
+                                       (e[0] - top, e[1] - left, e[2] - e[0], e[3] - e[1]))
+                    plans[a] = (plan, sorted(plans[a][1] + plans[b][1]))
+                    del plans[b]
+                    merged = True
+                    break
+            if merged:
+                break
+    return plans
+
+
+def plan_update_passes(plans, budget):
+    """How BatchCodec.update_regions groups update plans (of any containers) into passes: -> [[indices into plans]],
+    plans of one tile size per pass, grouped by bitcoding.plan_passes over their P_0 shapes so that a pass's padded
+    windows hold at most `budget` pixels (a window larger than that is a pass of its own)."""
+    from .bitcoding import plan_passes
+    by_tile = {}
+    for i, p in enumerate(plans):
+        by_tile.setdefault(p.tile, []).append(i)
+    passes = []
+    for idxs in by_tile.values():
+        shapes = [(plans[i].window[2] - plans[i].window[0], plans[i].window[3] - plans[i].window[1]) for i in idxs]
+        passes += [[idxs[j] for j in grp] for grp in plan_passes(shapes, budget)]
+    return passes
