@@ -156,6 +156,53 @@ int l3c_splice_streams(const uint8_t *old_dev, int64_t old_bytes, const uint8_t 
                        const int64_t *seg_host, int64_t *seg_dev, int n_seg, uint8_t *out_dev, int64_t out_bytes,
                        void *stream);
 
+/* Layout and splice of region updates whose new stream lengths stay in device memory (DESIGN §4.12, "Serving
+ * updates").  One stream of a container, in container stream order: */
+typedef struct {
+    int64_t fixed_off;          /* its offset if every stream of the container had length 0                    */
+    int64_t old_off, old_len;   /* where its bytes lie in the old container                                    */
+    int64_t src;                /* -1: unchanged; else index i into the call's new lengths, slot_off and caps  */
+} l3c_update_stream_t;
+
+/* One container of the call (all int64): */
+typedef struct {
+    int64_t first_stream, n_streams;  /* its streams: streams_dev[first_stream, first_stream + n_streams)          */
+    int64_t fixed_total;              /* its size if every stream had length 0                                     */
+    int64_t old_base, old_bytes;      /* the old container at old_dev + old_base, old_bytes long                   */
+    int64_t out_base, out_cap;        /* the new one goes to out_dev + out_base and may take up to out_cap bytes    */
+    int64_t first_seg, n_new;         /* its n_new re-encoded streams; its 2 n_new + 1 segments at seg_dev +        */
+                                      /* 4 first_seg, their chunk prefix at chunk0_dev + first_seg + (its index)   */
+} l3c_update_container_t;
+
+/* One CTA per container.  len[s] = old_len[s] for an unchanged stream, new_len_dev[src] for a re-encoded one;
+ * new_off[s] = fixed_off[s] + exclusive_scan(len)[s] and the size is fixed_total + sum(len).  Writes the size to
+ * info_dev[k] and the container's segments in the form of l3c_splice_streams, int64 [2 n_new + 1][4] =
+ * (src, src_off, dst_off, bytes): segment 0 the run of the old container before the first re-encoded stream's
+ * length field, then per re-encoded stream j (ascending) its new bytes (src 1, from slot_off_dev[src] of the slots,
+ * to out_base + new_off) and the run of the old container after it (src 0, up to the next re-encoded stream's length
+ * field or the end).  Runs may be empty.  Offsets are absolute: src_off in the old buffer or the slots, dst_off in the
+ * output.  chunk0_dev gets, per container, the exclusive prefix over its segments of l3c_splice_streams_dev's chunks
+ * (one per 4 KB of a segment, at least one for src 1) and their total; a container with an error gets no chunks.
+ * info_dev[n_containers] is an error flag, zeroed on `stream` first: bit 0 a new length above its cap (the coder
+ * clamps its writes to out_cap), bit 1 an inconsistent input (a descriptor outside the arrays, a source index out of
+ * range, re-encoded streams other than n_new, a size above out_cap).  L3C_EINVAL for null pointers or negative
+ * counts, before any GPU work; n_containers = 0 only clears the flag. */
+int l3c_update_layout(const l3c_update_container_t *conts_dev, int n_containers,
+                      const l3c_update_stream_t *streams_dev, int64_t n_streams, const int32_t *new_len_dev,
+                      const int64_t *slot_off_dev, const int64_t *caps_dev, int64_t n_new,
+                      int64_t *seg_dev, int64_t *chunk0_dev, int64_t n_seg, int64_t *info_dev, void *stream);
+
+/* The splice of l3c_splice_streams from the segments l3c_update_layout left in device memory: one warp per 4 KB
+ * chunk, grid rows over the containers.  Each segment is checked in the kernel: source 0 or 1, its bytes inside its
+ * container's old bytes (src 0) or the slots (src 1, below 2^32), its destination, length field included, inside the
+ * container's [out_base, out_base + out_cap) and out_dev.  A segment that fails is not copied and sets bit 1 of
+ * *flag_dev.  n_seg: the segments of seg_dev (a container whose segments fall outside them is skipped).  max_chunks: the most chunks a container can have (sizes the grid; any value is correct).  L3C_EINVAL
+ * for null pointers or negative counts. */
+int l3c_splice_streams_dev(const l3c_update_container_t *conts_dev, int n_containers, const int64_t *seg_dev,
+                           const int64_t *chunk0_dev, int64_t n_seg, const uint8_t *old_dev, int64_t old_bytes,
+                           const uint8_t *slots_dev, int64_t slot_bytes, uint8_t *out_dev, int64_t out_bytes,
+                           int64_t max_chunks, int64_t *flag_dev, void *stream);
+
 /* intervals_dev[i] = lut_dev[sym_dev[i]], i < n -- coding intervals when all pixels share one CDF row
  * (uniform prior of the coarsest scale, bitcoding.py:171-186). lut entry = c_low | (c_high-1)<<16, 256 entries.
  * intervals_dev must not be sym_dev or lut_dev; n above 2^31 - 1 CTAs of 256 is refused. */

@@ -37,6 +37,11 @@ PRECISIONS = {'fp32': PREC_FP32, 'tf32': PREC_TF32, 'f16': PREC_F16, 'f16x2': PR
 ENC_STREAM_DTYPE = [('intervals', '<u8'), ('out', '<u8'), ('n_sym', '<u4'), ('out_cap', '<u4')]
 DEC_STREAM_DTYPE = [('table', '<u8'), ('in', '<u8'), ('sym_out', '<u8'), ('state', '<u8'),
                     ('row_pitch', '<i8'), ('n_sym', '<u4'), ('in_len', '<u4')]
+# l3c_update_stream_t / l3c_update_container_t (l3c_update_layout)
+UPDATE_STREAM_DTYPE = [('fixed_off', '<i8'), ('old_off', '<i8'), ('old_len', '<i8'), ('src', '<i8')]
+UPDATE_CONTAINER_DTYPE = [('first_stream', '<i8'), ('n_streams', '<i8'), ('fixed_total', '<i8'), ('old_base', '<i8'),
+                          ('old_bytes', '<i8'), ('out_base', '<i8'), ('out_cap', '<i8'), ('first_seg', '<i8'),
+                          ('n_new', '<i8')]
 # l3c_code_src_t (section F)
 CODE_SRC_DTYPE = [('table', '<u8'), ('targets', '<u8'), ('means', '<u8'), ('log_scales', '<u8'), ('probs', '<u8'),
                   ('sym', '<u8'), ('n_sym', '<i8'), ('Lp', '<i4'), ('K', '<i4')]
@@ -95,6 +100,10 @@ _SIGNATURES = {
     'l3c_pack_streams': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'l3c_splice_streams': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_int64,
                                    c_void_p]),
+    'l3c_update_layout': (c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                  c_void_p, c_int64, c_void_p, c_void_p]),
+    'l3c_splice_streams_dev': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p,
+                                       c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     'l3c_partition_streams': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_partition_streams2': (c_int, [c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'l3c_set_conv_launch_limits': (c_int, [c_int, c_int]),

@@ -318,6 +318,15 @@ class Bitcoding(object):
         work, for every refusal of update_region, naming the container and the edit."""
         return self.codec.update_regions(datas, edits)
 
+    def update_regions_begin(self, datas, edits, lane=None):
+        """update_regions without a host wait until job.finish(), which returns the same bytes (DESIGN §4.12, "Serving
+        updates").  The parse, the plan and every ValueError of update_regions happen here, before any GPU work; the
+        rest is queued on the current stream and the new containers are laid out and spliced on the GPU.  job.counts
+        holds the call's per-container statistics.  lane: one of decode_lanes(...), as in decode_regions -- the caller
+        has made `lane.main` current, and the old-pixel decodes use the lane's decoder streams, so updates run beside
+        the region decodes and decode_batch calls of other lanes."""
+        return self.codec.update_regions_begin(datas, edits, lane=lane)
+
 
 class _ListEncodeJob:
     """encode_batch_begin: the codec jobs of its passes (one for a batch tensor); finish() -> (containers, bpsps) in

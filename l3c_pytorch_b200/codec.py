@@ -44,7 +44,7 @@ def _on_device(fn):
     Blueprint(device='cuda:1') must not depend on the caller having called torch.cuda.set_device(1)."""
     @functools.wraps(fn)
     def wrapped(self, *a, **kw):
-        dev = self.codec.blueprint.device if isinstance(self, EncodeJob) else self.blueprint.device
+        dev = self.codec.blueprint.device if isinstance(self, (EncodeJob, UpdateJob)) else self.blueprint.device
         if dev.type != 'cuda':
             return fn(self, *a, **kw)
         with torch.cuda.device(dev):
@@ -276,6 +276,32 @@ def splice_segments(old_off, old_len, total_old, new_off, cols, lens, slot_off, 
     return seg[(seg[:, 0] == 1) | (seg[:, 3] > 0)]
 
 
+def update_layout_inputs(containers, caps):
+    """The inputs of l3c_update_layout for the containers of an update call, from what the host knows before the new
+    stream lengths exist.  containers: per container (scales, tile, old_base, old_bytes, cols, src): parse_container's
+    scales and the tile size, where the old container lies in the uploaded buffer and its size, the ascending columns of
+    its re-encoded streams and each one's index into the call's new lengths and caps (int64).  Each new container is
+    given an upper bound of its size, old_bytes + sum(caps[src] - old length), rounded up to 16, and they follow one
+    another in the output in input order.  -> (containers UPDATE_CONTAINER_DTYPE, streams UPDATE_STREAM_DTYPE, int64
+    output offset of every container, output bytes)."""
+    conts = np.zeros(len(containers), _lib.UPDATE_CONTAINER_DTYPE)
+    streams, starts = [], np.zeros(len(containers), np.int64)
+    pos = first = seg = 0
+    for k, (scales, tile, base, nbytes, cols, src) in enumerate(containers):
+        old = np.concatenate([np.asarray(st, np.int64).reshape(-1, 2) for (_, _, _, st) in scales])
+        fixed_total, fixed_off = ContainerLayout([(i, C, H, W) for i, (C, H, W, _) in enumerate(scales)],
+                                                 tile).offsets(np.zeros(len(old), np.int64))
+        d = np.zeros(len(old), _lib.UPDATE_STREAM_DTYPE)
+        d['fixed_off'], d['old_off'], d['old_len'], d['src'] = fixed_off, old[:, 0], old[:, 1], -1
+        d['src'][cols] = src
+        cap = (nbytes + int((np.asarray(caps, np.int64)[src] - old[cols, 1]).sum()) + 15) & ~15
+        conts[k] = (first, len(old), fixed_total, base, nbytes, pos, cap, seg, len(cols))
+        streams.append(d)
+        starts[k] = pos
+        pos, first, seg = pos + cap, first + len(old), seg + 2 * len(cols) + 1
+    return conts, np.concatenate(streams) if streams else np.zeros(0, _lib.UPDATE_STREAM_DTYPE), starts, pos
+
+
 def container_tile(data):
     """tile size (th, tw) of a tiled container, None for the reference layout."""
     if len(data) >= 16 and bytes(data[8:12]) == TILED_MAGIC:
@@ -407,6 +433,62 @@ class _UpdateJob(object):
     def __init__(self, data, pad_tuple, parsed, tile, rects, patches, plans, whole):
         self.data, self.pad_tuple, self.parsed, self.tile = data, pad_tuple, parsed, tile
         self.rects, self.patches, self.plans, self.whole = rects, patches, plans, whole
+
+
+def _host_counts(job):
+    """updates_counts of a container whose edit list is empty or that takes the whole path (_UpdateJob)."""
+    total = job.plans[0][0].total_streams if job.plans else sum(len(st) for (_, _, _, st) in job.parsed)
+    if not job.plans:
+        return {'streams': 0, 'total': total, 'window_pixels': 0, 'whole': False, 'plans': 0}
+    _, H, W = job.parsed[-1][:3]
+    return {'streams': total, 'total': total, 'window_pixels': H * W, 'whole': True, 'plans': len(job.plans)}
+
+
+class _WindowWork(object):
+    """What BatchCodec._enqueue_windows queued for the window path of an update call."""
+    __slots__ = ('blob', 'starts', 'upload_ms', 't_enqueue', 'keep', 'caps', 'slot_off', 'slots', 'lens_dev', 'cols',
+                 'sl', 'counts')
+
+
+class UpdateJob(object):
+    """An update_regions call in flight (BatchCodec.update_regions_begin).  counts: one dict per container, with the
+    keys of BatchCodec.updates_counts.  finish() -> the new container bytes in input order, as update_regions returns
+    them.  It is the only place that waits for the GPU: one small copy of the window path's sizes and error flag,
+    then its bytes, and the whole-path containers' EncodeJob.finish()."""
+
+    def __init__(self, codec, outs, counts, whole, window):
+        self.codec, self.counts = codec, counts
+        self._outs = outs                  # containers done on the host (empty edit lists), None elsewhere
+        self._whole = whole                # [(i, EncodeJob)]
+        self._window = window              # None or (input indices, output starts, out, info_host, ready, stream, keep)
+
+    @_on_device
+    def finish(self):
+        if self._outs is None:
+            raise RuntimeError('UpdateJob.finish() was called before')
+        outs, self._outs = self._outs, None
+        if self._window is not None:
+            idx, starts, out, info_host, ready, stream, _ = self._window
+            ready.synchronize()
+            info = info_host.numpy().astype(np.int64)
+            sizes, flag = info[:-1], int(info[-1])
+            if flag & 1:
+                raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
+            if flag:
+                raise RuntimeError('region update: a splice segment fell outside its buffer (flag %d)' % flag)
+            end = int((starts + sizes).max())
+            host = torch.empty(end, dtype=torch.uint8, pin_memory=True)
+            with torch.cuda.stream(stream):
+                host.copy_(out[:end], non_blocking=True)
+                stream.synchronize()
+            buf = host.numpy()
+            for i, s0, n in zip(idx, starts, sizes):
+                outs[i] = buf[s0:s0 + n].tobytes()
+            self._window = None
+        for i, job in self._whole:
+            outs[i] = job.finish()[0][0]
+        self._whole = []
+        return outs
 
 
 class BatchCodec(object):
@@ -1457,19 +1539,13 @@ class BatchCodec(object):
                                  'whole': 0.0}
         outs, counts, window = [None] * len(jobs), [None] * len(jobs), []
         for i, job in enumerate(jobs):
-            total = job.plans[0][0].total_streams if job.plans else sum(len(st) for (_, _, _, st) in job.parsed)
             if not job.plans:
                 outs[i] = bytes(job.data)
-                counts[i] = {'streams': 0, 'total': total, 'window_pixels': 0, 'whole': False, 'plans': 0}
+                counts[i] = _host_counts(job)
             elif job.whole:
                 t0 = time.perf_counter()
-                left, _, top, _ = job.pad_tuple
-                img, _ = self.decode_batch([job.data], to_host=False)
-                for (y, x, h, w), patch in zip(job.rects, job.patches):
-                    img[:, :, top + y:top + y + h, left + x:left + x + w] = patch
-                outs[i] = self.encode_batch(img, job.pad_tuple, tile=job.tile)[0][0]
-                counts[i] = {'streams': total, 'total': total, 'window_pixels': img.shape[2] * img.shape[3],
-                             'whole': True, 'plans': len(job.plans)}
+                outs[i] = self._whole_begin(job).finish()[0][0]
+                counts[i] = _host_counts(job)
                 self.updates_stage_ms['whole'] += (time.perf_counter() - t0) * 1e3
             else:
                 window.append(i)
@@ -1479,20 +1555,120 @@ class BatchCodec(object):
         self.updates_counts = counts
         return outs
 
+    def _whole_begin(self, job, lane=None):
+        """update_regions' whole path for one container, queued: decode it (lane: as in decode_batch), paste every
+        patch in order, encode_begin the image -> its EncodeJob."""
+        left, _, top, _ = job.pad_tuple
+        img, _ = self.decode_batch([job.data], to_host=False, lane=lane)
+        for (y, x, h, w), patch in zip(job.rects, job.patches):
+            img[:, :, top + y:top + y + h, left + x:left + x + w] = patch
+        return self.encode_begin(img, job.pad_tuple, tile=job.tile)
+
+    @_on_device
+    def update_regions_begin(self, datas, edits, lane=None):
+        """update_regions queued without a host wait (DESIGN §4.12, "Serving updates") -> UpdateJob, whose finish()
+        returns the bytes update_regions returns and whose `counts` are the call's updates_counts (this codec's
+        updates_counts and updates_stage_ms are left as they are).  The host parse and plan (plan_updates) run here and
+        raise every ValueError of update_regions before any launch.  Everything else is queued on the current stream:
+        the window path up to the new stream lengths (_enqueue_windows), then l3c_update_layout lays out and
+        l3c_splice_streams_dev splices every new container from those lengths in device memory, and the sizes and the
+        error flag start on their way to the host; a whole-path container is decoded, pasted and encode_begin'd.
+        lane: as in decode_regions -- the caller has made `lane.main` current, and the old-pixel decodes run their range
+        decoders on the lane's decoder streams.  Buffers the queued work reads stay alive on the job until finish()."""
+        jobs = self.plan_updates(datas, edits)
+        cur = torch.cuda.current_stream()
+        outs, counts, whole, window = [None] * len(jobs), [None] * len(jobs), [], []
+        for i, job in enumerate(jobs):
+            for patch in job.patches:
+                patch.record_stream(cur)            # the caller's tensor, read on this stream
+            if not job.plans:
+                outs[i] = bytes(job.data)
+                counts[i] = _host_counts(job)
+            elif job.whole:
+                whole.append((i, self._whole_begin(job, lane)))
+                counts[i] = _host_counts(job)
+            else:
+                window.append(i)
+        tail = None
+        if window:
+            sel = [jobs[i] for i in window]
+            w = self._enqueue_windows(sel, lane, hold=True)
+            conts, streams, starts, size = update_layout_inputs(
+                [(job.parsed, job.tile, w.starts[k], len(job.data), w.cols[k], w.sl[k]) for k, job in enumerate(sel)],
+                w.caps)
+            out = torch.empty(max(size, 1), dtype=torch.uint8, device=w.blob.device)
+            info, keep = E.update_splice(conts, streams, w.lens_dev, w.slot_off[:-1], w.caps, w.blob, w.slots, out)
+            info_host = torch.empty(info.shape, dtype=torch.int64, pin_memory=True)
+            info_host.copy_(info, non_blocking=True)
+            ready = torch.cuda.Event()
+            ready.record(cur)
+            for i, c in zip(window, w.counts):
+                counts[i] = c
+            tail = (window, starts, out, info_host, ready, cur, (jobs, w, keep, info))
+        return UpdateJob(self, outs, counts, whole, tail)
+
     def _update_windows(self, jobs):
         """update_regions' window path (DESIGN §4.12, "Batches of updates") for the jobs of one call -> ([bytes],
-        [counts]).  One upload of the containers, read by the old-pixel decodes and the splice.  The plans are grouped
-        into passes of one tile size whose windows fit TILED_ENCODE_BAND_PIXELS (bitcoding.plan_passes).  Per pass: the
-        old pixels of every window from region passes (_decode_planned), the patches pasted in order, then per plan the
-        encoders and the coding on its windows (_encode_windows, _code_rects) and one range-coder launch for every new
-        stream of the pass.  A stream that two separate plans re-encode is coded once (both give the same bytes).  Then
-        one l3c_splice_streams launch assembles every new container and one copy brings them to the host."""
+        [counts]).  _enqueue_windows queues everything up to the new stream lengths; they come to the host, and one
+        l3c_splice_streams launch assembles every new container from host-made segments and one copy brings them to
+        the host."""
+        stage = self.updates_stage_ms
+        w = self._enqueue_windows(jobs)
+        stage['upload'] = w.upload_ms
+        t0 = w.t_enqueue
+        # ---- the new stream lengths, in the call's stream order, to the host (the layout depends on them)
+        lens_h = torch.empty(w.lens_dev.shape, dtype=torch.int32, pin_memory=True)
+        lens_h.copy_(w.lens_dev, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        lens = lens_h.numpy().astype(np.int64)
+        _check_lens(lens, w.caps)
+        stage['gpu'] = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        # ---- splice: every container's segments, one launch, one copy to the host
+        segs, sizes, out_starts, pos = [], [], [], 0
+        for k, job in enumerate(jobs):
+            cols, sl = w.cols[k], w.sl[k]
+            layout = ContainerLayout([(i, C, H, W) for i, (C, H, W, _) in enumerate(job.parsed)], job.tile)
+            old_len = np.concatenate([np.asarray(st, np.int64).reshape(-1, 2)[:, 1] for (_, _, _, st) in job.parsed])
+            _, old_off = layout.offsets(old_len)
+            new_len = old_len.copy()
+            new_len[cols] = lens[sl]
+            total, new_off = layout.offsets(new_len)
+            segs.append(splice_segments(old_off, old_len, len(job.data), new_off, cols, lens[sl], w.slot_off[sl],
+                                        w.starts[k], pos))
+            sizes.append(total)
+            out_starts.append(pos)
+            pos += (total + 15) & ~15
+        out = torch.empty(pos, dtype=torch.uint8, device=w.blob.device)
+        E.splice_streams(w.blob, w.slots, np.concatenate(segs), out)
+        host = torch.empty(out.shape, dtype=torch.uint8, pin_memory=True)
+        host.copy_(out, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        buf = host.numpy()
+        outs = [buf[s:s + n].tobytes() for s, n in zip(out_starts, sizes)]
+        stage['splice'] = (time.perf_counter() - t0) * 1e3
+        return outs, w.counts
+
+    def _enqueue_windows(self, jobs, lane=None, hold=False):
+        """The part of update_regions' window path that runs without a host wait, shared by update_regions and
+        update_regions_begin: everything up to the new stream lengths in device memory.  One upload of the containers,
+        read by the old-pixel decodes and the splice.  The plans are grouped into passes of one tile size whose windows
+        fit TILED_ENCODE_BAND_PIXELS (region.plan_update_passes).  Per pass: the old pixels of every window from region
+        passes (_decode_planned; on the lane's decoder streams with `lane`), the patches pasted in order, then per plan
+        the encoders and the coding on its windows (_encode_windows, _code_rects) and one range-coder launch for every
+        new stream of the pass.  A stream that two separate plans re-encode is coded once (both give the same bytes).
+        hold: keep every pass's intervals alive in `keep` (they are freed after each pass otherwise).
+        -> _WindowWork: blob and starts (_upload), upload_ms and t_enqueue (the host clock after the upload), caps and
+        slot_off (int64 per new stream, in the call's stream order), slots, lens_dev (int32 on the device) and, per
+        job, cols (the ascending columns of its re-encoded streams), sl (their indices into lens_dev) and counts."""
         from .region import plan_region, plan_update_passes, rect_streams
         dev = self.blueprint.device
-        stage, t0 = self.updates_stage_ms, time.perf_counter()
-        blob, starts = _upload([job.data for job in jobs], dev)
-        stage['upload'] = (time.perf_counter() - t0) * 1e3
+        w = _WindowWork()
         t0 = time.perf_counter()
+        w.blob, w.starts = _upload([job.data for job in jobs], dev)
+        w.t_enqueue = time.perf_counter()
+        w.upload_ms = (w.t_enqueue - t0) * 1e3
+        w.keep = []
         geo = self._geometry()
         # ---- host: every plan's streams (duplicates across a container's plans dropped) and its slot in one buffer
         items = []
@@ -1511,6 +1687,7 @@ class BatchCodec(object):
         caps = _slot_cap(np.concatenate([kp[1] for _, _, keep in items for _, kp in sorted(keep.items())]))
         slot_off = np.concatenate([[0], np.cumsum(caps)])
         slots = torch.empty(max(int(slot_off[-1]), 1), dtype=torch.uint8, device=dev)
+        w.caps, w.slot_off, w.slots = caps, slot_off, slots
         passes = plan_update_passes([plan for _, plan, _ in items], TILED_ENCODE_BAND_PIXELS)
         first = np.zeros(len(items) + 1, np.int64)          # each plan's first stream in the call's stream order
         first[1:] = np.cumsum([sum(kp[0].size for kp in keep.values()) for _, _, keep in items])
@@ -1527,15 +1704,15 @@ class BatchCodec(object):
                 rplans.append(plan_region([s[:3] for s in job.parsed], job.pad_tuple, job.tile, geo,
                                           (u[0] - top, u[1] - left, u[2] - u[0], u[3] - u[1])))
                 imgs.append((u, torch.zeros(1, 3, P[2] - P[0], P[3] - P[1], dtype=torch.uint8, device=dev)))
-            olds = self._decode_planned(blob, starts[[items[t][0] for t in ps]],
-                                        [[st for (_, _, _, st) in jobs[items[t][0]].parsed] for t in ps], rplans)
+            olds = self._decode_planned(w.blob, w.starts[[items[t][0] for t in ps]],
+                                        [[st for (_, _, _, st) in jobs[items[t][0]].parsed] for t in ps], rplans, lane)
             for t, (u, img), old in zip(ps, imgs, olds):
                 k, plan, _ = items[t]
                 job, P = jobs[k], plan.window
                 img[:, :, u[0] - P[0]:u[2] - P[0], u[1] - P[1]:u[3] - P[1]] = old
                 left, _, top, _ = job.pad_tuple
-                for (y, x, h, w), patch in zip(job.rects, job.patches):
-                    e = (y + top, x + left, y + top + h, x + left + w)
+                for (y, x, h, w_), patch in zip(job.rects, job.patches):
+                    e = (y + top, x + left, y + top + h, x + left + w_)
                     c = (max(e[0], P[0]), max(e[1], P[1]), min(e[2], P[2]), min(e[3], P[3]))
                     if c[0] < c[2] and c[1] < c[3]:
                         img[:, :, c[0] - P[0]:c[2] - P[0], c[1] - P[1]:c[3] - P[1]] = \
@@ -1569,49 +1746,26 @@ class BatchCodec(object):
             desc = np.concatenate(descs)
             if desc.size:
                 lens_parts.append((np.concatenate(order), E.ac_encode_streams(desc, dev)[1]))
+            if hold:
+                w.keep.extend(keep_alive)
             del keep_alive, coded
-        # ---- the new stream lengths, in the call's stream order, to the host (the layout depends on them)
-        lens_dev = torch.empty(int(first[-1]), dtype=torch.int32, device=dev)
+        # ---- the new stream lengths in the call's stream order
+        w.lens_dev = torch.empty(int(first[-1]), dtype=torch.int32, device=dev)
         for order, ln in lens_parts:
-            lens_dev[E._to_device_async(order, dev)] = ln
-        lens_h = torch.empty(lens_dev.shape, dtype=torch.int32, pin_memory=True)
-        lens_h.copy_(lens_dev, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        lens = lens_h.numpy().astype(np.int64)
-        _check_lens(lens, caps)
-        stage['gpu'] = (time.perf_counter() - t0) * 1e3
-        t0 = time.perf_counter()
-        # ---- splice: every container's segments, one launch, one copy to the host
-        segs, sizes, out_starts, counts, pos = [], [], [], [], 0
-        for k, job in enumerate(jobs):
+            w.lens_dev[E._to_device_async(order, dev)] = ln
+        # ---- per job: its re-encoded streams in container order, where their lengths are, and the call's counts
+        w.cols, w.sl, w.counts = [], [], []
+        for k in range(len(jobs)):
             mine = [t for t, it in enumerate(items) if it[0] == k]
             cols = np.concatenate([kp[0] for t in mine for _, kp in sorted(items[t][2].items())])
             sl = np.concatenate([np.arange(first[t], first[t + 1]) for t in mine])
             order = np.argsort(cols, kind='stable')
-            cols, sl = cols[order], sl[order]
-            layout = ContainerLayout([(i, C, H, W) for i, (C, H, W, _) in enumerate(job.parsed)], job.tile)
-            old_len = np.concatenate([np.asarray(st, np.int64).reshape(-1, 2)[:, 1] for (_, _, _, st) in job.parsed])
-            _, old_off = layout.offsets(old_len)
-            new_len = old_len.copy()
-            new_len[cols] = lens[sl]
-            total, new_off = layout.offsets(new_len)
-            segs.append(splice_segments(old_off, old_len, len(job.data), new_off, cols, lens[sl], slot_off[sl],
-                                        starts[k], pos))
-            sizes.append(total)
-            out_starts.append(pos)
-            pos += (total + 15) & ~15
-            counts.append({'streams': int(cols.size), 'total': items[mine[0]][1].total_streams,
-                           'window_pixels': sum(items[t][1].window_pixels for t in mine), 'whole': False,
-                           'plans': len(mine)})
-        out = torch.empty(pos, dtype=torch.uint8, device=dev)
-        E.splice_streams(blob, slots, np.concatenate(segs), out)
-        host = torch.empty(out.shape, dtype=torch.uint8, pin_memory=True)
-        host.copy_(out, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        buf = host.numpy()
-        outs = [buf[s:s + n].tobytes() for s, n in zip(out_starts, sizes)]
-        stage['splice'] = (time.perf_counter() - t0) * 1e3
-        return outs, counts
+            w.cols.append(cols[order])
+            w.sl.append(sl[order])
+            w.counts.append({'streams': int(cols.size), 'total': items[mine[0]][1].total_streams,
+                             'window_pixels': sum(items[t][1].window_pixels for t in mine), 'whole': False,
+                             'plans': len(mine)})
+        return w
 
     def _code_pass_serial(self, plans, imgs, tiles):
         """The encoders and the coding of the update plans of one pass, plan after plan, on their windows as update_region

@@ -1358,6 +1358,180 @@ splice_streams_kernel(const int64_t *__restrict__ seg, int n_seg, const uint8_t 
     }
 }
 
+// ---- layout and splice of region updates from device-resident lengths (l3c_update_layout, l3c_splice_streams_dev)
+constexpr int LAYOUT_THREADS = 256;
+constexpr int64_t UPD_SLOT_OVERFLOW = 1, UPD_INCONSISTENT = 2;
+
+// Exclusive scan of (a, b) over the CTA; *ta / *tb get the CTA's totals.  ws: LAYOUT_THREADS / 32 pairs of shared
+// memory; every thread calls it.
+__device__ __forceinline__ void block_scan2(int64_t a, int64_t b, int64_t *ws, int64_t &ea, int64_t &eb,
+                                            int64_t &ta, int64_t &tb) {
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    constexpr int NW = LAYOUT_THREADS / 32;
+    int64_t x = a, y = b;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int64_t px = __shfl_up_sync(0xffffffffu, x, o), py = __shfl_up_sync(0xffffffffu, y, o);
+        if (lane >= o) x += px, y += py;
+    }
+    if (lane == 31) ws[2 * wid] = x, ws[2 * wid + 1] = y;
+    __syncthreads();
+    if (wid == 0) {
+        int64_t u = lane < NW ? ws[2 * lane] : 0, v = lane < NW ? ws[2 * lane + 1] : 0;
+#pragma unroll
+        for (int o = 1; o < NW; o <<= 1) {
+            const int64_t pu = __shfl_up_sync(0xffffffffu, u, o), pv = __shfl_up_sync(0xffffffffu, v, o);
+            if (lane >= o) u += pu, v += pv;
+        }
+        if (lane < NW) ws[2 * lane] = u, ws[2 * lane + 1] = v;
+    }
+    __syncthreads();
+    ea = (wid ? ws[2 * wid - 2] : 0) + x - a;
+    eb = (wid ? ws[2 * wid - 1] : 0) + y - b;
+    ta = ws[2 * NW - 2];
+    tb = ws[2 * NW - 1];
+    __syncthreads();                                   // ws is reused by the next call
+}
+
+// a container's segments [first_seg, first_seg + 2 n_new + 1) lie in the segment array of n_seg
+__device__ __forceinline__ bool update_segs_ok(const l3c_update_container_t &c, int64_t n_seg) {
+    return c.n_new >= 0 && c.n_new <= n_seg && c.first_seg >= 0 && c.first_seg <= n_seg - (2 * c.n_new + 1);
+}
+
+__device__ __forceinline__ bool update_container_ok(const l3c_update_container_t &c, int64_t n_streams, int64_t n_seg) {
+    return update_segs_ok(c, n_seg) && c.first_stream >= 0 && c.n_streams >= 0 && c.first_stream <= n_streams - c.n_streams &&
+           c.n_new <= c.n_streams && c.old_base >= 0 && c.old_bytes >= 0 && c.out_base >= 0 && c.out_cap >= 0;
+}
+
+__global__ void __launch_bounds__(LAYOUT_THREADS)
+update_layout_kernel(const l3c_update_container_t *__restrict__ conts, const l3c_update_stream_t *__restrict__ streams,
+                     int64_t n_streams, const int32_t *__restrict__ new_len, const int64_t *__restrict__ slot_off,
+                     const int64_t *__restrict__ caps, int64_t n_new, int64_t *__restrict__ seg,
+                     int64_t *__restrict__ chunk0, int64_t n_seg, int64_t *__restrict__ info, int n_containers) {
+    __shared__ int64_t ws[2 * (LAYOUT_THREADS / 32)];
+    __shared__ int64_t err;
+    const int k = blockIdx.x;
+    const l3c_update_container_t c = conts[k];
+    if (threadIdx.x == 0) err = 0;
+    __syncthreads();
+    if (!update_container_ok(c, n_streams, n_seg)) {
+        // nothing of this container is placed: no segments, and no chunks where its chunk total can be located
+        if (threadIdx.x == 0) {
+            info[k] = 0;
+            if (update_segs_ok(c, n_seg)) chunk0[c.first_seg + k + 2 * c.n_new + 1] = 0;
+            atomicOr((unsigned long long *)(info + n_containers), (unsigned long long)UPD_INCONSISTENT);
+        }
+        return;
+    }
+    int64_t *sg = seg + 4 * c.first_seg;
+    const int64_t m = c.n_new, ns = 2 * m + 1;
+    // ---- new offsets: one chunk of LAYOUT_THREADS streams per step, the running sums carried across
+    int64_t base_len = 0, base_new = 0;
+    for (int64_t s0 = 0; s0 < c.n_streams; s0 += LAYOUT_THREADS) {
+        const int64_t s = s0 + threadIdx.x;
+        int64_t len = 0, is_new = 0;
+        l3c_update_stream_t st{};
+        if (s < c.n_streams) {
+            st = streams[c.first_stream + s];
+            len = st.old_len;
+            if (st.src >= 0) {
+                is_new = 1;
+                if (st.src >= n_new) {
+                    atomicOr((unsigned long long *)&err, (unsigned long long)UPD_INCONSISTENT);
+                    len = 0;
+                } else {
+                    len = new_len[st.src];
+                    if (len < 0 || len > caps[st.src]) atomicOr((unsigned long long *)&err, (unsigned long long)UPD_SLOT_OVERFLOW);
+                }
+            }
+        }
+        int64_t ex_len, ex_new, t_len, t_new;
+        block_scan2(len, is_new, ws, ex_len, ex_new, t_len, t_new);
+        const int64_t j = base_new + ex_new;
+        if (is_new && j < m && st.src < n_new) {
+            const int64_t off = c.out_base + st.fixed_off + base_len + ex_len;
+            int64_t *a = sg + 4 * (2 * j + 1), *b = a + 4;
+            a[0] = 1, a[1] = slot_off[st.src], a[2] = off, a[3] = len;
+            b[0] = 0, b[1] = c.old_base + st.old_off + st.old_len, b[2] = off + len;       // b[3] below
+        }
+        base_len += t_len;
+        base_new += t_new;
+    }
+    const int64_t total = c.fixed_total + base_len;
+    if (threadIdx.x == 0) {
+        sg[0] = 0, sg[1] = c.old_base, sg[2] = c.out_base;
+        if (base_new != m || total > c.out_cap) atomicOr((unsigned long long *)&err, (unsigned long long)UPD_INCONSISTENT);
+        info[k] = total;
+    }
+    __syncthreads();
+    // ---- every run ends at the length field of the next new stream or at the container's end: unchanged bytes
+    // keep their distances, so its size follows from the destinations
+    if (base_new == m)
+        for (int64_t j = threadIdx.x; j <= m; j += LAYOUT_THREADS) {
+            const int64_t end = j < m ? sg[4 * (2 * j + 1) + 2] - 4 : c.out_base + total;
+            sg[4 * (2 * j) + 3] = end - sg[4 * (2 * j) + 2];
+            if (end < sg[4 * (2 * j) + 2]) atomicOr((unsigned long long *)&err, (unsigned long long)UPD_INCONSISTENT);
+        }
+    __syncthreads();
+    const bool bad = err != 0;
+    // ---- chunks per segment (SPLICE_CHUNK bytes each, one for an empty new stream: its length field), prefix
+    int64_t *ch = chunk0 + c.first_seg + k;
+    int64_t base = 0;
+    for (int64_t i0 = 0; i0 < ns; i0 += LAYOUT_THREADS) {
+        const int64_t i = i0 + threadIdx.x;
+        int64_t n = 0;
+        if (i < ns && !bad) {
+            const int64_t b = sg[4 * i + 3];
+            n = b > 0 ? (b + SPLICE_CHUNK - 1) / SPLICE_CHUNK : sg[4 * i];
+        }
+        int64_t ex, unused, t, t2;
+        block_scan2(n, 0, ws, ex, unused, t, t2);
+        if (i < ns) ch[i] = base + ex;
+        base += t;
+    }
+    if (threadIdx.x == 0) {
+        ch[ns] = base;
+        if (bad) atomicOr((unsigned long long *)(info + n_containers), (unsigned long long)err);
+    }
+}
+
+__global__ void __launch_bounds__(SPLICE_THREADS)
+splice_streams_dev_kernel(const l3c_update_container_t *__restrict__ conts, int k0, const int64_t *__restrict__ seg,
+                          const int64_t *__restrict__ chunk0, int64_t n_seg, const uint8_t *__restrict__ old,
+                          int64_t old_bytes, const uint8_t *__restrict__ slots, int64_t slot_bytes,
+                          uint8_t *__restrict__ out, int64_t out_bytes, int64_t *__restrict__ flag) {
+    const int k = k0 + blockIdx.y;
+    const l3c_update_container_t c = conts[k];
+    if (!update_segs_ok(c, n_seg)) return;            // l3c_update_layout flagged it
+    const int64_t ns = 2 * c.n_new + 1;
+    const int64_t *sg = seg + 4 * c.first_seg, *ch = chunk0 + c.first_seg + k;
+    const int64_t total = ch[ns];
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (SPLICE_THREADS / 32);
+    for (int64_t w = (int64_t)blockIdx.x * (SPLICE_THREADS / 32) + (threadIdx.x >> 5); w < total; w += warps) {
+        int64_t lo = 0, hi = ns - 1;                   // the segment s with ch[s] <= w < ch[s + 1]
+        while (lo < hi) {
+            const int64_t mid = (lo + hi + 1) >> 1;
+            if (ch[mid] <= w) lo = mid; else hi = mid - 1;
+        }
+        const int64_t kind = sg[4 * lo], so = sg[4 * lo + 1], d = sg[4 * lo + 2], n = sg[4 * lo + 3];
+        const int64_t s_lo = kind ? 0 : c.old_base, s_hi = kind ? slot_bytes : min(c.old_base + c.old_bytes, old_bytes);
+        const int64_t d_lo = max(c.out_base, (int64_t)0), d_hi = min(c.out_base + c.out_cap, out_bytes);
+        const bool ok = (kind == 0 || kind == 1) && n >= 0 && (kind == 0 || n <= 0xffffffffll) && so >= s_lo &&
+                        so <= s_hi - n && d - 4 * kind >= d_lo && d <= d_hi - n;
+        if (!ok) {
+            if (lane == 0) atomicOr((unsigned long long *)flag, (unsigned long long)UPD_INCONSISTENT);
+            continue;
+        }
+        const int64_t b0 = (w - ch[lo]) * SPLICE_CHUNK, b1 = min(b0 + SPLICE_CHUNK, n);
+        const uint8_t *src = (kind ? slots : old) + so;
+        uint8_t *dst = out + d;
+        if (kind && b0 == 0 && lane < 4)                  // the new stream's u32 length, little-endian
+            dst[lane - 4] = (uint8_t)((uint64_t)n >> (8 * lane));
+        for (int64_t i = b0 + lane; i < b1; i += 32) dst[i] = src[i];
+    }
+}
+
 // intervals from a shared 256-entry LUT (uniform prior: every pixel has the same CDF row)
 __global__ void lut_intervals_kernel(const uint8_t *__restrict__ sym, const uint32_t *__restrict__ lut,
                                      int64_t n, uint32_t *__restrict__ iv) {
@@ -1607,6 +1781,52 @@ extern "C" int l3c_splice_streams(const uint8_t *old_dev, int64_t old_bytes, con
                                                                                                 old_dev, slots_dev,
                                                                                                 out_dev);
     L3C_LAUNCH_CHECK("splice_streams_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_update_layout(const l3c_update_container_t *conts_dev, int n_containers,
+                                 const l3c_update_stream_t *streams_dev, int64_t n_streams, const int32_t *new_len_dev,
+                                 const int64_t *slot_off_dev, const int64_t *caps_dev, int64_t n_new, int64_t *seg_dev,
+                                 int64_t *chunk0_dev, int64_t n_seg, int64_t *info_dev, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(n_containers >= 0 && n_streams >= 0 && n_new >= 0 && n_seg >= 0,
+                "l3c_update_layout: n_containers=%d n_streams=%lld n_new=%lld n_seg=%lld", n_containers,
+                (long long)n_streams, (long long)n_new, (long long)n_seg);
+    L3C_REQUIRE(info_dev, "l3c_update_layout: null info_dev");
+    L3C_REQUIRE(n_containers == 0 || (conts_dev && streams_dev && seg_dev && chunk0_dev &&
+                                      (n_new == 0 || (new_len_dev && slot_off_dev && caps_dev))),
+                "l3c_update_layout: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    L3C_CUDA(cudaMemsetAsync(info_dev + n_containers, 0, sizeof(int64_t), st));
+    if (n_containers == 0) return L3C_OK;
+    update_layout_kernel<<<n_containers, LAYOUT_THREADS, 0, st>>>(conts_dev, streams_dev, n_streams, new_len_dev,
+                                                                   slot_off_dev, caps_dev, n_new, seg_dev, chunk0_dev,
+                                                                   n_seg, info_dev, n_containers);
+    L3C_LAUNCH_CHECK("update_layout_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_splice_streams_dev(const l3c_update_container_t *conts_dev, int n_containers,
+                                      const int64_t *seg_dev, const int64_t *chunk0_dev, int64_t n_seg,
+                                      const uint8_t *old_dev, int64_t old_bytes, const uint8_t *slots_dev, int64_t slot_bytes, uint8_t *out_dev,
+                                      int64_t out_bytes, int64_t max_chunks, int64_t *flag_dev, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(n_containers >= 0 && n_seg >= 0 && old_bytes >= 0 && slot_bytes >= 0 && out_bytes >= 0 &&
+                    max_chunks >= 0,
+                "l3c_splice_streams_dev: n_containers=%d n_seg=%lld old_bytes=%lld slot_bytes=%lld out_bytes=%lld "
+                "max_chunks=%lld", n_containers, (long long)n_seg, (long long)old_bytes, (long long)slot_bytes,
+                (long long)out_bytes, (long long)max_chunks);
+    if (n_containers == 0 || max_chunks == 0) return L3C_OK;
+    L3C_REQUIRE(conts_dev && seg_dev && chunk0_dev && old_dev && slots_dev && out_dev && flag_dev,
+                "l3c_splice_streams_dev: null pointer");
+    const int64_t blocks = (max_chunks + SPLICE_THREADS / 32 - 1) / (SPLICE_THREADS / 32);
+    for (int k0 = 0; k0 < n_containers; k0 += 65535) {
+        dim3 grid((unsigned)(blocks < 65535 ? blocks : 65535), n_containers - k0 < 65535 ? n_containers - k0 : 65535);
+        splice_streams_dev_kernel<<<grid, SPLICE_THREADS, 0, (cudaStream_t)stream>>>(
+            conts_dev, k0, seg_dev, chunk0_dev, n_seg, old_dev, old_bytes, slots_dev, slot_bytes, out_dev, out_bytes,
+            flag_dev);
+        L3C_LAUNCH_CHECK("splice_streams_dev_kernel");
+    }
     return L3C_OK;
 }
 

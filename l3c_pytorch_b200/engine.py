@@ -1096,6 +1096,33 @@ def splice_streams(old, slots, seg, out):
     LAUNCHES['n'] += int(seg.shape[0] > 0)
 
 
+def update_splice(conts, streams, new_len, slot_off, caps, old, slots, out):
+    """l3c_update_layout, then l3c_splice_streams_dev: the containers conts (UPDATE_CONTAINER_DTYPE) with their streams
+    (UPDATE_STREAM_DTYPE), numpy, are laid out from the device lengths new_len (int32) and spliced from the uint8 device
+    buffers old and slots into out, without a host wait.  slot_off / caps: int64 numpy [new_len.numel()].  Everything
+    host-side is uploaded in one asynchronous copy.  -> (info, keep): info int64 [len(conts) + 1] on the device, the
+    new sizes and the error flag; keep: the device tensors the launches read, to be kept alive until they ran."""
+    n_c, n_s, n_new = conts.shape[0], streams.shape[0], int(new_len.numel())
+    n_seg = int((2 * conts['n_new'] + 1).sum())
+    host = np.concatenate([conts.view(np.int64).reshape(-1), streams.view(np.int64).reshape(-1),
+                           np.asarray(slot_off, np.int64), np.asarray(caps, np.int64)])
+    up = _to_device_async(host, out.device)
+    a, b = conts.size * 9, conts.size * 9 + streams.size * 4
+    seg = torch.empty(4 * n_seg + n_seg + n_c, dtype=torch.int64, device=out.device)
+    info = torch.empty(n_c + 1, dtype=torch.int64, device=out.device)
+    ptr = lambda t, i: ctypes.c_void_p(t.data_ptr() + 8 * i)
+    check(lib.l3c_update_layout(ptr(up, 0), n_c, ptr(up, a), n_s, _ptr(new_len), ptr(up, b), ptr(up, b + n_new), n_new,
+                                _ptr(seg), ptr(seg, 4 * n_seg), n_seg, _ptr(info), _stream_ptr()))
+    LAUNCHES['n'] += int(n_c > 0)
+    # a container's chunks: one per 4 KB of its bytes, plus one per segment boundary
+    max_chunks = int((conts['out_cap'] // 4096 + 2 * conts['n_new'] + 2).max()) if n_c else 0
+    check(lib.l3c_splice_streams_dev(ptr(up, 0), n_c, _ptr(seg), ptr(seg, 4 * n_seg), n_seg, _ptr(old), old.numel(),
+                                     _ptr(slots), slots.numel(), _ptr(out), out.numel(), max_chunks, ptr(info, n_c),
+                                     _stream_ptr()))
+    LAUNCHES['n'] += -(-n_c // 65535) if max_chunks else 0
+    return info, (up, seg, new_len, old, slots, out)
+
+
 COARSE_PITCH = 96     # uint16 per coarse record (l3c_dmll_build_coarse)
 
 
