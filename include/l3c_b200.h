@@ -103,7 +103,8 @@ typedef struct {
     uint32_t out_cap;           /* multiple of 4                                                */
 } l3c_enc_stream_t;
 
-/* out_len_dev[i] = bytes produced by stream i (if > out_cap the slot content is truncated). */
+/* out_len_dev[i] = bytes produced by stream i (if > out_cap the slot content is truncated; a stream of 2^32 bytes or
+ * more reports 2^32 - 1).  out_len is unsigned: read it as uint32, not int32. */
 int l3c_ac_encode_streams(const l3c_enc_stream_t *streams_dev, int n_streams,
                           uint32_t *out_len_dev, void *stream);
 
@@ -114,8 +115,12 @@ typedef struct {
     uint8_t *sym_out;           /* dev: n_sym decoded symbols, uint8; for L > 256 n_sym           */
                                 /*      little-endian uint16, 2-byte aligned.  Nothing past n_sym  */
                                 /*      symbols is written.                                       */
-    uint32_t *state;            /* dev: 4 words of coder state (low, high, value, bitpos);        */
-                                /*      lets one stream be decoded in several launches (chunks)   */
+    uint32_t *state;            /* dev: coder state (low, high, value, code bits read); lets one  */
+                                /*      stream be decoded in several launches (chunks).  4 words, */
+                                /*      word 3 the low 32 bits of the bits read; a stream with    */
+                                /*      in_len >= 2^28 takes a 5th word, their high 32 bits.  A    */
+                                /*      shorter stream read 2^32 bits or more, far past its end,  */
+                                /*      sets bit 31 of word 0 (low is below 2^31)                 */
     int64_t row_pitch;          /* entries between consecutive rows; 0 = one shared row.  Every   */
                                 /*      row is read whole: 32 entries for L <= 32, 256 for L <= 256,*/
                                 /*      round_up(L, 8) for L > 256, 16-byte aligned.  Entries past */

@@ -37,6 +37,9 @@ PRECISIONS = {'fp32': PREC_FP32, 'tf32': PREC_TF32, 'f16': PREC_F16, 'f16x2': PR
 ENC_STREAM_DTYPE = [('intervals', '<u8'), ('out', '<u8'), ('n_sym', '<u4'), ('out_cap', '<u4')]
 DEC_STREAM_DTYPE = [('table', '<u8'), ('in', '<u8'), ('sym_out', '<u8'), ('state', '<u8'),
                     ('row_pitch', '<i8'), ('n_sym', '<u4'), ('in_len', '<u4')]
+# uint32 words of a decoder stream's saved state that fit every stream: (low, high, value, code bits read: low word,
+# high word); streams below 2^28 bytes use only the first 4
+DEC_STATE_WORDS = 5
 # l3c_update_stream_t / l3c_update_container_t (l3c_update_layout)
 UPDATE_STREAM_DTYPE = [('fixed_off', '<i8'), ('old_off', '<i8'), ('old_len', '<i8'), ('src', '<i8')]
 UPDATE_CONTAINER_DTYPE = [('first_stream', '<i8'), ('n_streams', '<i8'), ('fixed_total', '<i8'), ('old_base', '<i8'),

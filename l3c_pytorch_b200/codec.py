@@ -91,6 +91,11 @@ def _enc_descs(ptrs, n_sym, dev):
     return caps, slots, desc
 
 
+def _host_lens(words):
+    """the range coder's uint32 output lengths, as the int32 words a device tensor holds them -> int64"""
+    return np.asarray(words).view(np.uint32).astype(np.int64)
+
+
 def _check_lens(lens, caps):
     if (lens > caps).any():
         raise RuntimeError('range coder output exceeded its slot (corrupt CDF?)')
@@ -385,7 +390,7 @@ class EncodeJob:
     def finish(self, to_host=True):
         N, per_img = self.caps.shape
         self.coded.synchronize()                                                   # sync #1 (tiny)
-        lens = self.lens_host.numpy().astype(np.int64).reshape(N, per_img)
+        lens = _host_lens(self.lens_host.numpy()).reshape(N, per_img)
         _check_lens(lens, self.caps)
         with torch.cuda.stream(self.stream):
             # ---- container layout + gather + single D2H
@@ -885,8 +890,8 @@ class BatchCodec(object):
             n_chunks = int(os.environ.get('L3C_RGB_CHUNKS', 64))
         csz = max(2048, -(-HW // n_chunks))
         csz = -(-csz // 64) * 64
-        state = torch.zeros(N * C * 4, dtype=torch.int32, device=dev)
-        d['state'][:] = state.data_ptr() + 16 * (np.arange(N)[:, None] * C + np.arange(C)[None, :])
+        state = torch.zeros(N * C * _lib.DEC_STATE_WORDS, dtype=torch.int32, device=dev)
+        d['state'][:] = state.data_ptr() + 4 * _lib.DEC_STATE_WORDS * (np.arange(N)[:, None] * C + np.arange(C)[None, :])
         descs = [E._desc_to_device(np.ascontiguousarray(d[:, c]), dev) for c in range(C)]
         cur = torch.cuda.current_stream()
         if lane is None:
@@ -1454,7 +1459,7 @@ class BatchCodec(object):
         slots_h.copy_(slots, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         del ivs
-        lens = lens_h.numpy().astype(np.int64)
+        lens = _host_lens(lens_h.numpy())
         _check_lens(lens, caps)
         slot_off = desc['out'].astype(np.int64) - slots.data_ptr()
 
@@ -1620,7 +1625,7 @@ class BatchCodec(object):
         lens_h = torch.empty(w.lens_dev.shape, dtype=torch.int32, pin_memory=True)
         lens_h.copy_(w.lens_dev, non_blocking=True)
         torch.cuda.current_stream().synchronize()
-        lens = lens_h.numpy().astype(np.int64)
+        lens = _host_lens(lens_h.numpy())
         _check_lens(lens, w.caps)
         stage['gpu'] = (time.perf_counter() - t0) * 1e3
         t0 = time.perf_counter()

@@ -3,6 +3,7 @@
 // implemented on top of the batched kernels of range_coder.cu / dmll.cu.
 #include <string.h>
 
+#include <algorithm>
 #include <mutex>
 #include <vector>
 
@@ -128,7 +129,9 @@ struct DevBuf {
 
 static int run_encode(const uint32_t *iv_dev, int64_t n_sym, uint8_t *out_host, size_t out_cap,
                       size_t *out_len) {
-    const size_t cap = (((size_t)n_sym * 17 + 7) / 8 + 64 + 3) & ~(size_t)3;
+    // the slot bound (17 bits per symbol + the terminator), clamped to the largest uint32 multiple of 4: above it
+    // the coder's saturated length exceeds the slot and the call fails instead of wrapping
+    const size_t cap = std::min<size_t>((((size_t)n_sym * 17 + 7) / 8 + 64 + 3) & ~(size_t)3, 0xFFFFFFFCu);
     DevBuf out, desc, len;
     if (int e = out.alloc(cap)) return e;
     if (int e = desc.alloc(sizeof(l3c_enc_stream_t))) return e;

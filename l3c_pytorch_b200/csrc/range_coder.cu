@@ -316,12 +316,13 @@ __device__ __forceinline__ void emit_records(const l3c_enc_stream_t &st, const u
         em.emit(rec.x, rec.y & 0xFFu, rec.y >> 8);
     }
     BitSink &sink = em.sink;
-    const uint32_t total = sink.wpos * 4u + (uint32_t)((sink.nacc + 7) >> 3);
+    // in 64 bits: a stream of 2^32 bytes or more reports 2^32 - 1, which exceeds every out_cap
+    const uint64_t total = 4ull * sink.wpos + (uint64_t)((sink.nacc + 7) >> 3);
     if (sink.nacc > 0) {
         const uint32_t w = (uint32_t)(sink.acc << (32 - sink.nacc));
         if (lane == 0 && sink.wpos < sink.cap_words) sink.out[sink.wpos] = __byte_perm(w, 0, 0x0123);
     }
-    if (lane == 0) *out_len = total;
+    if (lane == 0) *out_len = (uint32_t)min(total, (uint64_t)0xFFFFFFFFu);
 }
 
 // SPC = streams per CTA.  Coding warps are warps 0..SPC-1, emitter warps SPC..2*SPC-1 (the decoders' layout).
@@ -357,45 +358,50 @@ ac_encode_kernel(const l3c_enc_stream_t *__restrict__ streams, int n_streams, ui
 // MSB-first bit reader over a byte stream that may start at ANY address (streams are decoded in
 // place from the container): words are fetched from the 4-byte aligned address below the stream and
 // the first `8*mis` bits are simply skipped; bytes past the end read as zero (torchac.cpp:109-112).
+// Positions never wrap: the window is a 32-bit WORD index (streams are below 2^32 bytes, so words below 2^30 + 1)
+// and only bits 0..4 of `pos` are used, so the counter itself may wrap; the bit position is 32 * wbase + (pos & 31),
+// formed in 64 bits where it leaves the kernel (save_stream).
 struct BitSource {
     const uint32_t *base;
-    uint32_t end_byte;     // mis + in_len: first byte (relative to base) that is past the stream
+    uint32_t wend;         // words (relative to base) holding at least one byte of the stream: ceil((mis + in_len) / 4)
+    uint32_t last_mask;    // the bytes of word wend - 1 that lie inside the stream (big-endian mask)
     uint32_t wbase;        // word index of the upper half of `win`
     uint64_t win;          // words wbase, wbase+1
     uint32_t nextw;        // word wbase+2, ready to use
     uint32_t raw;          // word wbase+3 as loaded (little-endian, unmasked): consumed one refill
                            // later, so its load latency never lands on the coder's serial chain
-    uint32_t pos;          // next unread bit, relative to base; invariant 0 <= pos - 32*wbase < 32
+    uint32_t pos;          // next unread bit: bit (pos & 31) of word wbase; the higher bits are meaningless
 
-    __device__ __forceinline__ uint32_t load_raw(uint32_t i) const {
-        return ((int)end_byte - (int)(4u * i) > 0) ? __ldg(base + i) : 0u;
-    }
+    __device__ __forceinline__ uint32_t load_raw(uint32_t i) const { return (i < wend) ? __ldg(base + i) : 0u; }
     __device__ __forceinline__ uint32_t finish(uint32_t w_raw, uint32_t i) const {   // big-endian, zero past the end
-        const int rem = (int)end_byte - (int)(4u * i);
-        uint32_t w = __byte_perm(w_raw, 0, 0x0123);
-        if (rem < 4) w = (rem <= 0) ? 0u : (w & (0xFFFFFFFFu << (8 * (4 - rem))));
-        return w;
+        const uint32_t w = __byte_perm(w_raw, 0, 0x0123);
+        return w & ((i + 1u < wend) ? FULL : ((i + 1u == wend) ? last_mask : 0u));
     }
     __device__ __forceinline__ uint32_t word(uint32_t i) const { return finish(load_raw(i), i); }
     __device__ __forceinline__ uint32_t open(const uint8_t *in, uint32_t len) {
         const uintptr_t a = reinterpret_cast<uintptr_t>(in);
         const uint32_t mis = (uint32_t)(a & 3u);
         base = reinterpret_cast<const uint32_t *>(a - mis);
-        end_byte = mis + len;
+        const uint64_t end = (uint64_t)mis + len;          // up to 2^32 + 2: not a 32-bit quantity
+        wend = (uint32_t)((end + 3u) >> 2);
+        last_mask = (end & 3u) ? (FULL << (8u * (4u - (uint32_t)(end & 3u)))) : FULL;
         return 8u * mis;                                   // bit position of the first code bit
     }
-    __device__ __forceinline__ void seek(uint32_t p) {
-        wbase = p >> 5;
+    __device__ __forceinline__ void seek(uint64_t p) {
+        wbase = (uint32_t)(p >> 5);
         win = ((uint64_t)word(wbase) << 32) | (uint64_t)word(wbase + 1);
         nextw = word(wbase + 2);
         raw = load_raw(wbase + 3);
-        pos = p;
+        pos = (uint32_t)p;
     }
+    __device__ __forceinline__ uint64_t position() const { return 32ull * wbase + (pos & 31u); }
     // the next 32 bits (not consumed)
     __device__ __forceinline__ uint32_t peek32() const { return (uint32_t)((win << (pos & 31u)) >> 32); }
+    // (pos & 31) + n <= 63: the window moves by one word exactly when bit 5 of pos flips
     __device__ __forceinline__ void skip(uint32_t n) {     // n <= 32
+        const uint32_t p0 = pos;
         pos += n;
-        if ((pos >> 5) != wbase) {
+        if ((p0 ^ pos) & 32u) {
             win = (win << 32) | (uint64_t)nextw;
             wbase++;
             nextw = finish(raw, wbase + 2);
@@ -404,11 +410,12 @@ struct BitSource {
     }
     // same as skip(), written so that it compiles to predicated straight-line code (fast decode loops)
     __device__ __forceinline__ void skip_flat(uint32_t n) {
+        const uint32_t p0 = pos;
         pos += n;
-        const bool cross = (pos >> 5) != wbase;
+        const bool cross = ((p0 ^ pos) & 32u) != 0u;
         const uint32_t fin = finish(raw, wbase + 3);       // becomes word (wbase+1)+2
         const uint32_t idx = wbase + 4u;
-        const bool fetch = cross & ((int)end_byte - (int)(4u * idx) > 0);
+        const bool fetch = cross & (idx < wend);
         win = cross ? ((win << 32) | (uint64_t)nextw) : win;
         nextw = cross ? fin : nextw;
         // predicated load straight into `raw` (no select behind it: a select would wait for the load).
@@ -427,6 +434,14 @@ struct BitSource {
         return v;
     }
 };
+
+// The saved state (l3c_dec_stream_t.state): low, high, value, then the code bits read, word 3 their low 32 bits.  A
+// stream of LONG_STREAM_BYTES or more also keeps their high bits in word 4, so its state takes 5 words; a shorter one
+// takes 4.  Every position inside a shorter stream is below 2^31 + 64 bits, so one of 2^32 or more lies far past its
+// end, where only zeros are read: such a position is saved as its low 32 bits with bit 31 of word 0 set (a saved low
+// never has it, as every renormalisation clears it) and restored as past the end.
+constexpr uint32_t LONG_STREAM_BYTES = 1u << 28;
+constexpr uint32_t PAST_END = 0x80000000u;
 
 // count of torchac.cpp:327 in the reference's modular 64-bit arithmetic (only needed when the code
 // value has left [low, high], i.e. on corrupt or foreign input) -- kept out of line on purpose
@@ -447,9 +462,9 @@ struct CoderState {
         dv = value;
     }
     __device__ __forceinline__ void restore(const uint32_t *st) {
-        low = st[0];
-        r = st[1] - st[0];
-        dv = st[2] - st[0];
+        low = st[0] & ~PAST_END;
+        r = st[1] - low;
+        dv = st[2] - low;
     }
     __device__ __forceinline__ void save(uint32_t *st) const {
         st[0] = low;
@@ -523,17 +538,23 @@ __device__ __forceinline__ uint32_t open_stream(const l3c_dec_stream_t &st, uint
         cs.reset(src.take(32));
     } else {
         cs.restore(st.state);
-        src.seek(st.state[3] + bit0);
+        const uint64_t hi = (st.in_len >= LONG_STREAM_BYTES) ? st.state[4] : (st.state[0] & PAST_END) ? 1u : 0u;
+        src.seek(((hi << 32) | st.state[3]) + bit0);
     }
     return bit0;
 }
 
-// one lane per stream
+// one lane per stream (the layout: LONG_STREAM_BYTES above)
 __device__ __forceinline__ void save_stream(const l3c_dec_stream_t &st, const CoderState &cs, const BitSource &src,
                                             uint32_t bit0) {
     if (st.state != nullptr) {
         cs.save(st.state);
-        st.state[3] = src.pos - bit0;
+        const uint64_t bits = src.position() - bit0;
+        st.state[3] = (uint32_t)bits;
+        if (st.in_len >= LONG_STREAM_BYTES)
+            st.state[4] = (uint32_t)(bits >> 32);
+        else if (bits >> 32)
+            st.state[0] |= PAST_END;
     }
 }
 

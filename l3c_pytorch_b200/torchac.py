@@ -133,10 +133,33 @@ def row_bytes(L):
     return 2 * np.where(L <= 32, 32, np.where(L <= 256, 256, (L + 7) // 8 * 8))
 
 
+SLOT_CAP_MAX = (1 << 32) - 4        # the encoder's out_cap is a uint32 multiple of 4
+
+
+def slot_caps(n_sym):
+    """encoder slot bytes of streams of n_sym symbols: 17 bits per symbol (every symbol on a 1-count interval) and the
+    terminator, clamped to SLOT_CAP_MAX (from about 2.02e9 symbols on; such a stream must code below 16 bits per
+    symbol, else _pack_offsets refuses it)"""
+    n = np.asarray(n_sym, np.int64)
+    return np.minimum(((n * 17 + 7) // 8 + 64 + 3) & ~3, SLOT_CAP_MAX)
+
+
 def enc_scratch_bytes(n_sym):
     """encode scratch of streams of n_sym symbols: 4 B of intervals per symbol and the coder's output slot"""
-    n = np.asarray(n_sym, np.int64)
-    return 4 * n + (((n * 17 + 7) // 8 + 64 + 3) & ~3)
+    return 4 * np.asarray(n_sym, np.int64) + slot_caps(n_sym)
+
+
+def _pack_offsets(len_words, caps, streams):
+    """The encoder's output lengths of the streams `streams` (uint32, as the int32 words of the device buffer) ->
+    (lengths int64, pack offsets int64 [len + 1]).  RuntimeError, before anything is packed, when a stream did not fit
+    its slot: the coder then wrote only its first caps bytes."""
+    lens = np.asarray(len_words).view(np.uint32).astype(np.int64)
+    over = np.flatnonzero(lens > caps)
+    if over.size:
+        k = int(over[0])
+        raise RuntimeError('stream %d: range coder output of %d bytes exceeded its slot of %d bytes (rows not strictly '
+                           'increasing?)' % (int(streams[k]), int(lens[k]), int(caps[k])))
+    return lens, np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
 
 
 def plan_decode(n_sym, L, cap=None):
@@ -314,7 +337,7 @@ def _encode_group(dev, src, n, Lp, cuda_syms, g):
     ng_src = np.ascontiguousarray(src[g])
     sym_off = np.concatenate([[0], np.cumsum(n[g])]).astype(np.int64)
     total = int(sym_off[-1])
-    caps = (((n[g] * 17 + 7) // 8 + 64 + 3) & ~3).astype(np.int64)
+    caps = slot_caps(n[g])
     slot_off = np.concatenate([[0], np.cumsum(caps)])
     src_dev = E._desc_to_device(ng_src, dev)
     off_dev = E._to_device_async(sym_off, dev)
@@ -335,14 +358,12 @@ def _encode_group(dev, src, n, Lp, cuda_syms, g):
     host = torch.empty(2 * ng, dtype=torch.int32, pin_memory=True)
     host.copy_(bad_lens, non_blocking=True)
     torch.cuda.current_stream().synchronize()
-    bad, lens = host.numpy()[:ng].astype(np.int64), host.numpy()[ng:].astype(np.int64)
+    bad = host.numpy()[:ng].astype(np.int64)
     for k in np.flatnonzero(bad >= 0):
         i = int(g[k])
         sym = int(cuda_syms[i][int(bad[k])].item()) if cuda_syms is not None else None
         raise RuntimeError('stream %d: symbol %s at position %d outside [0,%d]' % (i, sym, int(bad[k]), int(Lp[i]) - 2))
-    if (lens > caps).any():
-        raise RuntimeError('range coder output exceeded its slot (rows not strictly increasing?)')
-    dst = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    lens, dst = _pack_offsets(host.numpy()[ng:], caps, g)
     blob = torch.empty(int(dst[-1]) + 16, dtype=torch.uint8, device=dev)
     dst_dev = E._to_device_async(dst[:-1], dev)
     esz = np.dtype(_lib.ENC_STREAM_DTYPE).itemsize
@@ -395,7 +416,7 @@ def _decode_batch(dev, src, n, Lp, strings, to_cpu):
         blob = host_in.to(dev, non_blocking=True)
         out8 = torch.empty(max(n8, 1), dtype=torch.uint8, device=dev)
         out16 = torch.empty(max(n16, 1), dtype=torch.int16, device=dev)
-        state = torch.empty(4 * m, dtype=torch.int32, device=dev)
+        state = torch.empty(_lib.DEC_STATE_WORDS * m, dtype=torch.int32, device=dev)
         rows = torch.empty(max(int((np.minimum(n[s] - f, c) * row_bytes(L[s])).sum()) for s, f, c in chunks) // 2,
                            dtype=torch.int16, device=dev)
         alphabets = sorted(set(L.tolist()), key=lambda x: (x > 256, x))     # narrow first: the wide launch waits
@@ -412,7 +433,7 @@ def _decode_batch(dev, src, n, Lp, strings, to_cpu):
             dd['table'] = rows.data_ptr() + 2 * (row_off[:-1] - first * pitch[act])
             dd['in'] = blob.data_ptr() + in_off[act]
             dd['sym_out'] = np.where(wide[act], out16.data_ptr() + 2 * out_off[act], out8.data_ptr() + out_off[act])
-            dd['state'] = state.data_ptr() + 16 * act
+            dd['state'] = state.data_ptr() + 4 * _lib.DEC_STATE_WORDS * act
             dd['row_pitch'] = pitch[act]
             dd['n_sym'] = n[act]
             dd['in_len'] = in_len[act]
