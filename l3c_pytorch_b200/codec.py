@@ -314,10 +314,28 @@ def container_tile(data):
     return None
 
 
+def _walk_streams(data, pos, n, out):
+    """Read n streams (u32 length, then its bytes) from pos: -> the position after them, their (offset, length)
+    appended to `out` unless it is None.  ValueError where the file ends first."""
+    for _ in range(n):
+        if pos + 4 > len(data):
+            raise ValueError('truncated stream length')
+        ln, = struct.unpack_from('<I', data, pos)
+        pos += 4
+        if pos + ln > len(data):
+            raise ValueError('stream runs past the end of the file')
+        if out is not None:
+            out.append((pos, ln))
+        pos += ln
+    return pos
+
+
 def parse_container(data):
     """-> (pad_tuple, [(C, H, W, [(offset, length), ...])] coarse -> fine); tiled containers (container_tile)
     list C * tiles streams per scale.  Raises ValueError on a malformed file (the reference asserts on the
-    magic, bitcoding.py:154)."""
+    magic, bitcoding.py:154) and on a padding tuple that leaves no pixel of the finest scale on an axis.
+    The work is bounded by the file's size, whatever its headers declare: a scale whose streams' length fields and
+    separator cannot fit in the bytes left is refused before anything is built per stream."""
     if len(data) < 8:
         raise ValueError('container too short')
     pad_tuple = struct.unpack_from('<4H', data, 0)
@@ -333,20 +351,22 @@ def parse_container(data):
             raise ValueError('truncated scale header')
         C, H, W = struct.unpack_from('<BHH', data, pos)
         pos += 5
+        n = C * (1 if tile is None else -(-H // tile[0]) * -(-W // tile[1]))
+        if 4 * n + 4 > len(data) - pos:
+            # the walk fails within (len(data) - pos) / 4 fields; it only names where, as for a truncated file
+            _walk_streams(data, pos, n, None)
+            raise ValueError('scale separator missing: not a valid .l3c file')
         streams = []
-        for _ in range(C * len(tile_grid(H, W, tile))):
-            if pos + 4 > len(data):
-                raise ValueError('truncated stream length')
-            n, = struct.unpack_from('<I', data, pos)
-            pos += 4
-            if pos + n > len(data):
-                raise ValueError('stream runs past the end of the file')
-            streams.append((pos, n))
-            pos += n
+        pos = _walk_streams(data, pos, n, streams)
         if data[pos:pos + 4] != MAGIC:
             raise ValueError('scale separator missing: not a valid .l3c file')
         pos += 4
         scales.append((C, H, W, streams))
+    if scales:
+        left, right, top, bottom = pad_tuple
+        _, H, W, _ = scales[-1]
+        if left + right >= W or top + bottom >= H:
+            raise ValueError('padding tuple %r leaves no pixel of the %dx%d image' % (pad_tuple, H, W))
     return pad_tuple, scales
 
 
@@ -863,9 +883,8 @@ class BatchCodec(object):
             raise ValueError('decode_batch needs containers of identical shape')
         if any(len(sh) != len(shapes_of[0]) for sh in shapes_of):
             raise ValueError('decode_batch: containers with different numbers of scales')
-        for sh in shapes_of:
-            for (_, H, W) in sh:
-                check_plane(H, W, 'decode_batch')
+        for sh in {tuple(sh): sh for sh in shapes_of}.values():
+            self._check_shapes(sh)                  # before the upload: nothing is sized from a header it refuses
         blob, starts = _upload(datas, dev)
         offs = np.array([[starts[n] + o for (_, _, _, st) in parsed[n][1] for (o, _) in st] for n in range(N)],
                         np.int64)
