@@ -138,6 +138,30 @@ typedef struct {
 int l3c_ac_decode_streams(const l3c_dec_stream_t *streams_dev, int n_streams, int L,
                           uint32_t first, uint32_t count, void *stream);
 
+/* Seek points (DESIGN §4.13).  A seek point of a stream is the decoder's state before one of its symbols j: low, high
+ * and the code bits read, 32 + the sum of the renormalisation shifts of the symbols before j (64 bits), plus whether
+ * the last of those shifts was an "underflow" shift: then the code value is the last 32 code bits read with bit 31
+ * flipped, else those bits.  From a seek point the symbols from j on decode without the ones before it. */
+
+/* l3c_ac_encode_streams, same bytes and lengths, that also records a seek point before symbol j of stream i for
+ * j = every, 2 every, ... < n_sym: point j / every - 1 is the 4 words at points_dev[i] + 4 (j / every - 1) =
+ * (low, high, bits: low word, bits: high word | underflow flag << 31).  points_dev: device array of n_streams device
+ * pointers (a stream with no points may have null).  every: a positive multiple of 32. */
+int l3c_ac_encode_streams_seek(const l3c_enc_stream_t *streams_dev, int n_streams, uint32_t *out_len_dev,
+                               uint32_t every, uint32_t *const *points_dev, void *stream);
+
+/* Segment decode: every descriptor is one segment of a stream, decoded whole in one launch, all segments in
+ * parallel.  table and sym_out point at the segment's first symbol, n_sym is its length, in / in_len the whole
+ * stream.  state: null for a segment that starts at the stream's head, else its seek point as 5 words (low, high,
+ * flip, bits: low word, bits: high word), flip 0 or 0x80000000 (the underflow flag in bit 31); it is only read.  The
+ * segment's final symbol is decoded like any other.  L from 1 to 256 (l3c_ac_decode_streams' rows); larger alphabets
+ * are refused (L3C_EINVAL). */
+int l3c_ac_decode_segments(const l3c_dec_stream_t *segs_dev, int n_segs, int L, void *stream);
+
+/* l3c_ac_decode_segments for L = 256 whose `table`s point at coarse records (as l3c_ac_decode_streams_coarse). */
+int l3c_ac_decode_segments_coarse(const l3c_dec_stream_t *segs_dev, int n_segs, const float *targets_dev,
+                                  void *stream);
+
 /* Copies the first min(len_dev[i], out_cap) bytes of encoder slot i (a stream that outgrew its slot is truncated as
  * the slot holds it) to blob_dev + dst_off_dev[i] (byte offsets, any alignment: the final .l3c container layout, so
  * ONE device->host copy returns a whole batch).  Nothing else of the blob is written.  Any number of streams; more

@@ -62,6 +62,9 @@ _SIGNATURES = {
                                                              c_void_p]),
     'l3c_ac_encode_streams': (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     'l3c_ac_decode_streams': (c_int, [c_void_p, c_int, c_int, c_uint32, c_uint32, c_void_p]),
+    'l3c_ac_encode_streams_seek': (c_int, [c_void_p, c_int, c_void_p, c_uint32, c_void_p, c_void_p]),
+    'l3c_ac_decode_segments': (c_int, [c_void_p, c_int, c_int, c_void_p]),
+    'l3c_ac_decode_segments_coarse': (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     'l3c_uniform_cdf_row': (c_int, [c_int, c_void_p]),
     'l3c_lut_intervals': (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     'l3c_dmll_intervals': (c_int, [c_void_p] * 3 + [c_int] * 6 + [c_void_p, c_void_p]),

@@ -18,10 +18,11 @@ import torch
 
 from . import auto_crop, pad, part_suffix_helper
 from .blueprint import MultiscaleBlueprint
-from .codec import BatchCodec, MAGIC
+from .codec import BatchCodec, MAGIC, parse_container
 from .times import NoOp
 
 _MAGIC_VALUE_SEP = MAGIC
+SEEK_SUFFIX = '.seek'          # a container's seek index beside it (DESIGN §4.13)
 
 # Largest N * Hmax * Wmax (padded pixels of the batch tensor) coded in one ragged pass: 16 images of up to 768 x 768
 # (tools/bench_mixed.py) -- the activations, mixture parameters and CDF rows of such a pass fit an 80 GB GPU.
@@ -112,7 +113,7 @@ class Bitcoding(object):
             return plan_passes([tuple(t.shape[-2:]) for (t, _) in prepared])
         return _groups((tuple(t.shape), pt) for (t, pt) in prepared)
 
-    def _begin_pass(self, prepared, idxs):
+    def _begin_pass(self, prepared, idxs, seek=None):
         """Enqueue the encode of prepared[idxs] as one batch on the current stream -> codec EncodeJob.  Images of
         different shapes are placed top-left in a zero batch of the largest extent (a ragged batch)."""
         imgs = [prepared[i][0] for i in idxs]
@@ -121,16 +122,19 @@ class Bitcoding(object):
         if all(sh == shapes[0] for sh in shapes):
             batch = torch.cat(imgs, 0) if len(imgs) > 1 else imgs[0]
             pt = pts[0] if all(p == pts[0] for p in pts) else pts
-            return self.codec.encode_begin(batch, pt, tile=self.tile, recursive=self.recursive)
+            return self.codec.encode_begin(batch, pt, tile=self.tile, recursive=self.recursive, seek=seek)
         Hb, Wb = max(h for (h, _) in shapes), max(w for (_, w) in shapes)
         batch = torch.zeros(len(imgs), 3, Hb, Wb, dtype=torch.uint8, device=self._device())
         for k, t in enumerate(imgs):
             batch[k, :, :t.shape[2], :t.shape[3]] = t[0]
-        return self.codec.encode_begin(batch, pts, tile=self.tile, extents=shapes, recursive=self.recursive)
+        return self.codec.encode_begin(batch, pts, tile=self.tile, extents=shapes, recursive=self.recursive, seek=seek)
 
-    def encode(self, img, pout):
-        """img: int64 (or uint8) CHW / 1CHW tensor with values 0..255; writes `pout`; returns bpsp."""
+    def encode(self, img, pout, seek=None):
+        """img: int64 (or uint8) CHW / 1CHW tensor with values 0..255; writes `pout`; returns bpsp.
+        seek = K (reference layout): also writes the container's seek index (DESIGN §4.13) to `pout + '.seek'`, and
+        for auto-crops `pout.partN.seek` beside every part."""
         assert not os.path.isfile(pout)
+        assert seek is None or not os.path.isfile(pout + SEEK_SUFFIX)
         if len(img.shape) == 3:
             img = img.unsqueeze(0)
         assert len(img.shape) == 4 and img.shape[0] == 1 and img.shape[1] == 3, img.shape
@@ -147,22 +151,27 @@ class Bitcoding(object):
             stale = [q for q in part_suffix_helper.existing_parts(pout) if q not in pouts]
             assert not any(os.path.isfile(q) for q in pouts) and not stale, \
                 'part files of {} already exist: {}'.format(pout, [q for q in pouts if os.path.isfile(q)] + stale)
-            bpsps = self._encode_many(crops, pouts)
+            assert seek is None or not any(os.path.isfile(q + SEEK_SUFFIX) for q in pouts), \
+                'seek indexes of the parts of {} already exist'.format(pout)
+            bpsps = self._encode_many(crops, pouts, seek)
             for crop, bpsp in zip(crops, bpsps):
                 combinator.add(bpsp, np.prod(crop.shape[-2:]))
             return combinator.get_bpsp()
-        return self._encode_many([img], [pout])[0]
+        return self._encode_many([img], [pout], seek)[0]
 
-    def _encode_many(self, imgs, pouts):
+    def _encode_many(self, imgs, pouts, seek=None):
         """Images are coded in ragged passes (any mix of shapes, plan_passes) where the codec supports them;
         otherwise, and with compare_with_theory, images of equal (padded) shape are coded as one batch."""
         prepared = [self._prepare(im) for im in imgs]
-        if not self.compare_with_theory and self.codec.ragged_unsupported(self.tile) is None:
-            datas, bpsps = self._encode_prepared(prepared).finish()
-            for i, dta in enumerate(datas):
+        if seek is not None or (not self.compare_with_theory and self.codec.ragged_unsupported(self.tile) is None):
+            res = self._encode_prepared(prepared, seek).finish()
+            for i, dta in enumerate(res[0]):
                 with open(pouts[i], 'wb') as f:
                     f.write(dta)
-            return bpsps
+                if seek is not None:
+                    with open(pouts[i] + SEEK_SUFFIX, 'wb') as f:
+                        f.write(res[2][i])
+            return res[1]
         bpsps = [None] * len(imgs)
         for idxs in _groups((tuple(t.shape), pt) for (t, pt) in prepared):
             batch = torch.cat([prepared[i][0] for i in idxs], 0)
@@ -194,7 +203,8 @@ class Bitcoding(object):
         return bpsps
 
     def decode(self, pin, _recurse_part=True):
-        """-> decoded image, int64 1CHW (on the GPU)."""
+        """-> decoded image, int64 1CHW (on the GPU).  A seek index beside a file (`pin + '.seek'`, `pin.partN.seek`)
+        is used (decode_batch(seeks=)); ValueError naming the index when it does not match its file."""
         if _recurse_part and part_suffix_helper.contains_part_suffix(pin):
             paths = part_suffix_helper.iter_part_suffixes(pin)
             parts = self._decode_many(paths)
@@ -203,25 +213,36 @@ class Bitcoding(object):
         return self._decode_many([pin])[0]
 
     def _decode_many(self, paths):
-        datas = []
+        from . import seek as _seek
+        datas, seeks = [], []
         for p in paths:
             with open(p, 'rb') as f:
                 datas.append(f.read())
-        return self.decode_batch(datas)
+            sk = None
+            if os.path.isfile(p + SEEK_SUFFIX):
+                with open(p + SEEK_SUFFIX, 'rb') as f:
+                    sk = f.read()
+                try:
+                    _seek.parse_index(sk, datas[-1])
+                except ValueError as e:
+                    raise ValueError('%s: %s' % (p + SEEK_SUFFIX, e))
+            seeks.append(sk)
+        return self.decode_batch(datas, seeks if any(sk is not None for sk in seeks) else None)
 
     # ------------------------------------------------------------------------------------------
     # H100-first batch API
-    def encode_batch(self, imgs_u8):
+    def encode_batch(self, imgs_u8, seek=None):
         """imgs_u8: uint8 [N,3,H,W] (any device), or a list / tuple of uint8 [3,H,W] / [1,3,H,W] images of any
-        sizes -> (list of container bytes, bpsp list) in input order."""
-        return self.encode_batch_begin(imgs_u8).finish()
+        sizes -> (list of container bytes, bpsp list) in input order.  seek = K (reference layout): -> (containers,
+        bpsps, seek indexes), the containers the same bytes (BatchCodec.encode_begin)."""
+        return self.encode_batch_begin(imgs_u8, seek=seek).finish()
 
-    def _encode_prepared(self, prepared):
+    def _encode_prepared(self, prepared, seek=None):
         """Enqueue the passes of `prepared` on the current stream -> _ListEncodeJob."""
-        jobs = [(idxs, self._begin_pass(prepared, idxs)) for idxs in self._passes(prepared)]
-        return _ListEncodeJob(jobs, [int(np.prod(t.shape[1:])) for (t, _) in prepared])
+        jobs = [(idxs, self._begin_pass(prepared, idxs, seek)) for idxs in self._passes(prepared)]
+        return _ListEncodeJob(jobs, [int(np.prod(t.shape[1:])) for (t, _) in prepared], seek is not None)
 
-    def encode_batch_begin(self, imgs_u8, stream=None):
+    def encode_batch_begin(self, imgs_u8, stream=None, seek=None):
         """Asynchronous encode_batch: enqueues the upload and the whole GPU side on `stream` (default:
         the current stream) and returns a job at once; job.finish() -> (containers, bpsps).  With
         `stream=self.side_stream(N)` the encode runs beside a decode_batch of another batch: the
@@ -238,7 +259,7 @@ class Bitcoding(object):
                 why = self.codec.ragged_unsupported(self.tile)
                 if why is not None and len({tuple(t.shape) for (t, _) in prepared}) > 1:
                     raise NotImplementedError(why)
-                return self._encode_prepared(prepared)
+                return self._encode_prepared(prepared, seek)
         pt = pad.padding_tuple(imgs_u8.shape[-2], imgs_u8.shape[-1], self.pad_factor())
         stream = stream if stream is not None else torch.cuda.current_stream(self._device())
         with torch.cuda.stream(stream):
@@ -246,9 +267,9 @@ class Bitcoding(object):
             if any(pt):
                 x = torch.nn.functional.pad(x, pt, 'constant')
             x = x.contiguous()
-            job = self.codec.encode_begin(x, pt, tile=self.tile, recursive=self.recursive)
+            job = self.codec.encode_begin(x, pt, tile=self.tile, recursive=self.recursive, seek=seek)
         N = x.shape[0]
-        return _ListEncodeJob([(list(range(N)), job)], [int(np.prod(x.shape[1:]))] * N)
+        return _ListEncodeJob([(list(range(N)), job)], [int(np.prod(x.shape[1:]))] * N, seek is not None)
 
     def side_stream(self, n_images, n_lanes=1):
         """Stream for encode_batch_begin() calls that should overlap decode_batch calls of `n_images` each."""
@@ -260,9 +281,12 @@ class Bitcoding(object):
         decode of one batch is bound by the serial chain of its range coder and leaves most of the GPU idle."""
         return self.codec.lanes(self._device(), 3 * n_images, n_lanes)[0]
 
-    def decode_batch(self, datas, lane=None):
+    def decode_batch(self, datas, seeks=None, lane=None):
         """list of container bytes (any mix of shapes) -> list of int64 1CHW tensors (GPU).  Ragged passes
-        (plan_passes) where the codec supports them, else one pass per shape."""
+        (plan_passes) where the codec supports them, else one pass per shape.  seeks: a seek index (bytes) or None
+        per container: the streams of an indexed container decode as parallel segments (DESIGN §4.13)."""
+        if seeks is not None and len(seeks) != len(datas):
+            raise ValueError('%d seek indexes for %d containers' % (len(seeks), len(datas)))
         from .codec import parse_container, container_tile
         parsed = [parse_container(d) for d in datas]
         if self.codec.ragged_unsupported(container_tile(datas[0]) if datas else None) is None and \
@@ -272,7 +296,8 @@ class Bitcoding(object):
             passes = _groups((tuple((C, H, W) for (C, H, W, _) in scales), pt) for (pt, scales) in parsed)
         outs = [None] * len(datas)
         for idxs in passes:
-            S, _ = self.codec.decode_batch([datas[i] for i in idxs], to_host=False, lane=lane)
+            S, _ = self.codec.decode_batch([datas[i] for i in idxs], to_host=False, lane=lane,
+                                           seeks=None if seeks is None else [seeks[i] for i in idxs])
             for k, i in enumerate(idxs):
                 pt, scales = parsed[i]
                 H, W = scales[-1][1:3] if scales else S.shape[-2:]
@@ -280,6 +305,22 @@ class Bitcoding(object):
                 if any(pt):
                     img = pad.undo_pad(img, *pt)
                 outs[i] = img
+        return outs
+
+    def seek_index(self, datas, every=None):
+        """Seek indexes (sidecar bytes, DESIGN §4.13) of reference-layout containers, e.g. files the reference or an
+        earlier encode wrote, from one serial decode (BatchCodec.seek_index); every = K, default 4096."""
+        from . import seek as _seek
+        every = _seek.DEFAULT_EVERY if every is None else every
+        parsed = [parse_container(d) for d in datas]
+        if self.codec.ragged_unsupported() is None and all(len(p[1]) for p in parsed):
+            passes = plan_passes([p[1][-1][1:3] for p in parsed])
+        else:
+            passes = _groups(tuple((C, H, W) for (C, H, W, _) in scales) for (_, scales) in parsed)
+        outs = [None] * len(datas)
+        for idxs in passes:
+            for i, sk in zip(idxs, self.codec.seek_index([datas[i] for i in idxs], every)):
+                outs[i] = sk
         return outs
 
     def decode_region(self, data, region, level=0, lane=None):
@@ -332,16 +373,21 @@ class _ListEncodeJob:
     """encode_batch_begin: the codec jobs of its passes (one for a batch tensor); finish() -> (containers, bpsps) in
     input order."""
 
-    def __init__(self, jobs, nsubs):
-        self.jobs, self.nsubs = jobs, nsubs
+    def __init__(self, jobs, nsubs, seek=False):
+        self.jobs, self.nsubs, self.seek = jobs, nsubs, seek
 
     def finish(self):
+        """-> (containers, bpsps), and their seek indexes third when the encode records them"""
         datas = [None] * len(self.nsubs)
+        seeks = [None] * len(self.nsubs)
         for idxs, job in self.jobs:
-            d, _ = job.finish(to_host=True)
+            d, info = job.finish(to_host=True)
             for k, i in enumerate(idxs):
                 datas[i] = d[k]
-        return datas, [len(d) * 8 / n for d, n in zip(datas, self.nsubs)]
+                if self.seek:
+                    seeks[i] = info['seeks'][k]
+        bpsps = [len(d) * 8 / n for d, n in zip(datas, self.nsubs)]
+        return (datas, bpsps, seeks) if self.seek else (datas, bpsps)
 
 
 # --- header field helpers (bitcoding.py:326-375), little-endian -------------------------------

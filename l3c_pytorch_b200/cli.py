@@ -1,12 +1,17 @@
 """Single-image command line: the encode/decode half of the reference's `l3c.py`
 (/root/reference/src/l3c.py:74-129) on the H100 path.
 
-    python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt enc IMG OUT.l3c [--overwrite]
+    python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt enc IMG OUT.l3c [--overwrite] [--seek K]
+    python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt idx IN.l3c [--every K]
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png
     python -m l3c_pytorch_b200.cli --config cr_rgb_shared --ckpt CKPT.pt enc IMG OUT.l3c --recursive auto
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt dec IN.l3c OUT.png --region Y,X,H,W [--level K]
     python -m l3c_pytorch_b200.cli --config cr --ckpt CKPT.pt upd IN.l3c PATCH.png Y,X OUT.l3c [--overwrite]
                                                                   [--edit PATCH2.png Y2,X2 ...]
+
+`enc --seek K` also writes OUT.l3c.seek, the file's seek index (DESIGN §4.13): the range coder's state every K
+symbols, with which `dec` decodes every stream as parallel segments; the .l3c file itself is unchanged.  `idx`
+writes the index of an existing file (one written by the reference, say).
 
 `upd --edit PATCH.png Y,X` (repeatable) applies more edits after the positional one, in order, in one call that
 re-encodes every tile the edits reach once (DESIGN §4.12, "Batches of updates").
@@ -27,6 +32,7 @@ import numpy as np
 import torch
 
 from . import codec
+from .bitcoding import SEEK_SUFFIX
 
 
 class EncodeError(Exception):
@@ -78,18 +84,24 @@ def write_image(img_1chw, path):
     Image.fromarray(arr).save(path)
 
 
-def encode(bc, img_p, pout, overwrite=False):
-    if os.path.isfile(pout) or os.path.isfile(pout + '.part0'):
+def encode(bc, img_p, pout, overwrite=False, seek=None):
+    if os.path.isfile(pout) or os.path.isfile(pout + '.part0') or os.path.isfile(pout + SEEK_SUFFIX):
         if not overwrite:
             raise EncodeError('{} exists. Consider --overwrite.'.format(pout))
+        # the parts and every seek index beside them: a stale index would no longer match its file
         for q in [pout] + [pout + '.part%d' % i for i in range(4096)]:
+            if os.path.isfile(q + SEEK_SUFFIX):
+                os.remove(q + SEEK_SUFFIX)
             if os.path.isfile(q):
                 os.remove(q)
             elif q != pout:
                 break
     # a tiled file holds one image of any size (DESIGN §4.10): read up to the largest plane the kernels index
     img = read_image(img_p, codec.MAX_PLANE_PIXELS if bc.tile is not None else None)
-    bpsp = bc.encode(img, pout)
+    try:
+        bpsp = bc.encode(img, pout) if seek is None else bc.encode(img, pout, seek=seek)
+    except ValueError as err:
+        raise EncodeError(str(err))
     print('Encoded {} -> {}: {:.4f} bpsp'.format(img_p, pout, bpsp))
     return bpsp
 
@@ -100,9 +112,35 @@ def decode(bc, pin, png_out):
             pin = pin + '.part0'
         else:
             raise DecodeError('File not found: {}'.format(pin))
-    img = bc.decode(pin)
+    try:
+        img = bc.decode(pin)
+    except ValueError as err:
+        raise DecodeError(str(err))
     write_image(img, png_out)
     print('Decoded {} -> {}'.format(pin, png_out))
+
+
+def index(bc, pin, every=None, overwrite=False):
+    """writes the seek index of pin (and of its .partN files) beside it -> the paths written"""
+    from . import part_suffix_helper
+    paths = [pin] if os.path.isfile(pin) else part_suffix_helper.existing_parts(pin)
+    if not paths:
+        raise DecodeError('File not found: {}'.format(pin))
+    if not overwrite and any(os.path.isfile(q + SEEK_SUFFIX) for q in paths):
+        raise EncodeError('{} exists. Consider --overwrite.'.format(paths[0] + SEEK_SUFFIX))
+    datas = []
+    for q in paths:
+        with open(q, 'rb') as f:
+            datas.append(f.read())
+    try:
+        seeks = bc.seek_index(datas, every)
+    except ValueError as err:
+        raise DecodeError(str(err))
+    for q, sk in zip(paths, seeks):
+        with open(q + SEEK_SUFFIX, 'wb') as f:
+            f.write(sk)
+        print('Indexed {} -> {}: {} bytes'.format(q, q + SEEK_SUFFIX, len(sk)))
+    return [q + SEEK_SUFFIX for q in paths]
 
 
 def recursive_of(args, config_ms):
@@ -129,6 +167,13 @@ def build_parser():
                    help='write ONE tiled file (tiles of TH x TW coded as independent streams) for an image of any '
                         'size, no .partN crops; `dec` decodes it in bands and `dec --region` reads crops of it.  Not '
                         'readable by the reference')
+    e.add_argument('--seek', default=None, type=int, metavar='K',
+                   help='also write OUT.seek, a seek index of the coder state every K symbols (a multiple of 32; '
+                        '4096 is a good default) with which `dec` decodes the streams in parallel')
+    x = sub.add_parser('idx', help='write IN.l3c.seek, the seek index of an existing reference-layout file')
+    x.add_argument('inp')
+    x.add_argument('--every', default=None, type=int, metavar='K', help='symbols between seek points (4096)')
+    x.add_argument('--overwrite', action='store_true')
     d = sub.add_parser('dec')
     d.add_argument('inp')
     d.add_argument('out_png')
@@ -244,7 +289,9 @@ def main(argv=None):
     bc = Bitcoding(bp, recursive=recursive_of(a, bp.net.config_ms), tile=tile, crop=tile is None)
     try:
         if a.mode == 'enc':
-            encode(bc, a.img, a.out, a.overwrite)
+            encode(bc, a.img, a.out, a.overwrite, a.seek)
+        elif a.mode == 'idx':
+            index(bc, a.inp, a.every, a.overwrite)
         elif a.mode == 'upd':
             try:
                 update_region(bc, a.inp, a.patch, a.pos, a.out, a.overwrite, a.edit)

@@ -33,6 +33,7 @@ import torch
 
 from . import _lib
 from . import engine as E
+from . import seek as _seek
 from .dmll import non_shared_get_K
 
 MAGIC = b'\x46\xE2\x84\x92'          # bitcoding.py:36
@@ -396,6 +397,8 @@ class EncodeJob:
     encode_batch.  shapes: [(scale, C, H, W)] of the batch tensors; shapes_of / pads: the container shapes
     [(scale, C, h_n, w_n)] and the padding tuple of every image; caps: slot bytes [N][streams per image]."""
 
+    seek = None        # (K, point counts per stream, device points int32 [points][4]): encode_begin(seek=K)
+
     def __init__(self, codec, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, keep):
         self.codec, self.shapes, self.shapes_of, self.pads, self.tile, self.out = codec, shapes, shapes_of, pads, tile, out
         self.caps, self.desc_dev, self.lens_dev = caps, desc_dev, lens_dev
@@ -425,10 +428,16 @@ class EncodeJob:
                 pieces_all.append(pieces)
                 sizes.append(total)
                 pos += (total + 15) & ~15
-            blob = torch.empty(pos + 16, dtype=torch.uint8, device=self.lens_dev.device)
+            # seek points (encode_begin(seek=K)) ride behind the containers: one copy to the host for both
+            n_pt = 0 if self.seek is None else self.seek[2].shape[0]
+            blob = torch.empty(pos + 16 + 16 * n_pt, dtype=torch.uint8, device=self.lens_dev.device)
             E.pack_streams(self.desc_dev, self.lens_dev, dst.reshape(-1), N * per_img, blob)
             info = dict(sizes=sizes, starts=starts, lens=lens, shapes=self.shapes, shapes_of=self.shapes_of,
                         out=self.out, stream_offsets=dst, tile=self.tile)
+            if n_pt:
+                blob[pos + 16:].view(torch.int32).view(n_pt, 4).copy_(self.seek[2])
+            if self.seek is not None:
+                info['seek_points'] = blob[pos + 16:].view(torch.int32).view(n_pt, 4)
             if not to_host:
                 self.packed = torch.cuda.Event()
                 self.packed.record(self.stream)
@@ -446,7 +455,23 @@ class EncodeJob:
             for (o, b) in pieces_all[n]:
                 buf[s0 + o:s0 + o + len(b)] = np.frombuffer(b, np.uint8)
             datas.append(buf[s0:s0 + sizes[n]].tobytes())
+        if self.seek is not None:
+            info['seeks'] = self._seek_indexes(datas, buf[pos + 16:].view(np.uint32).reshape(-1, 4), per_img)
         return datas, info
+
+    def _seek_indexes(self, datas, words, per_img):
+        """the sidecar bytes of every container from the recorded points (l3c_ac_encode_streams_seek's layout)"""
+        every, counts, _ = self.seek
+        words = words.astype(np.int64)
+        first = np.cumsum(counts) - counts
+        out = []
+        for n, dta in enumerate(datas):
+            cnt = counts[n * per_img:(n + 1) * per_img]
+            a = int(first[n * per_img]) if cnt.size else 0
+            w = words[a:a + int(cnt.sum())]
+            out.append(_seek.write_index(dta, every, cnt, w[:, 0], w[:, 1], w[:, 3] & 0x80000000,
+                                         w[:, 2] | ((w[:, 3] & 0x7FFFFFFF) << 32)))
+        return out
 
 
 class _UpdateJob(object):
@@ -516,6 +541,73 @@ class UpdateJob(object):
         return outs
 
 
+class _SegmentDecode(object):
+    """decode_device's stream hook for seek-indexed images (DESIGN §4.13): the seek points of the batch uploaded once,
+    and per call one l3c_ac_decode_segments launch of every segment of the descriptors' streams.  blob / offs as in
+    decode_device; seeks: seek.SeekIndex or None per image."""
+
+    def __init__(self, blob, offs, seeks):
+        N, P = offs.shape
+        self.dev = blob.device
+        addr = blob.data_ptr() + offs.reshape(-1)
+        every = np.full(N * P, 1 << 40, np.int64)            # no index: one segment per stream
+        first = np.zeros(N * P, np.int64)
+        words, base = [], 0
+        for n, sk in enumerate(seeks):
+            if sk is None:
+                continue
+            if sk.counts.size != P:
+                raise ValueError('seek index %d lists %d streams, the container has %d' % (n, sk.counts.size, P))
+            every[n * P:(n + 1) * P] = sk.every
+            first[n * P:(n + 1) * P] = base + sk.first
+            words.append(sk.state_words())
+            base += sk.low.size
+        order = np.argsort(addr, kind='stable')
+        self.addr, self.every, self.first = addr[order], every[order], first[order]
+        w = np.concatenate(words) if words else np.zeros((0, _seek.STATE_WORDS), np.uint32)
+        self.states = E._to_device_async(np.concatenate([w.reshape(-1), [0]]).astype(np.uint32).view(np.int32),
+                                         self.dev)
+
+    def decode(self, dmll, desc, coarse):
+        segs = _seek.plan_segments(desc, self.addr, self.every, self.first, self.states.data_ptr())
+        E.ac_decode_segments(segs, self.dev, dmll.L, dmll.targets(self.dev) if coarse else None)
+
+
+class _StateRecorder(object):
+    """decode_device's stream hook for BatchCodec.seek_index: decodes the descriptors' streams serially in launches of
+    `every` symbols and copies their saved states (l3c_dec_stream_t.state) into `points` after each launch, where the
+    stream has symbols left.  n_sym int64 [N][P]: symbols of every stream, in offs' order."""
+
+    def __init__(self, blob, offs, n_sym, every):
+        self.dev, self.every = blob.device, every
+        self.counts = _seek.point_counts(n_sym.reshape(-1), every)
+        self.first = np.concatenate([[0], np.cumsum(self.counts)[:-1]]).astype(np.int64)
+        addr = blob.data_ptr() + offs.reshape(-1)
+        self.order = np.argsort(addr, kind='stable')
+        self.addr = addr[self.order]
+        self.points = torch.zeros(int(self.counts.sum()), _lib.DEC_STATE_WORDS, dtype=torch.int32, device=self.dev)
+
+    def decode(self, dmll, desc, coarse):
+        M, K = desc.size, self.every
+        k = self.order[np.searchsorted(self.addr, desc['in'].astype(np.int64))]
+        state = torch.zeros(M, _lib.DEC_STATE_WORDS, dtype=torch.int32, device=self.dev)
+        desc = desc.copy()
+        desc['state'] = state.data_ptr() + 4 * _lib.DEC_STATE_WORDS * np.arange(M)
+        desc_dev = E._desc_to_device(desc, self.dev)
+        n = desc['n_sym'].astype(np.int64)
+        tg = dmll.targets(self.dev) if coarse else None
+        for first in range(0, int(n.max()) if M else 0, K):
+            if coarse:
+                E.ac_decode_streams_coarse(None, self.dev, tg, first, K, desc_dev, M)
+            else:
+                E.ac_decode_streams(None, self.dev, dmll.L, first, K, desc_dev, M)
+            sel = np.nonzero(n > first + K)[0]
+            if sel.size:
+                rows = self.first[k[sel]] + first // K
+                self.points.index_copy_(0, E._to_device_async(rows, self.dev),
+                                        state.index_select(0, E._to_device_async(sel.astype(np.int64), self.dev)))
+
+
 class BatchCodec(object):
     def __init__(self, blueprint):
         self.blueprint = blueprint
@@ -578,15 +670,16 @@ class BatchCodec(object):
 
     # ------------------------------------------------------------------------------------------
     def encode_batch(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, to_host=True, tile=None, extents=None,
-                     recursive=0):
+                     recursive=0, seek=None):
         """imgs_u8: uint8 [N,3,H,W] on the GPU, H and W multiples of 2**num_scales.  pad_tuple: the padding
         tuple written into every container, or a list of one per image.
         Returns a list of N container byte strings (or, with to_host=False, the device blob,
         per-image sizes and offsets, leaving the bytes in HBM).  `out`: a precomputed network Out.
         tile = (th, tw): tiled containers (ContainerLayout).
         extents = [(h_n, w_n)]: a ragged batch (encode_begin).
-        recursive = R: recursive containers (encode_begin)."""
-        return self.encode_begin(imgs_u8, pad_tuple, out, tile, extents, recursive).finish(to_host)
+        recursive = R: recursive containers (encode_begin).
+        seek = K: also seek indexes (encode_begin); info['seeks'] holds them."""
+        return self.encode_begin(imgs_u8, pad_tuple, out, tile, extents, recursive, seek).finish(to_host)
 
     def ragged_unsupported(self, tile=None):
         """Why this codec cannot code a ragged batch (a message naming it), or None when it can."""
@@ -616,7 +709,8 @@ class BatchCodec(object):
         return ext
 
     @_on_device
-    def encode_begin(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, tile=None, extents=None, recursive=0):
+    def encode_begin(self, imgs_u8, pad_tuple=(0, 0, 0, 0), out=None, tile=None, extents=None, recursive=0,
+                     seek=None):
         """First half of encode_batch: enqueues the whole GPU side of an encode (networks, intervals,
         the range-coder launch, the copy of the stream lengths to pinned memory) on the CURRENT stream
         and returns without waiting.  EncodeJob.finish() completes it.  Lets a caller overlap the
@@ -629,8 +723,16 @@ class BatchCodec(object):
         bottlenecks, reference layout only.  Extents that all equal the tensor are the equal-size call.
         recursive = R > 0 (RGB baselines, DESIGN §4.7): the last trained scale codes its own thumbnails R more
         times (forward(auto_recurse=R)); H and W must be multiples of 2**(num_scales + R); every stream of the
-        batch is still coded in one range-coder launch.  `out`, if given, must come from forward(auto_recurse=R)."""
+        batch is still coded in one range-coder launch.  `out`, if given, must come from forward(auto_recurse=R).
+        seek = K (reference layout only, DESIGN §4.13): the range coder also records every stream's state every K
+        symbols (l3c_ac_encode_streams_seek; the containers are the same bytes) and finish() returns a seek index per
+        container in info['seeks'].  ValueError with tile= and for a K that is not a multiple of 32 in [32, 2^24]."""
         assert imgs_u8.dtype == torch.uint8 and imgs_u8.dim() == 4 and imgs_u8.shape[1] == 3
+        if seek is not None:
+            if tile is not None:
+                raise ValueError('seek indexes are for the reference layout; tiled containers (tile=%s) decode their '
+                                 'tiles in parallel already' % (tuple(tile),))
+            seek = _seek.check_every(seek)
         recursive = self.check_recursive(recursive)
         dev = imgs_u8.device
         N, _, Hb, Wb = imgs_u8.shape
@@ -677,8 +779,17 @@ class BatchCodec(object):
         si, elem, n_sym, _ = stream_layout([[s[1:] for s in sh] for sh in shapes_of], tile)
         bases = np.array([iv.data_ptr() for iv in ivs], np.int64)
         caps, slots, desc = _enc_descs(bases[si] + elem * 4, n_sym, dev)
-        desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
-        return EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, (imgs_u8, ivs, slots))
+        if seek is None:
+            desc_dev, lens_dev = E.ac_encode_streams(desc, dev)
+            return EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev, (imgs_u8, ivs, slots))
+        counts = _seek.point_counts(desc['n_sym'], seek)
+        points = torch.empty(max(1, int(counts.sum())), 4, dtype=torch.int32, device=dev)
+        desc_dev, lens_dev, ptrs = E.ac_encode_streams_seek(desc, dev, seek, points,
+                                                            np.cumsum(counts) - counts)
+        job = EncodeJob(self, shapes, shapes_of, pads, tile, out, caps, desc_dev, lens_dev,
+                        (imgs_u8, ivs, slots, ptrs))
+        job.seek = (seek, counts, points[:int(counts.sum())])
+        return job
 
     @staticmethod
     def encode_banded(shape, tile, extents=None, out=None):
@@ -868,13 +979,19 @@ class BatchCodec(object):
 
     # ------------------------------------------------------------------------------------------
     @_on_device
-    def decode_batch(self, datas, to_host=True, lane=None):
+    def decode_batch(self, datas, to_host=True, lane=None, seeks=None):
         """datas: list of container byte strings of equally shaped images -- or, where ragged batches are supported
         (ragged_unsupported), of any mix of shapes: image n then is the top-left H_n x W_n of the result (the
         finest scale of its container), zero elsewhere.
+        seeks: one seek index (sidecar bytes, seek.parse_index) or None per container: containers with one decode
+        every stream as parallel segments (decode_device), the others serially; the same result either way.
         Returns (uint8 [N,3,H,W] incl. padding, pad_tuple list)."""
         dev = self.blueprint.device
         N = len(datas)
+        if seeks is not None:
+            if len(seeks) != N:
+                raise ValueError('%d seek indexes for %d containers' % (len(seeks), N))
+            seeks = [None if sk is None else _seek.parse_index(sk, dta) for sk, dta in zip(seeks, datas)]
         parsed = [parse_container(d) for d in datas]
         tile = container_tile(datas[0])
         shapes_of = [[(C, H, W) for (C, H, W, _) in p[1]] for p in parsed]
@@ -889,11 +1006,55 @@ class BatchCodec(object):
         offs = np.array([[starts[n] + o for (_, _, _, st) in parsed[n][1] for (o, _) in st] for n in range(N)],
                         np.int64)
         lens = np.array([[ln for (_, _, _, st) in parsed[n][1] for (_, ln) in st] for n in range(N)], np.int64)
-        S = self.decode_device(blob, offs, lens, shapes_of, lane=lane, tile=tile)
+        S = self.decode_device(blob, offs, lens, shapes_of, lane=lane, tile=tile, seeks=seeks)
         pads = [p[0] for p in parsed]
         if to_host:
             return S.cpu(), pads
         return S, pads
+
+    @_on_device
+    def seek_index(self, datas, every=_seek.DEFAULT_EVERY, lane=None):
+        """Seek indexes (sidecar bytes, DESIGN §4.13) of reference-layout containers, e.g. ones the reference or an
+        earlier encode wrote: one serial decode of the batch (containers as decode_batch takes them) in launches of
+        `every` symbols, the decoders' saved states copied aside on the device after each.  The same bytes as
+        encode_begin(..., seek=every) writes for the same containers.  ValueError for a tiled container or an
+        interval that is not a multiple of 32 in [32, 2^24]."""
+        every = _seek.check_every(every)
+        n_sym = [_seek.stream_symbols(dta) for dta in datas]
+        dev = self.blueprint.device
+        N = len(datas)
+        parsed = [parse_container(d) for d in datas]
+        shapes_of = [[(C, H, W) for (C, H, W, _) in p[1]] for p in parsed]
+        if any(sh != shapes_of[0] for sh in shapes_of) and self.ragged_unsupported() is not None:
+            raise ValueError('seek_index needs containers of identical shape')
+        if any(len(sh) != len(shapes_of[0]) for sh in shapes_of):
+            raise ValueError('seek_index: containers with different numbers of scales')
+        for sh in {tuple(sh): sh for sh in shapes_of}.values():
+            self._check_shapes(sh)
+        blob, starts = _upload(datas, dev)
+        offs = np.array([[starts[n] + o for (_, _, _, st) in parsed[n][1] for (o, _) in st] for n in range(N)],
+                        np.int64)
+        lens = np.array([[ln for (_, _, _, st) in parsed[n][1] for (_, ln) in st] for n in range(N)], np.int64)
+        rec = _StateRecorder(blob, offs, np.stack(n_sym), every)
+        self.decode_device(blob, offs, lens, shapes_of, lane=lane, _streams=rec.decode)
+        words = rec.points.cpu().numpy().view(np.uint32).astype(np.int64)
+        # the saved state (l3c_dec_stream_t.state) -> (low, high, flip, bits)
+        pt_stream = np.repeat(np.arange(N * offs.shape[1]), rec.counts)
+        pt_len = lens.reshape(-1)[pt_stream]
+        long_ = pt_len >= (1 << 28)
+        past = (words[:, 0] >> 31) & 1
+        bits = words[:, 3] | (np.where(long_, words[:, 4], past) << 32)
+        low = words[:, 0] & 0x7FFFFFFF
+        host = np.zeros(int(starts[-1]) + len(datas[-1]) if N else 0, np.uint8)
+        for n, dta in enumerate(datas):
+            host[starts[n]:starts[n] + len(dta)] = np.frombuffer(dta, np.uint8)
+        flip = (words[:, 2] ^ _seek.code_windows(host, offs.reshape(-1)[pt_stream], pt_len, bits)) & 0x80000000
+        out, P = [], offs.shape[1]
+        for n in range(N):
+            cnt = rec.counts[n * P:(n + 1) * P]
+            a, b = rec.first[n * P], rec.first[n * P] + cnt.sum()
+            out.append(_seek.write_index(datas[n], every, cnt, low[a:b], words[a:b, 1], flip[a:b], bits[a:b]))
+        return out
 
     def _decode_rgb_pipelined(self, l, S, tg, C, K, L, table, d, dev, n_chunks=None, lane=None, coarse=False):
         """RGB scale: channel c's means depend on the decoded channels < c at the same pixel
@@ -1024,7 +1185,7 @@ class BatchCodec(object):
 
     def _decode_scales(self, blob, offs, lens, layout, channels, recursive, lane, network, rows, raster,
                        symbols=lambda idx, S: S, features=lambda idx, F: F,
-                       row_pitch=lambda dmll: E.table_pitch(dmll.L), bands=lambda idx: None):
+                       row_pitch=lambda dmll: E.table_pitch(dmll.L), bands=lambda idx: None, streams=None):
         """The coarse-to-fine walk of every decode: full decodes of equal-size, tiled and ragged batches
         (decode_device) and region passes (decode_region_pass).  blob: the uploaded containers; offs / lens int64
         [N][streams per image] in the order of the stream_layout `layout`, where every stream reads its bytes in place;
@@ -1047,6 +1208,8 @@ class BatchCodec(object):
             from the [N][C][T] descriptors d;
           raster(idx, Sp) -> S [N][C][H][W]; symbols(idx, S), features(idx, F) -> what of them the next network reads
             (all of it by default);
+          streams(dmll, desc, coarse) -> None: decodes the streams of the descriptors desc in place of one
+            l3c_ac_decode_streams launch (seek-indexed decodes, DESIGN §4.13); coarse: the tables hold coarse records;
           bands(idx) -> None, or the bands (region.plan_bands) the scale is decoded in (DESIGN §4.10): then per band
             network(..., band) runs on the band's window of the whole coarser scale, rows(..., band) builds the band's
             rows into a table of the band's own stream planes, the band's streams decode into those planes and their
@@ -1061,6 +1224,9 @@ class BatchCodec(object):
             Sp = torch.empty(N, C, int(layout[3][idx]), dtype=torch.uint8, device=dev)     # symbols in stream order
 
             def decode(dsc):
+                if streams is not None:
+                    coarse = not uniform and row_pitch(dmll) == E.COARSE_PITCH
+                    return self._on_decoder_stream(lane, lambda: streams(dmll, dsc, coarse))
                 self._on_decoder_stream(lane, lambda: E.ac_decode_streams(dsc, dev, dmll.L))
 
             def steps(build):
@@ -1120,7 +1286,7 @@ class BatchCodec(object):
         return S
 
     @_on_device
-    def decode_device(self, blob, offs, lens, shapes, lane=None, tile=None):
+    def decode_device(self, blob, offs, lens, shapes, lane=None, tile=None, seeks=None, _streams=None):
         """Decode streams that already sit in HBM: `blob` uint8 device buffer (readable 4 bytes past
         every stream), offs/lens int64 [N][streams per image] in container order (coarse -> fine,
         channel-major), shapes [(C,H,W)] coarse -> fine.  Returns uint8 [N,3,H,W] on the device.
@@ -1132,9 +1298,17 @@ class BatchCodec(object):
         shapes may also be one list per image: a ragged batch (DESIGN §4.6) when they differ; image n then is the
         top-left H_n x W_n of the result, zero elsewhere.
         The scales are walked by _decode_scales; between stream and raster planes lies a view, l3c_reorder_tiles
-        (tiled) or l3c_ragged_pack (ragged)."""
+        (tiled) or l3c_ragged_pack (ragged).
+        seeks: one seek.SeekIndex (or None) per image (reference layout only, DESIGN §4.13): every stream of an image
+        with an index decodes as segments from its seek points, one l3c_ac_decode_segments launch per bottleneck or
+        uniform scale and per RGB channel, whose rows are built whole first.  Images without one decode serially."""
         dev = blob.device
         N = offs.shape[0]
+        # _streams: _StateRecorder.decode (seek_index)
+        if seeks is not None and any(sk is not None for sk in seeks):
+            if tile is not None:
+                raise ValueError('seek indexes are for reference-layout containers, not tiled ones')
+            _streams = _SegmentDecode(blob, offs, seeks).decode
         if shapes and isinstance(shapes[0][0], (tuple, list)):
             shapes_of = [[tuple(int(v) for v in s) for s in sh] for sh in shapes]
             if len(shapes_of) != N:
@@ -1201,7 +1375,13 @@ class BatchCodec(object):
                 l = E.ragged_pack(l, 1, H, W, ext_dev(idx), plane, True)
             l = l.view(N, 1, plane, l.shape[-1])
             Sv = Sp.view(N, C, 1, plane)
-            if dmll.rgb_scale:
+            if dmll.rgb_scale and _streams is not None:
+                # every channel's rows whole, then all its segments in one launch (steps)
+                if coarse(dmll):
+                    steps(lambda c: E.dmll_build_coarse(l, Sv, tg, K, dmll.L, c, table))
+                else:
+                    steps(lambda c: E.dmll_build_table(l, Sv, tg, C, K, dmll.L, True, c, table))
+            elif dmll.rgb_scale:
                 self._decode_rgb_pipelined(l, Sv, tg, C, K, dmll.L, table, d.reshape(N, C), dev, lane=lane,
                                            coarse=coarse(dmll))
             else:
@@ -1218,7 +1398,7 @@ class BatchCodec(object):
         return self._decode_scales(
             blob, offs, lens, stream_layout(shapes_of, tile), [s[0] for s in shapes_of[0]], Rs.pop(), lane,
             network, rows, raster, row_pitch=lambda dmll: E.COARSE_PITCH if coarse(dmll) else E.table_pitch(dmll.L),
-            bands=bands)
+            bands=bands, streams=_streams)
 
     def _geometry(self):
         """region.DecoderGeometry of this codec's network, built once."""

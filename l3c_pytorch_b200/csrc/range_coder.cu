@@ -226,10 +226,16 @@ __device__ __forceinline__ uint32_t shl64_hi(uint64_t x, uint32_t n) {
 // The shifted low is not masked to 31 bits on the chain: its bit 31 only flips bit 31 of low and high, which leaves
 // low ^ high (k), the underflow bits below the first differing one (u) and every later low's bits 0..30 unchanged;
 // the record and the terminator clear it.
+// SEEK (l3c_ac_encode_streams_seek): before symbol j = every, 2 every, ... < n (every a multiple of 32: the start of a
+// batch), lane 0 writes the decoder's low and high to words 0 and 1 of point j / every - 1 at `pts`; the width of the
+// previous symbol gives high: r + 1 = width << s.
+template <bool SEEK = false>
 __device__ __forceinline__ void encode_records(const uint32_t *__restrict__ iv, uint32_t n, uint2 (*ring)[32],
-                                               uint32_t bar0, int lane) {
+                                               uint32_t bar0, int lane, uint32_t every = 0u,
+                                               uint32_t *__restrict__ pts = nullptr) {
     uint32_t next = (lane < n) ? __ldg(iv + lane) : 0u;
     uint32_t lowp = 0u, s = 32u;
+    uint32_t wlast = 0u;                                   // SEEK: width - 1 of the last symbol coded
     uint64_t xl, xh;
     {
         const uint32_t v = __shfl_sync(FULL, next, 0);
@@ -261,6 +267,7 @@ __device__ __forceinline__ void encode_records(const uint32_t *__restrict__ iv, 
         }                                                                                                          \
         lowp = low;                                                                                                \
         s = k + u;                                                                                                 \
+        if constexpr (SEEK) wlast = wm1;                                                                           \
     }
 
     uint32_t b = 0;
@@ -268,6 +275,15 @@ __device__ __forceinline__ void encode_records(const uint32_t *__restrict__ iv, 
         const uint32_t mine = next;
         const uint32_t nb = base + 32 + lane;
         next = (nb < n) ? __ldg(iv + nb) : 0u;              // prefetch the next 32 intervals
+        if constexpr (SEEK) {
+            if (base != 0u && base % every == 0u && lane == 0) {
+                const uint32_t lowc = shl_c(lowp, s) & 0x7FFFFFFFu;
+                const uint32_t sp = min(s, 63u);
+                uint32_t *pt = pts + 4u * (base / every - 1u);
+                pt[0] = lowc;
+                pt[1] = lowc + (uint32_t)((((uint64_t)wlast + 1ull) << sp) - 1ull);
+            }
+        }
         uint32_t rec_low = 0u, rec_ku = 0u;
         if (n - base >= 32u) {
 #pragma unroll
@@ -295,8 +311,17 @@ __device__ __forceinline__ void encode_records(const uint32_t *__restrict__ iv, 
 }
 
 // Emitter warp: the batches of 32 records in order, then the termination record; writes the words and out_len.
+// SEEK: after the batch that ends before a point, lane 0 writes words 2 and 3 of the point: the code bits the decoder
+// has read there, 32 + the sum of k + u over the symbols before it (64 bits: word 2 the low, word 3 the high word), and
+// in bit 31 of word 3 whether the last renormalisation shift before it was an underflow shift.  Such a shift
+// subtracts 2^30 from the code value before shifting it (torchac.cpp:360), so after it the value is the last 32 code
+// bits read with bit 31 flipped; after an "equal MSB" shift it is those bits.  Symbols with no shift leave it as it was.
+template <bool SEEK = false>
 __device__ __forceinline__ void emit_records(const l3c_enc_stream_t &st, const uint2 (*ring)[32], uint32_t *stage,
-                                             uint32_t bar0, int lane, uint32_t *out_len) {
+                                             uint32_t bar0, int lane, uint32_t *out_len, uint32_t every = 0u,
+                                             uint32_t *__restrict__ pts = nullptr) {
+    uint64_t bits = 32u;
+    uint32_t flip = 0u;
     Emitter em;
     em.stage = stage;
     em.pending = 0u;
@@ -313,6 +338,20 @@ __device__ __forceinline__ void emit_records(const l3c_enc_stream_t &st, const u
         const uint2 rec = ring[slot][lane];
         mbar_arrive(bar0 + 8 * (ENC_RING + slot));                                              // empty[slot]
         if (b == n_batches) em.pending += 1u;
+        if constexpr (SEEK) {
+            if (b < n_batches) {
+                const uint32_t k = rec.y & 0xFFu, u = rec.y >> 8;
+                bits += __reduce_add_sync(FULL, k + u);
+                const uint32_t shifted = __ballot_sync(FULL, k + u != 0u);
+                if (shifted) flip = __shfl_sync(FULL, u, 31 - __clz((int)shifted)) != 0u ? 0x80000000u : 0u;
+                const uint32_t end = 32u * (b + 1u);
+                if (end < st.n_sym && end % every == 0u && lane == 0) {
+                    uint32_t *pt = pts + 4u * (end / every - 1u);
+                    pt[2] = (uint32_t)bits;
+                    pt[3] = (uint32_t)(bits >> 32) | flip;
+                }
+            }
+        }
         em.emit(rec.x, rec.y & 0xFFu, rec.y >> 8);
     }
     BitSink &sink = em.sink;
@@ -349,6 +388,35 @@ ac_encode_kernel(const l3c_enc_stream_t *__restrict__ streams, int n_streams, ui
         encode_records(st.intervals, st.n_sym, s_ring[sslot], bar0, lane);
     else
         emit_records(st, s_ring[sslot], s_stage[sslot], bar0, lane, out_len + sid);
+}
+
+// ac_encode_kernel that also records the decoder's state every `every` symbols (l3c_ac_encode_streams_seek): the
+// same bytes; points[sid] receives 4 words per point (encode_records / emit_records with SEEK)
+template <int SPC>
+__global__ void __launch_bounds__(64 * SPC)
+ac_encode_seek_kernel(const l3c_enc_stream_t *__restrict__ streams, int n_streams, uint32_t *__restrict__ out_len,
+                      uint32_t every, uint32_t *const *__restrict__ points) {
+    __shared__ uint2 s_ring[SPC][ENC_RING][32];
+    __shared__ uint32_t s_stage[SPC][STAGE_WORDS];
+    __shared__ __align__(8) uint64_t s_bar[SPC][2 * ENC_RING];
+    const int warp_id = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int sslot = warp_id % SPC;
+    const uint32_t bar0 = smem_u32(s_bar[sslot]);
+    if (warp_id < SPC && lane == 0) {
+#pragma unroll
+        for (int i = 0; i < 2 * ENC_RING; ++i) mbar_init(bar0 + 8 * i, 32);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const int sid = blockIdx.x * SPC + sslot;
+    if (sid >= n_streams) return;
+    const l3c_enc_stream_t st = streams[sid];
+    uint32_t *pts = points[sid];
+    if (warp_id < SPC)
+        encode_records<true>(st.intervals, st.n_sym, s_ring[sslot], bar0, lane, every, pts);
+    else
+        emit_records<true>(st, s_ring[sslot], s_stage[sslot], bar0, lane, out_len + sid, every, pts);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -530,10 +598,20 @@ __device__ __forceinline__ bool chunk_of(uint32_t n, uint32_t first, uint32_t co
 
 // Opens the stream at symbol `first`: at its head when first == 0, else where the previous launch saved its state.
 // Returns the bit position of the stream's first code bit (save_stream() needs it).
+// SEG (segment mode, l3c_ac_decode_segments): first is 0 and a non-null `state` holds a seek point (low, high, flip,
+// bits: low word, high word): the code value is the 32 code bits ending at `bits`, bit 31 flipped by `flip`.
+template <bool SEG = false>
 __device__ __forceinline__ uint32_t open_stream(const l3c_dec_stream_t &st, uint32_t first, BitSource &src,
                                                 CoderState &cs) {
     const uint32_t bit0 = src.open(st.in, st.in_len);
-    if (first == 0) {
+    if (SEG && st.state != nullptr) {
+        const uint64_t bits = ((uint64_t)st.state[4] << 32) | st.state[3];
+        src.seek(bit0 + bits - 32u);
+        const uint32_t value = src.take(32) ^ st.state[2];
+        cs.low = st.state[0];
+        cs.r = st.state[1] - cs.low;
+        cs.dv = value - cs.low;
+    } else if (first == 0) {
         src.seek(bit0);
         cs.reset(src.take(32));
     } else {
@@ -613,6 +691,8 @@ __device__ __forceinline__ void store_group(uint8_t *out, const uint32_t (&packe
 // lane, one compare and one max-reduction.  Groups of 8 symbols run as straight-line speculative code
 // (see v3::ac_decode_kernel); a group that trips the sticky flag is replayed with exact_step().
 // ---------------------------------------------------------------------------------------------
+// SEG: every descriptor is a segment (l3c_ac_decode_segments), decoded whole from its seek point
+template <bool SEG = false>
 __global__ void __launch_bounds__(32)
 ac_decode32_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, int L,
                    uint32_t first, uint32_t count) {
@@ -626,7 +706,7 @@ ac_decode32_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, 
 
     BitSource src;
     CoderState cs;
-    const uint32_t bit0 = open_stream(st, first, src, cs);
+    const uint32_t bit0 = open_stream<SEG>(st, first, src, cs);
 
     const uint16_t *__restrict__ table = st.table;
     const int64_t pitch = st.row_pitch;
@@ -705,7 +785,7 @@ ac_decode32_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, 
 #pragma unroll 1
     for (uint32_t i = base; i < last; ++i) exact(i);
 
-    if (lane == 0) save_stream(st, cs, src, bit0);
+    if (!SEG && lane == 0) save_stream(st, cs, src, bit0);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -782,7 +862,8 @@ __device__ __forceinline__ bool spec_group(CoderState &cs, BitSource &src, const
 //     passes) -- except entry L when it shares a pair of spec_group's select tree with entry L-1 (odd L): a 0 there
 //     would pass and hide entry L-1, so it repeats entry L-1's proposal, which passes exactly when that one does;
 //   * only entries m < L count towards the symbol index.
-template <bool FULLROW, int SPC>
+// SEG: segment mode (see ac_decode32_kernel)
+template <bool FULLROW, int SPC, bool SEG = false>
 __global__ void __launch_bounds__(64 * SPC)
 ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, int L, uint32_t first, uint32_t count) {
     extern __shared__ __align__(16) uint8_t dec_smem[];
@@ -894,7 +975,7 @@ ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, in
     // ============================ decoder warp ============================
     BitSource src;
     CoderState cs;
-    const uint32_t bit0 = open_stream(st, first, src, cs);
+    const uint32_t bit0 = open_stream<SEG>(st, first, src, cs);
     for (uint32_t gi = 0; gi < n_groups; ++gi) {
         const uint32_t g = gi & 1u;
         mbar_wait(bar0 + 8 * g, (gi >> 1) & 1u);                              // full[g]
@@ -935,7 +1016,7 @@ ac_decode_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, in
         __syncwarp();
         mbar_arrive(bar0 + 16 + 8 * g);                                       // empty[g]
     }
-    if (lane == 0) save_stream(st, cs, src, bit0);
+    if (!SEG && lane == 0) save_stream(st, cs, src, bit0);
 }
 
 }  // namespace v3
@@ -1067,7 +1148,8 @@ __device__ __forceinline__ bool spec_group(CoderState &cs, BitSource &src, const
 }
 
 // streams: row_pitch >= COARSE_REC_U16 (uint16), table 4-byte aligned; targets_dev: the 256 RGB bin targets
-template <int SPC>
+// SEG: segment mode (see ac_decode32_kernel)
+template <int SPC, bool SEG = false>
 __global__ void __launch_bounds__(64 * SPC, 1)
 ac_decode_coarse_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_streams, const float *__restrict__ targets,
                         uint32_t first, uint32_t count) {
@@ -1152,7 +1234,7 @@ ac_decode_coarse_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_stre
     // ============================ decoder warp ============================
     BitSource src;
     CoderState cs;
-    const uint32_t bit0 = open_stream(st, first, src, cs);
+    const uint32_t bit0 = open_stream<SEG>(st, first, src, cs);
     uint8_t *__restrict__ sym_out = st.sym_out;
     for (uint32_t gi = 0; gi < n_groups; ++gi) {
         const uint32_t g = gi & 1u;
@@ -1188,7 +1270,7 @@ ac_decode_coarse_kernel(const l3c_dec_stream_t *__restrict__ streams, int n_stre
         mbar_arrive(bar0 + 16 + 8 * g);                                          // empty[g]
         if (lane == 0) store_group(sym_out + ibase, packed, min(last - ibase, (uint32_t)G));
     }
-    if (lane == 0) save_stream(st, cs, src, bit0);
+    if (!SEG && lane == 0) save_stream(st, cs, src, bit0);
 }
 
 }  // namespace coarse
@@ -1603,6 +1685,28 @@ extern "C" int l3c_ac_encode_streams(const l3c_enc_stream_t *streams_dev, int n_
     return L3C_OK;
 }
 
+extern "C" int l3c_ac_encode_streams_seek(const l3c_enc_stream_t *streams_dev, int n_streams, uint32_t *out_len_dev,
+                                          uint32_t every, uint32_t *const *points_dev, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(n_streams >= 0, "l3c_ac_encode_streams_seek: n_streams=%d", n_streams);
+    L3C_REQUIRE(every >= 32u && every % 32u == 0u, "l3c_ac_encode_streams_seek: every=%u is not a positive multiple "
+                "of 32", every);
+    if (n_streams == 0) return L3C_OK;
+    L3C_REQUIRE(streams_dev && out_len_dev && points_dev, "l3c_ac_encode_streams_seek: null pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int spc = encoder_spc();
+    if (spc == 4)
+        ac_encode_seek_kernel<4><<<ceil_div(n_streams, 4), 256, 0, st>>>(streams_dev, n_streams, out_len_dev, every,
+                                                                          points_dev);
+    else if (spc == 2)
+        ac_encode_seek_kernel<2><<<ceil_div(n_streams, 2), 128, 0, st>>>(streams_dev, n_streams, out_len_dev, every,
+                                                                          points_dev);
+    else
+        ac_encode_seek_kernel<1><<<n_streams, 64, 0, st>>>(streams_dev, n_streams, out_len_dev, every, points_dev);
+    L3C_LAUNCH_CHECK("ac_encode_seek_kernel");
+    return L3C_OK;
+}
+
 extern "C" int l3c_set_encoder_streams_per_cta(int spc) {
     L3C_REQUIRE(spc == 0 || spc == 1 || spc == 2 || spc == 4,
                 "l3c_set_encoder_streams_per_cta: spc=%d not in {0, 1, 2, 4}", spc);
@@ -1624,17 +1728,17 @@ static int decoder_spc() {
     return forced ? forced : env_spc;
 }
 
-template <bool FULLROW>
+template <bool FULLROW, bool SEG = false>
 void launch_decode(const l3c_dec_stream_t *streams, int n, int L, uint32_t first, uint32_t count, int spc,
                    cudaStream_t st) {
     using v3::ac_decode_kernel;
     using v3::STREAM_SMEM;
     if (spc == 4)
-        ac_decode_kernel<FULLROW, 4><<<ceil_div(n, 4), 256, 4 * STREAM_SMEM, st>>>(streams, n, L, first, count);
+        ac_decode_kernel<FULLROW, 4, SEG><<<ceil_div(n, 4), 256, 4 * STREAM_SMEM, st>>>(streams, n, L, first, count);
     else if (spc == 2)
-        ac_decode_kernel<FULLROW, 2><<<ceil_div(n, 2), 128, 2 * STREAM_SMEM, st>>>(streams, n, L, first, count);
+        ac_decode_kernel<FULLROW, 2, SEG><<<ceil_div(n, 2), 128, 2 * STREAM_SMEM, st>>>(streams, n, L, first, count);
     else
-        ac_decode_kernel<FULLROW, 1><<<n, 64, STREAM_SMEM, st>>>(streams, n, L, first, count);
+        ac_decode_kernel<FULLROW, 1, SEG><<<n, 64, STREAM_SMEM, st>>>(streams, n, L, first, count);
 }
 }  // namespace l3c
 
@@ -1735,6 +1839,58 @@ extern "C" int l3c_ac_decode_streams_coarse(const l3c_dec_stream_t *streams_dev,
     // logged under the decoder family's name, like every v3 variant: a decode makes the same launches whether its
     // RGB scale reads coarse records or full rows
     L3C_LAUNCH_CHECK("ac_decode_kernel");
+    return L3C_OK;
+}
+
+// segment mode: every descriptor is decoded whole (first 0, every symbol), from its seek point when `state` is set
+extern "C" int l3c_ac_decode_segments(const l3c_dec_stream_t *segs_dev, int n_segs, int L, void *stream) {
+    using namespace l3c;
+    L3C_REQUIRE(n_segs >= 0, "l3c_ac_decode_segments: n_segs=%d", n_segs);
+    L3C_REQUIRE(L >= 1 && L <= 256, "l3c_ac_decode_segments: L=%d not in [1,256]", L);
+    if (n_segs == 0) return L3C_OK;
+    L3C_REQUIRE(segs_dev, "l3c_ac_decode_segments: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (L <= 32) {
+        ac_decode32_kernel<true><<<n_segs, 32, 0, st>>>(segs_dev, n_segs, L, 0u, 0xFFFFFFFFu);
+    } else {
+        const int spc = decoder_spc();
+        static bool configured_dev[64] = {};
+        bool &configured = configured_dev[current_device_slot()];
+        if (!configured) {
+            L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode_kernel<true, 4, true>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * v3::STREAM_SMEM));
+            L3C_CUDA(cudaFuncSetAttribute(v3::ac_decode_kernel<false, 4, true>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * v3::STREAM_SMEM));
+            configured = true;
+        }
+        if (L == 256)
+            launch_decode<true, true>(segs_dev, n_segs, L, 0u, 0xFFFFFFFFu, spc, st);
+        else
+            launch_decode<false, true>(segs_dev, n_segs, L, 0u, 0xFFFFFFFFu, spc, st);
+    }
+    L3C_LAUNCH_CHECK("ac_decode_segments");
+    return L3C_OK;
+}
+
+extern "C" int l3c_ac_decode_segments_coarse(const l3c_dec_stream_t *segs_dev, int n_segs, const float *targets_dev,
+                                             void *stream) {
+    using namespace l3c;
+    using coarse::ac_decode_coarse_kernel;
+    L3C_REQUIRE(n_segs >= 0, "l3c_ac_decode_segments_coarse: n_segs=%d", n_segs);
+    if (n_segs == 0) return L3C_OK;
+    L3C_REQUIRE(segs_dev && targets_dev, "l3c_ac_decode_segments_coarse: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int spc = decoder_spc();
+    if (spc == 4)
+        ac_decode_coarse_kernel<4, true><<<ceil_div(n_segs, 4), 256, coarse::smem_bytes(4), st>>>(
+            segs_dev, n_segs, targets_dev, 0u, 0xFFFFFFFFu);
+    else if (spc == 2)
+        ac_decode_coarse_kernel<2, true><<<ceil_div(n_segs, 2), 128, coarse::smem_bytes(2), st>>>(
+            segs_dev, n_segs, targets_dev, 0u, 0xFFFFFFFFu);
+    else
+        ac_decode_coarse_kernel<1, true><<<n_segs, 64, coarse::smem_bytes(1), st>>>(segs_dev, n_segs, targets_dev, 0u,
+                                                                                    0xFFFFFFFFu);
+    L3C_LAUNCH_CHECK("ac_decode_segments_coarse");
     return L3C_OK;
 }
 

@@ -1175,3 +1175,28 @@ def ac_decode_streams(desc_np, device, L, first=0, count=None, desc_dev=None, n=
     check(lib.l3c_ac_decode_streams(_ptr(desc_dev), n, L, first, count, _stream_ptr()))
     LAUNCHES['n'] += 1
     return desc_dev
+
+
+def ac_encode_streams_seek(desc_np, device, every, points_dev, point_off):
+    """ac_encode_streams that also records seek points every `every` symbols (l3c_ac_encode_streams_seek): stream i's
+    points go to points_dev (int32 [points][4]) from row point_off[i] on.  Returns (desc_dev, lens_dev int32)."""
+    n = desc_np.shape[0]
+    desc = _desc_to_device(desc_np, device)
+    ptrs = _to_device_async(points_dev.data_ptr() + 16 * np.asarray(point_off, np.int64), device)
+    lens = torch.empty(n, dtype=torch.int32, device=device)
+    check(lib.l3c_ac_encode_streams_seek(_ptr(desc), n, _ptr(lens), int(every), _ptr(ptrs), _stream_ptr()))
+    LAUNCHES['n'] += int(n > 0)
+    return desc, lens, ptrs
+
+
+def ac_decode_segments(segs_np, device, L, targets=None):
+    """l3c_ac_decode_segments on the segment descriptors segs_np (DEC_STREAM_DTYPE); with `targets`, the coarse
+    variant (tables of coarse records).  -> the uploaded descriptors (keep them alive until the launch ran)."""
+    n = segs_np.shape[0]
+    segs = _desc_to_device(segs_np, device)
+    if targets is None:
+        check(lib.l3c_ac_decode_segments(_ptr(segs), n, L, _stream_ptr()))
+    else:
+        check(lib.l3c_ac_decode_segments_coarse(_ptr(segs), n, _ptr(targets), _stream_ptr()))
+    LAUNCHES['n'] += int(n > 0)
+    return segs
