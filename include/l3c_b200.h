@@ -506,6 +506,15 @@ int l3c_decode_rgb_pipelined(const float *l_dev, uint8_t *sym_dev, const float *
  * l3c_dmll_build_table builds (cdf[256] = 2^16 is implied).  sym_dev: the decoded R (and G) symbols for c > 0. */
 int l3c_dmll_build_coarse(const float *l_dev, const uint8_t *sym_dev, const float *targets_dev, int N, int HW, int K,
                           int L, int c, int pix0, int npix, uint16_t *rec_dev, void *stream);
+/* l3c_dmll_build_coarse on decoder windows (region decodes of seek-indexed reference-layout containers, DESIGN §4.13
+ * "Regions"): image n's parameters are the rectangle geo_dev[n] = (oy, ox, H_n, W_n) (int32 [N][4], 16-byte aligned)
+ * of l_dev NHWC [N][Hl][Wl][120]; its records and decoded symbols are in the raster order of that H_n x W_n rectangle,
+ * in planes of `plane` elements (record of sub-pixel p of channel c at rec_dev[((n*3 + c)*plane + p) * 96]),
+ * max_hw = max_n H_n * W_n.  Null pointers, L != 256, c outside 0..2, c > 0 without sym_dev and max_hw outside
+ * 1..plane are refused (L3C_EINVAL) before anything is launched. */
+int l3c_dmll_build_coarse_windows(const float *l_dev, int Hl, int Wl, const int *geo_dev, int max_hw, int plane,
+                                  const uint8_t *sym_dev, const float *targets_dev, int N, int K, int L, int c,
+                                  uint16_t *rec_dev, void *stream);
 /* l3c_ac_decode_streams for L = 256 with every stream's `table` pointing at coarse records (row_pitch >= 96, 4-byte
  * aligned); targets_dev: the 256 bin targets the records were built with.  The entries between two coarse entries
  * are evaluated on demand, with the builder's arithmetic: symbols and saved states equal a full-row decode. */

@@ -102,6 +102,8 @@ _SIGNATURES = {
     'l3c_decode_rgb_pipelined': (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_void_p, c_int, c_void_p, c_int, c_void_p,
                                          c_void_p, c_void_p, c_int]),
     'l3c_dmll_build_coarse': (c_int, [c_void_p] * 3 + [c_int] * 7 + [c_void_p, c_void_p]),
+    'l3c_dmll_build_coarse_windows': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int] + [c_void_p] * 2 +
+                                      [c_int] * 4 + [c_void_p, c_void_p]),
     'l3c_ac_decode_streams_coarse': (c_int, [c_void_p, c_int, c_void_p, c_uint32, c_uint32, c_void_p]),
     'l3c_pack_streams': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'l3c_splice_streams': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_int64,

@@ -66,6 +66,34 @@ def stitch(parts):
     return torch.cat(rows, dim=2)
 
 
+def part_rects(shapes):
+    """shapes: (H, W) of every part of an image, unpadded, in `stitch` order (the parts' file order) -> the (y, x, h, w)
+    each one covers in the stitched image.  ValueError for anything `stitch` would not build as a grid: a part count
+    that is not the square of a power of two, a grid row whose parts differ in height or a grid column whose parts differ in width."""
+    shapes = [(int(h), int(w)) for (h, w) in shapes]
+    side = math.isqrt(len(shapes))
+    if not shapes or side * side != len(shapes) or side & (side - 1):
+        # iter_crops splits in quadrants: a grid is 2^k x 2^k parts (stitch fails on any other square)
+        raise ValueError('Invalid number of parts {}'.format(len(shapes)))
+    pos = _crop_positions(side)
+    grid = [None] * len(shapes)
+    for i, p in enumerate(pos):
+        grid[p] = shapes[i]
+    heights = [{grid[r * side + c][0] for c in range(side)} for r in range(side)]
+    widths = [{grid[r * side + c][1] for r in range(side)} for c in range(side)]
+    for r, hs in enumerate(heights):
+        if len(hs) != 1:
+            raise ValueError('parts of grid row {} have different heights {}'.format(r, sorted(hs)))
+    for c, ws in enumerate(widths):
+        if len(ws) != 1:
+            raise ValueError('parts of grid column {} have different widths {}'.format(c, sorted(ws)))
+    ys, xs = [0], [0]
+    for hs, ws in zip(heights, widths):
+        ys.append(ys[-1] + hs.pop())
+        xs.append(xs[-1] + ws.pop())
+    return [(ys[p // side], xs[p % side]) + shapes[i] for i, p in enumerate(pos)]
+
+
 class CropLossCombinator(object):
     """bpsp of several crops -> one bpsp, weighted by crop size (auto_crop.py:139-152)."""
 

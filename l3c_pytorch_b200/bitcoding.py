@@ -323,22 +323,94 @@ class Bitcoding(object):
                 outs[i] = sk
         return outs
 
-    def decode_region(self, data, region, level=0, lane=None):
-        """One region of a tiled container (DESIGN §4.8) -> int64 1CHW tensor (GPU), equal bit for bit to the same
-        crop of decode_batch([data])[0].  region = (y, x, h, w): at level 0 in the coordinates decode() returns (the
-        unpadded image); at level k >= 1 (RGB baselines) in those of the stored scale-k thumbnail.  Only the tile
-        streams and decoder windows the region depends on are decoded.  ValueError, before any GPU work, for an
-        untiled container, a container this model did not write, an empty region or one outside the image, and a
-        level that does not exist.  lane: as in decode_batch (BatchCodec.lanes; the caller has made `lane.main`
-        current)."""
-        return self.decode_regions([data], [region], [level], lane=lane)[0]
+    def decode_region(self, data, region, level=0, lane=None, seek=None):
+        """One region of a tiled container, or of a reference-layout one with its seek index `seek` (sidecar bytes;
+        DESIGN §4.8, §4.13 "Regions") -> int64 1CHW tensor (GPU), equal bit for bit to the same crop of
+        decode_batch([data])[0].  region = (y, x, h, w): at level 0 in the coordinates decode() returns (the unpadded
+        image); at level k >= 1 (RGB baselines) in those of the stored scale-k thumbnail.  Only the tile streams (the
+        segments of the row bands) and decoder windows the region depends on are decoded.  ValueError, before any GPU
+        work, for a reference-layout container without an index, an index of another container, a container this model
+        did not write, an empty region or one outside the image, and a level that does not exist.  lane: as in
+        decode_batch (BatchCodec.lanes; the caller has made `lane.main` current)."""
+        return self.decode_regions([data], [region], [level], lane=lane, seeks=None if seek is None else [seek])[0]
 
-    def decode_regions(self, datas, regions, levels=None, lane=None):
+    def decode_regions(self, datas, regions, levels=None, lane=None, seeks=None):
         """decode_region for many (container, region[, level]) pairs -> list of int64 1CHW tensors in input order.
-        In f16 and f16x2 the pairs of one level and tile size decode in one pass, whatever the shapes of their regions
-        and images; in tf32 / fp32 pairs whose plans have equal window shapes share one pass and the others run one
-        after another (BatchCodec.decode_regions)."""
-        return [S.long() for S in self.codec.decode_regions(datas, regions, levels, lane=lane)]
+        seeks: None, or one seek index (bytes) or None per container.  In f16 and f16x2 the pairs of one level and tile
+        size (or of indexed reference-layout containers) decode in one pass, whatever the shapes of their regions and
+        images; in tf32 / fp32 pairs whose plans have equal window shapes share one pass and the others run one after
+        another (BatchCodec.decode_regions)."""
+        return [S.long() for S in self.codec.decode_regions(datas, regions, levels, lane=lane, seeks=seeks)]
+
+    def decode_region_file(self, pin, region, level=0, lane=None):
+        """decode_region of a file: a tiled container as it is; a reference-layout one with its seek index
+        `pin + '.seek'`; an image the reference stored in parts (`pin.partN`, or `pin` when only the parts exist) from
+        the parts the region touches, each with its own `.seek` index, in one decode_regions call, the crops stitched
+        (auto_crop.part_rects).  -> int64 1CHW tensor (GPU), the same crop of decode(pin).  ValueError, before any GPU
+        work, naming the file, for a missing or mismatched index and for tiled parts (a large tiled image is one
+        container, crop=False); for level > 0 of an image in parts; and for what decode_regions refuses."""
+        from . import seek as _seek
+        from .codec import container_tile
+
+        def read(p):
+            with open(p, 'rb') as f:
+                return f.read()
+
+        def index_of(p, data):
+            if not os.path.isfile(p + SEEK_SUFFIX):
+                raise ValueError('{} is a reference-layout file: a region decode needs its seek index {} '
+                                 '(`idx {}`)'.format(p, p + SEEK_SUFFIX, p))
+            sk = read(p + SEEK_SUFFIX)
+            try:
+                _seek.parse_index(sk, data)
+            except ValueError as e:
+                raise ValueError('%s: %s' % (p + SEEK_SUFFIX, e))
+            return sk
+
+        if not os.path.isfile(pin) and os.path.isfile(pin + part_suffix_helper.make_part_suffix(0)):
+            pin = pin + part_suffix_helper.make_part_suffix(0)
+        if not part_suffix_helper.contains_part_suffix(pin):
+            data = read(pin)
+            if container_tile(data) is not None:
+                return self.decode_region(data, region, level, lane)
+            return self.decode_region(data, region, level, lane, seek=index_of(pin, data))
+        paths = part_suffix_helper.iter_part_suffixes(pin)
+        datas = [read(p) for p in paths]
+        for p, d in zip(paths, datas):
+            if container_tile(d) is not None:
+                raise ValueError('{} is a tiled part: region decode of part files reads reference-layout parts with '
+                                 'seek indexes (a large tiled image is one container, crop=False)'.format(p))
+        if level != 0:
+            raise ValueError('level {}: the parts of {} are crops of the image, not of its thumbnails'.format(
+                level, pin))
+        seeks = [index_of(p, d) for p, d in zip(paths, datas)]
+        shapes = []
+        for d in datas:
+            (left, right, top, bottom), scales = parse_container(d)
+            if not scales:
+                raise ValueError('an empty part container')
+            shapes.append((scales[-1][1] - top - bottom, scales[-1][2] - left - right))
+        rects = auto_crop.part_rects(shapes)
+        Ht, Wt = max(r[0] + r[2] for r in rects), max(r[1] + r[3] for r in rects)
+        if len(region) != 4:
+            raise ValueError('region must be (y, x, h, w), got %r' % (region,))
+        y, x, h, w = (int(v) for v in region)
+        if h < 1 or w < 1:
+            raise ValueError('empty region %r' % (tuple(region),))
+        if y < 0 or x < 0 or y + h > Ht or x + w > Wt:
+            raise ValueError('region %r lies outside the %dx%d image' % (tuple(region), Ht, Wt))
+        sel, subs = [], []
+        for i, (py, px, ph, pw) in enumerate(rects):
+            y0, x0, y1, x1 = max(y, py), max(x, px), min(y + h, py + ph), min(x + w, px + pw)
+            if y0 < y1 and x0 < x1:
+                sel.append(i)
+                subs.append((y0 - py, x0 - px, y1 - y0, x1 - x0))
+        pieces = self.decode_regions([datas[i] for i in sel], subs, lane=lane, seeks=[seeks[i] for i in sel])
+        out = torch.empty(1, 3, h, w, dtype=torch.int64, device=self._device())
+        for i, (sy, sx, sh, sw), piece in zip(sel, subs, pieces):
+            oy, ox = rects[i][0] + sy - y, rects[i][1] + sx - x
+            out[:, :, oy:oy + sh, ox:ox + sw] = piece
+        return out
 
     def update_region(self, data, pos, patch):
         """A tiled container with the pixels at pos = (y, x) replaced by `patch` (DESIGN §4.12) -> the new container

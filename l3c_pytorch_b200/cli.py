@@ -11,7 +11,8 @@
 
 `enc --seek K` also writes OUT.l3c.seek, the file's seek index (DESIGN §4.13): the range coder's state every K
 symbols, with which `dec` decodes every stream as parallel segments; the .l3c file itself is unchanged.  `idx`
-writes the index of an existing file (one written by the reference, say).
+writes the index of an existing file (one written by the reference, say).  With it, `dec --region` reads a crop of
+a reference-layout file, or of an image stored in `.partN` parts, from the row bands the crop needs.
 
 `upd --edit PATCH.png Y,X` (repeatable) applies more edits after the positional one, in order, in one call that
 re-encodes every tile the edits reach once (DESIGN §4.12, "Batches of updates").
@@ -178,7 +179,9 @@ def build_parser():
     d.add_argument('inp')
     d.add_argument('out_png')
     d.add_argument('--region', default=None, type=parse_region, metavar='Y,X,H,W',
-                   help='tiled files: decode only this crop (DESIGN §4.8), decoding only the tiles it depends on')
+                   help='decode only this crop, and only the tiles (DESIGN §4.8) or, for reference-layout files '
+                        'and their .partN parts, the row bands of the seek index written by `idx` (§4.13) it '
+                        'depends on')
     d.add_argument('--level', default=0, type=int, metavar='K',
                    help='with --region, RGB baselines: the crop is of the stored scale-K thumbnail (0 = the image)')
     u = sub.add_parser('upd', help='tiled L3C files: write OUT.l3c, IN.l3c with the pixels at Y,X replaced by '
@@ -228,20 +231,12 @@ def parse_region(text):
 
 
 def decode_region(bc, pin, png_out, region, level=0):
-    """`dec --region`: one crop of a tiled file.  ValueError for crop files (`.partN`, an image coded in parts) and
-    for what Bitcoding.decode_region refuses."""
-    from . import part_suffix_helper
-    if not os.path.isfile(pin):
-        if os.path.isfile(pin + '.part0'):
-            raise ValueError('{} is stored in parts ({}.part0, ...): region decode of part files is not '
-                             'supported'.format(pin, pin))
+    """`dec --region`: one crop of a tiled file, of a reference-layout file with its seek index (`idx IN.l3c` writes
+    it), or of an image the reference stored in parts (`.partN` files, each with its index) --
+    Bitcoding.decode_region_file.  ValueError for what that refuses, e.g. a missing index or tiled parts."""
+    if not os.path.isfile(pin) and not os.path.isfile(pin + '.part0'):
         raise DecodeError('File not found: {}'.format(pin))
-    if part_suffix_helper.contains_part_suffix(pin):
-        raise ValueError('{} is one part of an image coded in parts: region decode of part files is not '
-                         'supported'.format(pin))
-    with open(pin, 'rb') as f:
-        data = f.read()
-    img = bc.decode_region(data, region, level)
+    img = bc.decode_region_file(pin, region, level)
     write_image(img, png_out)
     print('Decoded region {} (level {}) of {} -> {}'.format(region, level, pin, png_out))
 

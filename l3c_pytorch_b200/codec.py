@@ -544,9 +544,12 @@ class UpdateJob(object):
 class _SegmentDecode(object):
     """decode_device's stream hook for seek-indexed images (DESIGN §4.13): the seek points of the batch uploaded once,
     and per call one l3c_ac_decode_segments launch of every segment of the descriptors' streams.  blob / offs as in
-    decode_device; seeks: seek.SeekIndex or None per image."""
+    decode_device; seeks: seek.SeekIndex or None per image.
+    A region pass (decode_region_pass) gives the first P streams of every container (those of the scales its plans
+    walk) and ranges = (start, lo, hi) int64 [N][P]: the stream symbol a descriptor's table and symbols start at and
+    the symbols [lo, hi) to decode (seek.plan_segments)."""
 
-    def __init__(self, blob, offs, seeks):
+    def __init__(self, blob, offs, seeks, ranges=None):
         N, P = offs.shape
         self.dev = blob.device
         addr = blob.data_ptr() + offs.reshape(-1)
@@ -556,20 +559,22 @@ class _SegmentDecode(object):
         for n, sk in enumerate(seeks):
             if sk is None:
                 continue
-            if sk.counts.size != P:
+            if sk.counts.size != P and (ranges is None or sk.counts.size < P):
                 raise ValueError('seek index %d lists %d streams, the container has %d' % (n, sk.counts.size, P))
             every[n * P:(n + 1) * P] = sk.every
-            first[n * P:(n + 1) * P] = base + sk.first
+            first[n * P:(n + 1) * P] = base + sk.first[:P]
             words.append(sk.state_words())
             base += sk.low.size
         order = np.argsort(addr, kind='stable')
         self.addr, self.every, self.first = addr[order], every[order], first[order]
+        self.ranges = (None,) * 3 if ranges is None else tuple(np.asarray(r, np.int64).reshape(-1)[order]
+                                                               for r in ranges)
         w = np.concatenate(words) if words else np.zeros((0, _seek.STATE_WORDS), np.uint32)
         self.states = E._to_device_async(np.concatenate([w.reshape(-1), [0]]).astype(np.uint32).view(np.int32),
                                          self.dev)
 
     def decode(self, dmll, desc, coarse):
-        segs = _seek.plan_segments(desc, self.addr, self.every, self.first, self.states.data_ptr())
+        segs = _seek.plan_segments(desc, self.addr, self.every, self.first, self.states.data_ptr(), *self.ranges)
         E.ac_decode_segments(segs, self.dev, dmll.L, dmll.targets(self.dev) if coarse else None)
 
 
@@ -1185,7 +1190,8 @@ class BatchCodec(object):
 
     def _decode_scales(self, blob, offs, lens, layout, channels, recursive, lane, network, rows, raster,
                        symbols=lambda idx, S: S, features=lambda idx, F: F,
-                       row_pitch=lambda dmll: E.table_pitch(dmll.L), bands=lambda idx: None, streams=None):
+                       row_pitch=lambda dmll: E.table_pitch(dmll.L), bands=lambda idx: None, streams=None,
+                       zero=False):
         """The coarse-to-fine walk of every decode: full decodes of equal-size, tiled and ragged batches
         (decode_device) and region passes (decode_region_pass).  blob: the uploaded containers; offs / lens int64
         [N][streams per image] in the order of the stream_layout `layout`, where every stream reads its bytes in place;
@@ -1210,6 +1216,8 @@ class BatchCodec(object):
             (all of it by default);
           streams(dmll, desc, coarse) -> None: decodes the streams of the descriptors desc in place of one
             l3c_ac_decode_streams launch (seek-indexed decodes, DESIGN §4.13); coarse: the tables hold coarse records;
+          zero: the stream planes start zeroed (a region pass over bands leaves the symbols before a seek point
+            undecoded);
           bands(idx) -> None, or the bands (region.plan_bands) the scale is decoded in (DESIGN §4.10): then per band
             network(..., band) runs on the band's window of the whole coarser scale, rows(..., band) builds the band's
             rows into a table of the band's own stream planes, the band's streams decode into those planes and their
@@ -1221,7 +1229,8 @@ class BatchCodec(object):
         bn8, F, S = None, None, None
         self._mark('start')
         for idx, ((scale, dmll, uniform), C) in enumerate(zip(self.iter_scale_dmll(recursive), channels)):
-            Sp = torch.empty(N, C, int(layout[3][idx]), dtype=torch.uint8, device=dev)     # symbols in stream order
+            Sp = (torch.zeros if zero else torch.empty)(N, C, int(layout[3][idx]), dtype=torch.uint8,
+                                                        device=dev)                        # symbols in stream order
 
             def decode(dsc):
                 if streams is not None:
@@ -1408,47 +1417,65 @@ class BatchCodec(object):
         return self._geo
 
     # ------------------------------------------------------------------------------------------
-    def plan_regions(self, datas, regions, levels=None):
+    def plan_regions(self, datas, regions, levels=None, seeks=None):
         """Parse, validate and plan (region.plan_region) every (container, region, level) of a decode_regions call,
-        before any GPU work: -> ([(pad_tuple, scales)] parsed, [RegionPlan]).  ValueError for an untiled
-        container, a container this model cannot have written, an empty region or one outside the image, and a
-        level that does not exist."""
+        before any GPU work: -> ([(pad_tuple, scales)] parsed, [RegionPlan]).  seeks: None, or one seek index
+        (sidecar bytes) or None per container; every index is parsed (seek.parse_index) first, and a reference-layout
+        container with one is planned in bands (RegionPlan.seek holds its SeekIndex).  ValueError for a
+        reference-layout container without an index, a malformed or mismatched index, a container this model cannot
+        have written, an empty region or one outside the image, and a level that does not exist."""
         from .region import DecoderGeometry, plan_region
         if len(regions) != len(datas):
             raise ValueError('%d regions for %d containers' % (len(regions), len(datas)))
         levels = [0] * len(datas) if levels is None else list(levels)
         if len(levels) != len(datas):
             raise ValueError('%d levels for %d containers' % (len(levels), len(datas)))
+        seeks = [None] * len(datas) if seeks is None else list(seeks)
+        if len(seeks) != len(datas):
+            raise ValueError('%d seek indexes for %d containers' % (len(seeks), len(datas)))
+        indexes = []
+        for i, (sk, dta) in enumerate(zip(seeks, datas)):
+            try:
+                indexes.append(None if sk is None else _seek.parse_index(sk, dta))
+            except ValueError as err:
+                raise ValueError('seek index %d: %s' % (i, err))
         geo = DecoderGeometry(self.net)
         parsed, plans = [], []
-        for i, (dta, reg, lev) in enumerate(zip(datas, regions, levels)):
+        for i, (dta, reg, lev, sk) in enumerate(zip(datas, regions, levels, indexes)):
             pt, scales = parse_container(dta)
             tile = container_tile(dta)
-            if tile is None:
+            if tile is None and sk is None:
                 raise ValueError('container %d: region decode needs a tiled container (written with '
-                                 'Bitcoding(..., tile=(th, tw))); the streams of the reference layout are serial' % i)
+                                 'Bitcoding(..., tile=(th, tw))) or the seek index of a reference-layout one '
+                                 '(Bitcoding.seek_index, `idx IN.l3c`); the streams of the reference layout are serial'
+                                 % i)
             shapes = [(C, H, W) for (C, H, W, _) in scales]
             try:
                 self._check_shapes(shapes)
             except ValueError as err:
                 raise ValueError('container %d was not written by this model: %s' % (i, err))
             parsed.append((pt, scales))
-            plans.append(plan_region(shapes, pt, tile, geo, reg, lev))
+            plan = plan_region(shapes, pt, tile, geo, reg, lev, every=None if sk is None else sk.every)
+            plan.seek = sk
+            plans.append(plan)
         return parsed, plans
 
     @_on_device
-    def decode_regions(self, datas, regions, levels=None, lane=None):
-        """Decode one region of each tiled container (DESIGN §4.8): -> [uint8 [1, C, h, w] on the device] in input
-        order, each equal to the same crop of the full decode (at level k >= 1, of the stored scale-k plane).  Only the
-        tile streams and decoder windows the region depends on are decoded.  In f16 and f16x2, pairs whose plans walk
+    def decode_regions(self, datas, regions, levels=None, lane=None, seeks=None):
+        """Decode one region of each container (DESIGN §4.8): -> [uint8 [1, C, h, w] on the device] in input order,
+        each equal to the same crop of the full decode (at level k >= 1, of the stored scale-k plane).  Only the tile
+        streams and decoder windows the region depends on are decoded.  In f16 and f16x2, pairs whose plans walk
         the same scales with the same tile size (RegionPlan.pass_key) share one ragged pass: one network pass per scale
         on a padded batch of their windows and one range-decoder launch per channel step; pairs of equal
         RegionPlan.shape_key share an equal-shape pass, and in tf32 / fp32 the groups of equal shape_key run one after
         another (region.plan_passes, decode_region_pass; REGION_RAGGED_PASS = False forces that grouping everywhere).
         regions: (y, x, h, w) each; levels: None (all 0) or one int each.
+        seeks: None, or one seek index (sidecar bytes) or None per container: a reference-layout container needs one
+        and decodes full-width bands, each channel's stream from the seek point before its band (DESIGN §4.13
+        "Regions"); its passes never include tiled containers.
         lane: as in decode_batch -- the caller has made `lane.main` current; the range decoders run on the lane's
         decoder streams."""
-        parsed, plans = self.plan_regions(datas, regions, levels)
+        parsed, plans = self.plan_regions(datas, regions, levels, seeks)
         blob, starts = _upload(datas, self.blueprint.device)
         self.region_counts = {'streams': 0, 'symbols': 0}          # of this call: every pass adds to them
         return self._decode_planned(blob, starts, [[st for (_, _, _, st) in p[1]] for p in parsed], plans, lane)
@@ -1479,11 +1506,17 @@ class BatchCodec(object):
         the pass's largest, plan n top-left (get_P_nhwc(windows=)), and the kernels take per-image rectangles
         (l3c_crop_rects, l3c_dmll_build_table_windows, l3c_reorder_tiles_images); each plan's per-channel tile streams
         are padded with empty ones to the pass's largest tile count (stream_layout(pad_tiles=True)).
+        Band plans of seek-indexed reference-layout containers (tile None, DESIGN §4.13 "Regions"): every scale's
+        rectangle is a full-width band, one stream per channel whose segments over ScalePlan.seg are decoded
+        (_SegmentDecode), laid out for the kernels as one tile (region.band_tile); the RGB scale builds coarse records
+        (l3c_dmll_build_coarse_windows) where the whole-file decode does (f16, L = 256, K = 10), and the band's symbols
+        before its seek point stay zero.
         -> [uint8 [1, C, h_n, w_n]], the regions.  lane: as in decode_device."""
         dev = blob.device
         N = len(plans)
         p0 = plans[0]
         tile = p0.tile
+        band = tile is None
         K = self.net.config_ms.prob.K
 
         def size(r):
@@ -1507,6 +1540,17 @@ class BatchCodec(object):
 
         rects_of = [[(sp.C,) + size(sp.rect) for sp in p.scales] for p in plans]
 
+        def ktile(idx):
+            # the tile the layout kernels see: the container's, or for bands one that puts them in raster order
+            if not band:
+                return tile
+            from .region import band_tile
+            return band_tile(plans, idx)
+
+        def coarse(dmll):
+            # as decode_device's coarse(): the RGB scale of a seek-indexed decode in f16 from coarse records
+            return band and dmll.rgb_scale and dmll.L == 256 and K == 10 and E.f16_mode()
+
         def network(idx, scale, bn8, F):
             wins = [size(p.scales[idx].window) for p in plans]
             l, F = self.net.get_P_nhwc(scale, bn8, F, windows=wins if len(set(wins)) > 1 else None)
@@ -1517,21 +1561,27 @@ class BatchCodec(object):
             C, plane = Sp.shape[1:]
             tg = dmll.targets(dev)
             ext = [r[idx][1:] for r in rects_of]
+            if coarse(dmll):
+                geo = rows_dev([p.scales[idx].out[:2] + e for p, e in zip(plans, ext)])
+                max_hw = max(h * w for h, w in ext)
+                return steps(lambda c: E.dmll_build_coarse_windows(l, geo, max_hw, plane, Sp, tg, K, dmll.L, c, table))
             if ragged:
                 geo = rows_dev([p.scales[idx].out[:2] + e for p, e in zip(plans, ext)])
                 max_hw = max(h * w for h, w in ext)
                 steps(lambda c: E.dmll_build_table_windows(l, geo, max_hw, plane, Sp, tg, C, K, dmll.L, c >= 0, c,
-                                                           table, tile))
+                                                           table, ktile(idx)))
             else:
                 (oy, ox), (H, W) = p0.scales[idx].out[:2], ext[0]
                 steps(lambda c: E.dmll_build_table_window(l, oy, ox, Sp, tg, C, K, dmll.L, c >= 0, c, table, H, W,
-                                                          tile))
+                                                          ktile(idx)))
 
         def raster(idx, Sp):
             ext = [r[idx][1:] for r in rects_of]
             H, W = pad(ext)
             if ragged:
-                return E.reorder_tiles_images(Sp, rows_dev(ext), H, W, tile)      # [N][C][H][W], zero-padded
+                return E.reorder_tiles_images(Sp, rows_dev(ext), H, W, ktile(idx))   # [N][C][H][W], zero-padded
+            if band:
+                return Sp.view(N, Sp.shape[1], H, W)                              # a band's stream order is raster
             return E.reorder_tiles(Sp, H, W, tile, False).view(N, Sp.shape[1], H, W)
 
         # the finer networks' inputs: their windows of this scale's symbols and, where they fuse them, of its features
@@ -1549,9 +1599,18 @@ class BatchCodec(object):
 
         layout = stream_layout(rects_of, tile, pad_tiles=ragged)
         self.region_counts['streams'] += int((layout[2] > 0).sum())        # the empty ones that pad a ragged pass aside
-        self.region_counts['symbols'] += int(layout[2].sum())
+        self.region_counts['symbols'] += sum(p.symbols for p in plans)
+        streams = None
+        if band:
+            # per stream (plan, scale, channel: the container's first streams, in order) its band's symbols
+            rng = np.array([[(sp.rect[0] * sp.W,) + sp.seg for sp in p.scales for _ in range(sp.C)] for p in plans],
+                           np.int64)
+            streams = _SegmentDecode(blob, offs, [p.seek for p in plans],
+                                     (rng[:, :, 0], rng[:, :, 1], rng[:, :, 2])).decode
         S = self._decode_scales(blob, offs, lens, layout, [r[0] for r in rects_of[0]], p0.recursive, lane,
-                                network, rows, raster, symbols, features)
+                                network, rows, raster, symbols, features,
+                                row_pitch=lambda dmll: E.COARSE_PITCH if coarse(dmll) else E.table_pitch(dmll.L),
+                                streams=streams, zero=band)
         return crop(S, [(p.region[0] - p.scales[-1].rect[0], p.region[1] - p.scales[-1].rect[1]) for p in plans],
                     [size(p.region) for p in plans], nhwc=False, split=True)
 

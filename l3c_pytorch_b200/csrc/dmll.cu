@@ -218,17 +218,35 @@ dmll_table_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym,
 // Coarse rows of RGB channel c (L = 256, raster stream order): per sub-pixel the record of dmll_math.cuh
 // (COARSE_REC_U16) -- channel_params() exactly as dmll_table_kernel computes them, and the entries cdf[8 i].  One
 // warp per record: lane l writes parameter word l and evaluates coarse entry l, 32 instead of 256 entries.
+// WIN (l3c_dmll_build_coarse_windows): every image n has its own rectangle geo[n] = (oy, ox, H_n, W_n) of a decoder
+// window's output, l_hw pixels per image and Wl wide; its records and the decoded symbols are in the raster order of
+// the H_n x W_n rectangle, in planes of HW (>= H_n * W_n) elements, and pix0 is 0.
+template <bool WIN = false>
 __global__ void __launch_bounds__(TB_THREADS)
 dmll_coarse_kernel(const float *__restrict__ l, const uint8_t *__restrict__ sym, const float *__restrict__ targets,
-                   int HW, int c, int pix0, int npix, uint16_t *__restrict__ rec) {
+                   int HW, int c, int pix0, int npix, uint16_t *__restrict__ rec, const int4 *__restrict__ geo = nullptr,
+                   int64_t l_hw = 0, int Wl = 0) {
     constexpr int K = 10, C = 3, Kp = 4 * C * K;
     __shared__ float s_par[TB_PIX][COARSE_PARAM_WORDS + 1];          // odd pitch: conflict-free column writes
     const int n = blockIdx.y;
+    int oy = 0, ox = 0, w = 1;
+    if constexpr (WIN) {
+        const int4 g = geo[n];
+        oy = g.x, ox = g.y, w = g.w;
+        npix = g.z * g.w;
+    }
     const int q0 = blockIdx.x * TB_PIX;
     const int np = min(TB_PIX, npix - q0);
+    if (WIN && np <= 0) return;                        // past this image's rectangle (uniform per CTA)
     if ((int)threadIdx.x < np) {
         const int p = pix0 + q0 + threadIdx.x;
-        const float *lp = l + ((size_t)n * HW + p) * Kp;
+        const float *lp;
+        if constexpr (WIN) {
+            const int py = p / w, px = p - py * w;
+            lp = l + ((size_t)n * l_hw + (size_t)(oy + py) * Wl + ox + px) * Kp;
+        } else {
+            lp = l + ((size_t)n * HW + p) * Kp;
+        }
         float xr = 0.f, xg = 0.f;
         if (c >= 1) xr = (float)sym[((size_t)n * C + 0) * HW + p];
         if (c >= 2) xg = (float)sym[((size_t)n * C + 1) * HW + p];
@@ -856,6 +874,25 @@ extern "C" int l3c_dmll_build_coarse(const float *l_dev, const uint8_t *sym_dev,
     dmll_coarse_kernel<<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(l_dev, sym_dev, targets_dev, HW, c, pix0, npix,
                                                                       rec_dev);
     L3C_LAUNCH_CHECK("dmll_coarse_kernel");
+    return L3C_OK;
+}
+
+extern "C" int l3c_dmll_build_coarse_windows(const float *l_dev, int Hl, int Wl, const int *geo_dev, int max_hw,
+                                             int plane, const uint8_t *sym_dev, const float *targets_dev, int N,
+                                             int K, int L, int c, uint16_t *rec_dev, void *stream) {
+    using namespace l3c;
+    if (int e = check_common("l3c_dmll_build_coarse_windows", N, plane, 3, K, L, 1)) return e;
+    L3C_REQUIRE(L == 256, "l3c_dmll_build_coarse_windows: coarse rows exist for L=256 only, got L=%d", L);
+    L3C_REQUIRE(l_dev && targets_dev && rec_dev && geo_dev, "l3c_dmll_build_coarse_windows: null pointer");
+    L3C_REQUIRE(c >= 0 && c < 3 && (c == 0 || sym_dev),
+                "l3c_dmll_build_coarse_windows: c=%d (decoded symbols needed for c>0)", c);
+    L3C_REQUIRE(Hl >= 1 && Wl >= 1 && max_hw >= 1 && max_hw <= plane,
+                "l3c_dmll_build_coarse_windows: %dx%d parameter plane, max_hw=%d plane=%d", Hl, Wl, max_hw, plane);
+    L3C_REQUIRE(((uintptr_t)geo_dev & 15) == 0, "l3c_dmll_build_coarse_windows: geo must be 16-byte aligned");
+    dim3 grid(ceil_div(max_hw, TB_PIX), N);
+    dmll_coarse_kernel<true><<<grid, TB_THREADS, 0, (cudaStream_t)stream>>>(
+        l_dev, sym_dev, targets_dev, plane, c, 0, 0, rec_dev, (const int4 *)geo_dev, (int64_t)Hl * Wl, Wl);
+    L3C_LAUNCH_CHECK("dmll_coarse_windows_kernel");
     return L3C_OK;
 }
 

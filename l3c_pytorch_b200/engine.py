@@ -1135,6 +1135,17 @@ def dmll_build_coarse(l, sym, targets, K, L, c, rec, pix0=0, npix=None):
     LAUNCHES['n'] += 1
 
 
+def dmll_build_coarse_windows(l, geo_dev, max_hw, plane, sym, targets, K, L, c, rec):
+    """dmll_build_coarse on decoder windows (l3c_dmll_build_coarse_windows): image n's parameters are the rectangle
+    geo_dev[n] = (oy, ox, H_n, W_n) (int32 [N, 4] on the device) of l NHWC [N,Hl,Wl,Kp]; its records and `sym` in the
+    raster order of that rectangle, in planes of `plane` elements."""
+    N, Hl, Wl, _ = l.shape
+    assert l.is_contiguous() and geo_dev.shape == (N, 4) and geo_dev.dtype == torch.int32
+    check(lib.l3c_dmll_build_coarse_windows(_ptr(l), Hl, Wl, _ptr(geo_dev), int(max_hw), int(plane), _ptr(sym),
+                                            _ptr(targets), N, K, L, c, _ptr(rec), _stream_ptr()))
+    LAUNCHES['n'] += 1
+
+
 def ac_decode_streams_coarse(desc_np, device, targets, first=0, count=None, desc_dev=None, n=None):
     """ac_decode_streams (L = 256) for streams whose `table` points at coarse records (row_pitch COARSE_PITCH)."""
     if desc_dev is None:

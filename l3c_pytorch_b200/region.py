@@ -15,6 +15,11 @@ full run.  `plan_region` walks the scales fine to coarse:
 At a clipped edge the window edge is the image edge, so the kernels' zero padding is the image's own.  Rectangles
 are tile-aligned (their start on a tile boundary, their end on one or at the plane's edge), so `tile_grid` cuts them
 into the same tiles, in the same order, as the full plane.
+
+A reference-layout container with a seek index (DESIGN §4.13 "Regions") is planned in full-width bands instead: its
+plane is one stream per channel in raster order, so the symbols a scale needs are the rows [a, b) of the finer window
+(of the region at the finest level), and its stream decodes them from the seek point at or before the band's first
+symbol (ScalePlan.seg).
 """
 import numpy as np
 
@@ -85,10 +90,14 @@ class ScalePlan(object):
     grid (tile_grid order).  For a scale with a decoder network: window, the bn_{s+1} rectangle (coarser scale's
     coordinates) its network runs on; out, the rectangle of that network's output (2x the window) that is exact
     and used, i.e. rect relative to 2 * window's origin; fused, whether the coarser decoder's features are added.
-    The uniform-prior scale has window = out = None."""
-    __slots__ = ('idx', 'scale', 'C', 'H', 'W', 'rect', 'tiles', 'window', 'out', 'fused')
+    The uniform-prior scale has window = out = None.
+    seg: None for a tiled container; for a band of a reference-layout container (every channel one stream, tiles
+    [0]) the symbols (s0, s1) of every channel's stream that are decoded: s0 the seek point at or before the band's
+    first needed symbol, s1 = b * W.  rect is then (s0 // W, 0, b, W), and its symbols before s0 are not decoded."""
+    __slots__ = ('idx', 'scale', 'C', 'H', 'W', 'rect', 'tiles', 'window', 'out', 'fused', 'seg')
 
     def __init__(self, **kw):
+        self.seg = None
         for k, v in kw.items():
             setattr(self, k, v)
 
@@ -98,7 +107,8 @@ class ScalePlan(object):
 
     @property
     def symbols(self):
-        return self.C * _area(self.rect)
+        """symbols handed to the range decoder"""
+        return self.C * (_area(self.rect) if self.seg is None else self.seg[1] - self.seg[0])
 
     @property
     def window_pixels(self):
@@ -110,17 +120,20 @@ class ScalePlan(object):
                 self.fused, len(self.tiles))
 
     def __repr__(self):
-        return 'ScalePlan(scale=%d, rect=%s, tiles=%d, window=%s, out=%s, fused=%s)' % (
-            self.scale, self.rect, len(self.tiles), self.window, self.out, self.fused)
+        return 'ScalePlan(scale=%d, rect=%s, tiles=%d, window=%s, out=%s, fused=%s%s)' % (
+            self.scale, self.rect, len(self.tiles), self.window, self.out, self.fused,
+            '' if self.seg is None else ', seg=%s' % (self.seg,))
 
 
 class RegionPlan(object):
     """plan_region's result: scales coarse -> fine (the finest is the requested level), the region in that level's
-    plane, and the totals."""
+    plane, and the totals.  tile None: bands of a reference-layout container whose seek points lie every `every`
+    symbols; `seek`, its parsed index (seek.SeekIndex), is set by BatchCodec.plan_regions."""
 
-    def __init__(self, scales, region, level, tile, n_scales, recursive):
+    def __init__(self, scales, region, level, tile, n_scales, recursive, every=None):
         self.scales, self.region, self.level, self.tile = scales, region, level, tile
         self.n_scales, self.recursive = n_scales, recursive
+        self.every, self.seek = every, None
 
     @property
     def tiles(self):
@@ -156,17 +169,24 @@ class RegionPlan(object):
             self.level, self.region, self.tiles, self.symbols, self.window_pixels)
 
 
-def plan_region(shapes, pad_tuple, tile, config, region, level=0):
+def plan_region(shapes, pad_tuple, tile, config, region, level=0, every=None):
     """shapes: [(C, H, W)] of a container's scales, coarse -> fine; pad_tuple: its (left, right, top, bottom);
     tile: its (th, tw), None for the reference layout; config: a MultiscaleNetwork or its DecoderGeometry;
     region = (y, x, h, w): at level 0 in unpadded image coordinates, at level k >= 1 (RGB baselines) in the
-    coordinates of the stored scale-k plane.  -> RegionPlan.  ValueError for an untiled container, an empty region
-    or one outside the image, and a level that does not exist."""
+    coordinates of the stored scale-k plane; every: the interval K of the seek index of a reference-layout container.
+    -> RegionPlan.  A reference-layout plan is one full-width band per scale: rows [a, b) of the finer window (of the
+    region at the finest level), and of every channel's stream the symbols [K floor(a W / K), b W) (ScalePlan.seg).
+    ValueError for an untiled container without `every`, an empty region or one outside the image, and a level that
+    does not exist."""
     geo = geometry_of(config)
-    if tile is None:
-        raise ValueError('region decode needs a tiled container (written with Bitcoding(..., tile=(th, tw))): '
-                         'the streams of the reference layout are serial')
-    tile = (int(tile[0]), int(tile[1]))
+    if tile is None and every is None:
+        raise ValueError('region decode needs a tiled container (written with Bitcoding(..., tile=(th, tw))) or the '
+                         'seek index of a reference-layout one (Bitcoding.seek_index, `idx IN.l3c`): the streams of '
+                         'the reference layout are serial')
+    if tile is not None:
+        tile = (int(tile[0]), int(tile[1]))
+    else:
+        every = int(every)
     n = len(shapes)
     recursive = n - geo.num_scales - 1
     if recursive < 0:
@@ -197,21 +217,36 @@ def plan_region(shapes, pad_tuple, tile, config, region, level=0):
     for idx in range(idx_f, -1, -1):
         C, H, W = shapes[idx]
         scale = n - 1 - idx
-        rect = _align(want, H, W, tile)
-        th, tw = tile
-        ntx = -(-W // tw)
-        tiles = [ty * ntx + tx for ty in range(rect[0] // th, -(-rect[2] // th))
-                 for tx in range(rect[1] // tw, -(-rect[3] // tw))]
+        seg = None
+        if tile is None:
+            # a full-width band: the stream decodes from the seek point at or before the band's first symbol, and
+            # its rows reach back to that point's row (those rows' CDFs are needed to decode up to the band)
+            seg = (want[0] * W // every * every, want[2] * W)
+            rect, tiles = (seg[0] // W, 0, want[2], W), [0]
+        else:
+            rect = _align(want, H, W, tile)
+            th, tw = tile
+            ntx = -(-W // tw)
+            tiles = [ty * ntx + tx for ty in range(rect[0] // th, -(-rect[2] // th))
+                     for tx in range(rect[1] // tw, -(-rect[3] // tw))]
         if idx == 0:                                                 # the uniform-prior thumbnail
             plans.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect, tiles=tiles, window=None,
-                                   out=None, fused=False))
+                                   out=None, fused=False, seg=seg))
             break
         Hc, Wc = shapes[idx - 1][1:]
         window, out, fused, want = _window(geo, scale, rect, H, W, Hc, Wc)
         plans.append(ScalePlan(idx=idx, scale=scale, C=C, H=H, W=W, rect=rect, tiles=tiles, window=window, out=out,
-                               fused=fused))
+                               fused=fused, seg=seg))
     plans.reverse()
-    return RegionPlan(plans, region_px, level, tile, n, recursive)
+    return RegionPlan(plans, region_px, level, tile, n, recursive, every)
+
+
+def band_tile(plans, idx):
+    """The tile the layout kernels (l3c_dmll_build_table_window(s), l3c_reorder_tiles(_images)) are given for scale idx
+    of a pass of reference-layout band plans: one row tall and as wide as the pass's widest band.  Tiles that span the
+    plane's width put it in raster order whatever their height, and with one row every in-tile product (th * W,
+    tw * h) stays at most the band's width."""
+    return (1, max(p.scales[idx].W for p in plans))
 
 
 def _window(geo, scale, rect, H, W, Hc, Wc, features=None):
@@ -269,7 +304,7 @@ def rect_columns(sp, T):
 
 def stream_columns(plan, tile):
     """Indices, in container order, of the planned streams of every scale: [[column in that scale's stream list]]
-    coarse -> fine (rect_columns)."""
+    coarse -> fine (rect_columns).  A band plan (tile None) lists every channel's one stream."""
     return [rect_columns(sp, len(tile_grid(sp.H, sp.W, tile))) for sp in plan.scales]
 
 

@@ -164,27 +164,38 @@ def code_windows(blob_host, offs, lens, bits):
     return (acc >> (8 - (p & 7))) & 0xFFFFFFFF
 
 
-def plan_segments(desc, in_addr, every, first_point, state_ptr):
+def plan_segments(desc, in_addr, every, first_point, state_ptr, start=None, lo=None, hi=None):
     """Segment descriptors (DEC_STREAM_DTYPE) of the decoder descriptors `desc` [M]: every stream cut into segments of
     its `every` symbols, segment s > 0 starting from seek point first_point + s - 1 of the batch's device state table
     at state_ptr (STATE_WORDS uint32 per point), segment 0 at the stream head.  in_addr: int64 sorted device addresses
     of the bytes of every stream of the batch; every / first_point: int64 per stream, in in_addr's order (a stream
-    without an index has every >= its n_sym: one segment).  Vectorised: no loop per segment."""
+    without an index has every >= its n_sym: one segment).
+    start / lo / hi (int64 per stream, in in_addr's order; None: 0, 0 and start + n_sym): a descriptor's table and
+    sym_out hold the stream's symbols from `start` on, and only [lo, hi) of them are needed (a band of a region decode,
+    DESIGN §4.13 "Regions").  Then only the segments that meet [lo, hi) are emitted: the first one from the seek point
+    at or before lo (which must not lie before `start`), the last one cut at hi.  Vectorised: no loop per segment."""
     addr = desc['in'].astype(np.int64)
     k = np.minimum(np.searchsorted(in_addr, addr), max(in_addr.size - 1, 0))
     if desc.size and (in_addr.size == 0 or (in_addr[k] != addr).any()):
         raise ValueError('a decoder descriptor reads no stream of the batch')
     K = np.asarray(every, np.int64)[k]
     n = desc['n_sym'].astype(np.int64)
-    nseg = np.maximum(1, -(-n // K))
+    base = np.zeros_like(n) if start is None else np.asarray(start, np.int64)[k]
+    a = base if lo is None else np.asarray(lo, np.int64)[k]
+    b = base + n if hi is None else np.asarray(hi, np.int64)[k]
+    j0 = a // K
+    if (j0 * K < base).any() or (b > base + n).any():
+        raise ValueError('a segment range reaches outside its descriptor\'s symbols')
+    nseg = np.maximum(1, -(-b // K) - j0)
     sid = np.repeat(np.arange(desc.size), nseg)
-    j = np.arange(sid.size) - np.repeat(np.cumsum(nseg) - nseg, nseg)
-    start = j * K[sid]
+    j = j0[sid] + np.arange(sid.size) - np.repeat(np.cumsum(nseg) - nseg, nseg)
+    at = j * K[sid]                                      # the segment's first symbol, in stream coordinates
+    rel = at - base[sid]                                 # ... and in the descriptor's
     segs = desc[sid].copy()
-    segs['n_sym'] = np.minimum(K[sid], n[sid] - start)
+    segs['n_sym'] = np.maximum(0, np.minimum(K[sid], b[sid] - at))
     pitch = desc['row_pitch'].astype(np.int64)[sid]
-    segs['table'] = desc['table'].astype(np.int64)[sid] + 2 * start * pitch
-    segs['sym_out'] = desc['sym_out'].astype(np.int64)[sid] + start
+    segs['table'] = desc['table'].astype(np.int64)[sid] + 2 * rel * pitch
+    segs['sym_out'] = desc['sym_out'].astype(np.int64)[sid] + rel
     pt = np.asarray(first_point, np.int64)[k][sid] + j - 1
     segs['state'] = np.where(j == 0, 0, state_ptr + 4 * STATE_WORDS * pt)
     return segs
