@@ -29,10 +29,11 @@ def _sigmoid(x):
     return 1.0 / (1.0 + np.exp(-x))
 
 
-def _params(kind, rng):
+def _params(kind, rng, N=N, H=H, W=W):
     """l [N, H, W, 4 C K] and symbols [N, C, HW]: 'peaked' = one dominant component with log-scales down to and below
     the -7 clamp (most entries saturated); 'broad' = random-init-like logits, means around the middle of [0, 255] and
     log-scales around 2-4 (few entries saturated); 'mixed' = either, per pixel."""
+    HW = H * W
     shp = (N, HW, C, K)
     dom = rng.integers(0, K, (N, HW, C))
     logit = rng.normal(0, 1, shp)

@@ -14,6 +14,7 @@ from l3c_pytorch_b200.codec import MAGIC, TILED_MAGIC, stream_layout
 from tests.test_gpu_coder_launches import make_stream
 
 M32 = 0xFFFFFFFF
+M64 = (1 << 64) - 1
 
 
 def record_points(cdf, data, L, every):
@@ -37,7 +38,8 @@ def record_points(cdf, data, L, every):
         if i and i % every == 0:
             pts.append((low, high, flip, 32 + pos[0] - 32))
         span = high - low + 1
-        count = ((value - low + 1) * 65536 - 1) // span & 0xFFFF
+        # in uint64 as the reference computes it: on junk input the value can lie below low, and the difference wraps
+        count = (((value - low + 1) * 65536 - 1) & M64) // span & 0xFFFF
         row = [int(v) for v in cdf[i, :L]]
         sym = max(m for m in range(L) if row[m] <= count) if row[0] <= count else 0
         out[i] = sym
